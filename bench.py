@@ -5,7 +5,7 @@ A "step" = one body of GHRegistration::ghicp_reg's while-loop (src/ghicp_reg.cpp
 excluded): calED + calCD_* + findcorrespondence* + transformestimation + adjustweight.
 Default workload = BASELINE.json configs[1]: 50k x 50k keypoints, BSC descriptors, KM matching, 6-DoF.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload ...]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload ...] [--dump-outputs DIR]
 
 Prints ONE JSON line (rank 0).  See DESIGN.md §Measurement for every field.
 """
@@ -50,7 +50,7 @@ def peaks():
             return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 class ClockSampler:
@@ -171,20 +171,7 @@ def make_scene(g, wl, n_override=None, seed=2):
     return sc
 
 
-# dram__bytes_read.sum + dram__bytes_write.sum of ONE k_stream launch, from the committed `ncu --set full` captures
-# (profiles/r01_summary.md); algorithmic bytes are 5.002e9
-# dram__bytes_read.sum + dram__bytes_write.sum of the dominant kernel's launch in an `ncu --set full` capture of the same command
-# (a constant from the committed capture, labelled with its source: a bench run is never taken under the profiler)
-NCU_TRAFFIC = {"config2": {"bytes": 5.038999e9 + 0.32185856e9,
-                           "source": "profiles/r02_ncu_k_stream_km.raw.csv (ncu --set full, k_stream<2,1,1,1,1>, round 2): "
-                                     "5.039 GB read (algorithmic 5.002 GB) + 0.322 GB written (counts, partial sums, edge list)"},
-               "config2-672": {"bytes": 5.038999e9 + 0.32185856e9,
-                               "source": "profiles/r02_ncu_k_stream_km.raw.csv (the same kernel and plane: the descriptor width only "
-                                         "changes the one-time FD build)"},
-               "config2-nnr": {"bytes": 5.179896e9 + 0.321731584e9,
-                               "source": "profiles/r02_ncu_k_stream_nnr.raw.csv (ncu --set full, k_stream<1,1,1,1,1>, round 2)"},
-               "config2-nn": {"bytes": 5.311e9, "source": "profiles/r01_summary.md (ncu --set full capture of k_stream NN, round 1)"}}
-
+H100_SMS = 132
 FT = {"none": 3, "bsc": 0, "fpfh": 2}
 CT = {"nn": 0, "nnr": 1, "km": 2}
 
@@ -305,6 +292,26 @@ def cpu_arm(g, wl, warmup, steps, sizes, fit_steps=3, threads=1, budget_s=240.0)
                 ms_per_step_sample=ms_sample, sample_n=n_s, extrapolated=extrap, fit=fit, registration=reg, ladder=rows)
 
 
+DUMP_MAX_ROWS = 1 << 20   # rows kept per array: with at most 3 float64 columns that is 24 MB per array, well under 64 MB in all
+
+
+def dump_outputs(out_dir, reg, st):
+    """What the last timed step handed to its caller: the step's statistics and transforms, its correspondence pairs and the
+    moved source keypoints, as float64 .npy files (stats.npy holds the IterStats fields named in `scalars`, in that order).  An array longer than DUMP_MAX_ROWS keeps a fixed seeded sample of rows."""
+    os.makedirs(out_dir, exist_ok=True)
+    sp, tp = reg.pairs()
+    scalars = ["iteration", "cor", "converged", "cd_mean", "cd_std", "penalty", "rmse", "rmse_after", "fdm", "fdstd", "iou",
+               "para1", "para2", "km_energy"]
+    arrays = {"stats": np.array([float(getattr(st, k)) for k in scalars]),
+              "rt": st.Rt_np(), "rt_tillnow": reg.Rt_tillnow(),
+              "pairs": np.stack([sp, tp], axis=1), "source": np.ascontiguousarray(reg.source())}
+    for name, a in arrays.items():
+        a = np.asarray(a, dtype=np.float64)
+        if a.ndim and len(a) > DUMP_MAX_ROWS:
+            a = a[np.sort(np.random.default_rng(0).choice(len(a), DUMP_MAX_ROWS, replace=False))]
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def main():
     # stdout carries exactly ONE JSON line: whatever libraries print on fd 1 while we run (NCCL's version banner, ...) goes to
     # stderr; the line itself is written to the saved descriptor at the end
@@ -336,6 +343,8 @@ def _main(saved_stdout):
     ap.add_argument("--n", type=int, default=0, help="override N=M (e.g. 4000: a size the reference runs WITHOUT extrapolation)")
     ap.add_argument("--cpu-sample", type=int, default=0, help="N=M of the CPU arm's main sample")
     ap.add_argument("--no-cpu", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned to DIR/<name>.npy (float64)")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3  # timing rule: >= 3 warm-up steps
@@ -505,6 +514,8 @@ def _main(saved_stdout):
     barrier()
     clocks = cs.summary()
     ms_per_step = allmax(wall * 1e3 / args.steps)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, reg, st)
 
     # ---- timed region 2: end to end through the host-facing API -----------------------------------
     # every step: host (pinned inside the library) -> device copy of the current source + target
@@ -545,23 +556,21 @@ def _main(saved_stdout):
     cost_ms = float(np.median(stage[:, 0]))
     stream_ms = float(np.median(stage[:, 6]))
     achieved = alg_bytes / (stream_ms * 1e-3) / 1e9 if stream_ms > 0 else 0.0
-    traffic = NCU_TRAFFIC.get(args.workload) if (not args.n and world == 1) else None
     roofline = {"kernel": "k_stream (calED+calCD+scan/gate+stats fused over the fp16 FD plane)", "bound": "hbm",
-                "kernel_ms": stream_ms,
+                "kernel_ms": stream_ms, "traffic": None,
                 "achieved": achieved, "peak": hbm_peak, "unit": "GB/s", "frac": achieved / hbm_peak,
-                "traffic": traffic["bytes"] if traffic else None, "traffic_source": traffic["source"] if traffic else None,
                 "peak_source": peak_src, "per_gpu": True, "rows_per_gpu": nloc,
                 "algorithmic_bytes_per_launch": alg_bytes, "sweeps_per_step": n_sweeps}
     if wl["ft"] == "fpfh":
         # matrix-free FPFH: O(N+M) bytes for N*M pair evaluations -> the FP32 pipe, not HBM, bounds the sweep.
         # Dominant kernel = k_ff_sweep<MAIN> (FP32 filter; ms_stream is its CUDA-event time).  Algorithmic work per pair
         # (DESIGN.md §3.5): 33 FFMA (histogram dot) + 12 (hi/lo coordinate differences, d2) + 8 (cost, bound, sum) = 53
-        # FP32-pipe instructions; peak = 148 SMs x 128 lanes x SM clock.
+        # FP32-pipe instructions; peak = SMs x 128 lanes x SM clock.
         pairs = float(nloc) * wl["M"]
         fast = stream_ms > 0
         t_ms = stream_ms if fast else cost_ms
-        sm_mhz = (clocks.get("sm_mhz") or 1965.0)
-        peak_ginstr = 148 * 128 * sm_mhz * 1e6 / 1e9
+        sm_mhz = (clocks.get("sm_mhz") or 1980.0)   # H100 SXM boost clock when no sample was taken
+        peak_ginstr = H100_SMS * 128 * sm_mhz * 1e6 / 1e9
         ach = 53.0 * pairs / (t_ms * 1e-3) / 1e9 if t_ms > 0 else 0.0
         roofline = {"kernel": "k_ff_sweep (FP32 filter over on-the-fly FPFH distances + exact FP64 refinement)" if fast
                     else "k_rowsweep_mf / k_colsweep_mf (exact all-double matrix-free sweeps)",

@@ -1,6 +1,6 @@
-"""gh-icp_b200 — B200-native GH-ICP registration inner loop (host-side Python face).
+"""gh-icp_b200 — GH-ICP registration inner loop for the H100 (host-side Python face).
 
-The product is `libghicp_b200.so` (hand-written sm_100a CUDA kernels behind the C ABI of
+The product is `libghicp_b200.so` (hand-written sm_90a CUDA kernels behind the C ABI of
 include/ghicp_b200.h).  This package is a thin ctypes binding plus a Python mirror of the reference's
 `GHRegistration` interface (include/ghicp_reg.h:74-132) used by tests/ and bench.py.  It never imports
 oracle/ and has no CPU fallback: without the compiled library or without a CUDA device it raises.

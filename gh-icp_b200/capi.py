@@ -57,7 +57,7 @@ def lib_path():
 
 
 def build_library(force=False):
-    """Compile gh-icp_b200/csrc for sm_100a in-tree (nvcc cross-compiles without a GPU)."""
+    """Compile gh-icp_b200/csrc for sm_90a in-tree (nvcc cross-compiles without a GPU)."""
     if force or not os.path.exists(_LIB):
         r = subprocess.run(["make", "-C", os.path.join(_HERE, "csrc"), "-j4"], capture_output=True, text=True)
         if r.returncode != 0:

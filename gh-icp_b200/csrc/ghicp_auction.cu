@@ -27,7 +27,7 @@ namespace {
 constexpr int UNASSIGNED = -1;
 constexpr int DUMMY = -2;
 constexpr int AUC_BLOCK = 256;
-constexpr int AUC_GRID = 148 * 4;
+constexpr int AUC_GRID = GHICP_SMS * 4;
 
 __device__ __forceinline__ unsigned long long d2ull(double v) { return (unsigned long long)__double_as_longlong(v); }
 
@@ -743,7 +743,7 @@ int km_auction_settled(Ctx *c, int n_rows, int n_cols, long long nnz_hint, doubl
   cudaMemcpyAsync(c->d_list[0], base_list, sizeof(int) * (size_t)n_rows, cudaMemcpyDeviceToDevice, st);
   cudaMemcpyAsync(&c->d_counters[0], &c->d_counters[2], sizeof(int), cudaMemcpyDeviceToDevice, st);
   static int blocks_per_sm = 0;
-  int n_sm = 148;
+  int n_sm = GHICP_SMS;
   cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, c->device);
   if (blocks_per_sm == 0) {
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, k_auction_persistent<false>, PA_THREADS, 0);
@@ -826,7 +826,7 @@ int km_auction(Ctx *c, int n_rows, int n_cols, long long nnz, double eps_final, 
   const int max_rounds = 4000000;
   // persistent cooperative launch geometry (all CTAs must be co-resident)
   static int coop_blocks_per_sm[2] = {0, 0};
-  int n_sm = 148;
+  int n_sm = GHICP_SMS;
   cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, c->device);
   if (coop_blocks_per_sm[0] == 0) {
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&coop_blocks_per_sm[0], k_auction_persistent<false>, PA_THREADS, 0);
@@ -883,7 +883,7 @@ int km_auction(Ctx *c, int n_rows, int n_cols, long long nnz, double eps_final, 
     if (ph + 1 == eps_list.size()) {
       unsigned long long *d_D = reinterpret_cast<unsigned long long *>(c->d_bid_aux);  // free scratch between rounds
       cudaMemsetAsync(d_D, 0, sizeof(unsigned long long), st);
-      GHICP_LAUNCH(k_free_price_sum, 148, 256, 0, st, n_cols, c->d_owner, c->d_price, d_D);
+      GHICP_LAUNCH(k_free_price_sum, GHICP_SMS, 256, 0, st, n_cols, c->d_owner, c->d_price, d_D);
       c->launches++;
       unsigned long long D_fx_host = 0ull;
       cudaMemcpyAsync(&D_fx_host, d_D, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st);

@@ -141,7 +141,7 @@ static int alloc_workspaces(Ctx *c) {
   c->nloc = std::max(0, std::min(N, c->r0 + c->shard) - c->r0);
   const int nmax = std::max(c->Npad, M);
   const int row_ctas = (N + 7) / 8;
-  int want = (148 * 4 + row_ctas - 1) / row_ctas;
+  int want = (GHICP_SMS * 4 + row_ctas - 1) / row_ctas;
   int lim = std::max(1, M / 2048);
   c->n_chunks = std::max(1, std::min(want, lim));
   if (c->cfg.corr_type == GHICP_CT_KM || c->world > 1) c->n_chunks = 1;  // one CSR / result segment per row
@@ -260,7 +260,7 @@ static int build_fd(Ctx *c) {
     if (rc) return rc;
     CK(c, cudaMemsetAsync(c->d_fd16, 0, fd_elems(c->fd_rows, c->M) * sizeof(uint16_t), c->stream));  // zero the panel padding
     {
-      // tensor-core build (tcgen05 kind::i8) when the descriptor fits its shared-memory tiling, else POPC
+      // tensor-core build (wgmma s8) when the descriptor fits its shared-memory tiling, else POPC
       cudaError_t e = (getenv("GHICP_FD_POPC") != nullptr) ? cudaErrorNotSupported : launch_fd_bsc_tc(c);
       if (e == cudaErrorNotSupported) { cudaGetLastError(); CK(c, launch_fd_bsc(c)); c->fd_tensor = false; }
       else { CK(c, e); c->fd_tensor = true; }
@@ -271,8 +271,8 @@ static int build_fd(Ctx *c) {
     // Stored float plane (4*N*M bytes) or matrix-free (ghicp_fpfh.cu: FD recomputed inside the sweeps, O(N+M) memory).
     // Both give bit-identical FD / CD values; auto mode stores the plane only while it is a modest share of the HBM.
     const size_t plane_bytes = fd_elems(c->fd_rows, c->M) * sizeof(float);
-    // auto: NN / NNR always go matrix-free (their sweeps then run the FP32-filter fast path, ~9x the all-double
-    // kernels at 200k x 200k on a B200, same correspondences); KM keeps the plane while it is a modest share of the HBM.
+    // auto: NN / NNR always go matrix-free (their sweeps then run the FP32-filter fast path, several times faster than the
+    // all-double kernels, same correspondences); KM keeps the plane while it is a modest share of the HBM.
     bool mf = c->cfg.fpfh_matrix_free > 0 || getenv("GHICP_FPFH_MATRIX_FREE") != nullptr;
     if (!mf && c->cfg.fpfh_matrix_free == 0) {
       size_t free_b = 0, total_b = 0;

@@ -1,15 +1,15 @@
-// ghicp_fdtc.cu — one-time BSC feature-distance build on the 5th-generation tensor cores (tcgen05 + TMEM).
+// ghicp_fdtc.cu — one-time BSC feature-distance build on the Hopper tensor cores (wgmma, integer kind).
 //
 // calFD_BSC (src/ghicp_reg.cpp:143-200): FD[i][j] = min_v Hamming(bscS[v][i], bscT[0][j]).
 // With descriptor bits mapped to +/-1 int8 (padding = 0) the Hamming distance is an integer GEMM:
 //      dot(a, b) = (#equal bits) - (#different bits) = bits - 2 * Hamming   =>   Hamming = (bits - dot) / 2
-// exactly (int32 accumulation of +/-1 products).  One CTA keeps a B tile = 256 (source, variant) rows
-// resident in shared memory and streams 128-row target tiles (A) through a double buffer; a single thread
-// issues tcgen05.mma.kind::i8 (M=128, N=256, K=32 per instruction) into one of two 256-column TMEM
-// accumulators while four warps drain the other one (tcgen05.ld), take the min over the V variants
-// (adjacent accumulator columns, in registers) and store fp16 into the panel-major FD plane.
+// exactly (int32 accumulation of +/-1 products).  One CTA keeps a B tile = TN (source, variant) rows resident in shared
+// memory and streams 64-row target tiles (A) through a ring of K-chunk stages (cp.async.bulk, one mbarrier per stage).
+// Two consumer warpgroups each own half of the B tile's columns and issue wgmma.mma_async m64n32k32.s32.s8.s8 from shared
+// memory into register accumulators; after a tile's last K-chunk they take the min over the V variants (adjacent
+// accumulator columns: in-thread pairs, plus one lane shuffle for V = 4) and store fp16 into the panel-major FD plane.
 // Operands sit in shared memory in the canonical K-major no-swizzle layout [k-chunk(16 B)][row][16 B]
-// (8-row x 16-byte core matrices back to back: SBO = 128 B, LBO = rows * 16 B).
+// (8-row x 16-byte core matrices back to back: SBO = 128 B between row groups, LBO = rows * 16 B between k-chunks).
 #include <cstdlib>
 #include <cuda_fp16.h>
 
@@ -19,9 +19,12 @@ namespace ghicp_b200 {
 
 namespace {
 
-constexpr int TC_TM = 128;   // target rows per A tile  (UMMA M)
-constexpr int TC_TN = 256;   // (source, variant) rows per B tile (UMMA N)
-constexpr int TC_THREADS = 256;
+constexpr int TC_TM = 64;         // target rows per A tile (wgmma M)
+constexpr int TC_NCH = 32;        // B columns per wgmma instruction (N)
+constexpr int TC_CONSUMERS = 2;   // warpgroups; each owns TN / 2 columns of the B tile
+constexpr int TC_THREADS = TC_CONSUMERS * 128 + 32;   // + one producer warp
+constexpr int KC_BYTES = 128;     // K bytes per row and ring stage (4 wgmma K-steps)
+constexpr int KC_STAGES = 4;
 
 #if !defined(GHICP_EMU_HOST)
 __device__ __forceinline__ unsigned smem_u32(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
@@ -65,31 +68,29 @@ __global__ void k_unpack_pm1(const uint64_t *__restrict__ words, int V, int n, i
 }
 
 #if defined(GHICP_EMU_HOST)
-// Host emulation (tests/harness/cuda_emu): mbarriers and bulk copies as in emu_mbarrier.h; tensor memory is an int32 array
-// [128 lanes][512 columns]; one tcgen05.mma kind::i8 K-step is the plain triple loop over the two no-swizzle K-major tiles
-// (k-chunk of 16 bytes outermost, rows 16 bytes apart: the layout k_unpack_pm1 writes); tcgen05.ld 32x32b.x32 gives thread
-// (warp w, lane l) the 32 columns of lane 32 w + l.  Blocks run one at a time, so one static TMEM serves the launch.
-static int emu_tmem[128][512];
+// Host emulation (tests/harness/cuda_emu): mbarriers and bulk copies as in emu_mbarrier.h; one wgmma m64n32k32 s8 is, for
+// the calling thread, the 16 accumulator elements of its fragment computed from the two no-swizzle K-major tiles (the
+// layout k_unpack_pm1 writes), so the fragment mapping of the epilogue is exercised as on the device.
 __device__ __forceinline__ void mbar_init1(unsigned long long *b, int count) { emu::bar_init(b, count); }
 __device__ __forceinline__ void mbar_wait_parity(unsigned long long *b, unsigned parity) { emu::bar_wait(b, parity); }
+__device__ __forceinline__ void mbar_arrive(unsigned long long *b) { emu::bar_arrive(b); }
 __device__ __forceinline__ void bulk_load(void *dst, const void *src, unsigned bytes, unsigned long long *bar) {
   emu::bar_arrive_expect_tx(bar, bytes);
   emu::bulk_copy(dst, src, bytes, bar);
 }
-inline void emu_umma_i8_at(int d_col, const signed char *A, const signed char *B, int TN, bool accumulate) {
-  // A, B point at the first 16-byte k-chunk of this K = 32 step; rows 16 bytes apart, the second k-chunk TM * 16 / TN * 16
-  // bytes further (the no-swizzle K-major layout k_unpack_pm1 writes)
-  for (int m = 0; m < TC_TM; ++m)
-    for (int n = 0; n < TN; ++n) {
-      int acc = accumulate ? emu_tmem[m][d_col + n] : 0;
-      for (int kk = 0; kk < 32; ++kk)
-        acc += (int)A[(size_t)(kk >> 4) * TC_TM * 16 + (size_t)m * 16 + (kk & 15)] * (int)B[(size_t)(kk >> 4) * TN * 16 + (size_t)n * 16 + (kk & 15)];
-      emu_tmem[m][d_col + n] = acc;
-    }
-}
-inline void emu_umma_i8(int d_col, const unsigned char *a_tile, const unsigned char *b_tile, int k, bool accumulate) {
-  emu_umma_i8_at(d_col, reinterpret_cast<const signed char *>(a_tile) + (size_t)k * 2 * TC_TM * 16,
-                 reinterpret_cast<const signed char *>(b_tile) + (size_t)k * 2 * TC_TN * 16, TC_TN, accumulate);
+// A: first 16-byte k-chunk of this K = 32 step of the 64-row stage (k-chunks TC_TM * 16 bytes apart); B: first k-chunk of the
+// step at the instruction's first column (k-chunks TN * 16 bytes apart)
+inline void emu_wgmma_s8(int d[16], const unsigned char *A, const unsigned char *B, int TN, bool accumulate) {
+  const int tid = (int)(emu::cur()->tidx.x & 127), warp = tid >> 5, lane = tid & 31;
+  for (int e = 0; e < 16; ++e) {
+    const int m = warp * 16 + (lane >> 2) + 8 * ((e >> 1) & 1);
+    const int n = 8 * (e >> 2) + 2 * (lane & 3) + (e & 1);
+    int acc = accumulate ? d[e] : 0;
+    for (int kk = 0; kk < 32; ++kk)
+      acc += (int)(signed char)A[(size_t)(kk >> 4) * TC_TM * 16 + (size_t)m * 16 + (kk & 15)] *
+             (int)(signed char)B[(size_t)(kk >> 4) * TN * 16 + (size_t)n * 16 + (kk & 15)];
+    d[e] = acc;
+  }
 }
 #else
 __device__ __forceinline__ void mbar_init1(unsigned long long *b, int count) {
@@ -102,8 +103,11 @@ __device__ __forceinline__ void mbar_wait_parity(unsigned long long *b, unsigned
                  : "=r"(ok) : "r"(smem_u32(b)), "r"(parity) : "memory");
   } while (!ok);
 }
-// One logical tile copy = many 2-4 KB bulk copies in flight (a single large cp.async.bulk is serviced with
-// little memory-level parallelism; measured 13 GB/s per SM for one 56 KB copy), all completing on one mbarrier.
+__device__ __forceinline__ void mbar_arrive(unsigned long long *b) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(b)) : "memory");
+}
+// One logical tile copy = several bulk copies of at most 4 KB in flight (a single large cp.async.bulk is serviced with little
+// memory-level parallelism), all completing on one mbarrier.
 __device__ __forceinline__ void bulk_load(void *dst, const void *src, unsigned bytes, unsigned long long *bar) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
   constexpr unsigned PIECE = 4096;
@@ -113,357 +117,186 @@ __device__ __forceinline__ void bulk_load(void *dst, const void *src, unsigned b
                  ::"r"(smem_u32((unsigned char *)dst + off)), "l"((const unsigned char *)src + off), "r"(n), "r"(smem_u32(bar)) : "memory");
   }
 }
-#endif
 
 __device__ __forceinline__ uint64_t make_desc(unsigned smem_addr, unsigned lbo_bytes, unsigned sbo_bytes) {
-  // SM100 shared-memory matrix descriptor: start address [0,14) (>>4), leading byte offset [16,30) (>>4),
-  // stride byte offset [32,46) (>>4), version = 1 at [46,48), layout type [61,64) = 0 (no swizzle)
+  // SM90 shared-memory matrix descriptor: start address [0,14) (>>4), leading byte offset [16,30) (>>4),
+  // stride byte offset [32,46) (>>4), base offset [49,52) = 0, layout type [62,64) = 0 (no swizzle)
   return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16) |
-         ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32) | (1ull << 46);
+         ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32);
 }
 
-// fences have no meaning on one host thread
-#if defined(GHICP_EMU_HOST)
-#define GHICP_TC_ASM(text) (void)0
-#else
-#define GHICP_TC_ASM(text) asm volatile(text ::: "memory")
+__device__ __forceinline__ void wgmma_s8(int d[16], uint64_t adesc, uint64_t bdesc, unsigned accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.s8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p;\n\t}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]),
+        "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
 #endif
 
-template <int V>
+// keeps the compiler from moving accumulator registers across the asynchronous MMA window
+template <int NC>
+__device__ __forceinline__ void fence_acc(int (&acc)[NC][16]) {
+#if !defined(GHICP_EMU_HOST)
+#pragma unroll
+  for (int c = 0; c < NC; ++c)
+#pragma unroll
+    for (int e = 0; e < 16; ++e) asm volatile("" : "+r"(acc[c][e])::"memory");
+#else
+  (void)acc;
+#endif
+}
+
+// B tile: TN (source, variant) rows x KP bytes, resident.  A tiles: TC_TM target rows, streamed in K-chunks of KC_BYTES through
+// KC_STAGES ring stages (warp 8 loads; every consumer warp hands a stage back on its `empty` barrier once its MMAs retired).
+template <int V, int TN>
 __global__ void __launch_bounds__(TC_THREADS, 1)
-k_fd_bsc_tc(const int8_t *__restrict__ T8c, const int8_t *__restrict__ S8c, unsigned short *__restrict__ fd, int N, int M,
-            size_t fd_rows, int row0, int nloc, int bits, int KP, int dbg) {
+k_fd_bsc_tc(const int8_t *__restrict__ T8c, const int8_t *__restrict__ S8c, unsigned short *__restrict__ fd, int M,
+            size_t fd_rows, int row0, int nloc, int bits, int KP) {
 #if defined(GHICP_EMU_HOST)
   unsigned char *smem = reinterpret_cast<unsigned char *>(emu::dyn_smem());   // host emulation: the launch's dynamic shared memory
 #else
   extern __shared__ __align__(128) unsigned char smem[];
 #endif
-  // barriers: [0,1] A tile landed, [2,3] MMA of tile done, [4,5] TMEM accumulator drained, [6] B tile landed
-  __shared__ __align__(8) unsigned long long s_bar[7];
-  __shared__ unsigned s_tmem_base;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  constexpr int SRC_PER_TILE = TC_TN / V;
-  const unsigned b_bytes = (unsigned)TC_TN * KP, a_bytes = (unsigned)TC_TM * KP;
-  unsigned char *Bs = smem;
-  unsigned char *As[2] = {smem + b_bytes, smem + b_bytes + a_bytes};
-  const int src_base = row0 + blockIdx.x * SRC_PER_TILE;   // first source row of this CTA's B tile
-  const int n_ttiles = (M + TC_TM - 1) / TC_TM;
-
-#if defined(GHICP_EMU_HOST)
-  if (tid == 0) s_tmem_base = 0;   // the whole emulated TMEM, column 0
-#else
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(&s_tmem_base)));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-#endif
-  if (tid == 0) {
-    mbar_init1(&s_bar[0], 1); mbar_init1(&s_bar[1], 1);
-    mbar_init1(&s_bar[2], 1); mbar_init1(&s_bar[3], 1);
-    mbar_init1(&s_bar[4], 128); mbar_init1(&s_bar[5], 128);
-    mbar_init1(&s_bar[6], 1);
-    GHICP_TC_ASM("fence.mbarrier_init.release.cluster;");
-  }
-  GHICP_TC_ASM("tcgen05.fence::before_thread_sync;");
-  __syncthreads();
-  GHICP_TC_ASM("tcgen05.fence::after_thread_sync;");
-  const unsigned tmem_base = s_tmem_base;
-
-  if (warp == 4 && lane == 0) {
-    // ===== producer + MMA issuer (one thread) =====
-    bulk_load(Bs, S8c + (size_t)blockIdx.x * b_bytes, b_bytes, &s_bar[6]);
-    // instruction descriptor (kind::i8): D = s32 [4,6)=2, A = s8 [7,10)=1, B = s8 [10,13)=1, K-major A and B,
-    // N>>3 at [17,23), M>>4 at [24,29)
-    const unsigned idesc = (2u << 4) | (1u << 7) | (1u << 10) | ((unsigned)(TC_TN >> 3) << 17) | ((unsigned)(TC_TM >> 4) << 24);
-    const int ksteps = KP / 32;
-#if !defined(GHICP_EMU_HOST)
-    const unsigned b_addr = smem_u32(Bs);
-#endif
-    bulk_load(As[0], T8c, a_bytes, &s_bar[0]);                      // A(0)
-    for (int t = 0; t < n_ttiles; ++t) {
-      const int s = t & 1;
-      const unsigned ph = (unsigned)((t >> 1) & 1);
-      if (t >= 2) mbar_wait_parity(&s_bar[4 + s], ph ^ 1);      // epilogue(t-2) drained TMEM buffer s
-      if (t == 0) mbar_wait_parity(&s_bar[6], 0);                // B landed
-      mbar_wait_parity(&s_bar[s], ph);                           // A(t) landed
-      GHICP_TC_ASM("tcgen05.fence::after_thread_sync;");
-      const unsigned d_tmem = tmem_base + (unsigned)(s * TC_TN);
-#if defined(GHICP_EMU_HOST)
-      for (int k = 0; k < ((dbg & 2) ? 1 : ksteps); ++k) emu_umma_i8((int)d_tmem, As[s], Bs, k, k > 0);
-      (void)idesc;
-      emu::bar_arrive(&s_bar[2 + s]);                              // tcgen05.commit: the MMAs above have completed
-#else
-      const unsigned a_addr = smem_u32(As[s]);
-      for (int k = 0; k < ((dbg & 2) ? 1 : ksteps); ++k) {
-        const uint64_t adesc = make_desc(a_addr + (unsigned)k * 2u * TC_TM * 16u, TC_TM * 16u, 128u);
-        const uint64_t bdesc = make_desc(b_addr + (unsigned)k * 2u * TC_TN * 16u, TC_TN * 16u, 128u);
-        const unsigned accumulate = k > 0 ? 1u : 0u;
-        asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, {%5, %5, %5, %5}, p;\n\t}\n"
-            ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(0u) : "memory");
-      }
-      asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(&s_bar[2 + s])) : "memory");
-#endif
-      // prefetch A(t+1) into the other buffer as soon as MMA(t-1) has finished reading it: the copy then
-      // overlaps MMA(t)
-      if (t + 1 < n_ttiles) {
-        const int s1 = (t + 1) & 1;
-        if (t >= 1) mbar_wait_parity(&s_bar[2 + s1], (unsigned)(((t - 1) >> 1) & 1));
-        bulk_load(As[s1], T8c + (size_t)(t + 1) * a_bytes, a_bytes, &s_bar[s1]);
-      }
-    }
-  } else if (warp < 4) {
-    // ===== epilogue warps: TMEM -> registers -> min over variants -> fp16 -> FD plane =====
-    for (int t = 0; t < n_ttiles; ++t) {
-      const int s = t & 1;
-      const unsigned ph = (unsigned)((t >> 1) & 1);
-      mbar_wait_parity(&s_bar[2 + s], ph);
-      GHICP_TC_ASM("tcgen05.fence::after_thread_sync;");
-      const int j = t * TC_TM + warp * 32 + lane;  // target column owned by this thread (TMEM lane)
-      const unsigned taddr0 = tmem_base + ((unsigned)(warp * 32) << 16) + (unsigned)(s * TC_TN);
-#pragma unroll 1
-      for (int cb = 0; cb < TC_TN; cb += 32) {
-        unsigned r[32];
-#if defined(GHICP_EMU_HOST)
-        for (int q = 0; q < 32; ++q) r[q] = (unsigned)emu_tmem[(taddr0 >> 16) + lane][(taddr0 & 0xffffu) + cb + q];
-#else
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-            : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-              "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-              "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-              "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-            : "r"(taddr0 + (unsigned)cb));
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#endif
-        if (j < M && !(dbg & 1)) {
-#pragma unroll
-          for (int q = 0; q < 32 / V; ++q) {
-            int best = (int)r[q * V];
-#pragma unroll
-            for (int v = 1; v < V; ++v) best = max(best, (int)r[q * V + v]);   // max dot = min Hamming
-            const int i = src_base + (cb / V) + q;
-            if (i < row0 + nloc) {
-              const int ham = (bits - best) >> 1;
-              fd[fd_index(fd_rows, i - row0, j)] = __half_as_ushort(__int2half_rn(ham));
-            }
-          }
-        }
-      }
-      GHICP_TC_ASM("tcgen05.fence::before_thread_sync;");
-#if defined(GHICP_EMU_HOST)
-      emu::bar_arrive(&s_bar[4 + s]);
-#else
-      asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&s_bar[4 + s])) : "memory");
-#endif
-    }
-  }
-  __syncthreads();
-#if !defined(GHICP_EMU_HOST)
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base));
-#endif
-}
-
-
-// ---- long descriptors (KP > 448, e.g. the 672-bit BSC of BASELINE.json config 2): K-chunked variant -----------------------
-// The B tile (TN (source, variant) rows x KP bytes) stays resident; the A tiles no longer fit twice, so they stream through
-// a ring of KC_STAGES stages of K = 96 bytes per row (3 MMA K-steps, 12 KB): warp 4 loads (cp.async.bulk per stage, the
-// stage's k-chunks are contiguous in the tile-canonical global layout), warp 5 issues the MMAs and hands a stage back with a
-// tcgen05.commit on its `free` barrier; the epilogue is the same as above.  TN = 256 / 128 / 64 by descriptor length.
-constexpr int KC_BYTES = 96;      // K bytes per row and stage
-constexpr int KC_STAGES = 4;
-
-template <int V, int TN>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-k_fd_bsc_tc_kc(const int8_t *__restrict__ T8c, const int8_t *__restrict__ S8c, unsigned short *__restrict__ fd, int N, int M,
-               size_t fd_rows, int row0, int nloc, int bits, int KP) {
-#if defined(GHICP_EMU_HOST)
-  unsigned char *smem = reinterpret_cast<unsigned char *>(emu::dyn_smem());
-#else
-  extern __shared__ __align__(128) unsigned char smem[];
-#endif
-  // barriers: full[4] stage landed, freeb[4] stage consumed, [8,9] MMA of tile done, [10,11] accumulator drained, [12] B landed
-  __shared__ __align__(8) unsigned long long s_bar[13];
-  __shared__ unsigned s_tmem_base;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  // barriers: full[KC_STAGES] stage landed, empty[KC_STAGES] stage consumed, [2 * KC_STAGES] B tile landed
+  __shared__ __align__(8) unsigned long long s_bar[2 * KC_STAGES + 1];
+  constexpr int NC = TN / TC_CONSUMERS / TC_NCH;    // wgmma instructions per K-step and warpgroup
   constexpr int SRC_PER_TILE = TN / V;
-  const unsigned b_bytes = (unsigned)TN * KP, a_bytes = (unsigned)TC_TM * KP;
   constexpr unsigned STAGE_BYTES = (unsigned)TC_TM * KC_BYTES;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const unsigned b_bytes = (unsigned)TN * KP, a_bytes = (unsigned)TC_TM * KP;
   unsigned char *Bs = smem;
   unsigned char *ring = smem + b_bytes;
-  const int src_base = row0 + blockIdx.x * SRC_PER_TILE;
+  const int src_base = row0 + blockIdx.x * SRC_PER_TILE;   // first source row of this CTA's B tile
   const int n_ttiles = (M + TC_TM - 1) / TC_TM;
   const int n_kc = (KP + KC_BYTES - 1) / KC_BYTES;
-  const long long n_chunks = (long long)n_ttiles * n_kc;
-  (void)N;
 
-#if defined(GHICP_EMU_HOST)
-  if (tid == 0) s_tmem_base = 0;
-#else
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(&s_tmem_base)));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-#endif
   if (tid == 0) {
-    for (int b = 0; b < 10; ++b) mbar_init1(&s_bar[b], 1);
-    mbar_init1(&s_bar[10], 128); mbar_init1(&s_bar[11], 128);
-    mbar_init1(&s_bar[12], 1);
-    GHICP_TC_ASM("fence.mbarrier_init.release.cluster;");
-  }
-  GHICP_TC_ASM("tcgen05.fence::before_thread_sync;");
-  __syncthreads();
-  GHICP_TC_ASM("tcgen05.fence::after_thread_sync;");
-  const unsigned tmem_base = s_tmem_base;
-
-  if (warp == 4 && lane == 0) {
-    // ===== loader =====
-    bulk_load(Bs, S8c + (size_t)blockIdx.x * b_bytes, b_bytes, &s_bar[12]);
-    for (long long g = 0; g < n_chunks; ++g) {
-      const int st = (int)(g % KC_STAGES);
-      const int t = (int)(g / n_kc), kc = (int)(g % n_kc);
-      if (g >= KC_STAGES) mbar_wait_parity(&s_bar[4 + st], (unsigned)(((g / KC_STAGES) - 1) & 1));   // MMAs of chunk g - STAGES done
-      const int kb = min(KC_BYTES, KP - kc * KC_BYTES);                                             // K bytes of this chunk
-      bulk_load(ring + (size_t)st * STAGE_BYTES, T8c + (size_t)t * a_bytes + (size_t)kc * KC_BYTES * TC_TM, (unsigned)kb * TC_TM,
-                &s_bar[st]);
+    for (int s = 0; s < KC_STAGES; ++s) {
+      mbar_init1(&s_bar[s], 1);
+      mbar_init1(&s_bar[KC_STAGES + s], TC_CONSUMERS * 4);
     }
-  } else if (warp == 5 && lane == 0) {
-    // ===== MMA issuer =====
-    const unsigned idesc = (2u << 4) | (1u << 7) | (1u << 10) | ((unsigned)(TN >> 3) << 17) | ((unsigned)(TC_TM >> 4) << 24);
+    mbar_init1(&s_bar[2 * KC_STAGES], 1);
 #if !defined(GHICP_EMU_HOST)
-    const unsigned b_addr = smem_u32(Bs), ring_addr = smem_u32(ring);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 #endif
-    mbar_wait_parity(&s_bar[12], 0);   // B landed
-    long long g = 0;
-    for (int t = 0; t < n_ttiles; ++t) {
-      const int s = t & 1;
-      if (t >= 2) mbar_wait_parity(&s_bar[10 + s], (unsigned)(((t >> 1) & 1) ^ 1));   // epilogue(t-2) drained accumulator s
-      const unsigned d_tmem = tmem_base + (unsigned)(s * TN);
-      for (int kc = 0; kc < n_kc; ++kc, ++g) {
+  }
+  __syncthreads();
+
+  if (warp == TC_CONSUMERS * 4) {
+    // ===== producer (one thread) =====
+    if (lane == 0) {
+      bulk_load(Bs, S8c + (size_t)blockIdx.x * b_bytes, b_bytes, &s_bar[2 * KC_STAGES]);
+      const long long n_chunks = (long long)n_ttiles * n_kc;
+      for (long long g = 0; g < n_chunks; ++g) {
         const int st = (int)(g % KC_STAGES);
-        mbar_wait_parity(&s_bar[st], (unsigned)((g / KC_STAGES) & 1));
-        GHICP_TC_ASM("tcgen05.fence::after_thread_sync;");
-        const int ks = min(KC_BYTES, KP - kc * KC_BYTES) / 32;
-        for (int k = 0; k < ks; ++k) {
-          const int kg = kc * (KC_BYTES / 32) + k;   // K-step index inside the B tile
-#if defined(GHICP_EMU_HOST)
-          emu_umma_i8_at((int)d_tmem, reinterpret_cast<const signed char *>(ring + (size_t)st * STAGE_BYTES) + (size_t)k * 2 * TC_TM * 16,
-                         reinterpret_cast<const signed char *>(Bs) + (size_t)kg * 2 * TN * 16, TN, kc > 0 || k > 0);
-          (void)idesc;
-#else
-          const uint64_t adesc = make_desc(ring_addr + (unsigned)st * STAGE_BYTES + (unsigned)k * 2u * TC_TM * 16u, TC_TM * 16u, 128u);
-          const uint64_t bdesc = make_desc(b_addr + (unsigned)kg * 2u * TN * 16u, TN * 16u, 128u);
-          const unsigned accumulate = (kc > 0 || k > 0) ? 1u : 0u;
-          asm volatile(
-              "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-              "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, {%5, %5, %5, %5}, p;\n\t}\n"
-              ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(0u) : "memory");
-#endif
-        }
-#if defined(GHICP_EMU_HOST)
-        emu::bar_arrive(&s_bar[4 + st]);
-        if (kc == n_kc - 1) emu::bar_arrive(&s_bar[8 + s]);
-#else
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(&s_bar[4 + st])) : "memory");
-        if (kc == n_kc - 1)
-          asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(&s_bar[8 + s])) : "memory");
-#endif
+        const int t = (int)(g / n_kc), kc = (int)(g % n_kc);
+        if (g >= KC_STAGES) mbar_wait_parity(&s_bar[KC_STAGES + st], (unsigned)(((g / KC_STAGES) - 1) & 1));
+        const int kb = min(KC_BYTES, KP - kc * KC_BYTES);   // K bytes of this chunk (a multiple of 32)
+        bulk_load(ring + (size_t)st * STAGE_BYTES, T8c + (size_t)t * a_bytes + (size_t)kc * KC_BYTES * TC_TM,
+                  (unsigned)kb * TC_TM, &s_bar[st]);
       }
     }
-  } else if (warp < 4) {
-    // ===== epilogue warps: TMEM -> registers -> min over variants -> fp16 -> FD plane =====
-    for (int t = 0; t < n_ttiles; ++t) {
-      const int s = t & 1;
-      const unsigned ph = (unsigned)((t >> 1) & 1);
-      mbar_wait_parity(&s_bar[8 + s], ph);
-      GHICP_TC_ASM("tcgen05.fence::after_thread_sync;");
-      const int j = t * TC_TM + warp * 32 + lane;
-      const unsigned taddr0 = tmem_base + ((unsigned)(warp * 32) << 16) + (unsigned)(s * TN);
-#pragma unroll 1
-      for (int cb = 0; cb < TN; cb += 32) {
-        unsigned r[32];
-#if defined(GHICP_EMU_HOST)
-        for (int q = 0; q < 32; ++q) r[q] = (unsigned)emu_tmem[(taddr0 >> 16) + lane][(taddr0 & 0xffffu) + cb + q];
-#else
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-            : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-              "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-              "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-              "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-            : "r"(taddr0 + (unsigned)cb));
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+    return;
+  }
+
+  // ===== consumer warpgroups: wgmma into registers, then min over variants -> fp16 -> FD plane =====
+  const int wg = warp >> 2, wl = warp & 3;
+  const int col0 = wg * (TN / TC_CONSUMERS);   // first B row (column of D) of this warpgroup
+  int acc[NC][16];
+#if !defined(GHICP_EMU_HOST)
+  const unsigned b_addr = smem_u32(Bs), ring_addr = smem_u32(ring);
 #endif
-        if (j < M) {
+  mbar_wait_parity(&s_bar[2 * KC_STAGES], 0);   // B landed
+  long long g = 0;
+  for (int t = 0; t < n_ttiles; ++t) {
+    for (int kc = 0; kc < n_kc; ++kc, ++g) {
+      const int st = (int)(g % KC_STAGES);
+      mbar_wait_parity(&s_bar[st], (unsigned)((g / KC_STAGES) & 1));
+      const int ks = min(KC_BYTES, KP - kc * KC_BYTES) / 32;
+#if defined(GHICP_EMU_HOST)
+      for (int k = 0; k < ks; ++k) {
+        const int kg = kc * (KC_BYTES / 32) + k;   // K-step index inside the B tile
+        for (int c = 0; c < NC; ++c)
+          emu_wgmma_s8(acc[c], ring + (size_t)st * STAGE_BYTES + (size_t)k * 2 * TC_TM * 16,
+                       Bs + (size_t)kg * 2 * TN * 16 + (size_t)(col0 + c * TC_NCH) * 16, TN, kc > 0 || k > 0);
+      }
+#else
+      fence_acc(acc);
+      asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+      for (int k = 0; k < ks; ++k) {
+        const int kg = kc * (KC_BYTES / 32) + k;
+        const uint64_t adesc = make_desc(ring_addr + (unsigned)st * STAGE_BYTES + (unsigned)k * 2u * TC_TM * 16u, TC_TM * 16u, 128u);
+        const unsigned accumulate = (kc > 0 || k > 0) ? 1u : 0u;
 #pragma unroll
-          for (int q = 0; q < 32 / V; ++q) {
-            int best = (int)r[q * V];
+        for (int c = 0; c < NC; ++c) {
+          const uint64_t bdesc = make_desc(b_addr + (unsigned)kg * 2u * TN * 16u + (unsigned)(col0 + c * TC_NCH) * 16u, TN * 16u, 128u);
+          wgmma_s8(acc[c], adesc, bdesc, accumulate);
+        }
+      }
+      asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+      asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+      fence_acc(acc);
+#endif
+      __syncwarp();                                          // every lane of the warp is past its reads of the stage
+      if (lane == 0) mbar_arrive(&s_bar[KC_STAGES + st]);   // this warp's MMAs no longer read the stage
+    }
+    // epilogue.  Fragment of m64nNk32: element e of a thread sits at row 16 wl + lane / 4 + 8 ((e >> 1) & 1) and column
+    // 8 (e >> 2) + 2 (lane & 3) + (e & 1) of its instruction's 32 columns
 #pragma unroll
-            for (int v = 1; v < V; ++v) best = max(best, (int)r[q * V + v]);   // max dot = min Hamming
-            const int i = src_base + (cb / V) + q;
-            if (i < row0 + nloc) {
-              const int ham = (bits - best) >> 1;
-              fd[fd_index(fd_rows, i - row0, j)] = __half_as_ushort(__int2half_rn(ham));
-            }
+    for (int c = 0; c < NC; ++c) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int j = t * TC_TM + wl * 16 + (lane >> 2) + 8 * h;   // target column of the FD plane
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          int best = max(acc[c][q * 4 + h * 2], acc[c][q * 4 + h * 2 + 1]);   // max dot = min Hamming
+          const int col = col0 + c * TC_NCH + 8 * q + 2 * (lane & 3);          // first of the two columns
+          if (V == 4) best = max(best, __shfl_xor_sync(0xffffffffu, best, 1));  // the other two variants sit in lane ^ 1
+          if (V == 4 && (lane & 1)) continue;
+          const int i = src_base + col / V;
+          if (j < M && i < row0 + nloc) {
+            const int ham = (bits - best) >> 1;
+            fd[fd_index(fd_rows, i - row0, j)] = __half_as_ushort(__int2half_rn(ham));
           }
         }
       }
-      GHICP_TC_ASM("tcgen05.fence::before_thread_sync;");
-#if defined(GHICP_EMU_HOST)
-      emu::bar_arrive(&s_bar[10 + s]);
-#else
-      asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&s_bar[10 + s])) : "memory");
-#endif
     }
   }
-  __syncthreads();
-#if !defined(GHICP_EMU_HOST)
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base));
-#endif
 }
 
 }  // namespace
 
-// Returns cudaErrorNotSupported when the shape does not fit this kernel (caller falls back to k_fd_bsc).
 #if defined(GHICP_EMU_HOST)
 #define GHICP_TC_OPT_IN_SMEM(kernel) (void)0
 #else
 #define GHICP_TC_OPT_IN_SMEM(kernel) cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
 #endif
 template <int V, int TN>
-static cudaError_t launch_kc(Ctx *c, const int8_t *T8, const int8_t *S8, int KP, int grid, size_t smem) {
-  GHICP_TC_OPT_IN_SMEM((k_fd_bsc_tc_kc<V, TN>));
-  GHICP_LAUNCH((k_fd_bsc_tc_kc<V, TN>), grid, TC_THREADS, smem, c->stream, T8, S8, c->d_fd16, c->N, c->M, c->fd_rows, c->r0, c->nloc,
+static cudaError_t launch_tc(Ctx *c, const int8_t *T8, const int8_t *S8, int KP, int grid, size_t smem) {
+  GHICP_TC_OPT_IN_SMEM((k_fd_bsc_tc<V, TN>));
+  GHICP_LAUNCH((k_fd_bsc_tc<V, TN>), grid, TC_THREADS, smem, c->stream, T8, S8, c->d_fd16, c->M, c->fd_rows, c->r0, c->nloc,
                c->bits, KP);
   return cudaGetLastError();
 }
 
+// Returns cudaErrorNotSupported when the shape does not fit this kernel (caller falls back to k_fd_bsc).
 cudaError_t launch_fd_bsc_tc(Ctx *c) {
   const int V = (c->cfg.dof == 6) ? 4 : 2;
   const int KP = (c->bits + 31) / 32 * 32;
   if (c->V < V || c->nloc <= 0) return cudaErrorNotSupported;
-  // short descriptors (<= 448 bits: the reference's 441): B tile + two whole A tiles resident; longer ones: B tile resident,
-  // A tiles streamed through the K-chunk ring, the B tile narrowed (256 / 128 / 64 rows) until it fits
-  const size_t smem_max = 227 * 1024;
-  const bool whole = (size_t)TC_TN * KP + 2 * (size_t)TC_TM * KP <= smem_max && getenv("GHICP_FDTC_KC") == nullptr;
+  // the B tile narrows (256 / 128 / 64 rows) until it and the A ring fit the 227 KB a block may opt in to
+  const size_t smem_max = 227 * 1024 - 128;   // less the kernel's static barriers
   const size_t ring_bytes = (size_t)KC_STAGES * TC_TM * KC_BYTES;
   int TN = 0;
-  if (!whole) {
-    for (int cand : {256, 128, 64})
-      if ((size_t)cand * KP + ring_bytes <= smem_max) { TN = cand; break; }
-    if (TN == 0) return cudaErrorNotSupported;
-  } else {
-    TN = TC_TN;
-  }
-  const size_t smem = whole ? (size_t)TC_TN * KP + 2 * (size_t)TC_TM * KP : (size_t)TN * KP + ring_bytes;
+  for (int cand : {256, 128, 64})
+    if ((size_t)cand * KP + ring_bytes <= smem_max) { TN = cand; break; }
+  if (TN == 0) return cudaErrorNotSupported;
+  const size_t smem = (size_t)TN * KP + ring_bytes;
   int8_t *T8 = nullptr, *S8 = nullptr;
   cudaError_t e;
-  const int dbg = getenv("GHICP_FDTC_DBG") ? atoi(getenv("GHICP_FDTC_DBG")) : 0;
   const int src_per_tile = TN / V;
   const int grid = (c->nloc + src_per_tile - 1) / src_per_tile;
   const int n_ttiles = (c->M + TC_TM - 1) / TC_TM;
@@ -478,21 +311,12 @@ cudaError_t launch_fd_bsc_tc(Ctx *c) {
                  c->nloc * V, S8);
     c->launches += 2;
   }
-  if (whole) {
-    if (V == 4) {
-      GHICP_TC_OPT_IN_SMEM(k_fd_bsc_tc<4>);
-      GHICP_LAUNCH(k_fd_bsc_tc<4>, grid, TC_THREADS, smem, c->stream, T8, S8, c->d_fd16, c->N, c->M, c->fd_rows, c->r0, c->nloc, c->bits, KP, dbg);
-    } else {
-      GHICP_TC_OPT_IN_SMEM(k_fd_bsc_tc<2>);
-      GHICP_LAUNCH(k_fd_bsc_tc<2>, grid, TC_THREADS, smem, c->stream, T8, S8, c->d_fd16, c->N, c->M, c->fd_rows, c->r0, c->nloc, c->bits, KP, dbg);
-    }
-    e = cudaGetLastError();
-  } else if (V == 4) {
-    e = TN == 256 ? launch_kc<4, 256>(c, T8, S8, KP, grid, smem) : TN == 128 ? launch_kc<4, 128>(c, T8, S8, KP, grid, smem)
-                                                                             : launch_kc<4, 64>(c, T8, S8, KP, grid, smem);
+  if (V == 4) {
+    e = TN == 256 ? launch_tc<4, 256>(c, T8, S8, KP, grid, smem) : TN == 128 ? launch_tc<4, 128>(c, T8, S8, KP, grid, smem)
+                                                                             : launch_tc<4, 64>(c, T8, S8, KP, grid, smem);
   } else {
-    e = TN == 256 ? launch_kc<2, 256>(c, T8, S8, KP, grid, smem) : TN == 128 ? launch_kc<2, 128>(c, T8, S8, KP, grid, smem)
-                                                                             : launch_kc<2, 64>(c, T8, S8, KP, grid, smem);
+    e = TN == 256 ? launch_tc<2, 256>(c, T8, S8, KP, grid, smem) : TN == 128 ? launch_tc<2, 128>(c, T8, S8, KP, grid, smem)
+                                                                             : launch_tc<2, 64>(c, T8, S8, KP, grid, smem);
   }
   c->launches++;
   cudaFreeAsync(T8, c->stream);

@@ -794,8 +794,8 @@ cudaError_t launch_fpfh_fast_sweep(Ctx *c, const CostParams &cp, bool pre, bool 
 cudaError_t launch_fpfh_fast_finish(Ctx *c, const CostParams &cp, bool with_cols) {
   const FfArgs a = ff_args(c, cp);
   GHICP_LAUNCH(k_ff_stats, 1, 1024, 0, c->stream, c->d_ff_part, (int)fpfh_fast_parts(c), c->d_xstats, c->rank);
-  GHICP_LAUNCH(k_ff_resolve, 148 * 4, 256, 0, c->stream, a, 0);
-  if (with_cols) GHICP_LAUNCH(k_ff_resolve, 148 * 4, 256, 0, c->stream, a, 1);
+  GHICP_LAUNCH(k_ff_resolve, GHICP_SMS * 4, 256, 0, c->stream, a, 0);
+  if (with_cols) GHICP_LAUNCH(k_ff_resolve, GHICP_SMS * 4, 256, 0, c->stream, a, 1);
   const int n = c->N > c->M ? c->N : c->M;
   GHICP_LAUNCH(k_ff_publish, (n + 255) / 256, 256, 0, c->stream, a, c->d_row_cd, c->d_row_idx,
                with_cols ? c->d_col_cd : (double *)nullptr, with_cols ? c->d_col_idx : (int *)nullptr, c->d_xstats, c->rank);
@@ -820,7 +820,7 @@ cudaError_t launch_fpfh_cand_block(Ctx *c, const CostParams &cp) {
   float *fd = reinterpret_cast<float *>(gain + c->xuse);
   cudaMemsetAsync(hdr, 0, sizeof(XBlockHdr), c->stream);
   GHICP_LAUNCH(k_ff_stats, 1, 1024, 0, c->stream, c->d_ff_part, (int)fpfh_fast_parts(c), c->d_xstats, c->rank);
-  GHICP_LAUNCH(k_ff_cand_block, 148 * 2, 256, 0, c->stream, a, c->d_iter, hdr, key, gain, fd, (unsigned long long)c->xuse);
+  GHICP_LAUNCH(k_ff_cand_block, GHICP_SMS * 2, 256, 0, c->stream, a, c->d_iter, hdr, key, gain, fd, (unsigned long long)c->xuse);
   GHICP_LAUNCH(k_ff_block_hdr, 1, 1, 0, c->stream, a, c->d_xstats + 4 * c->rank, hdr, (unsigned long long)c->xuse);
   c->launches += 3;
   return cudaGetLastError();

@@ -21,6 +21,10 @@
 
 namespace ghicp_b200 {
 
+// SM count of the H100 SXM the fixed grid-stride launch geometries are sized for (a multiple of it keeps every SM busy);
+// launches that must match the device query cudaDevAttrMultiProcessorCount instead.
+constexpr int GHICP_SMS = 132;
+
 // Feature-distance plane layout: PANEL-MAJOR.  The N x M plane is stored as ceil(M/256) column panels, each
 // a dense row-major [rows][256] block, so the 256-column panel a warp sweeps down the source rows is one
 // perfectly sequential HBM stream (512 B per row back to back) instead of 512 B reads at a 2*M-byte stride.
@@ -139,7 +143,7 @@ struct Ctx {
   double *d_tn = nullptr;  // target normals [3][M]
   bool have_normals = false;
   bool have_bsc = false, have_fpfh = false, fd_built = false;
-  bool fd_tensor = false;  // FD plane built by the tcgen05 kernel
+  bool fd_tensor = false;  // FD plane built by the tensor-core (wgmma) kernel
 
   // per-iteration workspaces
   int rows_per_cta = 8, n_chunks = 1;
@@ -251,7 +255,7 @@ struct KmResult {
 // ---- launchers (ghicp_kernels.cu) ---------------------------------------------------------------
 cudaError_t launch_pack_bsc(Ctx *c, const uint8_t *d_raw_s, const uint8_t *d_raw_t);
 cudaError_t launch_fd_bsc(Ctx *c);
-cudaError_t launch_fd_bsc_tc(Ctx *c);  // tcgen05 path; cudaErrorNotSupported when the shape does not fit
+cudaError_t launch_fd_bsc_tc(Ctx *c);  // wgmma path; cudaErrorNotSupported when the shape does not fit
 cudaError_t launch_fd_fpfh(Ctx *c);
 // mode: 0 rowmin+stats, 1 count (needs penalty in d_iter), 2 fill
 cudaError_t launch_rowsweep(Ctx *c, int mode, const CostParams &cp);

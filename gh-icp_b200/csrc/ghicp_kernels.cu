@@ -1,5 +1,5 @@
 // ghicp_kernels.cu — cost build, correspondence scans, pair statistics, rigid solve and update kernels
-// of the GH-ICP inner loop for sm_100a.  Compiled with --fmad=false: every arithmetic operation on
+// of the GH-ICP inner loop for sm_90a.  Compiled with --fmad=false: every arithmetic operation on
 // the exact path is a separately rounded IEEE operation, in the reference's evaluation order, so
 // CD(i,j) is bit-identical to the reference's double arithmetic (src/ghicp_reg.cpp:122,259,308).
 #include <algorithm>
@@ -900,7 +900,7 @@ cudaError_t launch_pair_fd_km(Ctx *c) {
     c->launches++;
     return cudaGetLastError();
   }
-  GHICP_LAUNCH(k_pair_fd_km, 148 * 2, 256, 0, c->stream, c->d_sp, c->d_tp, c->d_iter, c->d_rowptr, c->d_csr_col, c->d_csr_fd,
+  GHICP_LAUNCH(k_pair_fd_km, GHICP_SMS * 2, 256, 0, c->stream, c->d_sp, c->d_tp, c->d_iter, c->d_rowptr, c->d_csr_col, c->d_csr_fd,
                                                c->d_pair_fd);
   c->launches++;
   return cudaGetLastError();

@@ -65,8 +65,8 @@ cudaError_t exclusive_scan(const int *in, int *out, int n, cudaStream_t) {   // 
 }
 #else
 // Workspaces come from the device's stream-ordered pool (the whole pre-processing runs on one stream): a cudaMalloc /
-// cudaFree pair per temporary cost more host time than all the kernels of a 1 M-point scan together (measured on the
-// B200: 376 ms per scan against ~10 ms of kernels), cudaFree being a device-wide synchronisation.  The pool keeps what it
+// cudaFree pair per temporary costs more host time than all the kernels of a 1 M-point scan together, cudaFree being a
+// device-wide synchronisation.  The pool keeps what it
 // has handed out once (release threshold = unlimited), so the second scan of a pair allocates nothing new.
 inline void ppool_init() {
   static bool done = false;   // per process; set for the current device on first use
@@ -235,13 +235,10 @@ __device__ __forceinline__ void column_run(const GridArgs &g, int x, int y, int 
   s0 = g.cstart[lo]; s1 = g.cstart[u1];            // cstart holds nu + 1 entries
 }
 // Per-thread neighbour walks (k_pca, k_nms_round): every thread first resolves its nine column runs, then walks them in one
-// flat loop nest.  Round 1 shipped the walk as "for dx, for dy { column_run; for s }" reading the grid description straight
-// from the kernel parameters; on B200 hardware that kernel returned neighbour counts that were short for whole warps
-// (33 of 40 000 points, deterministic run to run, different under compute-sanitizer; the grid arrays validated clean on the
-// host and the CPU emulation of the same source passed).  Its SASS kept the dx / dy loop counters and re-loaded kernel
-// parameters in per-warp uniform registers across the divergent per-thread loops.  The form below — grid description copied
-// into per-thread registers, runs resolved before any point is touched — is exact on hardware (A/B log:
-// profiles/r02_k_pca_variants_b200.log, 0 mismatches of 320 000 points in every run).
+// flat loop nest, with the grid description copied into per-thread registers.  A form that walked "for dx, for dy
+// { column_run; for s }" reading the grid description straight from the kernel parameters returned neighbour counts short
+// for whole warps on hardware (its SASS re-loaded kernel parameters in per-warp uniform registers across the divergent
+// per-thread loops), while the CPU emulation of the same source passed.
 struct GridRegs {
   const float4 *sorted; const pu64 *ucell; const int *cstart; const int *order; int nu; float r2;
 };
@@ -395,7 +392,7 @@ cudaError_t build_grid(cudaStream_t st, const float *d_xyz, const int *d_ids, in
   int nu = 0;
   PCK(pmalloc(&d_box, 6));
   { const unsigned init[6] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u}; PCK(pcopy(d_box, init, sizeof(init), P_H2D, st)); }
-  GHICP_LAUNCH(k_bbox, n < 148 * 8 * PT ? blocks(n) : 148 * 8, PT, 0, st, d_xyz, d_ids, n, d_box, d_box + 3);
+  GHICP_LAUNCH(k_bbox, n < GHICP_SMS * 8 * PT ? blocks(n) : GHICP_SMS * 8, PT, 0, st, d_xyz, d_ids, n, d_box, d_box + 3);
   PCK(pcopy(h_box, d_box, sizeof(h_box), P_D2H, st)); PCK(psync(st));
   g->mnx = ord2f(h_box[0]); g->mny = ord2f(h_box[1]); g->mnz = ord2f(h_box[2]);
   g->inv = 1.0f / cell; g->r2 = cell * cell;
@@ -430,7 +427,7 @@ cudaError_t prep_voxel_downsample(cudaStream_t st, const float *d_xyz, int n, fl
     PCK(pmalloc(&d_box, 6));
     const unsigned init[6] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u};
     PCK(pcopy(d_box, init, sizeof(init), P_H2D, st));
-    GHICP_LAUNCH(k_bbox, n < 148 * 8 * PT ? blocks(n) : 148 * 8, PT, 0, st, d_xyz, (const int *)nullptr, n, d_box, d_box + 3);
+    GHICP_LAUNCH(k_bbox, n < GHICP_SMS * 8 * PT ? blocks(n) : GHICP_SMS * 8, PT, 0, st, d_xyz, (const int *)nullptr, n, d_box, d_box + 3);
     PCK(pcopy(h_box, d_box, sizeof(h_box), P_D2H, st)); PCK(psync(st));
     const float mn[3] = {ord2f(h_box[0]), ord2f(h_box[1]), ord2f(h_box[2])}, mx[3] = {ord2f(h_box[3]), ord2f(h_box[4]), ord2f(h_box[5])};
     const float inv = 1.0f / voxel_size;                                   // include/filter.hpp:30
@@ -541,7 +538,7 @@ cudaError_t prep_bounds(cudaStream_t st, const float *d_xyz, int n, float mn[3],
     PCK(pmalloc(&d_box, 6));
     const unsigned init[6] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u};
     PCK(pcopy(d_box, init, sizeof(init), P_H2D, st));
-    GHICP_LAUNCH(k_bbox, n < 148 * 8 * PT ? blocks(n) : 148 * 8, PT, 0, st, d_xyz, (const int *)nullptr, n, d_box, d_box + 3);
+    GHICP_LAUNCH(k_bbox, n < GHICP_SMS * 8 * PT ? blocks(n) : GHICP_SMS * 8, PT, 0, st, d_xyz, (const int *)nullptr, n, d_box, d_box + 3);
     PCK(pcopy(h_box, d_box, sizeof(h_box), P_D2H, st)); PCK(psync(st));
     for (int a = 0; a < 3; ++a) { mn[a] = ord2f(h_box[a]); mx[a] = ord2f(h_box[3 + a]); }
   }

@@ -1,4 +1,4 @@
-// ghicp_stream.cu — the streaming cost/correspondence kernel of the GH-ICP inner loop (sm_100a).
+// ghicp_stream.cu — the streaming cost/correspondence kernel of the GH-ICP inner loop (sm_90a).
 //
 // One pass over the N x M feature-distance plane (fp16, 2 B/pair — the only O(N*M) HBM traffic of an
 // iteration) fuses calED + calCD_* + the NN / NNR scans or the KM candidate gate
@@ -89,12 +89,10 @@ __device__ __forceinline__ void bulk_g2s(void *dst, const void *src, unsigned by
 
 enum { SM_NN = 0, SM_NNR = 1, SM_COUNT = 2, SM_FILL = 3, SM_PRE = 4, SM_PRE_COLS = 5 };
 
-#if defined(GHICP_EMU_HOST)
-// Host emulation of the PTX-only arithmetic: the approximate square root becomes the exact one (inside the filter's error
-// budget), a packed f32x2 operation is two scalar ones with the same single rounding, the mixed f16 x f16 + f32 FMA is an
-// fmaf of the converted halves (their product is exact in float).
+// Column pairs travel as one 64-bit value (two floats); Hopper has no packed f32x2 arithmetic, so fma2 / add2 are two scalar
+// operations with one rounding each.  fhfma = fd(fp16) * weight(fp16) + dist: the product of two halves is exact in float,
+// so the fmaf of the converted halves rounds once, like a mixed-precision FMA would.
 typedef unsigned long long u64;
-__device__ __forceinline__ float sqrt_approx(float x) { return sqrtf(x); }
 __device__ __forceinline__ u64 pack2(float lo, float hi) { return ((u64)__float_as_uint(hi) << 32) | __float_as_uint(lo); }
 __device__ __forceinline__ void unpack2(u64 v, float &lo, float &hi) { lo = __uint_as_float((unsigned)v); hi = __uint_as_float((unsigned)(v >> 32)); }
 __device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) {
@@ -103,28 +101,20 @@ __device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) {
 }
 __device__ __forceinline__ u64 add2(u64 a, u64 b) {
   float al, ah, bl, bh; unpack2(a, al, ah); unpack2(b, bl, bh);
-  return pack2(al + bl, ah + bh);
+  return pack2(__fadd_rn(al, bl), __fadd_rn(ah, bh));
 }
 __device__ __forceinline__ float fhfma(unsigned short h, unsigned short w, float c) {
   return fmaf(__half2float(__ushort_as_half(h)), __half2float(__ushort_as_half(w)), c);
 }
+#if defined(GHICP_EMU_HOST)
+// Host emulation of the PTX-only operations: the approximate square root becomes the exact one (inside the filter's error
+// budget), the streaming load a plain one.
+__device__ __forceinline__ float sqrt_approx(float x) { return sqrtf(x); }
 __device__ __forceinline__ uint4 ldg_stream(const uint4 *p) { return *p; }
 #else
 __device__ __forceinline__ float sqrt_approx(float x) {
   float r;
   asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
-  return r;
-}
-// packed FP32 pairs (FFMA2 / FADD2 on sm_100a): two columns per instruction, half the issue slots
-typedef unsigned long long u64;
-__device__ __forceinline__ u64 pack2(float lo, float hi) { u64 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi)); return r; }
-__device__ __forceinline__ void unpack2(u64 v, float &lo, float &hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) { u64 r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c)); return r; }
-__device__ __forceinline__ u64 add2(u64 a, u64 b) { u64 r; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-// cd = fd(fp16) * weight(fp16) + dist : one FHFMA (the half product is exact in fp32)
-__device__ __forceinline__ float fhfma(unsigned short h, unsigned short w, float c) {
-  float r;
-  asm("fma.rn.f32.f16 %0, %1, %2, %3;" : "=f"(r) : "h"(h), "h"(w), "f"(c));
   return r;
 }
 __device__ __forceinline__ uint4 ldg_stream(const uint4 *p) {
@@ -849,9 +839,9 @@ static int stream_rows_per_cta(const Ctx *c) {
   if (forced >= ST_RB_MIN && forced <= ST_RB) return forced / ST_UNROLL * ST_UNROLL;
   static int slots = 0;
   if (slots == 0) {
-    int n_sm = 148;
+    int n_sm = GHICP_SMS;
     cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, c->device);
-    slots = 2 * (n_sm > 0 ? n_sm : 148);
+    slots = 2 * (n_sm > 0 ? n_sm : GHICP_SMS);
   }
   const long long gx = (c->M + ST_CTA_COLS - 1) / ST_CTA_COLS;
   const int nloc = c->nloc > 0 ? c->nloc : 1;
@@ -986,8 +976,8 @@ cudaError_t launch_stream(Ctx *c, const CostParams &cp, int mode, bool stats) {
 
 cudaError_t launch_stream_resolve(Ctx *c, const CostParams &cp, bool with_cols) {
   StreamArgs a = make_args(c, cp);
-  GHICP_LAUNCH(k_resolve, 148 * 4, 256, 0, c->stream, a, 0);
-  if (with_cols) GHICP_LAUNCH(k_resolve, 148 * 4, 256, 0, c->stream, a, 1);
+  GHICP_LAUNCH(k_resolve, GHICP_SMS * 4, 256, 0, c->stream, a, 0);
+  if (with_cols) GHICP_LAUNCH(k_resolve, GHICP_SMS * 4, 256, 0, c->stream, a, 1);
   const int n = c->N > c->M ? c->N : c->M;
   GHICP_LAUNCH(k_publish, (n + 255) / 256, 256, 0, c->stream, a, c->d_row_cd, c->d_row_idx, with_cols ? c->d_col_cd : nullptr,
                                                     with_cols ? c->d_col_idx : nullptr, c->d_xstats, c->rank);
@@ -1037,7 +1027,7 @@ __global__ void k_count_valid(const double *__restrict__ gain, long long nnz, St
 }
 cudaError_t launch_count_valid(Ctx *c, long long nnz) {
   cudaMemsetAsync(&c->d_sdev->nnz_valid, 0, sizeof(unsigned long long), c->stream);
-  GHICP_LAUNCH(k_count_valid, 148 * 4, 256, 0, c->stream, c->d_csr_gain, nnz, c->d_sdev);
+  GHICP_LAUNCH(k_count_valid, GHICP_SMS * 4, 256, 0, c->stream, c->d_csr_gain, nnz, c->d_sdev);
   c->launches++;
   return cudaGetLastError();
 }
@@ -1047,14 +1037,14 @@ cudaError_t launch_scan_rows(Ctx *c) {
 cudaError_t launch_emit_scatter(Ctx *c, const CostParams &cp, unsigned long long n_emitted) {
   StreamArgs a = make_args(c, cp);
   const unsigned long long want = (n_emitted + 255) / 256;
-  const int blocks = (int)std::min<unsigned long long>(std::max<unsigned long long>(want, 1), 148ull * 8);
+  const int blocks = (int)std::min<unsigned long long>(std::max<unsigned long long>(want, 1), (unsigned long long)GHICP_SMS * 8);
   GHICP_LAUNCH(k_emit_scatter, blocks, 256, 0, c->stream, a, n_emitted);
   c->launches++;
   return cudaGetLastError();
 }
 cudaError_t launch_csr_check(Ctx *c, const CostParams &cp) {
   StreamArgs a = make_args(c, cp);
-  GHICP_LAUNCH(k_csr_check, 148 * 4, 256, 0, c->stream, a, c->d_iter, c->d_csr_gain);
+  GHICP_LAUNCH(k_csr_check, GHICP_SMS * 4, 256, 0, c->stream, a, c->d_iter, c->d_csr_gain);
   c->launches++;
   return cudaGetLastError();
 }
@@ -1069,7 +1059,7 @@ cudaError_t launch_emit_check(Ctx *c, const CostParams &cp) {
   unsigned long long *key = reinterpret_cast<unsigned long long *>(hdr + 1);
   double *gain = reinterpret_cast<double *>(key + c->xuse);
   float *fd = reinterpret_cast<float *>(gain + c->xuse);
-  GHICP_LAUNCH(k_emit_check, 148 * 2, 256, 0, c->stream, a, c->d_iter, c->d_xstats + 4 * c->rank, hdr, key, gain, fd,
+  GHICP_LAUNCH(k_emit_check, GHICP_SMS * 2, 256, 0, c->stream, a, c->d_iter, c->d_xstats + 4 * c->rank, hdr, key, gain, fd,
                (unsigned long long)c->xuse);
   c->launches++;
   return cudaGetLastError();

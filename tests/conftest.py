@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 def build_emulated_library(out_dir):
@@ -49,7 +49,7 @@ def emu_library_path(tmp_path_factory):
 def g(request):
     """The product package, with the library built (nvcc cross-compiles here without a GPU).
     Developer switch, never set by the driver: GHICP_TEST_EMULATED_ABI=1 runs the `-m gpu` tests on a machine WITHOUT a GPU
-    against the emulated library (all-double kernels; nothing about the TMA / tcgen05 kernels is exercised that way):
+    against the emulated library (all-double kernels; nothing about the TMA / wgmma kernels is exercised that way):
         GHICP_TEST_EMULATED_ABI=1 python -m pytest tests/test_gpu_parity.py -m gpu -q"""
     import ghicp_b200
     ghicp_b200.build_library()

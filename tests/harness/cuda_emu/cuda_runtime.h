@@ -125,6 +125,7 @@ inline double __dsub_rn(double a, double b) { return a - b; }     // built with 
 inline double __dadd_rn(double a, double b) { return a + b; }
 inline double __dmul_rn(double a, double b) { return a * b; }
 inline double __dsqrt_rn(double a) { return sqrt(a); }
+inline float __fadd_rn(float a, float b) { return a + b; }
 template <typename T> inline T __ldcg(const T *p) { return *p; }
 inline int __ffs(unsigned v) { return v ? __builtin_ctz(v) + 1 : 0; }
 inline unsigned __float_as_uint(float f) { unsigned u; memcpy(&u, &f, 4); return u; }

@@ -1,9 +1,9 @@
 // emu_library.cpp — the WHOLE C ABI of libghicp_b200.so built for the CPU through the host emulation shim
 // (tests/harness/cuda_emu): ghicp_capi.cu (context, iteration orchestration, every extern "C" entry point) on top of ALL of
 // the product's kernels — ghicp_kernels.cu, ghicp_stream.cu, ghicp_fdtc.cu, ghicp_auction.cu, ghicp_fpfh.cu,
-// ghicp_solvers.cu, ghicp_prep.cu — every CUDA thread a fiber.  The PTX of ghicp_stream.cu (mbarrier, cp.async.bulk, packed
-// f32x2 arithmetic) and of ghicp_fdtc.cu (tcgen05.alloc / mma kind::i8 / commit / ld, over an int32 array standing in for
-// tensor memory) has a host stand-in next to each asm statement.
+// ghicp_solvers.cu, ghicp_prep.cu — every CUDA thread a fiber.  The PTX of ghicp_stream.cu (mbarrier, cp.async.bulk) and of
+// ghicp_fdtc.cu (mbarrier, cp.async.bulk, wgmma s8 computed per thread on its accumulator fragment) has a host stand-in next
+// to each asm statement.
 // TEST INFRASTRUCTURE ONLY: tests/test_emulated_abi.py loads it explicitly to run the Python and C++ host layers, the
 // command-line driver and the GPU test functions themselves on a machine without a GPU.  The product never loads it;
 // libghicp_b200.so has no CPU path.

@@ -1,6 +1,6 @@
 """Run by tests/test_emulated_abi.py in a fresh process (the emulator reads its stress switches once): loads the emulated
 library given on the command line in place of libghicp_b200.so and checks, against the oracle,
-  * the tcgen05 FD build (ghicp_fdtc.cu: TMA tiles -> UMMA -> TMEM epilogue) on two shapes, bit for bit;
+  * the wgmma FD build (ghicp_fdtc.cu: TMA ring -> wgmma -> register epilogue) on two shapes, bit for bit;
   * a BSC + reciprocal-NN registration through the TMA streaming kernel (ghicp_stream.cu), pair lists per iteration.
 Exit status 0 = everything equal, 1 = a mismatch.  Test infrastructure only."""
 import os

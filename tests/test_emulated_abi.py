@@ -1,6 +1,6 @@
 """The WHOLE C ABI on the CPU: tests/harness/emu_library.cpp builds ghicp_capi.cu (context, iteration orchestration, every
 extern "C" entry point) on top of the product's own kernels through the host emulation shim — CUDA threads as fibers, device
-memory = the heap — the TMA streaming kernel of ghicp_stream.cu and the tcgen05 FD build of ghicp_fdtc.cu included (their
+memory = the heap — the TMA streaming kernel of ghicp_stream.cu and the wgmma FD build of ghicp_fdtc.cu included (their
 PTX statements have host stand-ins: mbarriers, bulk copies, packed arithmetic, tensor memory as an int32 array).
 
 This module loads that library IN PLACE OF libghicp_b200.so for the duration of a test (the product never does: it has no CPU
@@ -377,7 +377,7 @@ def test_cpp_mirror_fills_matchlist_pre_rec_in_km_mode(ge, tmp_path, monkeypatch
                                            ({"GHICP_EMU_SCHED": "5", "GHICP_EMU_TMA_DELAY": "40"}, True),
                                            ({"GHICP_EMU_NEGCTL_NOWAIT": "1", "GHICP_EMU_TMA_DELAY": "7"}, False)])
 def test_tma_and_tcgen05_kernels_under_random_scheduling_and_delayed_copies(emu_library_path, env, expect_ok):
-    """The streaming kernel and the tcgen05 FD build must not depend on which fiber runs first (GHICP_EMU_SCHED: a fresh
+    """The streaming kernel and the wgmma FD build must not depend on which fiber runs first (GHICP_EMU_SCHED: a fresh
     random order every scheduling sweep) nor on a bulk copy having landed before its mbarrier says so (GHICP_EMU_TMA_DELAY: the
     destination is poisoned and the bytes land 1..n ticks later).  Negative control: with every mbarrier wait turned into a no-op
     the same check must FAIL — the modes can see a forgotten wait."""

@@ -26,7 +26,7 @@ def make_pair(g, orc, scene, Ft, Ct, dof=6, solve_mode=1, **kw):
 
 
 # ---- one-time FD build ---------------------------------------------------------------------------
-# 672 / 700 bits: K-chunked tcgen05 kernel with a 256-row B tile; 1000 / 1400: 128 rows; 2048 (the fp16 plane's limit): 64 rows
+# 672 / 700 bits: wgmma kernel with a 256-row B tile; 1000 / 1400: 128 rows; 2048 (the fp16 plane's limit): 64 rows
 @pytest.mark.parametrize("bits,V,dof", [(441, 4, 6), (672, 4, 6), (441, 2, 4), (64, 4, 6), (9, 2, 4), (672, 2, 4), (700, 4, 6),
                                         (1000, 4, 6), (1400, 2, 4), (2048, 4, 6)])
 @pytest.mark.parametrize("N,M", [(257, 131), (64, 300)])
@@ -373,7 +373,7 @@ def test_dof4_two_variants_loop(g, orc):
 
 
 def test_bsc_672_bits_loop(g, orc):
-    """BASELINE.json names 672-bit BSC; 672 bits take the POPC FD kernel (the tcgen05 tiling holds <= 448)."""
+    """BASELINE.json names 672-bit BSC; 672 bits take the tensor-core FD kernel with its widest B tile."""
     sc = g.synth.add_bsc(g.synth.gen_points(400, 420, overlap=0.7, extent=(50, 50, 10), noise=0.03, seed=78), bits=672, V=4)
     reg, o = make_pair(g, orc, sc, g.FT_BSC, g.CT_NNR, solve_mode=1)
     assert np.array_equal(reg.fd(), o.fd())

@@ -297,7 +297,7 @@ def test_cuda_path_reproduces_committed_loop_fixture(g, scratch_cwd, name):
 # ---- the reference's own per-pair feature distances (tests/golden/feat_golden.npz) -------------------------------------
 @pytest.mark.parametrize("bits", [441, 672, 9, 64, 2048])
 def test_fd_bsc_equals_reference_hamming_fixture(g, bits):
-    """The FD build (tcgen05 / POPC) against Hamming distances produced by the REFERENCE's own
+    """The FD build (wgmma / POPC) against Hamming distances produced by the REFERENCE's own
     StereoBinaryFeature::hammingDistance (compiled verbatim in the build container, outputs committed)."""
     from test_oracle_golden import load_feat_golden
     z = load_feat_golden()

@@ -128,7 +128,7 @@ struct Stats {
   double est_us = 0;
   void add(const Stats &o) { rounds += o.rounds; grid_rounds += o.grid_rounds; tail_rounds += o.tail_rounds; bids += o.bids; edges += o.edges; est_us += o.est_us; }
 };
-// time model of one round (measured on the B200: ~58 us per full-grid round at iteration 0, ~20 us per CTA-0 round)
+// time model of one round (cost per full-grid round and per CTA-0 round: inputs of the model, not measurements)
 static void account(Stats &st, ll n_active, ll edges, int small_n) {
   st.rounds++; st.bids += n_active; st.edges += edges;
   if (n_active > small_n) { st.grid_rounds++; st.est_us += 12.0 + (double)edges * 12.0 / 2.5e6; }   // 2.5 TB/s effective on the CSR

@@ -17,4 +17,4 @@ for bits in [int(x) for x in sys.argv[1:]] or [441, 672]:
         reg.build_fd()
         out.append(round((time.perf_counter() - t0) * 1e3, 2))
         reg.close()
-    print("bits", bits, "POPC" if os.environ.get("GHICP_FD_POPC") else "tcgen05", "build_fd ms (3 builds in one process):", out, flush=True)
+    print("bits", bits, "POPC" if os.environ.get("GHICP_FD_POPC") else "wgmma", "build_fd ms (3 builds in one process):", out, flush=True)

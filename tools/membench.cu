@@ -1,5 +1,5 @@
 // membench.cu — read-bandwidth ceilings for the access patterns k_stream can use on the FD plane.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o membench membench.cu && ./membench
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o membench membench.cu && ./membench
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -71,27 +71,27 @@ int main() {
   const size_t bytes = 5ull << 30; unsigned char* d; unsigned* out;
   CK(cudaMalloc(&d, bytes)); CK(cudaMalloc(&out, 4)); CK(cudaMemset(d, 1, bytes));
   const size_t n16 = bytes / 16;
-  float ms = timeit([&] { k_linear<<<148 * 8, 256>>>((const uint4*)d, n16, out); });
+  float ms = timeit([&] { k_linear<<<132 * 8, 256>>>((const uint4*)d, n16, out); });
   printf("linear grid-stride uint4 x4           : %.3f ms  %.0f GB/s\n", ms, bytes / ms / 1e6);
   const size_t region = 128 * 1024;  // 256 rows x 512 B, like one warp's sweep of a panel
   const int nregions = (int)(bytes / region);
-  ms = timeit([&] { k_warpstream<4><<<148 * 2, 256>>>((const uint4*)d, region / 16, nregions, out); });
+  ms = timeit([&] { k_warpstream<4><<<132 * 2, 256>>>((const uint4*)d, region / 16, nregions, out); });
   printf("per-warp 128KB streams, LDG x4, 16w/SM: %.3f ms  %.0f GB/s\n", ms, bytes / ms / 1e6);
-  ms = timeit([&] { k_warpstream<8><<<148 * 2, 256>>>((const uint4*)d, region / 16, nregions, out); });
+  ms = timeit([&] { k_warpstream<8><<<132 * 2, 256>>>((const uint4*)d, region / 16, nregions, out); });
   printf("per-warp 128KB streams, LDG x8, 16w/SM: %.3f ms  %.0f GB/s\n", ms, bytes / ms / 1e6);
-  ms = timeit([&] { k_warpstream<8><<<148 * 4, 256>>>((const uint4*)d, region / 16, nregions, out); });
+  ms = timeit([&] { k_warpstream<8><<<132 * 4, 256>>>((const uint4*)d, region / 16, nregions, out); });
   printf("per-warp 128KB streams, LDG x8, 32w/SM: %.3f ms  %.0f GB/s\n", ms, bytes / ms / 1e6);
   cudaFuncSetAttribute(k_tma<2048, 6>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * 6 * 2048);
-  ms = timeit([&] { k_tma<2048, 6><<<148 * 2, 256, 8 * 6 * 2048>>>(d, region, nregions, out); });
+  ms = timeit([&] { k_tma<2048, 6><<<132 * 2, 256, 8 * 6 * 2048>>>(d, region, nregions, out); });
   printf("per-warp TMA bulk 2KB x6 stages, 16w/SM: %.3f ms  %.0f GB/s\n", ms, bytes / ms / 1e6);
   cudaFuncSetAttribute(k_tma<4096, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * 3 * 4096);
-  ms = timeit([&] { k_tma<4096, 3><<<148 * 2, 256, 8 * 3 * 4096>>>(d, region, nregions, out); });
+  ms = timeit([&] { k_tma<4096, 3><<<132 * 2, 256, 8 * 3 * 4096>>>(d, region, nregions, out); });
   printf("per-warp TMA bulk 4KB x3 stages, 16w/SM: %.3f ms  %.0f GB/s\n", ms, bytes / ms / 1e6);
   cudaFuncSetAttribute(k_tma<8192, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * 3 * 8192);
-  ms = timeit([&] { k_tma<8192, 3><<<148 * 2, 128, 4 * 3 * 8192>>>(d, region, nregions, out); });
+  ms = timeit([&] { k_tma<8192, 3><<<132 * 2, 128, 4 * 3 * 8192>>>(d, region, nregions, out); });
   printf("per-warp TMA bulk 8KB x3 stages,  8w/SM: %.3f ms  %.0f GB/s\n", ms, bytes / ms / 1e6);
   // strided 512 B segments (the old row-major plane): region = one segment, regions far apart
-  ms = timeit([&] { k_warpstream<1><<<148 * 8, 256>>>((const uint4*)d, 32, (int)(bytes / 512), out); });
+  ms = timeit([&] { k_warpstream<1><<<132 * 8, 256>>>((const uint4*)d, 32, (int)(bytes / 512), out); });
   printf("per-warp 512B segments round-robin     : %.3f ms  %.0f GB/s\n", ms, bytes / ms / 1e6);
   return 0;
 }
