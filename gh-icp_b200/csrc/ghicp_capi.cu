@@ -254,11 +254,12 @@ static int build_fd(Ctx *c) {
     if (!c->have_bsc) { set_error(c, "build_fd: BSC descriptors not set"); return GHICP_E_ARG; }
     const int Vneed = (c->cfg.dof == 6) ? 4 : 2;
     if (c->V < Vneed) { set_error(c, "build_fd: not enough BSC source variants for dof"); return GHICP_E_ARG; }
-    if (c->bits > 2048) { set_error(c, "build_fd: BSC descriptors longer than 2048 bits are not supported (fp16 FD plane)"); return GHICP_E_ARG; }
+    if (c->bits > 2048) { set_error(c, "build_fd: BSC descriptors longer than 2048 bits are not supported (12-bit FD plane)"); return GHICP_E_ARG; }
     c->fd_rows = (size_t)std::max(c->nloc, 1);
-    int rc = dev_alloc(c, &c->d_fd16, fd_elems(c->fd_rows, c->M));
+    const size_t plane_bytes = fd_plane_bytes(c->fd_rows, c->M, fd_hb(c->bits));
+    int rc = dev_alloc(c, &c->d_fd16, (plane_bytes + 1) / 2);
     if (rc) return rc;
-    CK(c, cudaMemsetAsync(c->d_fd16, 0, fd_elems(c->fd_rows, c->M) * sizeof(uint16_t), c->stream));  // zero the panel padding
+    CK(c, cudaMemsetAsync(c->d_fd16, 0, plane_bytes, c->stream));  // zero the quad / panel padding
     {
       // tensor-core build (wgmma s8) when the descriptor fits its shared-memory tiling, else POPC
       cudaError_t e = (getenv("GHICP_FD_POPC") != nullptr) ? cudaErrorNotSupported : launch_fd_bsc_tc(c);

@@ -7,7 +7,7 @@
 // memory and streams 64-row target tiles (A) through a ring of K-chunk stages (cp.async.bulk, one mbarrier per stage).
 // Two consumer warpgroups each own half of the B tile's columns and issue wgmma.mma_async m64n32k32.s32.s8.s8 from shared
 // memory into register accumulators; after a tile's last K-chunk they take the min over the V variants (adjacent
-// accumulator columns: in-thread pairs, plus one lane shuffle for V = 4) and store fp16 into the panel-major FD plane.
+// accumulator columns: in-thread pairs, plus one lane shuffle for V = 4) and store into the packed panel-major FD plane (ghicp_internal.h: fd_at).
 // Operands sit in shared memory in the canonical K-major no-swizzle layout [k-chunk(16 B)][row][16 B]
 // (8-row x 16-byte core matrices back to back: SBO = 128 B between row groups, LBO = rows * 16 B between k-chunks).
 #include <cstdlib>
@@ -151,9 +151,9 @@ __device__ __forceinline__ void fence_acc(int (&acc)[NC][16]) {
 
 // B tile: TN (source, variant) rows x KP bytes, resident.  A tiles: TC_TM target rows, streamed in K-chunks of KC_BYTES through
 // KC_STAGES ring stages (warp 8 loads; every consumer warp hands a stage back on its `empty` barrier once its MMAs retired).
-template <int V, int TN>
+template <int V, int TN, int HB>
 __global__ void __launch_bounds__(TC_THREADS, 1)
-k_fd_bsc_tc(const int8_t *__restrict__ T8c, const int8_t *__restrict__ S8c, unsigned short *__restrict__ fd, int M,
+k_fd_bsc_tc(const int8_t *__restrict__ T8c, const int8_t *__restrict__ S8c, unsigned char *__restrict__ fdq, int M,
             size_t fd_rows, int row0, int nloc, int bits, int KP) {
 #if defined(GHICP_EMU_HOST)
   unsigned char *smem = reinterpret_cast<unsigned char *>(emu::dyn_smem());   // host emulation: the launch's dynamic shared memory
@@ -202,7 +202,7 @@ k_fd_bsc_tc(const int8_t *__restrict__ T8c, const int8_t *__restrict__ S8c, unsi
     return;
   }
 
-  // ===== consumer warpgroups: wgmma into registers, then min over variants -> fp16 -> FD plane =====
+  // ===== consumer warpgroups: wgmma into registers, then min over variants -> packed FD plane =====
   const int wg = warp >> 2, wl = warp & 3;
   const int col0 = wg * (TN / TC_CONSUMERS);   // first B row (column of D) of this warpgroup
   int acc[NC][16];
@@ -244,22 +244,48 @@ k_fd_bsc_tc(const int8_t *__restrict__ T8c, const int8_t *__restrict__ S8c, unsi
       if (lane == 0) mbar_arrive(&s_bar[KC_STAGES + st]);   // this warp's MMAs no longer read the stage
     }
     // epilogue.  Fragment of m64nNk32: element e of a thread sits at row 16 wl + lane / 4 + 8 ((e >> 1) & 1) and column
-    // 8 (e >> 2) + 2 (lane & 3) + (e & 1) of its instruction's 32 columns
+    // 8 (e >> 2) + 2 (lane & 3) + (e & 1) of its instruction's 32 columns.  For one (c, h) the warp's values cover 8 aligned
+    // target columns (one lane of a panel) and, over q, 16 aligned source rows: with V = 2 each q is one whole quad block
+    // (row (lane & 3)), with V = 4 two consecutive q are (rows 2 (q & 1) + (lane & 3) / 2, even lanes).  The low bytes go
+    // straight to the plane, the high-bit words are OR-reduced over the warp and written by lane 0.
+    constexpr int QPQ = (V == 4) ? 2 : 1;   // fragment steps per quad
+    constexpr int QB = FD_LOW_BYTES + 128 * HB;
+    const size_t panel_stride = fd_quads(fd_rows) * QB;
+    const int irel0 = src_base - row0;        // a multiple of 4
 #pragma unroll
-    for (int c = 0; c < NC; ++c) {
+    for (int h = 0; h < 2; ++h) {
+      const int j = t * TC_TM + wl * 16 + (lane >> 2) + 8 * h;   // target column of the FD plane
+      const int jp = j & (FD_PANEL - 1), c8 = j & 7;
+      unsigned char *pbase = fdq + (size_t)(j >> 8) * panel_stride;
+      unsigned char *hbase = pbase + FD_LOW_BYTES + (jp >> 3) * 4;   // word 0 of lane 0's panel lane, quad 0
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int j = t * TC_TM + wl * 16 + (lane >> 2) + 8 * h;   // target column of the FD plane
+      for (int c = 0; c < NC; ++c) {
+        unsigned hw[HB];
+#pragma unroll
+        for (int w = 0; w < HB; ++w) hw[w] = 0u;
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
           int best = max(acc[c][q * 4 + h * 2], acc[c][q * 4 + h * 2 + 1]);   // max dot = min Hamming
-          const int col = col0 + c * TC_NCH + 8 * q + 2 * (lane & 3);          // first of the two columns
           if (V == 4) best = max(best, __shfl_xor_sync(0xffffffffu, best, 1));  // the other two variants sit in lane ^ 1
-          if (V == 4 && (lane & 1)) continue;
-          const int i = src_base + col / V;
-          if (j < M && i < row0 + nloc) {
-            const int ham = (bits - best) >> 1;
-            fd[fd_index(fd_rows, i - row0, j)] = __half_as_ushort(__int2half_rn(ham));
+          // source row of this value, relative to the plane: quad (col0 + 32 c + 8 q) / (4 V), row u in the quad
+          const int irel = irel0 + (col0 + c * TC_NCH + 8 * q + 2 * (lane & 3)) / V;
+          const int u = irel & 3;
+          if (!(V == 4 && (lane & 1)) && j < M && irel < nloc) {
+            const unsigned ham = (unsigned)((bits - best) >> 1);
+            pbase[(size_t)(irel >> 2) * QB + u * FD_PANEL + jp] = (unsigned char)ham;
+            const int wd = fd_hi_word(HB, u, c8);
+            const unsigned part = fd_hi_part(HB, u, c8, ham);
+#pragma unroll
+            for (int w = 0; w < HB; ++w) hw[w] |= (w == wd) ? part : 0u;
+          }
+          if (q % QPQ == QPQ - 1) {
+            const int iq = irel >> 2;   // the warp's quad (lane 0's row is in it)
+#pragma unroll
+            for (int w = 0; w < HB; ++w) {
+              const unsigned word = fd_lanes_or<32>(hw[w]);
+              if (lane == 0 && j < M && iq * 4 < nloc) *reinterpret_cast<unsigned *>(hbase + (size_t)iq * QB + w * 128) = word;
+              hw[w] = 0u;
+            }
           }
         }
       }
@@ -274,12 +300,22 @@ k_fd_bsc_tc(const int8_t *__restrict__ T8c, const int8_t *__restrict__ S8c, unsi
 #else
 #define GHICP_TC_OPT_IN_SMEM(kernel) cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
 #endif
-template <int V, int TN>
+template <int V, int TN, int HB>
 static cudaError_t launch_tc(Ctx *c, const int8_t *T8, const int8_t *S8, int KP, int grid, size_t smem) {
-  GHICP_TC_OPT_IN_SMEM((k_fd_bsc_tc<V, TN>));
-  GHICP_LAUNCH((k_fd_bsc_tc<V, TN>), grid, TC_THREADS, smem, c->stream, T8, S8, c->d_fd16, c->M, c->fd_rows, c->r0, c->nloc,
+  GHICP_TC_OPT_IN_SMEM((k_fd_bsc_tc<V, TN, HB>));
+  GHICP_LAUNCH((k_fd_bsc_tc<V, TN, HB>), grid, TC_THREADS, smem, c->stream, T8, S8, reinterpret_cast<unsigned char *>(c->d_fd16), c->M, c->fd_rows, c->r0, c->nloc,
                c->bits, KP);
   return cudaGetLastError();
+}
+
+template <int V>
+static cudaError_t launch_tc_hb(Ctx *c, const int8_t *T8, const int8_t *S8, int KP, int grid, size_t smem, int TN, int hb) {
+  if (hb == 1) return TN == 256 ? launch_tc<V, 256, 1>(c, T8, S8, KP, grid, smem) : TN == 128 ? launch_tc<V, 128, 1>(c, T8, S8, KP, grid, smem)
+                                                                                  : launch_tc<V, 64, 1>(c, T8, S8, KP, grid, smem);
+  if (hb == 2) return TN == 256 ? launch_tc<V, 256, 2>(c, T8, S8, KP, grid, smem) : TN == 128 ? launch_tc<V, 128, 2>(c, T8, S8, KP, grid, smem)
+                                                                                  : launch_tc<V, 64, 2>(c, T8, S8, KP, grid, smem);
+  return TN == 256 ? launch_tc<V, 256, 4>(c, T8, S8, KP, grid, smem) : TN == 128 ? launch_tc<V, 128, 4>(c, T8, S8, KP, grid, smem)
+                                                                     : launch_tc<V, 64, 4>(c, T8, S8, KP, grid, smem);
 }
 
 // Returns cudaErrorNotSupported when the shape does not fit this kernel (caller falls back to k_fd_bsc).
@@ -311,13 +347,10 @@ cudaError_t launch_fd_bsc_tc(Ctx *c) {
                  c->nloc * V, S8);
     c->launches += 2;
   }
-  if (V == 4) {
-    e = TN == 256 ? launch_tc<4, 256>(c, T8, S8, KP, grid, smem) : TN == 128 ? launch_tc<4, 128>(c, T8, S8, KP, grid, smem)
-                                                                             : launch_tc<4, 64>(c, T8, S8, KP, grid, smem);
-  } else {
-    e = TN == 256 ? launch_tc<2, 256>(c, T8, S8, KP, grid, smem) : TN == 128 ? launch_tc<2, 128>(c, T8, S8, KP, grid, smem)
-                                                                             : launch_tc<2, 64>(c, T8, S8, KP, grid, smem);
-  }
+  // the high-bit count of the plane is a template parameter, so the epilogue's bit positions are shifts by constants
+  const int hb = fd_hb(c->bits);
+  if (V == 4) e = launch_tc_hb<4>(c, T8, S8, KP, grid, smem, TN, hb);
+  else e = launch_tc_hb<2>(c, T8, S8, KP, grid, smem, TN, hb);
   c->launches++;
   cudaFreeAsync(T8, c->stream);
   cudaFreeAsync(S8, c->stream);

@@ -27,12 +27,59 @@ constexpr int GHICP_SMS = 132;
 
 // Feature-distance plane layout: PANEL-MAJOR.  The N x M plane is stored as ceil(M/256) column panels, each
 // a dense row-major [rows][256] block, so the 256-column panel a warp sweeps down the source rows is one
-// perfectly sequential HBM stream (512 B per row back to back) instead of 512 B reads at a 2*M-byte stride.
+// perfectly sequential HBM stream instead of short reads at a row stride.  fd_index / fd_elems address the
+// float FPFH plane in this order.
 constexpr int FD_PANEL = 256;
 __host__ __device__ inline size_t fd_index(size_t rows, int i, int j) {
   return ((size_t)(j >> 8) * rows + (size_t)i) * FD_PANEL + (size_t)(j & (FD_PANEL - 1));
 }
 __host__ __device__ inline size_t fd_elems(size_t rows, int M) { return (size_t)((M + FD_PANEL - 1) / FD_PANEL) * rows * FD_PANEL; }
+
+// The BSC plane holds integer Hamming distances 0 ... bits (<= 2048), PACKED exactly into 8 + hb bits per value:
+//   hb = 1 for bits <= 511, 2 for bits <= 1023, 4 up to 2048 (fd_hb).
+// Panels as above; inside a panel the rows are grouped in QUADS (4 rows: one k_stream TMA stage).  A quad block is
+//   [4][256] low bytes (row-major)  |  [hb][32] 32-bit words of high bits (word h of lane l at h * 32 + l)
+// where "lane" l = column / 8 of the panel: a lane's 8 columns x 4 rows are 16 column PAIRS k = 4 * row + column / 2, and
+// the high bits of pair k, value e (= column & 1) sit in word k / (16 / hb) at bit hb * (k % (16 / hb)) + 16 e.  Shifting
+// a word so that a pair lands on bits 8 and 24 puts both high parts right above their low bytes (k_stream's decode).
+// Rows are padded to whole quads and columns to whole panels; padding holds zeros.
+constexpr int FD_QUAD = 4;
+constexpr int FD_LOW_BYTES = FD_QUAD * FD_PANEL;   // 1024
+__host__ __device__ inline int fd_hb(int bits) { return bits <= 511 ? 1 : bits <= 1023 ? 2 : 4; }
+__host__ __device__ inline size_t fd_block_bytes(int hb) { return (size_t)FD_LOW_BYTES + 128 * (size_t)hb; }   // 1152 / 1280 / 1536
+__host__ __device__ inline size_t fd_quads(size_t rows) { return (rows + FD_QUAD - 1) / FD_QUAD; }
+__host__ __device__ inline size_t fd_plane_bytes(size_t rows, int M, int hb) {
+  return (size_t)((M + FD_PANEL - 1) / FD_PANEL) * fd_quads(rows) * fd_block_bytes(hb);
+}
+// byte offset of the quad block holding rows 4 (i / 4) ... of the panel of column j
+__host__ __device__ inline size_t fd_block_offset(size_t rows, int hb, int i, int j) {
+  return ((size_t)(j >> 8) * fd_quads(rows) + (size_t)(i >> 2)) * fd_block_bytes(hb);
+}
+// high-bit word (0 ... hb-1) and bit position of value (u, c): row u of the quad, column c of the lane
+// (pair k = 4u + c/2 in word k / (16/hb) at hb * (k mod 16/hb); hb = 1, 2, 4 -> log2(hb) = hb >> 1, shifts instead of divisions)
+__host__ __device__ inline int fd_hi_word(int hb, int u, int c) { return (4 * u + (c >> 1)) >> (4 - (hb >> 1)); }
+__host__ __device__ inline int fd_hi_bit(int hb, int u, int c) {
+  return hb * ((4 * u + (c >> 1)) & ((16 >> (hb >> 1)) - 1)) + 16 * (c & 1);
+}
+// exact decode of FD(i, j), i relative to the plane's first row
+__host__ __device__ inline unsigned fd_at(const void *plane, size_t rows, int hb, int i, int j) {
+  const unsigned char *blk = static_cast<const unsigned char *>(plane) + fd_block_offset(rows, hb, i, j);
+  const int u = i & 3, col = j & (FD_PANEL - 1), c = col & 7;
+  const unsigned hi = reinterpret_cast<const unsigned *>(blk + FD_LOW_BYTES)[fd_hi_word(hb, u, c) * 32 + (col >> 3)];
+  return (unsigned)blk[u * FD_PANEL + col] | (((hi >> fd_hi_bit(hb, u, c)) & ((1u << hb) - 1u)) << 8);
+}
+// OR of v over aligned groups of WIDTH lanes (the encoders' high-bit words); every lane of the warp must take part
+template <int WIDTH>
+__device__ __forceinline__ unsigned fd_lanes_or(unsigned v) {
+#if !defined(GHICP_EMU_HOST)
+  if (WIDTH == 32) return __reduce_or_sync(0xffffffffu, v);
+#endif
+#pragma unroll
+  for (int o = 1; o < WIDTH; o <<= 1) v |= __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+// encoder side: value v's contribution to its high-bit word (the words of a quad and lane are the OR over its 32 values)
+__host__ __device__ inline unsigned fd_hi_part(int hb, int u, int c, unsigned v) { return (v >> 8) << fd_hi_bit(hb, u, c); }
 
 // ---- small device-side structs -----------------------------------------------------------------
 // Parameters of one cost evaluation CD(i,j) (src/ghicp_reg.cpp:122, 224, 259, 308).
@@ -79,16 +126,16 @@ struct StreamDev {  // device-resident scalars of the streaming path
   unsigned long long emit_count;  // KM: gate hits appended to the edge list by the count pass (may exceed its capacity)
 };
 struct StreamArgs {
-  const unsigned short *fd;  // fp16 FD plane (panel-major) or nullptr (no feature)
+  const unsigned char *fd;   // packed BSC FD plane (fd_at) or nullptr (no feature)
   size_t fd_rows;            // rows of the plane held by this context
+  int fd_hb;                 // high bits per value of the plane (fd_hb)
   int N, M;
   int row0, nloc;            // source rows [row0, row0 + nloc) streamed by this context
   int rb;                    // source rows per CTA of this launch (<= ST_RB, a multiple of the batch)
   const float4 *S4, *T4;
   const double *s, *t;
   double scale, WED, WFD;
-  float b;               // feature weight in the filter's (kappa-scaled) domain
-  unsigned short bh;     // the same weight as fp16 bits (FHFMA operand)
+  float b;               // feature weight in the filter's (kappa-scaled) domain (an fp16 value when x2_ok)
   double kappa;          // scale of the filter domain relative to CD
   StreamDev *dev;
   unsigned *row_thr_init; unsigned long long *rowbest; int *rowidx;
@@ -126,7 +173,7 @@ struct Ctx {
   int V = 0, bits = 0, Bbytes = 0, W64 = 0;
   uint64_t *d_bs = nullptr;  // [V][W64][N]
   uint64_t *d_bt = nullptr;  // [W64][M]
-  uint16_t *d_fd16 = nullptr;  // [N][ldM]
+  uint16_t *d_fd16 = nullptr;  // packed FD plane, fd_plane_bytes(fd_rows, M, fd_hb(bits)) bytes (allocated in 16-bit units)
   // FPFH
   float *d_fs = nullptr, *d_ft = nullptr;  // raw [N][33], [M][33]
   float *d_fdf = nullptr;                  // [N][ldM] float FD
@@ -185,10 +232,9 @@ struct Ctx {
 
   // streaming path
   bool use_fast = true;
-  bool x2_ok = true;         // packed-FP32 / FHFMA variant usable this iteration
+  bool x2_ok = true;         // column-pair FP32 variant usable this iteration (feature weight exact in fp16)
   double kappa = 1.0;
   float b_eff = 0.f;
-  unsigned short bh_bits = 0;
   long long last_cands = 0;  // candidates the filter passed to exact evaluation last iteration
   int fallbacks = 0;         // iterations that fell back to the all-double cost kernels
   bool have_prev = false;    // d_row_idx / d_col_idx hold last iteration's partners

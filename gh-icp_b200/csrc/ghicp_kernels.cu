@@ -43,7 +43,7 @@ __global__ void k_pack_bsc(const uint8_t *__restrict__ raw, uint64_t *__restrict
 }
 
 // ---------------------------------------------------------------------------------------------
-// calFD_BSC (src/ghicp_reg.cpp:143-200): FD[i][j] = min_v popcount(bscS[v][i] ^ bscT[0][j]) → u16.
+// calFD_BSC (src/ghicp_reg.cpp:143-200): FD[i][j] = min_v popcount(bscS[v][i] ^ bscT[0][j]) → the packed plane (fd_at).
 // CTA = 128 threads = 128 target columns x 32 source rows; source words staged in shared memory.
 // ---------------------------------------------------------------------------------------------
 constexpr int FDB_ROWS = 32;
@@ -51,8 +51,8 @@ constexpr int FDB_THREADS = 128;
 template <int V>
 __global__ void __launch_bounds__(FDB_THREADS) k_fd_bsc(const uint64_t *__restrict__ bs,
                                                          const uint64_t *__restrict__ bt,
-                                                         uint16_t *__restrict__ fd, int N, int M, size_t ldM,
-                                                         int W64, int row0, int nloc) {
+                                                         unsigned char *__restrict__ fdq, int hb, int N, int M,
+                                                         size_t ldM, int W64, int row0, int nloc) {
 #if defined(GHICP_EMU_HOST)
   uint64_t *s_words = reinterpret_cast<uint64_t *>(emu::dyn_smem());  // host emulation: the launch's dynamic shared memory
 #else
@@ -68,7 +68,9 @@ __global__ void __launch_bounds__(FDB_THREADS) k_fd_bsc(const uint64_t *__restri
     s_words[k] = (i < iend) ? bs[(size_t)vw * N + i] : 0ull;
   }
   __syncthreads();
-  if (j >= M) return;
+  // every lane stays to the end: the high-bit words of the packed plane are OR-reduced over the 8 lanes of a quad block's lane
+  const bool live = j < M;
+  const int jj = live ? j : M - 1;
   for (int rc = 0; rc < FDB_ROWS; rc += 8) {
     int acc[8][V];
 #pragma unroll
@@ -76,7 +78,7 @@ __global__ void __launch_bounds__(FDB_THREADS) k_fd_bsc(const uint64_t *__restri
 #pragma unroll
       for (int v = 0; v < V; ++v) acc[r][v] = 0;
     for (int w = 0; w < W64; ++w) {
-      const uint64_t tw = bt[(size_t)w * M + j];
+      const uint64_t tw = bt[(size_t)w * M + jj];
 #pragma unroll
       for (int v = 0; v < V; ++v) {
         const uint64_t *sw = &s_words[(v * W64 + w) * FDB_ROWS + rc];
@@ -84,14 +86,28 @@ __global__ void __launch_bounds__(FDB_THREADS) k_fd_bsc(const uint64_t *__restri
         for (int r = 0; r < 8; ++r) acc[r][v] += __popcll(sw[r] ^ tw);
       }
     }
+    // rows i0 + rc ... + 7 are two whole quads (i0 - row0 and rc are multiples of 4)
 #pragma unroll
-    for (int r = 0; r < 8; ++r) {
-      int i = i0 + rc + r;
-      if (i < iend) {
+    for (int qd = 0; qd < 2; ++qd) {
+      unsigned hw[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+      for (int u = 0; u < FD_QUAD; ++u) {
+        const int r = FD_QUAD * qd + u, i = i0 + rc + r;
         int m = acc[r][0];
 #pragma unroll
         for (int v = 1; v < V; ++v) m = min(m, acc[r][v]);
-        fd[fd_index(ldM, i - row0, j)] = __half_as_ushort(__int2half_rn(m));
+        if (!live || i >= iend) m = 0;
+        else fdq[fd_block_offset(ldM, hb, i - row0, j) + u * FD_PANEL + (j & (FD_PANEL - 1))] = (unsigned char)m;
+        const int c = j & 7, wd = fd_hi_word(hb, u, c);
+        const unsigned part = fd_hi_part(hb, u, c, (unsigned)m);
+#pragma unroll
+        for (int w = 0; w < 4; ++w) hw[w] |= (w == wd) ? part : 0u;
+      }
+      const int iq = i0 + rc + FD_QUAD * qd;
+      for (int w = 0; w < hb; ++w) {
+        const unsigned word = fd_lanes_or<8>(hw[w]);   // a warp's 32 columns are four whole lanes of the panel
+        if ((j & 7) == 0 && live && iq < iend)
+          reinterpret_cast<unsigned *>(fdq + fd_block_offset(ldM, hb, iq - row0, j) + FD_LOW_BYTES)[w * 32 + ((j & (FD_PANEL - 1)) >> 3)] = word;
       }
     }
   }
@@ -155,7 +171,8 @@ __global__ void __launch_bounds__(FPT *FPT) k_fd_fpfh(const float *__restrict__ 
 struct SweepArgs {
   const double *s;  // [3][N]
   const double *t;  // [3][M]
-  const uint16_t *fd16;
+  const unsigned char *fdq;  // packed BSC plane (fd_at)
+  int hb;
   const float *fdf;
   size_t ldM;
   int N, M, n_chunks, cols_per_chunk;
@@ -212,9 +229,8 @@ __global__ void __launch_bounds__(SWEEP_THREADS) k_rowsweep(const SweepArgs a) {
         const double sx = s_src[0][r], sy = s_src[1][r], sz = s_src[2][r];
         double fdv[COLS_PER_THREAD];
         if (FT == GHICP_FT_BSC) {
-          const uint2 q = *reinterpret_cast<const uint2 *>(a.fd16 + fd_index(a.ldM, i0 + r - a.row0, j));
-          fdv[0] = h2d(q.x & 0xffffu); fdv[1] = h2d(q.x >> 16);
-          fdv[2] = h2d(q.y & 0xffffu); fdv[3] = h2d(q.y >> 16);
+#pragma unroll
+          for (int c = 0; c < COLS_PER_THREAD; ++c) fdv[c] = (double)fd_at(a.fdq, a.ldM, a.hb, i0 + r - a.row0, j + c);
         } else if (FT == GHICP_FT_FPFH) {
           const float4 q = *reinterpret_cast<const float4 *>(a.fdf + fd_index(a.ldM, i0 + r - a.row0, j));
           fdv[0] = (double)q.x; fdv[1] = (double)q.y; fdv[2] = (double)q.z; fdv[3] = (double)q.w;
@@ -295,7 +311,8 @@ constexpr int CT = 8;
 constexpr int COL_THREADS = 256;
 struct ColArgs {
   const double *s, *t;
-  const uint16_t *fd16;
+  const unsigned char *fdq;  // packed BSC plane (fd_at)
+  int hb;
   const float *fdf;
   size_t ldM;
   int N, M;
@@ -325,11 +342,8 @@ __global__ void __launch_bounds__(COL_THREADS) k_colsweep(const ColArgs a) {
     const double sx = sxp[i], sy = syp[i], sz = szp[i];
     double fdv[CT];
     if (FT == GHICP_FT_BSC) {
-      const uint4 q = *reinterpret_cast<const uint4 *>(a.fd16 + fd_index(a.ldM, i - a.row0, j0));
-      fdv[0] = h2d(q.x & 0xffffu); fdv[1] = h2d(q.x >> 16);
-      fdv[2] = h2d(q.y & 0xffffu); fdv[3] = h2d(q.y >> 16);
-      fdv[4] = h2d(q.z & 0xffffu); fdv[5] = h2d(q.z >> 16);
-      fdv[6] = h2d(q.w & 0xffffu); fdv[7] = h2d(q.w >> 16);
+#pragma unroll
+      for (int c = 0; c < CT; ++c) fdv[c] = (double)fd_at(a.fdq, a.ldM, a.hb, i - a.row0, j0 + c);
     } else if (FT == GHICP_FT_FPFH) {
       const float4 q0 = *reinterpret_cast<const float4 *>(a.fdf + fd_index(a.ldM, i - a.row0, j0));
       const float4 q1 = *reinterpret_cast<const float4 *>(a.fdf + fd_index(a.ldM, i - a.row0, j0 + 4));
@@ -372,7 +386,7 @@ __global__ void __launch_bounds__(1024) k_finalize(const double *__restrict__ pa
                                                    const int *__restrict__ part_idx, int n_chunks, int row0, int nloc,
                                                    const double *__restrict__ part_stats, int n_parts,
                                                    double *__restrict__ row_cd, int *__restrict__ row_idx,
-                                                   float *__restrict__ row_fd, const uint16_t *__restrict__ fd16,
+                                                   float *__restrict__ row_fd, const unsigned char *__restrict__ fdq, int hb,
                                                    const float *__restrict__ fdf, size_t fd_rows,
                                                    double *__restrict__ xstats /* [world][2] */, int rank) {
   __shared__ double smem[2 * 32];
@@ -382,7 +396,7 @@ __global__ void __launch_bounds__(1024) k_finalize(const double *__restrict__ pa
     for (int c = 1; c < n_chunks; ++c) lexmin(v, ix, part_cd[(size_t)i * n_chunks + c], part_idx[(size_t)i * n_chunks + c]);
     row_cd[i] = v;
     row_idx[i] = ix;
-    row_fd[i] = fd16 ? (float)h2d(fd16[fd_index(fd_rows, i - row0, ix)]) : (fdf ? fdf[fd_index(fd_rows, i - row0, ix)] : 0.f);
+    row_fd[i] = fdq ? (float)fd_at(fdq, fd_rows, hb, i - row0, ix) : (fdf ? fdf[fd_index(fd_rows, i - row0, ix)] : 0.f);
   }
   double acc[2] = {0.0, 0.0};
   for (int p = threadIdx.x; p < n_parts; p += blockDim.x) {
@@ -748,13 +762,13 @@ __global__ void k_apply(double *__restrict__ s, int N, const DevIter *__restrict
   s[2 * (size_t)N + i] = ((Rt[2] * x + Rt[6] * y) + Rt[10] * z) + Rt[14];
 }
 
-__global__ void k_fd_to_double(const uint16_t *__restrict__ fd16, const float *__restrict__ fdf, size_t ldM,
+__global__ void k_fd_to_double(const unsigned char *__restrict__ fdq, int hb, const float *__restrict__ fdf, size_t ldM,
                                int N, int M, int row0, int nloc, double *__restrict__ out) {
   const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= (size_t)N * M) return;
   const int i = (int)(idx / M), j = (int)(idx % M);
   if (i < row0 || i >= row0 + nloc) { out[idx] = 0.0; return; }  // rows held by another rank
-  out[idx] = fd16 ? h2d(fd16[fd_index(ldM, i - row0, j)]) : (fdf ? (double)fdf[fd_index(ldM, i - row0, j)] : 0.0);
+  out[idx] = fdq ? (double)fd_at(fdq, ldM, hb, i - row0, j) : (fdf ? (double)fdf[fd_index(ldM, i - row0, j)] : 0.0);
 }
 
 // KM: FD of every kept pair, looked up in the candidate CSR (every rank holds the full CSR, not the full plane)
@@ -817,9 +831,11 @@ cudaError_t launch_fd_bsc(Ctx *c) {
   dim3 grid((c->M + FDB_THREADS - 1) / FDB_THREADS, (c->nloc + FDB_ROWS - 1) / FDB_ROWS);
   size_t smem = (size_t)V * c->W64 * FDB_ROWS * sizeof(uint64_t);
   if (V == 4)
-    GHICP_LAUNCH(k_fd_bsc<4>, grid, FDB_THREADS, smem, c->stream, c->d_bs, c->d_bt, c->d_fd16, c->N, c->M, c->fd_rows, c->W64, c->r0, c->nloc);
+    GHICP_LAUNCH(k_fd_bsc<4>, grid, FDB_THREADS, smem, c->stream, c->d_bs, c->d_bt, reinterpret_cast<unsigned char *>(c->d_fd16), fd_hb(c->bits),
+                 c->N, c->M, c->fd_rows, c->W64, c->r0, c->nloc);
   else
-    GHICP_LAUNCH(k_fd_bsc<2>, grid, FDB_THREADS, smem, c->stream, c->d_bs, c->d_bt, c->d_fd16, c->N, c->M, c->fd_rows, c->W64, c->r0, c->nloc);
+    GHICP_LAUNCH(k_fd_bsc<2>, grid, FDB_THREADS, smem, c->stream, c->d_bs, c->d_bt, reinterpret_cast<unsigned char *>(c->d_fd16), fd_hb(c->bits),
+                 c->N, c->M, c->fd_rows, c->W64, c->r0, c->nloc);
   c->launches++;
   return cudaGetLastError();
 }
@@ -841,7 +857,7 @@ cudaError_t launch_fd_fpfh(Ctx *c) {
 
 cudaError_t launch_rowsweep(Ctx *c, int mode, const CostParams &cp) {
   SweepArgs a{};
-  a.s = c->d_s; a.t = c->d_t; a.fd16 = c->d_fd16; a.fdf = c->d_fdf; a.ldM = c->fd_rows;
+  a.s = c->d_s; a.t = c->d_t; a.fdq = reinterpret_cast<const unsigned char *>(c->d_fd16); a.hb = fd_hb(c->bits); a.fdf = c->d_fdf; a.ldM = c->fd_rows;
   a.N = c->N; a.M = c->M; a.n_chunks = c->n_chunks;
   a.row0 = c->r0; a.nloc = c->nloc;
   int cpc = (c->M + c->n_chunks - 1) / c->n_chunks;
@@ -864,7 +880,7 @@ cudaError_t launch_rowsweep(Ctx *c, int mode, const CostParams &cp) {
 
 cudaError_t launch_colsweep(Ctx *c, const CostParams &cp) {
   ColArgs a{};
-  a.s = c->d_s; a.t = c->d_t; a.fd16 = c->d_fd16; a.fdf = c->d_fdf; a.ldM = c->fd_rows;
+  a.s = c->d_s; a.t = c->d_t; a.fdq = reinterpret_cast<const unsigned char *>(c->d_fd16); a.hb = fd_hb(c->bits); a.fdf = c->d_fdf; a.ldM = c->fd_rows;
   a.N = c->N; a.M = c->M; a.row0 = c->r0; a.nloc = c->nloc; a.cp = cp; a.col_cd = c->d_col_cd; a.col_idx = c->d_col_idx;
   dim3 grid((c->M + CT - 1) / CT);
   cudaError_t e = dispatch_ft(c->cfg.feature_type, [&](auto ft) {
@@ -881,7 +897,7 @@ cudaError_t launch_finalize_stats(Ctx *c, const CostParams &cp, const LoopScalar
   (void)cp; (void)ls;
   const int n_parts = ((c->nloc + TR - 1) / TR) * c->n_chunks;
   GHICP_LAUNCH(k_finalize, 1, 1024, 0, c->stream, c->d_part_cd, c->d_part_idx, c->n_chunks, c->r0, c->nloc, c->d_part_stats,
-                                        n_parts, c->d_row_cd, c->d_row_idx, c->d_row_fd, c->d_fd16, c->d_fdf,
+                                        n_parts, c->d_row_cd, c->d_row_idx, c->d_row_fd, reinterpret_cast<const unsigned char *>(c->d_fd16), fd_hb(c->bits), c->d_fdf,
                                         c->fd_rows, c->d_xstats, c->rank);
   c->launches++;
   return cudaGetLastError();
@@ -985,7 +1001,7 @@ cudaError_t launch_apply(Ctx *c, bool guard_overflow) {
 
 cudaError_t launch_get_fd(Ctx *c, double *d_out) {
   const size_t total = (size_t)c->N * c->M;
-  GHICP_LAUNCH(k_fd_to_double, (unsigned)((total + 255) / 256), 256, 0, c->stream, c->d_fd16, c->d_fdf, c->fd_rows, c->N, c->M, c->r0, c->nloc, d_out);
+  GHICP_LAUNCH(k_fd_to_double, (unsigned)((total + 255) / 256), 256, 0, c->stream, reinterpret_cast<const unsigned char *>(c->d_fd16), fd_hb(c->bits), c->d_fdf, c->fd_rows, c->N, c->M, c->r0, c->nloc, d_out);
   c->launches++;
   return cudaGetLastError();
 }

@@ -1,6 +1,6 @@
 // ghicp_stream.cu — the streaming cost/correspondence kernel of the GH-ICP inner loop (sm_90a).
 //
-// One pass over the N x M feature-distance plane (fp16, 2 B/pair — the only O(N*M) HBM traffic of an
+// One pass over the N x M feature-distance plane (packed, 9 / 10 / 12 bits per pair — the only O(N*M) HBM traffic of an
 // iteration) fuses calED + calCD_* + the NN / NNR scans or the KM candidate gate
 // (src/ghicp_reg.cpp:114-139, 216-293, 348-365, 622-650, 715-733) and the CD mean / std reductions
 // (:228, 264-272).  ED and CD are never stored.
@@ -14,8 +14,9 @@
 // centroid, then cd32 = sqrt.approx(d2') + WFD*fd.   |cd32 - cd64| <= margin (see k_margin).
 //
 // Thread mapping: a warp owns a 256-column panel (lane = 8 consecutive columns whose T operands stay in
-// registers) and sweeps ST_RB source rows; per row a lane issues one 16-byte load of the FD plane
-// (512 contiguous bytes per warp and row).  Row minima are warp-reduced with one REDUX per row.
+// registers) and sweeps ST_RB source rows, one quad block of the packed plane (4 rows, ghicp_internal.h) per TMA stage;
+// per row a lane reads its 8 low bytes, per quad its hb words of high bits, and decodes in registers.  Row minima are
+// warp-reduced with one REDUX per row.
 #include <climits>
 #include <cstdlib>
 #include <cuda_fp16.h>
@@ -34,25 +35,28 @@ constexpr int ST_CTA_COLS = ST_WARPS * ST_PANEL;  // 2048
 constexpr int ST_RB = 256;                        // source rows per CTA (upper bound; StreamArgs::rb is what a launch uses)
 constexpr int ST_RB_MIN = 64;
 // tuning knobs (compile-time; tools/build_variants.sh builds A/B libraries with other values)
-#ifndef GHICP_ST_UNROLL
-#define GHICP_ST_UNROLL 4
+#ifndef GHICP_ST_RING_KB
+#define GHICP_ST_RING_KB 12
 #endif
-#ifndef GHICP_ST_STAGES
-#define GHICP_ST_STAGES 6
+#ifndef GHICP_ST_QPS
+#define GHICP_ST_QPS 4
 #endif
 #ifndef GHICP_ST_MINB
 #define GHICP_ST_MINB 2
 #endif
-constexpr int ST_UNROLL = GHICP_ST_UNROLL;
+constexpr int ST_UNROLL = FD_QUAD;   // rows per batch = one quad block of the packed plane (part of its format)
 constexpr unsigned INF_BITS = 0x7f800000u;
-// TMA staging of the FD plane: every warp runs its own ring of ST_STAGES stages; a stage holds ST_UNROLL
-// row segments of the warp's 256-column panel (512 B each), brought in by cp.async.bulk (TMA engine,
-// UBLKCP) and signalled on one mbarrier per stage.  No registers are tied up by loads in flight.
-constexpr int ST_STAGES = GHICP_ST_STAGES;
-constexpr int ST_SEG_BYTES = ST_PANEL * 2;                   // 512
-constexpr int ST_STAGE_BYTES = ST_UNROLL * ST_SEG_BYTES;     // 2048
-constexpr int ST_RING_BYTES = ST_STAGES * ST_STAGE_BYTES;    // per warp
+// TMA staging of the FD plane: every warp runs its own ring of stages in at most GHICP_ST_RING_KB; a stage holds ST_QPS
+// consecutive quad blocks of the warp's 256-column panel (fd_block_bytes(hb) = 1152 / 1280 / 1536 B each), brought in by ONE
+// cp.async.bulk (TMA engine, UBLKCP) and signalled on one mbarrier per stage.  No registers are tied up by loads in flight.
+// Four quads per stage (two stages) measured fastest on the H100: fewer, larger copies beat more bytes in flight.
+constexpr int ST_RING_BYTES = GHICP_ST_RING_KB * 1024;   // per warp
 constexpr int ST_DYN_SMEM = ST_WARPS * ST_RING_BYTES;
+constexpr int ST_QPS = GHICP_ST_QPS;                     // quad blocks (batches) per stage
+template <int HB> __host__ __device__ constexpr int st_quad_bytes() { return FD_LOW_BYTES + 128 * HB; }
+template <int HB> __host__ __device__ constexpr int st_stage_bytes() { return ST_QPS * st_quad_bytes<HB>(); }
+template <int HB> __host__ __device__ constexpr int st_stages() { return ST_RING_BYTES / st_stage_bytes<HB>(); }
+constexpr int ST_MAX_STAGES = ST_RING_BYTES / (ST_QPS * (FD_LOW_BYTES + 128));
 
 #if defined(GHICP_EMU_HOST)
 __device__ __forceinline__ void fence_proxy_async() {}     // one OS thread: program order is memory order
@@ -63,7 +67,14 @@ __device__ __forceinline__ void mbar_init(unsigned long long *bar, int count) { 
 __device__ __forceinline__ void mbar_expect_tx(unsigned long long *bar, unsigned bytes) { emu::bar_arrive_expect_tx(bar, bytes); }
 __device__ __forceinline__ void mbar_wait(unsigned long long *bar, unsigned parity) { emu::bar_wait(bar, parity); }
 __device__ __forceinline__ void bulk_g2s(void *dst, const void *src, unsigned bytes, unsigned long long *bar) { emu::bulk_copy(dst, src, bytes, bar); }
+__device__ __forceinline__ unsigned byte_perm(unsigned x, unsigned y, unsigned sel) {   // PRMT, default mode
+  const unsigned long long xy = ((unsigned long long)y << 32) | x;
+  unsigned r = 0;
+  for (int n = 0; n < 4; ++n) r |= (unsigned)((xy >> (8 * ((sel >> (4 * n)) & 7))) & 0xffu) << (8 * n);
+  return r;
+}
 #else
+__device__ __forceinline__ unsigned byte_perm(unsigned x, unsigned y, unsigned sel) { return __byte_perm(x, y, sel); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void fence_mbarrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ unsigned smem_u32(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
@@ -90,8 +101,7 @@ __device__ __forceinline__ void bulk_g2s(void *dst, const void *src, unsigned by
 enum { SM_NN = 0, SM_NNR = 1, SM_COUNT = 2, SM_FILL = 3, SM_PRE = 4, SM_PRE_COLS = 5 };
 
 // Column pairs travel as one 64-bit value (two floats); Hopper has no packed f32x2 arithmetic, so fma2 / add2 are two scalar
-// operations with one rounding each.  fhfma = fd(fp16) * weight(fp16) + dist: the product of two halves is exact in float,
-// so the fmaf of the converted halves rounds once, like a mixed-precision FMA would.
+// operations with one rounding each.
 typedef unsigned long long u64;
 __device__ __forceinline__ u64 pack2(float lo, float hi) { return ((u64)__float_as_uint(hi) << 32) | __float_as_uint(lo); }
 __device__ __forceinline__ void unpack2(u64 v, float &lo, float &hi) { lo = __uint_as_float((unsigned)v); hi = __uint_as_float((unsigned)(v >> 32)); }
@@ -103,24 +113,14 @@ __device__ __forceinline__ u64 add2(u64 a, u64 b) {
   float al, ah, bl, bh; unpack2(a, al, ah); unpack2(b, bl, bh);
   return pack2(__fadd_rn(al, bl), __fadd_rn(ah, bh));
 }
-__device__ __forceinline__ float fhfma(unsigned short h, unsigned short w, float c) {
-  return fmaf(__half2float(__ushort_as_half(h)), __half2float(__ushort_as_half(w)), c);
-}
 #if defined(GHICP_EMU_HOST)
 // Host emulation of the PTX-only operations: the approximate square root becomes the exact one (inside the filter's error
-// budget), the streaming load a plain one.
+// budget).
 __device__ __forceinline__ float sqrt_approx(float x) { return sqrtf(x); }
-__device__ __forceinline__ uint4 ldg_stream(const uint4 *p) { return *p; }
 #else
 __device__ __forceinline__ float sqrt_approx(float x) {
   float r;
   asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
-  return r;
-}
-__device__ __forceinline__ uint4 ldg_stream(const uint4 *p) {
-  uint4 r;
-  asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
   return r;
 }
 #endif
@@ -130,6 +130,24 @@ __device__ __forceinline__ unsigned long long ord64(double v) {  // CD >= 0: bit
 __device__ __forceinline__ float half_lo(unsigned w) { return __half2float(__ushort_as_half((unsigned short)(w & 0xffffu))); }
 __device__ __forceinline__ float half_hi(unsigned w) { return __half2float(__ushort_as_half((unsigned short)(w >> 16))); }
 
+// Decode of column pair p (columns 2p, 2p+1 of the lane) of quad row u from the staged quad block: lo4 = the 4 low bytes
+// of columns 4 (p / 2) ..., hw = the lane's high-bit words.  One PRMT spreads the two low bytes to bits 0 and 16, one shift
+// brings the pair's high bits to bits 8 (and 24) and one LOP3 ORs them in: two 16-bit patterns fd0, fd1.  Read as fp16, a
+// pattern v <= 2048 is exactly v * 2^-24 (subnormal below 1024, exponent field 1 below 2048, 2^-13 for 2048), so the usual
+// fp16 -> f32 conversion yields f = fd * 2^-24 exactly, and fmaf(f, 2^24 b, dist) == fmaf(fd, b, dist) bit for bit: the
+// product is exact either way and the FMA rounds once.
+template <int HB>
+__device__ __forceinline__ void fd_pair(unsigned lo4, const unsigned (&hw)[HB], int u, int p, float &f0, float &f1) {
+  constexpr int PPW = 16 / HB;                       // pairs per high-bit word
+  constexpr unsigned MASK = HB == 1 ? 0x01000100u : HB == 2 ? 0x03000300u : 0x0f000f00u;
+  const int k = 4 * u + p;
+  const int sh = HB * (k % PPW) - 8;
+  const unsigned hv = sh >= 0 ? hw[k / PPW] >> sh : hw[k / PPW] << -sh;
+  const unsigned h2 = byte_perm(lo4, 0u, (p & 1) ? 0x4342u : 0x4140u) | (hv & MASK);
+  f0 = half_lo(h2);
+  f1 = half_hi(h2);
+}
+
 // exact CD(i,j), the reference's operation order, no FMA contraction (src/ghicp_reg.cpp:122,224,259)
 __device__ GHICP_NOINLINE double exact_cd(const StreamArgs &a, int i, int j) {
   const double sx = a.s[i], sy = a.s[(size_t)a.N + i], sz = a.s[2 * (size_t)a.N + i];
@@ -138,7 +156,7 @@ __device__ GHICP_NOINLINE double exact_cd(const StreamArgs &a, int i, int j) {
   const double d2 = __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
   const double ed = __dmul_rn(a.scale, __dsqrt_rn(d2));
   if (a.fd) {
-    const double fd = (double)__half2float(__ushort_as_half(a.fd[fd_index(a.fd_rows, i - a.row0, j)]));
+    const double fd = (double)fd_at(a.fd, a.fd_rows, a.fd_hb, i - a.row0, j);
     return __dadd_rn(__dmul_rn(a.WED, ed), __dmul_rn(a.WFD, fd));
   }
   return ed;
@@ -276,7 +294,7 @@ __device__ GHICP_NOINLINE void emit_hits(const StreamArgs &a, int *s_cnt_r, int 
   }
 }
 
-template <int MODE, bool HAS_FD, bool STATS, bool FULL, bool TMA, bool X2>
+template <int MODE, bool HAS_FD, bool STATS, bool FULL, int HB, bool X2>
 __device__ __forceinline__ void sweep(const StreamArgs &a, const float4 *s_S4, const float *s_S8, unsigned *s_thr, int *s_cnt,
                                       int r0, int nrows, int j0, int lane, double &dsum, double &dsq,
                                       unsigned char *ring, unsigned long long *bars) {
@@ -303,10 +321,6 @@ __device__ __forceinline__ void sweep(const StreamArgs &a, const float4 *s_S4, c
       Tz2[p] = pack2(Tz[2 * p], Tz[2 * p + 1]); Tw2[p] = pack2(Tw[2 * p], Tw[2 * p + 1]);
     }
   }
-  // keep the fp16 weight in a per-thread (vector) register: FHFMA takes no uniform-register operand, and a
-  // value the compiler can prove warp-uniform would be re-materialised from the constant bank per use
-  // (bit 31 of a running-minimum word is always 0 — a positive float — but only known at run time)
-  const unsigned short bh = (unsigned short)(a.bh | (unsigned short)(s_thr[0] >> 31));
   const float margin = a.dev->margin;
   const float m2 = 2.f * margin;
   if (MODE == SM_NNR) {
@@ -314,47 +328,43 @@ __device__ __forceinline__ void sweep(const StreamArgs &a, const float4 *s_S4, c
     for (int c = 0; c < ST_CPL; ++c) colrun[c] += m2;   // (padding columns: cd = +inf never passes a finite threshold)
   }
   const float thr_hi = a.dev->thr_hi;
-  const float b = a.b;
-  const bool lane_loads = true;  // the panel-major plane is allocated in whole panels (zero padded)
-  const unsigned short *fdp = HAS_FD ? a.fd + fd_index(a.fd_rows, r0 - a.row0, j0) : nullptr;
+  const float b24 = a.b * 16777216.f;   // 2^24 b, exact: the decoded FD values carry the factor 2^-24 (fd_pair)
   // ---- TMA ring bookkeeping (warp-private) ----
+  constexpr int STAGES = st_stages<HB>(), STAGE_BYTES = st_stage_bytes<HB>(), QUAD_BYTES = st_quad_bytes<HB>();
   const int panel = j0 - lane * ST_CPL;
-  const unsigned short *panel_base = (HAS_FD && TMA) ? a.fd + fd_index(a.fd_rows, r0 - a.row0, panel) : nullptr;
+  // rows are padded to whole quads (r0 - row0 is a multiple of 4): a batch is one whole quad block, a stage ST_QPS of them
+  // (fewer in the CTA's last stage)
+  const unsigned char *panel_base = HAS_FD ? a.fd + fd_block_offset(a.fd_rows, HB, r0 - a.row0, panel) : nullptr;
   const int nbatch = (nrows + ST_UNROLL - 1) / ST_UNROLL;
-  auto issue = [&](int k) {  // lane 0 only
-    const int stage = k % ST_STAGES;
-    const int rows = min(ST_UNROLL, nrows - k * ST_UNROLL);
-    // panel-major plane: the ST_UNROLL row segments of a stage are contiguous -> ONE bulk copy
-    mbar_expect_tx(&bars[stage], (unsigned)rows * ST_SEG_BYTES);
-    bulk_g2s(ring + stage * ST_STAGE_BYTES, panel_base + (size_t)(k * ST_UNROLL) * FD_PANEL, (unsigned)rows * ST_SEG_BYTES,
-             &bars[stage]);
+  const int nstage = (nbatch + ST_QPS - 1) / ST_QPS;
+  auto issue = [&](int st) {  // lane 0 only
+    const int slot = st % STAGES;
+    const unsigned bytes = (unsigned)(min(ST_QPS, nbatch - st * ST_QPS) * QUAD_BYTES);
+    mbar_expect_tx(&bars[slot], bytes);
+    bulk_g2s(ring + slot * STAGE_BYTES, panel_base + (size_t)st * STAGE_BYTES, bytes, &bars[slot]);
   };
-  // (the first ST_STAGES batches were issued by the kernel prologue, before the operand staging)
+  // (the first STAGES stages were issued by the kernel prologue, before the operand staging)
 
   for (int rb = 0; rb < nrows; rb += ST_UNROLL) {
-    uint4 q[ST_UNROLL];
-    if (HAS_FD && TMA) {
-      const int k = rb / ST_UNROLL;
-      const int stage = k % ST_STAGES;
-      mbar_wait(&bars[stage], (unsigned)((k / ST_STAGES) & 1));
-    } else if (HAS_FD) {
+    uint2 lo[ST_UNROLL];
+    unsigned hw[HB];
+    // per-batch base addresses: everything inside the unrolled rows is base + immediate
+    const int kb = rb / ST_UNROLL, kst = kb / ST_QPS;
+    const unsigned char *qbase = HAS_FD ? ring + (kst % STAGES) * STAGE_BYTES + (kb % ST_QPS) * QUAD_BYTES : nullptr;
+    if (HAS_FD) {
+      if (kb % ST_QPS == 0) mbar_wait(&bars[kst % STAGES], (unsigned)((kst / STAGES) & 1));
 #pragma unroll
-      for (int u = 0; u < ST_UNROLL; ++u) {
-        const int r = min(rb + u, nrows - 1);
-        q[u] = lane_loads ? ldg_stream(reinterpret_cast<const uint4 *>(fdp + (size_t)r * FD_PANEL)) : make_uint4(0, 0, 0, 0);
-      }
+      for (int w = 0; w < HB; ++w) hw[w] = reinterpret_cast<const unsigned *>(qbase + FD_LOW_BYTES)[w * 32 + lane];
     }
     float psum = 0.f, psq = 0.f;
     u64 psum2 = 0ull, psq2 = 0ull;
-    // per-batch base addresses: everything inside the unrolled rows is base + immediate
-    const unsigned char *qbase = (HAS_FD && TMA) ? ring + ((rb / ST_UNROLL) % ST_STAGES) * ST_STAGE_BYTES + lane * 16 : nullptr;
     const float *s8base = s_S8 + rb * 8;
     const float4 *s4base = s_S4 + rb;
     unsigned *thrbase = s_thr + rb;
     auto compute_row = [&](const int u, float (&cd)[ST_CPL]) {
         const float4 S = X2 ? make_float4(0.f, 0.f, 0.f, 0.f) : s4base[u];
-        if (HAS_FD && TMA)  // just-in-time read of this row's 8 values from the staged segment
-          q[u] = *reinterpret_cast<const uint4 *>(qbase + u * ST_SEG_BYTES);
+        if (HAS_FD)  // just-in-time read of this row's 8 low bytes from the staged quad block
+          lo[u] = *reinterpret_cast<const uint2 *>(qbase + u * FD_PANEL + lane * ST_CPL);
                 if (X2) {
           const ulonglong2 sA = *reinterpret_cast<const ulonglong2 *>(s8base + u * 8);      // (sx,sx) (sy,sy)
           const ulonglong2 sB = *reinterpret_cast<const ulonglong2 *>(s8base + u * 8 + 4);  // (sz,sz) (sw,sw)
@@ -369,9 +379,10 @@ __device__ __forceinline__ void sweep(const StreamArgs &a, const float4 *s_S4, c
             d0 = sqrt_approx(fabsf(d0));   // |.|: a slightly negative d2' (cancellation) stays inside the margin
             d1 = sqrt_approx(fabsf(d1));
             if (HAS_FD) {
-              const unsigned w = (p == 0) ? q[u].x : (p == 1) ? q[u].y : (p == 2) ? q[u].z : q[u].w;
-              cd[2 * p] = fhfma((unsigned short)(w & 0xffffu), bh, d0);
-              cd[2 * p + 1] = fhfma((unsigned short)(w >> 16), bh, d1);
+              float f0, f1;
+              fd_pair<HB>(p < 2 ? lo[u].x : lo[u].y, hw, u, p, f0, f1);
+              cd[2 * p] = fmaf(f0, b24, d0);
+              cd[2 * p + 1] = fmaf(f1, b24, d1);
             } else {
               cd[2 * p] = d0;
               cd[2 * p + 1] = d1;
@@ -388,15 +399,18 @@ __device__ __forceinline__ void sweep(const StreamArgs &a, const float4 *s_S4, c
               if (j0 + c < a.M) { psum += cd[c]; psq = fmaf(cd[c], cd[c], psq); }
           }
         } else {
+        float fdf[ST_CPL];
+        if (HAS_FD) {
+#pragma unroll
+          for (int p = 0; p < ST_CPL / 2; ++p) fd_pair<HB>(p < 2 ? lo[u].x : lo[u].y, hw, u, p, fdf[2 * p], fdf[2 * p + 1]);
+        }
 #pragma unroll
         for (int c = 0; c < ST_CPL; ++c) {
           float d2 = fmaf(S.x, Tx[c], fmaf(S.y, Ty[c], fmaf(S.z, Tz[c], Tw[c] + S.w)));
           d2 = fmaxf(d2, 0.f);
           const float dist = sqrt_approx(d2);
           if (HAS_FD) {
-            const unsigned w = (c < 2) ? q[u].x : (c < 4) ? q[u].y : (c < 6) ? q[u].z : q[u].w;
-            const float fdf = (c & 1) ? half_hi(w) : half_lo(w);
-            cd[c] = fmaf(b, fdf, dist);
+            cd[c] = fmaf(fdf[c], b24, dist);
           } else {
             cd[c] = dist;
           }
@@ -538,13 +552,12 @@ __device__ __forceinline__ void sweep(const StreamArgs &a, const float4 *s_S4, c
         }
       }
     }
-    if (HAS_FD && TMA) {
-      // every lane has consumed its values: hand the stage back to the TMA engine for batch k + ST_STAGES
-      const int k = rb / ST_UNROLL;
+    if (HAS_FD && (kb % ST_QPS == ST_QPS - 1 || kb == nbatch - 1)) {
+      // every lane has consumed the stage's values: hand it back to the TMA engine for stage kst + STAGES
       __syncwarp();
-      if (lane == 0 && k + ST_STAGES < nbatch) {
+      if (lane == 0 && kst + STAGES < nstage) {
         fence_proxy_async();
-        issue(k + ST_STAGES);
+        issue(kst + STAGES);
       }
     }
     if (STATS) {
@@ -566,15 +579,16 @@ __device__ __forceinline__ void sweep(const StreamArgs &a, const float4 *s_S4, c
   }
 }
 
-template <int MODE, bool HAS_FD, bool STATS, bool TMA, bool X2>
-__global__ void __launch_bounds__(ST_THREADS, (TMA && !X2) ? 3 : GHICP_ST_MINB) k_stream(const StreamArgs a) {
+// two CTAs per SM: the FD variants are held there by their 2 x 96 KB rings anyway, and a tighter bound only costs spills
+template <int MODE, bool HAS_FD, bool STATS, int HB, bool X2>
+__global__ void __launch_bounds__(ST_THREADS, GHICP_ST_MINB) k_stream(const StreamArgs a) {
   __shared__ __align__(16) float s_S8[X2 ? ST_RB * 8 : 8];
 #if defined(GHICP_EMU_HOST)
   unsigned char *s_ring = reinterpret_cast<unsigned char *>(emu::dyn_smem());   // host emulation: the launch's dynamic shared memory
 #else
-  extern __shared__ __align__(128) unsigned char s_ring[];   // [ST_WARPS][ST_RING_BYTES] when TMA
+  extern __shared__ __align__(128) unsigned char s_ring[];   // [ST_WARPS][ST_RING_BYTES] when HAS_FD
 #endif
-  __shared__ __align__(8) unsigned long long s_bar[ST_WARPS][ST_STAGES];
+  __shared__ __align__(8) unsigned long long s_bar[ST_WARPS][ST_MAX_STAGES];
   __shared__ float4 s_S4[ST_RB];
   __shared__ unsigned s_thr[ST_RB];
   __shared__ int s_cnt[ST_RB];
@@ -582,20 +596,21 @@ __global__ void __launch_bounds__(ST_THREADS, (TMA && !X2) ? 3 : GHICP_ST_MINB) 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int r0 = a.row0 + blockIdx.y * a.rb;
   const int nrows = min(a.rb, a.row0 + a.nloc - r0);
-  if (TMA && HAS_FD) {
+  if (HAS_FD) {
     // start the FD stream first: the operand staging below overlaps with the first bulk copies in flight
+    constexpr int STAGES = st_stages<HB>(), STAGE_BYTES = st_stage_bytes<HB>(), QUAD_BYTES = st_quad_bytes<HB>();
     const int panel0 = blockIdx.x * ST_CTA_COLS + warp * ST_PANEL;
     if (lane == 0) {
-      for (int st = 0; st < ST_STAGES; ++st) mbar_init(&s_bar[warp][st], 1);
+      for (int st = 0; st < STAGES; ++st) mbar_init(&s_bar[warp][st], 1);
       fence_mbarrier_init();
       if (panel0 < a.M) {
-        const unsigned short *pb = a.fd + fd_index(a.fd_rows, r0 - a.row0, panel0);
+        const unsigned char *pb = a.fd + fd_block_offset(a.fd_rows, HB, r0 - a.row0, panel0);
         const int nbatch = (nrows + ST_UNROLL - 1) / ST_UNROLL;
-        for (int k = 0; k < min(ST_STAGES, nbatch); ++k) {
-          const int rows = min(ST_UNROLL, nrows - k * ST_UNROLL);
-          mbar_expect_tx(&s_bar[warp][k], (unsigned)rows * ST_SEG_BYTES);
-          bulk_g2s(s_ring + warp * ST_RING_BYTES + k * ST_STAGE_BYTES, pb + (size_t)(k * ST_UNROLL) * FD_PANEL,
-                   (unsigned)rows * ST_SEG_BYTES, &s_bar[warp][k]);
+        const int nstage = (nbatch + ST_QPS - 1) / ST_QPS;
+        for (int st = 0; st < min(STAGES, nstage); ++st) {
+          const unsigned bytes = (unsigned)(min(ST_QPS, nbatch - st * ST_QPS) * QUAD_BYTES);
+          mbar_expect_tx(&s_bar[warp][st], bytes);
+          bulk_g2s(s_ring + warp * ST_RING_BYTES + st * STAGE_BYTES, pb + (size_t)st * STAGE_BYTES, bytes, &s_bar[warp][st]);
         }
       }
     }
@@ -612,15 +627,15 @@ __global__ void __launch_bounds__(ST_THREADS, (TMA && !X2) ? 3 : GHICP_ST_MINB) 
     s_cnt[r] = 0;
   }
   __syncthreads();
-  unsigned char *ring = TMA ? s_ring + warp * ST_RING_BYTES : nullptr;
+  unsigned char *ring = HAS_FD ? s_ring + warp * ST_RING_BYTES : nullptr;
   const int panel = blockIdx.x * ST_CTA_COLS + warp * ST_PANEL;
   const int j0 = panel + lane * ST_CPL;
   double dsum = 0.0, dsq = 0.0;
   if (panel < a.M) {
     if (panel + ST_PANEL <= a.M)
-      sweep<MODE, HAS_FD, STATS, true, TMA, X2>(a, s_S4, s_S8, s_thr, s_cnt, r0, nrows, j0, lane, dsum, dsq, ring, s_bar[warp]);
+      sweep<MODE, HAS_FD, STATS, true, HB, X2>(a, s_S4, s_S8, s_thr, s_cnt, r0, nrows, j0, lane, dsum, dsq, ring, s_bar[warp]);
     else
-      sweep<MODE, HAS_FD, STATS, false, TMA, X2>(a, s_S4, s_S8, s_thr, s_cnt, r0, nrows, j0, lane, dsum, dsq, ring, s_bar[warp]);
+      sweep<MODE, HAS_FD, STATS, false, HB, X2>(a, s_S4, s_S8, s_thr, s_cnt, r0, nrows, j0, lane, dsum, dsq, ring, s_bar[warp]);
   }
   if (STATS) {
 #pragma unroll
@@ -668,7 +683,7 @@ __global__ void k_publish(const StreamArgs a, double *row_cd, int *row_idx, doub
     row_cd[k] = __longlong_as_double((long long)a.rowbest[k]);
     const int j = a.rowidx[k];
     row_idx[k] = j;
-    a.row_fd[k] = (a.fd && j >= 0 && j < a.M) ? __half2float(__ushort_as_half(a.fd[fd_index(a.fd_rows, k - a.row0, j)])) : 0.f;
+    a.row_fd[k] = (a.fd && j >= 0 && j < a.M) ? (float)fd_at(a.fd, a.fd_rows, a.fd_hb, k - a.row0, j) : 0.f;
   }
   if (col_cd && k < a.M) {
     col_cd[k] = __longlong_as_double((long long)a.colbest[k]);
@@ -713,7 +728,7 @@ __global__ void __launch_bounds__(256) k_csr_check(const StreamArgs a, const Dev
     for (long long k = b + lane; k < e; k += 32) {
       const int j = a.csr_col[k];
       const double cd = exact_cd(a, i, j);
-      a.csr_fd[k] = a.fd ? __half2float(__ushort_as_half(a.fd[fd_index(a.fd_rows, i - a.row0, j)])) : 0.f;
+      a.csr_fd[k] = a.fd ? (float)fd_at(a.fd, a.fd_rows, a.fd_hb, i - a.row0, j) : 0.f;
       if (cd < penalty) { csr_gain[k] = penalty - cd; ++valid; }
       else csr_gain[k] = -1e300;
     }
@@ -761,7 +776,7 @@ __global__ void __launch_bounds__(256) k_emit_check(const StreamArgs a, const De
     const double cd = exact_cd(a, i, j);
     xkey[k] = e;
     xgain[k] = cd < penalty ? penalty - cd : -1e300;   // src/ghicp_reg.cpp:362-363 (strict <)
-    xfd[k] = a.fd ? __half2float(__ushort_as_half(a.fd[fd_index(a.fd_rows, i - a.row0, j)])) : 0.f;
+    xfd[k] = a.fd ? (float)fd_at(a.fd, a.fd_rows, a.fd_hb, i - a.row0, j) : 0.f;
   }
 }
 __device__ __forceinline__ const XBlockHdr *xblock_hdr(const unsigned char *blocks, size_t block_bytes, int r) {
@@ -812,14 +827,14 @@ __global__ void k_xscatter(const unsigned char *__restrict__ blocks, size_t bloc
 static int stream_rows_per_cta(const Ctx *c);
 static StreamArgs make_args(Ctx *c, const CostParams &cp) {
   StreamArgs a{};
-  a.fd = (c->cfg.feature_type == GHICP_FT_BSC) ? c->d_fd16 : nullptr;
-  a.fd_rows = c->fd_rows; a.N = c->N; a.M = c->M;
+  a.fd = (c->cfg.feature_type == GHICP_FT_BSC) ? reinterpret_cast<const unsigned char *>(c->d_fd16) : nullptr;
+  a.fd_rows = c->fd_rows; a.fd_hb = fd_hb(c->bits); a.N = c->N; a.M = c->M;
   a.row0 = c->r0; a.nloc = c->nloc; a.rb = stream_rows_per_cta(c);
   a.row_fd = c->d_row_fd; a.csr_fd = c->d_csr_fd;
   a.S4 = reinterpret_cast<const float4 *>(c->d_S4); a.T4 = reinterpret_cast<const float4 *>(c->d_T4);
   a.s = c->d_s; a.t = c->d_t;
   a.scale = cp.scale; a.WED = cp.WED; a.WFD = cp.WFD;
-  a.b = c->b_eff; a.bh = c->bh_bits; a.kappa = c->kappa;
+  a.b = c->b_eff; a.kappa = c->kappa;
   a.dev = c->d_sdev;
   a.row_thr_init = c->d_row_thr; a.rowbest = c->d_rowbest; a.rowidx = c->d_rowidx2;
   a.col_thr_init = nullptr; a.colbest = c->d_colbest; a.colidx = c->d_colidx2;
@@ -873,18 +888,16 @@ static int stream_num_parts_now(const Ctx *c) {
 cudaError_t launch_stream_prep(Ctx *c, const CostParams &cp, int for_km_gate) {
   const bool bsc = c->cfg.feature_type == GHICP_FT_BSC;
   // The filter works in a domain scaled by kappa = half(WFD)/WFD (|kappa - 1| <= 2^-11) so that the feature
-  // weight is exactly representable in fp16 and cd32 = FHFMA(fd, w_h, dist): argmin and threshold tests are
+  // weight is exactly representable in fp16 and cd32 = fmaf(fd, w_h, dist): argmin and threshold tests are
   // invariant under the positive scaling; sums are scaled back in k_finalize_fast.
   double kappa = 1.0;
   c->x2_ok = true;
-  c->bh_bits = 0;
   c->b_eff = 0.f;
   if (bsc) {
     const __half wh = __float2half_rn((float)cp.WFD);
     const float whf = __half2float(wh);
     if (cp.WFD >= 6.2e-5 && whf > 0.f) {
       kappa = (double)whf / cp.WFD;
-      c->bh_bits = __half_as_ushort(wh);
       c->b_eff = whf;
     } else {           // weight below the fp16 normal range: scalar FFMA path with the float weight
       c->x2_ok = false;
@@ -933,24 +946,31 @@ cudaError_t launch_stream(Ctx *c, const CostParams &cp, int mode, bool stats) {
   if (mode == SM_NNR || mode == SM_PRE_COLS) a.col_thr_init = c->d_col_thr;
   const dim3 grid = stream_grid(c);
   const bool fd = a.fd != nullptr;
-  static const bool use_tma = getenv("GHICP_STREAM_LDG") == nullptr;
 #if defined(GHICP_EMU_HOST)
 #define GHICP_STREAM_OPT_IN_SMEM(kernel) (void)0
 #else
 #define GHICP_STREAM_OPT_IN_SMEM(kernel) cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ST_DYN_SMEM)
 #endif
+#define LAUNCH_FD(MODE, ST, HB)                                                                                \
+  do {                                                                                                         \
+    if (c->x2_ok) {                                                                                            \
+      GHICP_STREAM_OPT_IN_SMEM((k_stream<MODE, true, ST, HB, true>));                                          \
+      GHICP_LAUNCH((k_stream<MODE, true, ST, HB, true>), grid, ST_THREADS, ST_DYN_SMEM, c->stream, a);         \
+    } else {                                                                                                   \
+      GHICP_STREAM_OPT_IN_SMEM((k_stream<MODE, true, ST, HB, false>));                                         \
+      GHICP_LAUNCH((k_stream<MODE, true, ST, HB, false>), grid, ST_THREADS, ST_DYN_SMEM, c->stream, a);        \
+    }                                                                                                          \
+  } while (0)
 #define LAUNCH(MODE, FD, ST)                                                                                   \
   do {                                                                                                         \
-    if (FD && use_tma && c->x2_ok) {                                                                           \
-      GHICP_STREAM_OPT_IN_SMEM((k_stream<MODE, FD, ST, true, true>));                                             \
-      GHICP_LAUNCH((k_stream<MODE, FD, ST, true, true>), grid, ST_THREADS, ST_DYN_SMEM, c->stream, a);                    \
-    } else if (FD && use_tma) {                                                                                \
-      GHICP_STREAM_OPT_IN_SMEM((k_stream<MODE, FD, ST, true, false>));                                            \
-      GHICP_LAUNCH((k_stream<MODE, FD, ST, true, false>), grid, ST_THREADS, ST_DYN_SMEM, c->stream, a);                   \
+    if (FD) {                                                                                                  \
+      if (a.fd_hb == 1) LAUNCH_FD(MODE, ST, 1);                                                                \
+      else if (a.fd_hb == 2) LAUNCH_FD(MODE, ST, 2);                                                           \
+      else LAUNCH_FD(MODE, ST, 4);                                                                             \
     } else if (c->x2_ok) {                                                                                     \
-      GHICP_LAUNCH((k_stream<MODE, FD, ST, false, true>), grid, ST_THREADS, 0, c->stream, a);                             \
+      GHICP_LAUNCH((k_stream<MODE, false, ST, 1, true>), grid, ST_THREADS, 0, c->stream, a);                   \
     } else {                                                                                                   \
-      GHICP_LAUNCH((k_stream<MODE, FD, ST, false, false>), grid, ST_THREADS, 0, c->stream, a);                            \
+      GHICP_LAUNCH((k_stream<MODE, false, ST, 1, false>), grid, ST_THREADS, 0, c->stream, a);                  \
     }                                                                                                          \
   } while (0)
 #define PICK(MODE)                                      \
@@ -970,6 +990,7 @@ cudaError_t launch_stream(Ctx *c, const CostParams &cp, int mode, bool stats) {
   }
 #undef PICK
 #undef LAUNCH
+#undef LAUNCH_FD
   c->launches++;
   return cudaGetLastError();
 }

@@ -1,6 +1,6 @@
 #!/bin/bash
 # A/B builds of libghicp_b200.so with other compile-time tuning knobs of the streaming kernel (ghicp_stream.cu:
-# GHICP_ST_UNROLL rows per batch, GHICP_ST_STAGES ring depth, GHICP_ST_MINB resident CTAs per SM).  Output:
+# GHICP_ST_RING_KB ring bytes per warp, GHICP_ST_MINB resident CTAs per SM; the batch is the plane's 4-row quad).  Output:
 # gh-icp_b200/variants/lib_<name>.so (git-ignored; select with GHICP_B200_LIB=<path> python bench.py ...).
 set -e
 cd "$(dirname "$0")/../gh-icp_b200/csrc"
