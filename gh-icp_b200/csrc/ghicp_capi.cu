@@ -24,8 +24,6 @@ void set_error(Ctx *c, const std::string &msg) {
   g_last_error = msg;
 }
 
-cudaError_t launch_solve_explicit(cudaStream_t stream, const double *d_s, const double *d_t, int n, DevIter *d_iter);
-
 #define CK(c, call)                                                                          \
   do {                                                                                       \
     cudaError_t e__ = (call);                                                                \
@@ -127,9 +125,27 @@ static void reset_loop_state(Ctx *c) {
   c->converge = false;
   c->last_mean = 0.0;
   for (int i = 0; i < 16; ++i) c->Rt_tillnow[i] = (i % 5 == 0) ? 1.0 : 0.0;
+  c->RouteHistory::reset();
 }
 
-static int ensure_edges(Ctx *c, long long nnz);
+static int ensure_edges(Ctx *c, long long nnz) {
+  const size_t need = (size_t)std::max<long long>(nnz, 1);
+  int rc;
+  if (need > c->csr_cap) {
+    size_t cap = need + need / 8 + 1024;
+    if ((rc = dev_alloc(c, &c->d_csr_col, cap))) return rc;
+    if ((rc = dev_alloc(c, &c->d_csr_gain, cap))) return rc;
+    if ((rc = dev_alloc(c, &c->d_csr_fd, cap))) return rc;
+    c->csr_cap = cap;
+  }
+  if (need > c->csc_cap) {
+    size_t cap = need + need / 8 + 1024;
+    if ((rc = dev_alloc(c, &c->d_csc_row, cap))) return rc;
+    if ((rc = dev_alloc(c, &c->d_csc_gain, cap))) return rc;
+    c->csc_cap = cap;
+  }
+  return GHICP_OK;
+}
 
 // workspaces that depend on (N, M)
 static int alloc_workspaces(Ctx *c) {
@@ -229,22 +245,17 @@ static int alloc_workspaces(Ctx *c) {
   return GHICP_OK;
 }
 
-static int ensure_edges(Ctx *c, long long nnz) {
-  const size_t need = (size_t)std::max<long long>(nnz, 1);
+// New keypoint counts: workspaces of the new size; descriptors, FD plane, normals, loop state and route history start over
+static int resize_keypoints(Ctx *c, int N, int M) {
+  if (N == c->N && M == c->M) return GHICP_OK;
+  c->N = N; c->M = M;
   int rc;
-  if (need > c->csr_cap) {
-    size_t cap = need + need / 8 + 1024;
-    if ((rc = dev_alloc(c, &c->d_csr_col, cap))) return rc;
-    if ((rc = dev_alloc(c, &c->d_csr_gain, cap))) return rc;
-    if ((rc = dev_alloc(c, &c->d_csr_fd, cap))) return rc;
-    c->csr_cap = cap;
+  if ((rc = dev_alloc(c, &c->d_s, 3 * (size_t)N)) || (rc = dev_alloc(c, &c->d_t, 3 * (size_t)M)) || (rc = alloc_workspaces(c))) {
+    c->N = c->M = 0;   // half-sized workspaces must not pass for a configured context: every later call answers "keypoints not set"
+    return rc;
   }
-  if (need > c->csc_cap) {
-    size_t cap = need + need / 8 + 1024;
-    if ((rc = dev_alloc(c, &c->d_csc_row, cap))) return rc;
-    if ((rc = dev_alloc(c, &c->d_csc_gain, cap))) return rc;
-    c->csc_cap = cap;
-  }
+  c->have_bsc = c->have_fpfh = c->fd_built = c->have_normals = false;
+  reset_loop_state(c);
   return GHICP_OK;
 }
 
@@ -260,27 +271,19 @@ static int build_fd(Ctx *c) {
     int rc = dev_alloc(c, &c->d_fd16, (plane_bytes + 1) / 2);
     if (rc) return rc;
     CK(c, cudaMemsetAsync(c->d_fd16, 0, plane_bytes, c->stream));  // zero the quad / panel padding
-    {
-      // tensor-core build (wgmma s8) when the descriptor fits its shared-memory tiling, else POPC
-      cudaError_t e = (getenv("GHICP_FD_POPC") != nullptr) ? cudaErrorNotSupported : launch_fd_bsc_tc(c);
-      if (e == cudaErrorNotSupported) { cudaGetLastError(); CK(c, launch_fd_bsc(c)); c->fd_tensor = false; }
-      else { CK(c, e); c->fd_tensor = true; }
-    }
+    // tensor-core build (wgmma s8) when the descriptor fits its shared-memory tiling, else POPC
+    cudaError_t e = (getenv("GHICP_FD_POPC") != nullptr) ? cudaErrorNotSupported : launch_fd_bsc_tc(c);
+    if (e == cudaErrorNotSupported) { cudaGetLastError(); CK(c, launch_fd_bsc(c)); }
+    else CK(c, e);
   } else if (c->cfg.feature_type == GHICP_FT_FPFH) {
     if (!c->have_fpfh) { set_error(c, "build_fd: FPFH descriptors not set"); return GHICP_E_ARG; }
     c->fd_rows = (size_t)std::max(c->nloc, 1);
-    // Stored float plane (4*N*M bytes) or matrix-free (ghicp_fpfh.cu: FD recomputed inside the sweeps, O(N+M) memory).
-    // Both give bit-identical FD / CD values; auto mode stores the plane only while it is a modest share of the HBM.
+    // Stored float plane (4*N*M bytes, fpfh_matrix_free = -1) or matrix-free (ghicp_fpfh.cu: FD recomputed inside the sweeps,
+    // O(N+M) memory).  Both give bit-identical FD / CD values.  Auto (0) is matrix-free for every correspondence mode: NN / NNR
+    // sweeps then run the FP32-filter fast path, several times faster than the all-double kernels with the same
+    // correspondences; KM runs the exact sweeps in iterations 0-1 and the filter's gate after.
     const size_t plane_bytes = fd_elems(c->fd_rows, c->M) * sizeof(float);
-    // auto: NN / NNR always go matrix-free (their sweeps then run the FP32-filter fast path, several times faster than the
-    // all-double kernels, same correspondences); KM keeps the plane while it is a modest share of the HBM.
-    bool mf = c->cfg.fpfh_matrix_free > 0 || getenv("GHICP_FPFH_MATRIX_FREE") != nullptr;
-    if (!mf && c->cfg.fpfh_matrix_free == 0) {
-      size_t free_b = 0, total_b = 0;
-      CK(c, cudaMemGetInfo(&free_b, &total_b));
-      (void)free_b; (void)total_b;
-      mf = true;   // auto = matrix-free for every correspondence mode (KM: exact sweeps in iterations 0-1, the filter's gate after)
-    }
+    const bool mf = c->cfg.fpfh_matrix_free >= 0 || getenv("GHICP_FPFH_MATRIX_FREE") != nullptr;
     c->fpfh_mf = mf;
     int rc;
     if (mf) {
@@ -290,20 +293,18 @@ static int build_fd(Ctx *c) {
       if ((rc = dev_alloc(c, &c->d_ftc, (size_t)c->M * 36))) return rc;
       if ((rc = dev_alloc(c, &c->d_ftcT, (size_t)c->M * 36))) return rc;
       CK(c, launch_fpfh_prepare(c));
-      // operands of the FP32 filter (fast NN / NNR path); KM keeps the exact sweeps
+      // operands of the FP32 filter (NN / NNR filter route, the KM gate of the settled route)
       c->fpfh_fast_ready = false;
-      {
-        if ((rc = dev_alloc(c, &c->d_ff_srec, (size_t)c->N * fpfh_fast_rec_floats()))) return rc;
-        if ((rc = dev_alloc(c, &c->d_ff_tnT, (size_t)c->M * 36))) return rc;
-        if ((rc = dev_alloc(c, &c->d_ff_tco, (size_t)c->M * 6))) return rc;
-        if ((rc = dev_alloc(c, &c->d_ff_part, fpfh_fast_parts(c)))) return rc;
-        if ((rc = dev_alloc(c, &c->d_ff_rowguess, (size_t)c->Npad))) return rc;
-        if ((rc = dev_alloc(c, &c->d_ff_colguess, (size_t)c->M))) return rc;
-        CK(c, cudaMemsetAsync(c->d_ff_rowguess, 0xff, sizeof(unsigned long long) * (size_t)c->Npad, c->stream));
-        CK(c, cudaMemsetAsync(c->d_ff_colguess, 0xff, sizeof(unsigned long long) * (size_t)c->M, c->stream));
-        CK(c, launch_fpfh_fast_build(c));
-        c->fpfh_fast_ready = true;
-      }
+      if ((rc = dev_alloc(c, &c->d_ff_srec, (size_t)c->N * fpfh_fast_rec_floats()))) return rc;
+      if ((rc = dev_alloc(c, &c->d_ff_tnT, (size_t)c->M * 36))) return rc;
+      if ((rc = dev_alloc(c, &c->d_ff_tco, (size_t)c->M * 6))) return rc;
+      if ((rc = dev_alloc(c, &c->d_ff_part, fpfh_fast_parts(c)))) return rc;
+      if ((rc = dev_alloc(c, &c->d_ff_rowguess, (size_t)c->Npad))) return rc;
+      if ((rc = dev_alloc(c, &c->d_ff_colguess, (size_t)c->M))) return rc;
+      CK(c, cudaMemsetAsync(c->d_ff_rowguess, 0xff, sizeof(unsigned long long) * (size_t)c->Npad, c->stream));
+      CK(c, cudaMemsetAsync(c->d_ff_colguess, 0xff, sizeof(unsigned long long) * (size_t)c->M, c->stream));
+      CK(c, launch_fpfh_fast_build(c));
+      c->fpfh_fast_ready = true;
     } else {
       if ((rc = dev_alloc(c, &c->d_fdf, fd_elems(c->fd_rows, c->M)))) return rc;
       CK(c, cudaMemsetAsync(c->d_fdf, 0, plane_bytes, c->stream));
@@ -334,7 +335,8 @@ static LoopScalars make_loop_scalars(const Ctx *c, const CostParams &cp) {
 }
 
 // Candidate edges a rank's block carries this iteration: twice the largest per-rank share of the last one (same on every
-// rank).  GHICP_KM_XUSE_MAX caps it (test hook: forces the overflow -> general-route fallback).
+// rank; the latency-bound all-gather carries what the graph needs, not what the buffers could hold).  GHICP_KM_XUSE_MAX caps
+// it (test hook: forces the overflow -> general-route fallback).
 static size_t settled_block_size(const Ctx *c) {
   size_t x = std::min(c->xcap, ((size_t)std::max<long long>(1024, 2 * c->last_max_local_nnz + 256) + 3) & ~(size_t)3);
   if (const char *ov = getenv("GHICP_KM_XUSE_MAX")) {
@@ -344,309 +346,284 @@ static size_t settled_block_size(const Ctx *c) {
   return x;
 }
 
-static int iterate_impl(Ctx *c, ghicp_iter_stats *out) {
-  if (c->N <= 0 || c->M <= 0) { set_error(c, "iterate: keypoints not set"); return GHICP_E_ARG; }
-  if (c->cfg.solver == GHICP_SOLVER_POINT_TO_PLANE && !c->have_normals) {
-    set_error(c, "iterate: GHICP_SOLVER_POINT_TO_PLANE needs ghicp_set_target_normals");
-    return GHICP_E_ARG;
-  }
-  int rc;
-  if ((rc = build_fd(c))) return rc;
-  c->launches = 0;
-  cudaStream_t st = c->stream;
-  const CostParams cp = make_cost_params(c);
-  const LoopScalars ls = make_loop_scalars(c, cp);
-  KmResult kres;
-  long long nnz = 0;
+// How one iteration computes its costs and correspondences (DESIGN.md §7).  Every route ends in the same solve and host tail.
+enum class Route {
+  FpfhFilter,       // FPFH, matrix-free: FP32 filter over on-the-fly FD + exact refinement (NN / NNR)
+  Stream,           // BSC or no feature: streaming filter pass + exact refinement (NN / NNR)
+  FpfhKmSettled,    // FPFH + KM, settled loop: the FP32 filter as the KM gate
+  StreamKmSettled,  // BSC + KM, settled loop: one streaming pass, one all-gather, no host round trip
+  StreamKmGeneral,  // BSC / no feature + KM: [statistics pass] + count pass [+ fill pass], CSR cuts read by the host
+  Exact,            // all-double kernels
+};
 
-  CK(c, cudaEventRecord(c->ev[0], st));
+static Route choose_route(const Ctx *c) {
   const int ft = c->cfg.feature_type, ct = c->cfg.corr_type;
-  const bool fast = c->use_fast && (ft == GHICP_FT_NONE || ft == GHICP_FT_BSC);
-  // FPFH: FP32 filter over on-the-fly feature distances + exact refinement (ghicp_fpfh.cu).  Taken when no decision
-  // depends on the CD mean, which a filter cannot reproduce in FPFH mode (heavy-tailed ED / FD^ex): NNR has no gate,
-  // NN's penalty is RMS*para1*scale*para2 from iteration 2 on (src/ghicp_reg.cpp:327-330).
-  const bool fpfh_fast = c->use_fast && ft == GHICP_FT_FPFH && c->fpfh_mf && c->fpfh_fast_ready && ct != GHICP_CT_KM &&
-                         (ct == GHICP_CT_NNR || c->iteration >= 2) && getenv("GHICP_FPFH_EXACT") == nullptr;
+  const bool stream = c->use_fast && (ft == GHICP_FT_NONE || ft == GHICP_FT_BSC);
+  const bool fpfh_filter = c->use_fast && ft == GHICP_FT_FPFH && c->fpfh_mf && c->fpfh_fast_ready &&
+                           getenv("GHICP_FPFH_EXACT") == nullptr;
+  if (ct != GHICP_CT_KM) {
+    // FPFH: the filter is taken when no decision depends on the CD mean, which a filter cannot reproduce in FPFH mode
+    // (heavy-tailed ED / FD^ex): NNR has no gate, NN's penalty is RMS*para1*scale*para2 from iteration 2 on
+    // (src/ghicp_reg.cpp:327-330).
+    if (fpfh_filter && (ct == GHICP_CT_NNR || c->iteration >= 2)) return Route::FpfhFilter;
+    return stream ? Route::Stream : Route::Exact;
+  }
   // Settled KM iteration?  Decided from quantities every rank holds identically (both routes contain collectives).
-  const long long nmax_km = std::max(c->N, c->M);
-  const bool km_sparse_history = ct == GHICP_CT_KM && c->iteration >= 2 && !c->km_settled_off && c->xcap > 0 &&
-                                 c->last_total_nnz >= 0 && (double)c->last_total_nnz <= 1.5 * (double)nmax_km &&
-                                 c->last_max_local_nnz >= 0 &&
-                                 (size_t)c->last_max_local_nnz + (size_t)c->last_max_local_nnz / 2 + 64 <= c->xcap &&
-                                 getenv("GHICP_KM_GENERAL") == nullptr && getenv("GHICP_KM_FILL") == nullptr;   // test hooks: general route
-  const bool km_settled = fast && ft != GHICP_FT_NONE && km_sparse_history;
+  const RouteHistory &h = *c;
+  const long long nmax = std::max(c->N, c->M);
+  const bool sparse_history = c->iteration >= 2 && !h.km_settled_off && c->xcap > 0 && h.last_total_nnz >= 0 &&
+                              (double)h.last_total_nnz <= 1.5 * (double)nmax && h.last_max_local_nnz >= 0 &&
+                              (size_t)h.last_max_local_nnz + (size_t)h.last_max_local_nnz / 2 + 64 <= c->xcap &&
+                              getenv("GHICP_KM_GENERAL") == nullptr && getenv("GHICP_KM_FILL") == nullptr;   // test hooks: general route
   // FPFH + KM, settled loop: the FP32 filter as the KM gate (penalty = RMS*para1*scale*para2 from iteration 2 on)
-  const bool fpfh_km_fast = c->use_fast && ft == GHICP_FT_FPFH && c->fpfh_mf && c->fpfh_fast_ready && c->d_cand[0] &&
-                            km_sparse_history && getenv("GHICP_FPFH_EXACT") == nullptr;
-  const bool settled_any = km_settled || fpfh_km_fast;
-  bool exact_fallback = !fast && !fpfh_fast && !fpfh_km_fast;
-  bool ev1_done = false, timed_stream = false;
-  int stream_passes = 0;
-  const bool sharded = c->world > 1;
-  if (fpfh_fast) {
-    const bool cols = (ct == GHICP_CT_NNR);
-    // guesses for the thresholds: last iteration's partners once the loop has settled, else an FP32 argmin pre-pass
-    const long long cand_budget = 6ll * ((long long)c->nloc + (cols ? c->M : 0));
-    const bool prepass = !c->have_prev || c->iteration <= 2 || c->last_cands > cand_budget;
-    CK(c, launch_fpfh_fast_prep(c));
-    if (prepass) { CK(c, launch_fpfh_fast_sweep(c, cp, true, cols)); ++stream_passes; }
-    CK(c, launch_fpfh_fast_seed(c, cp, cols, prepass));
-    CK(c, cudaEventRecord(c->ev[4], st));
-    CK(c, launch_fpfh_fast_sweep(c, cp, false, cols));
-    CK(c, cudaEventRecord(c->ev[5], st));
-    ++stream_passes; timed_stream = true;
-    CK(c, launch_fpfh_fast_finish(c, cp, cols));
-    CK(c, launch_rowfd_mf(c));
-    if ((rc = comm_exchange(c, 1 | 2 | (cols ? 4 : 0)))) return rc;
-    CK(c, launch_penalty(c, 0.0, ls));
-    if (cols && sharded) CK(c, launch_colmerge(c));
-    CK(c, cudaEventRecord(c->ev[1], st));
-    ev1_done = true;
-    if (cols) CK(c, launch_select_nnr(c));
-    else CK(c, launch_select_nn(c, 0.0));
-    CK(c, cudaMemcpyAsync(c->h_sdev, c->d_sdev, sizeof(StreamDev), cudaMemcpyDeviceToHost, st));
-    CK(c, cudaMemcpyAsync(c->h_iter, c->d_iter, sizeof(DevIter), cudaMemcpyDeviceToHost, st));
-    CK(c, cudaStreamSynchronize(st));
-    c->last_cands = (long long)c->h_sdev->cand_count[0] + (cols ? c->h_sdev->cand_count[1] : 0);
-    if (c->h_iter->overflow_any) exact_fallback = true;   // candidate buffer overflow (on any rank): exact sweeps
-    else c->have_prev = true;
-    c->fallbacks += exact_fallback ? 1 : 0;
-  } else if (fast && ct != GHICP_CT_KM) {
-    // ---- streaming path, NN / NNR: one pass = calED + calCD + row (and column) scans + statistics
-    const bool cols = (ct == GHICP_CT_NNR);
-    // a seed pass (FP32 minima only) keeps the refinement cheap whenever last iteration's partners are not
-    // a tight bound: the first iterations (the metric mix changes fastest) or when many candidates were seen
-    const long long cand_budget = 6ll * ((long long)c->nloc + (cols ? c->M : 0));
-    const bool prepass = !c->have_prev || c->iteration <= 2 || c->last_cands > cand_budget;
-    CK(c, launch_stream_prep(c, cp, 0));
-    CK(c, launch_stream_seed(c, cp, cols));
-    if (prepass) { CK(c, launch_stream(c, cp, cols ? 5 : 4, true)); ++stream_passes; }
-    CK(c, cudaEventRecord(c->ev[4], st));
-    CK(c, launch_stream(c, cp, cols ? 1 : 0, !prepass));
-    CK(c, cudaEventRecord(c->ev[5], st));
-    ++stream_passes; timed_stream = true;
-    CK(c, launch_finalize_fast(c, ls));
-    CK(c, launch_stream_resolve(c, cp, cols));
-    if ((rc = comm_exchange(c, 1 | 2 | (cols ? 4 : 0)))) return rc;   // the single exchange of the iteration
-    CK(c, launch_penalty(c, 0.0, ls));
-    if (cols && sharded) CK(c, launch_colmerge(c));
-    CK(c, cudaEventRecord(c->ev[1], st));
-    ev1_done = true;
-    // the NN gate depends on this iteration's statistics only for Ft=None and for BSC iterations 0-1
-    const bool stats_dependent = (ft == GHICP_FT_NONE) || (c->iteration <= 1);
-    if (cols) CK(c, launch_select_nnr(c));
-    else CK(c, launch_select_nn(c, stats_dependent ? 1e-5 : 0.0));
-    CK(c, cudaMemcpyAsync(c->h_sdev, c->d_sdev, sizeof(StreamDev), cudaMemcpyDeviceToHost, st));
-    CK(c, cudaMemcpyAsync(c->h_iter, c->d_iter, sizeof(DevIter), cudaMemcpyDeviceToHost, st));
-    CK(c, cudaStreamSynchronize(st));
-    // candidate buffer overflow (on any rank), or an NN gate decision inside the error band of the fast
-    // statistics: redo this iteration's cost stage with the all-double kernels (rare)
-    c->last_cands = (long long)c->h_sdev->cand_count[0] + (cols ? c->h_sdev->cand_count[1] : 0);
-    if (c->h_iter->overflow_any || (!cols && c->h_iter->ambiguous > 0)) exact_fallback = true;
-    else c->have_prev = true;
-    c->fallbacks += exact_fallback ? 1 : 0;
-  } else if (fpfh_km_fast) {
-    // ---- FPFH + KM, settled loop: one filter sweep with every row's threshold at the penalty; the exactly evaluated hits with
-    //      CD < penalty are the KM graph and travel as this rank's candidate block (the settled route below, same tail)
-    c->xuse = settled_block_size(c);
-    CK(c, launch_fpfh_fast_prep(c));
-    CK(c, launch_fpfh_gate_seed(c, cp, ls));
-    CK(c, cudaEventRecord(c->ev[4], st));
-    CK(c, launch_fpfh_fast_sweep(c, cp, false, false));
-    CK(c, cudaEventRecord(c->ev[5], st));
-    CK(c, launch_fpfh_cand_block(c, cp));
-    if ((rc = comm_allgather_bytes(c, c->d_xsend, c->d_xrecv, xblock_bytes(c->xuse)))) return rc;
-    CK(c, launch_xbuild(c));
-    CK(c, launch_penalty(c, 0.0, ls));        // CD mean (the filter's estimate) + the overflow flag; same penalty
-    CK(c, cudaEventRecord(c->ev[1], st));
-    stream_passes += 1; timed_stream = true; ev1_done = true;
-    if ((rc = km_auction_settled(c, c->N, c->M, c->last_total_nnz, c->KM_eps))) return rc;
-    CK(c, launch_select_km(c));
-    CK(c, launch_pair_fd_km(c));
-    CK(c, cudaMemcpyAsync(c->h_sdev, c->d_sdev, sizeof(StreamDev), cudaMemcpyDeviceToHost, st));
-    CK(c, cudaMemcpyAsync(c->h_xcounts, c->d_xcounts, sizeof(unsigned long long) * (size_t)c->world, cudaMemcpyDeviceToHost, st));
-    nnz = -1;
-  } else if (fast && km_settled) {
-    // ---- streaming path, KM, settled loop (sparse candidate graph, penalty independent of this iteration's CD):
-    //      one pass over the FD plane, the gate hits checked exactly where they were found, ONE all-gather of the
-    //      per-rank candidate blocks (none on one GPU), CSR / CSC / single-phase auction / selection enqueued behind it.
-    //      The host reads nothing until the iteration's final synchronize; a block overflow (flag travels with the
-    //      statistics, k_apply then leaves the keypoints alone) sends the iteration through the general route below.
-    c->emit_on = true;
-    // message size of this iteration: twice the largest per-rank share of the last one (the latency-bound all-gather carries
-    // what the graph needs, not what the buffers could hold); an overflow redoes the iteration on the general route
-    c->xuse = settled_block_size(c);
-    CK(c, launch_stream_prep(c, cp, 0));
-    CK(c, cudaMemsetAsync(c->d_cnt, 0, sizeof(int) * ((size_t)c->Npad + 2), st));
-    CK(c, launch_penalty_only(c, ls));        // src/ghicp_reg.cpp:279-282: independent of this iteration's CD
-    CK(c, launch_stream_gate(c, cp));
-    CK(c, cudaEventRecord(c->ev[4], st));
-    CK(c, launch_stream(c, cp, 2, true));
-    CK(c, cudaEventRecord(c->ev[5], st));
-    CK(c, launch_finalize_fast(c, ls));
-    CK(c, launch_emit_check(c, cp));
-    if ((rc = comm_allgather_bytes(c, c->d_xsend, c->d_xrecv, xblock_bytes(c->xuse)))) return rc;   // the iteration's one exchange
-    CK(c, launch_xbuild(c));
-    CK(c, launch_penalty(c, 0.0, ls));        // CD mean / std of all ranks' sums (+ the overflow flag)
-    CK(c, cudaEventRecord(c->ev[1], st));
-    stream_passes += 1; timed_stream = true; ev1_done = true;
-    if ((rc = km_auction_settled(c, c->N, c->M, c->last_total_nnz, c->KM_eps))) return rc;
-    CK(c, launch_select_km(c));
-    CK(c, launch_pair_fd_km(c));
-    CK(c, cudaMemcpyAsync(c->h_sdev, c->d_sdev, sizeof(StreamDev), cudaMemcpyDeviceToHost, st));
-    CK(c, cudaMemcpyAsync(c->h_xcounts, c->d_xcounts, sizeof(unsigned long long) * (size_t)c->world, cudaMemcpyDeviceToHost, st));
-    nnz = -1;  // filled from h_sdev after the final synchronize
-  } else if (fast) {
-    // ---- streaming path, KM: [statistics pass] + count pass + fill pass over the FD plane
-    const bool stats_first = (ft == GHICP_FT_NONE) || (c->iteration <= 1);
-    // the edge list pays off on sparse candidate graphs; on a dense one (first iterations) its single append
-    // counter would serialise millions of hits, so it is switched on from last iteration's count
-    c->emit_on = c->last_local_nnz >= 0 && (size_t)c->last_local_nnz + (size_t)c->last_local_nnz / 2 <= c->emit_cap;
-    CK(c, launch_stream_prep(c, cp, 0));
-    CK(c, cudaMemsetAsync(c->d_cnt, 0, sizeof(int) * ((size_t)c->Npad + 2), st));
-    if (stats_first) {
-      CK(c, cudaEventRecord(c->ev[4], st));
-      CK(c, launch_stream(c, cp, 2, true));   // gate disabled (thr = -1): statistics only
-      CK(c, cudaEventRecord(c->ev[5], st));
-      CK(c, launch_finalize_fast(c, ls));
-      if ((rc = comm_exchange(c, 1))) return rc;
-      CK(c, launch_penalty(c, 0.0, ls));
-      CK(c, launch_stream_gate(c, cp));
-      CK(c, cudaEventRecord(c->ev[1], st));
-      CK(c, launch_stream(c, cp, 2, false));
-      stream_passes += 2;
-    } else {
-      CK(c, launch_penalty_only(c, ls));      // src/ghicp_reg.cpp:279-282: independent of this iteration's CD
-      CK(c, launch_stream_gate(c, cp));
-      CK(c, cudaEventRecord(c->ev[4], st));
-      CK(c, launch_stream(c, cp, 2, true));
-      CK(c, cudaEventRecord(c->ev[5], st));
-      CK(c, launch_finalize_fast(c, ls));
-      if ((rc = comm_exchange(c, 1))) return rc;
-      CK(c, launch_penalty(c, 0.0, ls));
-      CK(c, cudaEventRecord(c->ev[1], st));
-      stream_passes += 1;
-    }
-    timed_stream = true;
-    ev1_done = true;
-    if ((rc = comm_gather_counts(c))) return rc;
-    CK(c, launch_scan_rows(c));
-    CK(c, cudaMemcpyAsync(c->h_iter, c->d_iter, sizeof(DevIter), cudaMemcpyDeviceToHost, st));
-    CK(c, cudaMemcpyAsync(c->h_sdev, c->d_sdev, sizeof(StreamDev), cudaMemcpyDeviceToHost, st));
-    if (sharded)
-      for (int r = 0; r <= c->world; ++r)
-        CK(c, cudaMemcpyAsync(&c->h_rowptr_cut[r], c->d_rowptr + std::min(c->N, r * c->shard), sizeof(long long),
-                              cudaMemcpyDeviceToHost, st));
-    CK(c, cudaStreamSynchronize(st));
-    const long long nnz_super = c->h_iter->nnz;
-    const double penalty = c->h_iter->penalty;
-    if ((rc = ensure_edges(c, nnz_super))) return rc;
-    if (nnz_super == 0) c->last_local_nnz = c->last_max_local_nnz = 0;
-    c->last_total_nnz = nnz_super;
-    c->km_settled_off = false;
-    if (nnz_super > 0) {
-      // this rank's gate hits were appended to the edge list by the count pass (when the list was on and did
-      // not overflow): scatter them; otherwise stream the plane a second time (fill pass)
-      const long long local_nnz = sharded ? c->h_rowptr_cut[c->rank + 1] - c->h_rowptr_cut[c->rank] : nnz_super;
-      const unsigned long long emitted = c->h_sdev->emit_count;
-      const bool force_fill = getenv("GHICP_KM_FILL") != nullptr;  // test hook: always take the fill pass
-      if (c->emit_on && emitted <= (unsigned long long)c->emit_cap && !force_fill) {
-        if (emitted > 0) CK(c, launch_emit_scatter(c, cp, emitted));
-      } else {
-        ++stream_passes;
-        CK(c, launch_stream(c, cp, 3, false));
-      }
-      c->last_local_nnz = local_nnz;
-      c->last_max_local_nnz = local_nnz;
-      if (sharded)
-        for (int r = 0; r < c->world; ++r)
-          c->last_max_local_nnz = std::max(c->last_max_local_nnz, c->h_rowptr_cut[r + 1] - c->h_rowptr_cut[r]);
-      CK(c, launch_csr_check(c, cp));
-      if (sharded) {
-        if ((rc = comm_gather_edges(c, c->h_rowptr_cut))) return rc;
-        CK(c, launch_count_valid(c, nnz_super));
-      }
-    }
-    if ((rc = km_auction(c, c->N, c->M, nnz_super, c->KM_eps, std::max(penalty, c->KM_eps), &kres))) return rc;
-    CK(c, launch_select_km(c));
-    CK(c, launch_pair_fd_km(c));
-    CK(c, cudaMemcpyAsync(c->h_sdev, c->d_sdev, sizeof(StreamDev), cudaMemcpyDeviceToHost, st));
-    nnz = -1;  // filled from h_sdev after the final synchronize
-  }
-  if (exact_fallback) {
-    // ---- all-double path (FPFH; forced; or fallback): calED + calCD_* (+ the row scan of NN / NNR)
-    const bool mf = (ft == GHICP_FT_FPFH) && c->fpfh_mf;   // matrix-free FPFH: FD recomputed inside the sweeps
-    CK(c, mf ? launch_rowsweep_mf(c, 0, cp) : launch_rowsweep(c, 0, cp));
-    CK(c, launch_finalize_stats(c, cp, ls));
-    if (mf) CK(c, launch_rowfd_mf(c));
-    if (ct == GHICP_CT_NNR) CK(c, mf ? launch_colsweep_mf(c, cp) : launch_colsweep(c, cp));
-    if ((rc = comm_exchange(c, 1 | 2 | (ct == GHICP_CT_NNR ? 4 : 0)))) return rc;
-    CK(c, launch_penalty(c, cp.pivot, ls));
-    if (ct == GHICP_CT_NNR && sharded) CK(c, launch_colmerge(c));
-    if (!ev1_done) CK(c, cudaEventRecord(c->ev[1], st));
-    if (ct == GHICP_CT_NN) {
-      CK(c, launch_select_nn(c));
-    } else if (ct == GHICP_CT_NNR) {
-      CK(c, launch_select_nnr(c));
-    } else {
-      // sharded: every rank counts, fills and checks the candidates of ITS rows with the all-double kernels; counts and
-      // edges travel like on the streaming path's general route (all-gather of the counts, one broadcast group of the edges)
-      if (sharded) CK(c, cudaMemsetAsync(c->d_cnt, 0, sizeof(int) * ((size_t)c->Npad + 2), st));
-      CK(c, mf ? launch_rowsweep_mf(c, 1, cp) : launch_rowsweep(c, 1, cp));
-      if (sharded && (rc = comm_gather_counts(c))) return rc;
-      CK(c, launch_scan_counts(c));
-      CK(c, cudaMemcpyAsync(c->h_iter, c->d_iter, sizeof(DevIter), cudaMemcpyDeviceToHost, st));
-      if (sharded)
-        for (int r = 0; r <= c->world; ++r)
-          CK(c, cudaMemcpyAsync(&c->h_rowptr_cut[r], c->d_rowptr + std::min(c->N, r * c->shard), sizeof(long long),
-                                cudaMemcpyDeviceToHost, st));
-      CK(c, cudaStreamSynchronize(st));
-      nnz = c->h_iter->nnz;
-      const double penalty = c->h_iter->penalty;
-      if ((rc = ensure_edges(c, nnz))) return rc;
-      if (nnz > 0) CK(c, mf ? launch_rowsweep_mf(c, 2, cp) : launch_rowsweep(c, 2, cp));
-      if (sharded && nnz > 0 && (rc = comm_gather_edges(c, c->h_rowptr_cut))) return rc;
-      c->last_total_nnz = nnz;
-      c->last_max_local_nnz = nnz;
-      if (sharded) {
-        c->last_max_local_nnz = 0;
-        for (int r = 0; r < c->world; ++r)
-          c->last_max_local_nnz = std::max(c->last_max_local_nnz, c->h_rowptr_cut[r + 1] - c->h_rowptr_cut[r]);
-      }
-      c->km_settled_off = false;
-      if ((rc = km_auction(c, c->N, c->M, nnz, c->KM_eps, std::max(penalty, c->KM_eps), &kres))) return rc;
-      CK(c, launch_select_km(c));
-      CK(c, launch_pair_fd_km(c));
-    }
-    if (ct != GHICP_CT_KM) c->have_prev = true;
-  }
-  CK(c, cudaEventRecord(c->ev[2], st));
-  // transformestimation (numeric core) + update of all source keypoints
-  CK(c, launch_solve(c, cp));
-  // opt-in estimators replace the transform (and the RMSE after it); the pair statistics stay k_solve's
-  if (c->cfg.solver != GHICP_SOLVER_SVD) CK(c, launch_solve_alt(c, c->cfg.solver));
-  CK(c, launch_apply(c, settled_any));
-  CK(c, cudaEventRecord(c->ev[3], st));
-  CK(c, cudaMemcpyAsync(c->h_iter, c->d_iter, sizeof(DevIter), cudaMemcpyDeviceToHost, st));
-  CK(c, cudaStreamSynchronize(st));
-  if (settled_any) {
-    if (c->h_iter->overflow_any) {   // some rank's candidate block overflowed: nothing was updated, take the general route
-      c->km_settled_off = true;
-      c->km_redone = true;
-      const int rc_redo = iterate_impl(c, out);
-      c->km_redone = false;
-      return rc_redo;
-    }
-    if ((rc = km_auction_settled_result(c, &kres))) return rc;
-    c->last_total_nnz = c->h_iter->nnz;
-    c->last_local_nnz = (long long)c->h_xcounts[c->rank];
-    c->last_max_local_nnz = 0;
-    for (int r = 0; r < c->world; ++r) c->last_max_local_nnz = std::max(c->last_max_local_nnz, (long long)c->h_xcounts[r]);
-    c->settled_iterations++;
-  }
-  if (nnz < 0) nnz = (long long)c->h_sdev->nnz_valid;
+  if (fpfh_filter && c->d_cand[0] && sparse_history) return Route::FpfhKmSettled;
+  if (!stream) return Route::Exact;
+  return (ft != GHICP_FT_NONE && sparse_history) ? Route::StreamKmSettled : Route::StreamKmGeneral;
+}
 
-  // ---- host tail (scalars only) -----------------------------------------------------------
+// What a route hands to the solve and the host tail.
+struct RouteResult {
+  long long nnz = 0;          // KM candidate edges (-1: the device's count, read after the final synchronize)
+  KmResult kres;
+  int stream_passes = 0;      // > 0: ev[4] / ev[5] were recorded around the route's main streaming pass
+  long long candidates = 0;   // NN / NNR filter routes: candidates the filter passed to exact evaluation
+  bool exact_redo = false;    // a filter route asks for the all-double redo of its cost stage (which then skips ev[1])
+};
+
+// Seed pre-pass (FP32 minima only) before an NN / NNR filter pass?  It keeps the refinement cheap whenever last iteration's
+// partners are not a tight bound: the first iterations (the metric mix changes fastest) or after many candidates.
+static bool want_prepass(const Ctx *c, bool cols) {
+  const long long cand_budget = 6ll * ((long long)c->nloc + (cols ? c->M : 0));
+  return !c->have_prev || c->iteration <= 2 || c->last_cands > cand_budget;
+}
+
+// Tail of the NN / NNR filter routes: exchange, penalty, selection, read-back.  A candidate buffer overflow (on any rank), or
+// an NN gate decision inside the error band of the fast statistics (amb_rel > 0), asks for the all-double redo (rare).
+static int nn_tail(Ctx *c, const LoopScalars &ls, bool cols, double amb_rel, RouteResult *r) {
+  int rc;
+  if ((rc = comm_exchange(c, EX_STATS | EX_ROWS | (cols ? EX_COLS : 0)))) return rc;
+  CK(c, launch_penalty(c, 0.0, ls));
+  if (cols && c->world > 1) CK(c, launch_colmerge(c));
+  CK(c, cudaEventRecord(c->ev[1], c->stream));
+  CK(c, cols ? launch_select_nnr(c) : launch_select_nn(c, amb_rel));
+  CK(c, cudaMemcpyAsync(c->h_sdev, c->d_sdev, sizeof(StreamDev), cudaMemcpyDeviceToHost, c->stream));
+  CK(c, cudaMemcpyAsync(c->h_iter, c->d_iter, sizeof(DevIter), cudaMemcpyDeviceToHost, c->stream));
+  CK(c, cudaStreamSynchronize(c->stream));
+  r->candidates = c->last_cands = (long long)c->h_sdev->cand_count[0] + (cols ? c->h_sdev->cand_count[1] : 0);
+  r->exact_redo = c->h_iter->overflow_any || (!cols && c->h_iter->ambiguous > 0);
+  if (!r->exact_redo) c->have_prev = true;
+  return GHICP_OK;
+}
+
+static int route_fpfh_filter(Ctx *c, const CostParams &cp, const LoopScalars &ls, RouteResult *r) {
+  const bool cols = c->cfg.corr_type == GHICP_CT_NNR;
+  const bool prepass = want_prepass(c, cols);
+  CK(c, launch_fpfh_fast_prep(c));
+  if (prepass) { CK(c, launch_fpfh_fast_sweep(c, cp, true, cols)); ++r->stream_passes; }
+  CK(c, launch_fpfh_fast_seed(c, cp, cols, prepass));
+  CK(c, cudaEventRecord(c->ev[4], c->stream));
+  CK(c, launch_fpfh_fast_sweep(c, cp, false, cols));
+  CK(c, cudaEventRecord(c->ev[5], c->stream));
+  ++r->stream_passes;
+  CK(c, launch_fpfh_fast_finish(c, cp, cols));
+  CK(c, launch_rowfd_mf(c));
+  return nn_tail(c, ls, cols, 0.0, r);
+}
+
+// one pass = calED + calCD + row (and column) scans + statistics
+static int route_stream(Ctx *c, const CostParams &cp, const LoopScalars &ls, RouteResult *r) {
+  const bool cols = c->cfg.corr_type == GHICP_CT_NNR;
+  const bool prepass = want_prepass(c, cols);
+  CK(c, launch_stream_prep(c, cp, 0));
+  CK(c, launch_stream_seed(c, cp, cols));
+  if (prepass) { CK(c, launch_stream(c, cp, cols ? SM_PRE_COLS : SM_PRE, true)); ++r->stream_passes; }
+  CK(c, cudaEventRecord(c->ev[4], c->stream));
+  CK(c, launch_stream(c, cp, cols ? SM_NNR : SM_NN, !prepass));
+  CK(c, cudaEventRecord(c->ev[5], c->stream));
+  ++r->stream_passes;
+  CK(c, launch_finalize_fast(c));
+  CK(c, launch_stream_resolve(c, cp, cols));
+  // the NN gate depends on this iteration's statistics only for Ft=None and for BSC iterations 0-1
+  const bool stats_dependent = c->cfg.feature_type == GHICP_FT_NONE || c->iteration <= 1;
+  return nn_tail(c, ls, cols, stats_dependent ? 1e-5 : 0.0, r);
+}
+
+// Tail of the two settled KM routes: ONE all-gather of the per-rank candidate blocks (none on one GPU), then CSR / CSC,
+// statistics, single-phase auction and selection; the host reads nothing until the iteration's final synchronize.
+static int km_settled_tail(Ctx *c, const LoopScalars &ls, RouteResult *r) {
+  int rc;
+  if ((rc = comm_allgather_bytes(c, c->d_xsend, c->d_xrecv, xblock_bytes(c->xuse)))) return rc;   // the iteration's one exchange
+  CK(c, launch_xbuild(c));
+  CK(c, launch_penalty(c, 0.0, ls));        // CD mean / std of all ranks' sums (+ the overflow flag); same penalty
+  CK(c, cudaEventRecord(c->ev[1], c->stream));
+  r->stream_passes = 1;
+  if ((rc = km_auction_settled(c, c->N, c->M, c->last_total_nnz, c->KM_eps))) return rc;
+  CK(c, launch_select_km(c));
+  CK(c, launch_pair_fd_km(c));
+  CK(c, cudaMemcpyAsync(c->h_sdev, c->d_sdev, sizeof(StreamDev), cudaMemcpyDeviceToHost, c->stream));
+  CK(c, cudaMemcpyAsync(c->h_xcounts, c->d_xcounts, sizeof(unsigned long long) * (size_t)c->world, cudaMemcpyDeviceToHost, c->stream));
+  r->nnz = -1;  // filled from h_sdev after the final synchronize
+  return GHICP_OK;
+}
+
+// FPFH + KM, settled loop: one filter sweep with every row's threshold at the penalty; the exactly evaluated hits with
+// CD < penalty are the KM graph and travel as this rank's candidate block
+static int route_fpfh_km_settled(Ctx *c, const CostParams &cp, const LoopScalars &ls, RouteResult *r) {
+  c->xuse = settled_block_size(c);
+  CK(c, launch_fpfh_fast_prep(c));
+  CK(c, launch_fpfh_gate_seed(c, cp, ls));
+  CK(c, cudaEventRecord(c->ev[4], c->stream));
+  CK(c, launch_fpfh_fast_sweep(c, cp, false, false));
+  CK(c, cudaEventRecord(c->ev[5], c->stream));
+  CK(c, launch_fpfh_cand_block(c, cp));
+  return km_settled_tail(c, ls, r);
+}
+
+// BSC + KM, settled loop (sparse candidate graph, penalty independent of this iteration's CD): one pass over the FD plane,
+// the gate hits checked exactly where they were found.  A block overflow (the flag travels with the statistics, k_apply then
+// leaves the keypoints alone) sends the iteration through the general route.
+static int route_stream_km_settled(Ctx *c, const CostParams &cp, const LoopScalars &ls, RouteResult *r) {
+  c->emit_on = true;
+  c->xuse = settled_block_size(c);
+  CK(c, launch_stream_prep(c, cp, 0));
+  CK(c, cudaMemsetAsync(c->d_cnt, 0, sizeof(int) * ((size_t)c->Npad + 2), c->stream));
+  CK(c, launch_penalty_only(c, ls));        // src/ghicp_reg.cpp:279-282: independent of this iteration's CD
+  CK(c, launch_stream_gate(c, cp));
+  CK(c, cudaEventRecord(c->ev[4], c->stream));
+  CK(c, launch_stream(c, cp, SM_COUNT, true));
+  CK(c, cudaEventRecord(c->ev[5], c->stream));
+  CK(c, launch_finalize_fast(c));
+  CK(c, launch_emit_check(c, cp));
+  return km_settled_tail(c, ls, r);
+}
+
+// The KM graph's size and per-rank shares (share(k) = candidate edges of rank k), noted for the next route choice
+template <class Share>
+static void note_km_graph(Ctx *c, long long total, Share share) {
+  RouteHistory &h = *c;
+  h.last_total_nnz = total;
+  h.last_local_nnz = share(c->rank);
+  h.last_max_local_nnz = 0;
+  for (int k = 0; k < c->world; ++k) h.last_max_local_nnz = std::max(h.last_max_local_nnz, share(k));
+}
+
+// End of the general KM routes: read back the edge count and penalty (sharded: and the CSR offsets at the shard boundaries),
+// make room for the edges, fill(nnz) enqueues this rank's edges, note the graph's shares, auction, selection, pairs' FD.
+template <class Fill>
+static int km_general_tail(Ctx *c, RouteResult *r, Fill fill) {
+  CK(c, cudaMemcpyAsync(c->h_iter, c->d_iter, sizeof(DevIter), cudaMemcpyDeviceToHost, c->stream));
+  if (c->world > 1)
+    for (int k = 0; k <= c->world; ++k)
+      CK(c, cudaMemcpyAsync(c->h_rowptr_cut + k, c->d_rowptr + std::min(c->N, k * c->shard), sizeof(long long),
+                            cudaMemcpyDeviceToHost, c->stream));
+  CK(c, cudaStreamSynchronize(c->stream));
+  const long long nnz = c->h_iter->nnz;
+  const double penalty = c->h_iter->penalty;
+  int rc;
+  if ((rc = ensure_edges(c, nnz)) || (rc = fill(nnz))) return rc;
+  note_km_graph(c, nnz, [&](int k) { return c->world > 1 ? c->h_rowptr_cut[k + 1] - c->h_rowptr_cut[k] : nnz; });
+  c->km_settled_off = false;
+  if ((rc = km_auction(c, c->N, c->M, nnz, c->KM_eps, std::max(penalty, c->KM_eps), &r->kres))) return rc;
+  CK(c, launch_select_km(c));
+  CK(c, launch_pair_fd_km(c));
+  r->nnz = nnz;
+  return GHICP_OK;
+}
+
+// BSC / no feature + KM, general: [statistics pass] + count pass + [fill pass] over the FD plane
+static int route_stream_km_general(Ctx *c, const CostParams &cp, const LoopScalars &ls, RouteResult *r) {
+  int rc;
+  // the penalty needs this iteration's CD statistics for Ft=None and in iterations 0-1: a statistics pass with the gate off
+  // (thr = -1) comes first, then the count pass; otherwise the penalty is known and the first pass counts
+  const bool stats_first = c->cfg.feature_type == GHICP_FT_NONE || c->iteration <= 1;
+  // the edge list pays off on sparse candidate graphs; on a dense one (first iterations) its single append
+  // counter would serialise millions of hits, so it is switched on from last iteration's count
+  c->emit_on = c->last_local_nnz >= 0 && (size_t)c->last_local_nnz + (size_t)c->last_local_nnz / 2 <= c->emit_cap;
+  CK(c, launch_stream_prep(c, cp, 0));
+  CK(c, cudaMemsetAsync(c->d_cnt, 0, sizeof(int) * ((size_t)c->Npad + 2), c->stream));
+  if (!stats_first) {
+    CK(c, launch_penalty_only(c, ls));      // src/ghicp_reg.cpp:279-282: independent of this iteration's CD
+    CK(c, launch_stream_gate(c, cp));
+  }
+  CK(c, cudaEventRecord(c->ev[4], c->stream));
+  CK(c, launch_stream(c, cp, SM_COUNT, true));
+  CK(c, cudaEventRecord(c->ev[5], c->stream));
+  CK(c, launch_finalize_fast(c));
+  if ((rc = comm_exchange(c, EX_STATS))) return rc;
+  CK(c, launch_penalty(c, 0.0, ls));
+  if (stats_first) CK(c, launch_stream_gate(c, cp));
+  CK(c, cudaEventRecord(c->ev[1], c->stream));
+  if (stats_first) CK(c, launch_stream(c, cp, SM_COUNT, false));
+  r->stream_passes = stats_first ? 2 : 1;
+  if ((rc = comm_gather_counts(c))) return rc;
+  CK(c, launch_scan_rows(c));
+  CK(c, cudaMemcpyAsync(c->h_sdev, c->d_sdev, sizeof(StreamDev), cudaMemcpyDeviceToHost, c->stream));
+  rc = km_general_tail(c, r, [&](long long nnz) -> int {
+    if (nnz <= 0) return GHICP_OK;
+    // this rank's gate hits were appended to the edge list by the count pass (when the list was on and did
+    // not overflow): scatter them; otherwise stream the plane a second time (fill pass)
+    const unsigned long long emitted = c->h_sdev->emit_count;
+    const bool force_fill = getenv("GHICP_KM_FILL") != nullptr;  // test hook: always take the fill pass
+    if (c->emit_on && emitted <= (unsigned long long)c->emit_cap && !force_fill) {
+      if (emitted > 0) CK(c, launch_emit_scatter(c, cp, emitted));
+    } else {
+      ++r->stream_passes;
+      CK(c, launch_stream(c, cp, SM_FILL, false));
+    }
+    CK(c, launch_csr_check(c, cp));
+    if (c->world > 1) {
+      if ((rc = comm_gather_edges(c, c->h_rowptr_cut))) return rc;
+      CK(c, launch_count_valid(c, nnz));
+    }
+    return GHICP_OK;
+  });
+  if (rc) return rc;
+  CK(c, cudaMemcpyAsync(c->h_sdev, c->d_sdev, sizeof(StreamDev), cudaMemcpyDeviceToHost, c->stream));
+  r->nnz = -1;  // filled from h_sdev after the final synchronize
+  return GHICP_OK;
+}
+
+// Row stage of the all-double kernels: row minima and CD statistics (+ the partners' FD for matrix-free FPFH)
+static int exact_row_stage(Ctx *c, const CostParams &cp, const LoopScalars &ls) {
+  const bool mf = (c->cfg.feature_type == GHICP_FT_FPFH) && c->fpfh_mf;   // matrix-free FPFH: FD recomputed inside the sweeps
+  CK(c, mf ? launch_rowsweep_mf(c, SWEEP_ROWMIN, cp) : launch_rowsweep(c, SWEEP_ROWMIN, cp));
+  CK(c, launch_finalize_stats(c, cp, ls));
+  if (mf) CK(c, launch_rowfd_mf(c));
+  return GHICP_OK;
+}
+
+// All-double route (FPFH; forced; or the redo after a filter route): calED + calCD_* (+ the row scan of NN / NNR)
+static int route_exact(Ctx *c, const CostParams &cp, const LoopScalars &ls, RouteResult *r) {
+  const int ct = c->cfg.corr_type;
+  const bool mf = (c->cfg.feature_type == GHICP_FT_FPFH) && c->fpfh_mf;
+  const bool sharded = c->world > 1;
+  int rc;
+  if ((rc = exact_row_stage(c, cp, ls))) return rc;
+  if (ct == GHICP_CT_NNR) CK(c, mf ? launch_colsweep_mf(c, cp) : launch_colsweep(c, cp));
+  if ((rc = comm_exchange(c, EX_STATS | EX_ROWS | (ct == GHICP_CT_NNR ? EX_COLS : 0)))) return rc;
+  CK(c, launch_penalty(c, cp.pivot, ls));
+  if (ct == GHICP_CT_NNR && sharded) CK(c, launch_colmerge(c));
+  if (!r->exact_redo) CK(c, cudaEventRecord(c->ev[1], c->stream));
+  if (ct != GHICP_CT_KM) {
+    CK(c, ct == GHICP_CT_NN ? launch_select_nn(c) : launch_select_nnr(c));
+    c->have_prev = true;
+    return GHICP_OK;
+  }
+  // sharded: every rank counts, fills and checks the candidates of ITS rows with the all-double kernels; counts and
+  // edges travel like on the streaming path's general route (all-gather of the counts, one broadcast group of the edges)
+  if (sharded) CK(c, cudaMemsetAsync(c->d_cnt, 0, sizeof(int) * ((size_t)c->Npad + 2), c->stream));
+  CK(c, mf ? launch_rowsweep_mf(c, SWEEP_COUNT, cp) : launch_rowsweep(c, SWEEP_COUNT, cp));
+  if (sharded && (rc = comm_gather_counts(c))) return rc;
+  CK(c, launch_scan_counts(c));
+  return km_general_tail(c, r, [&](long long nnz) -> int {
+    if (nnz <= 0) return GHICP_OK;
+    CK(c, mf ? launch_rowsweep_mf(c, SWEEP_FILL, cp) : launch_rowsweep(c, SWEEP_FILL, cp));
+    return sharded ? comm_gather_edges(c, c->h_rowptr_cut) : GHICP_OK;
+  });
+}
+
+// Host tail of an iteration (scalars only): convergence, IoU, Euler angles, adjustweight, Rt_tillnow, statistics; warnings
+static int host_tail(Ctx *c, const RouteResult &r, bool redone, ghicp_iter_stats *out) {
   const DevIter &h = *c->h_iter;
   const int cor_number = h.cor;
   c->last_cor = cor_number;
@@ -704,20 +681,71 @@ static int iterate_impl(Ctx *c, ghicp_iter_stats *out) {
     const int n = std::max(c->N, c->M);
     out->km_energy = (c->cfg.corr_type == GHICP_CT_KM) ? h.km_cd_sum + (double)(n - cor_number) * h.penalty : 0.0;
     out->ax = ax; out->ay = ay; out->az = az;
-    out->nnz = nnz; out->km_rounds = kres.rounds; out->km_phases = kres.phases;
+    out->nnz = r.nnz; out->km_rounds = r.kres.rounds; out->km_phases = r.kres.phases;
     out->gpu_launches = c->launches;
-    out->exact_fallback = (((fast || fpfh_fast) && exact_fallback) ? 1 : 0) | (c->km_redone ? 2 : 0);
+    out->exact_fallback = (r.exact_redo ? 1 : 0) | (redone ? 2 : 0);
     float ms;
     cudaEventElapsedTime(&ms, c->ev[0], c->ev[1]); out->ms_cost = ms;
     cudaEventElapsedTime(&ms, c->ev[1], c->ev[2]); out->ms_corr = ms;
     cudaEventElapsedTime(&ms, c->ev[2], c->ev[3]); out->ms_solve = ms;
     cudaEventElapsedTime(&ms, c->ev[0], c->ev[3]); out->ms_total = ms;
-    if (timed_stream) { cudaEventElapsedTime(&ms, c->ev[4], c->ev[5]); out->ms_stream = ms; }
-    out->stream_passes = stream_passes;
-    out->candidates = ((fast || fpfh_fast) && ct != GHICP_CT_KM) ? c->last_cands : 0;
+    if (r.stream_passes > 0) { cudaEventElapsedTime(&ms, c->ev[4], c->ev[5]); out->ms_stream = ms; }
+    out->stream_passes = r.stream_passes;
+    out->candidates = r.candidates;
   }
   c->iteration++;
   return warnings;
+}
+
+static int iterate_impl(Ctx *c, ghicp_iter_stats *out) {
+  if (c->N <= 0 || c->M <= 0) { set_error(c, "iterate: keypoints not set"); return GHICP_E_ARG; }
+  if (c->cfg.solver == GHICP_SOLVER_POINT_TO_PLANE && !c->have_normals) {
+    set_error(c, "iterate: GHICP_SOLVER_POINT_TO_PLANE needs ghicp_set_target_normals");
+    return GHICP_E_ARG;
+  }
+  int rc;
+  if ((rc = build_fd(c))) return rc;
+  const CostParams cp = make_cost_params(c);
+  const LoopScalars ls = make_loop_scalars(c, cp);
+  RouteResult r;
+  bool redone = false;   // reported as bit 1 of ghicp_iter_stats.exact_fallback
+  for (;;) {
+    const Route route = choose_route(c);
+    const bool settled = route == Route::FpfhKmSettled || route == Route::StreamKmSettled;
+    r = RouteResult();
+    c->launches = 0;
+    CK(c, cudaEventRecord(c->ev[0], c->stream));
+    switch (route) {
+      case Route::FpfhFilter: rc = route_fpfh_filter(c, cp, ls, &r); break;
+      case Route::Stream: rc = route_stream(c, cp, ls, &r); break;
+      case Route::FpfhKmSettled: rc = route_fpfh_km_settled(c, cp, ls, &r); break;
+      case Route::StreamKmSettled: rc = route_stream_km_settled(c, cp, ls, &r); break;
+      case Route::StreamKmGeneral: rc = route_stream_km_general(c, cp, ls, &r); break;
+      case Route::Exact: rc = route_exact(c, cp, ls, &r); break;
+    }
+    if (rc == GHICP_OK && r.exact_redo) rc = route_exact(c, cp, ls, &r);
+    if (rc) return rc;
+    CK(c, cudaEventRecord(c->ev[2], c->stream));
+    // transformestimation (numeric core) + update of all source keypoints
+    CK(c, launch_solve(c, cp));
+    // opt-in estimators replace the transform (and the RMSE after it); the pair statistics stay k_solve's
+    if (c->cfg.solver != GHICP_SOLVER_SVD) CK(c, launch_solve_alt(c, c->cfg.solver));
+    CK(c, launch_apply(c, settled));
+    CK(c, cudaEventRecord(c->ev[3], c->stream));
+    CK(c, cudaMemcpyAsync(c->h_iter, c->d_iter, sizeof(DevIter), cudaMemcpyDeviceToHost, c->stream));
+    CK(c, cudaStreamSynchronize(c->stream));
+    if (!settled) break;
+    if (!c->h_iter->overflow_any) {
+      if ((rc = km_auction_settled_result(c, &r.kres))) return rc;
+      note_km_graph(c, c->h_iter->nnz, [&](int k) { return (long long)c->h_xcounts[k]; });
+      break;
+    }
+    // some rank's candidate block overflowed: nothing was updated; the iteration runs again on the general route
+    c->km_settled_off = true;
+    redone = true;
+  }
+  if (r.nnz < 0) r.nnz = (long long)c->h_sdev->nnz_valid;
+  return host_tail(c, r, redone, out);
 }
 
 }  // namespace ghicp_b200
@@ -793,20 +821,7 @@ int ghicp_set_keypoints(ghicp_ctx *ctx, const double *sxyz, int N, const double 
   if (!c || !sxyz || !txyz || N <= 0 || M <= 0) { set_error(c, "set_keypoints: bad argument"); return GHICP_E_ARG; }
   int rc;
   if ((rc = use_device(c))) return rc;
-  const bool resize = (N != c->N || M != c->M);
-  if (resize) {
-    c->N = N; c->M = M;
-    c->ldM = ((size_t)M + 63) / 64 * 64;
-    if ((rc = dev_alloc(c, &c->d_s, 3 * (size_t)N)) || (rc = dev_alloc(c, &c->d_t, 3 * (size_t)M)) || (rc = alloc_workspaces(c))) {
-      c->N = c->M = 0;   // half-sized workspaces must not pass for a configured context: every later call answers "keypoints not set"
-      return rc;
-    }
-    c->have_bsc = c->have_fpfh = c->fd_built = false;
-    c->have_normals = false;
-    c->have_prev = false;
-    c->last_local_nnz = -1; c->last_total_nnz = -1; c->last_max_local_nnz = -1; c->km_settled_off = false;
-    reset_loop_state(c);
-  }
+  if ((rc = resize_keypoints(c, N, M))) return rc;
   const size_t need = 3 * ((size_t)N + M) * sizeof(double);
   if (need > c->h_stage_cap) {
     if (c->h_stage) cudaFreeHost(c->h_stage);
@@ -1011,11 +1026,8 @@ int ghicp_probe_rowmin(ghicp_ctx *ctx, int *idx, double *cd, double *cd_mean, do
   if ((rc = build_fd(c))) return rc;
   const CostParams cp = make_cost_params(c);
   const LoopScalars ls = make_loop_scalars(c, cp);
-  const bool mf = c->cfg.feature_type == GHICP_FT_FPFH && c->fpfh_mf;
-  CK(c, mf ? launch_rowsweep_mf(c, 0, cp) : launch_rowsweep(c, 0, cp));
-  CK(c, launch_finalize_stats(c, cp, ls));
-  if (mf) CK(c, launch_rowfd_mf(c));
-  if ((rc = comm_exchange(c, 1 | 2))) return rc;
+  if ((rc = exact_row_stage(c, cp, ls))) return rc;
+  if ((rc = comm_exchange(c, EX_STATS | EX_ROWS))) return rc;
   CK(c, launch_penalty(c, cp.pivot, ls));
   CK(c, cudaMemcpyAsync(c->h_iter, c->d_iter, sizeof(DevIter), cudaMemcpyDeviceToHost, c->stream));
   CK(c, cudaStreamSynchronize(c->stream));
@@ -1039,9 +1051,6 @@ int ghicp_reset(ghicp_ctx *ctx) {
   Ctx *c = reinterpret_cast<Ctx *>(ctx);
   if (!c) return GHICP_E_ARG;
   reset_loop_state(c);
-  c->have_prev = false;
-  c->last_local_nnz = -1; c->last_total_nnz = -1; c->last_max_local_nnz = -1; c->km_settled_off = false;
-  c->last_cands = 0;
   c->last_cor = 0;
   return GHICP_OK;
 }
@@ -1063,7 +1072,7 @@ int ghicp_km_solve(int device, const double *W, int n, int sp, int tp, double ep
   int rc = ghicp_create(&cfg, &ctx);
   if (rc) return rc;
   Ctx *c = reinterpret_cast<Ctx *>(ctx);
-  c->N = sp; c->M = tp; c->ldM = ((size_t)tp + 63) / 64 * 64;
+  c->N = sp; c->M = tp;
   rc = alloc_workspaces(c);
   if (rc) { ghicp_destroy(ctx); return rc; }
   // candidate edges: weight != -penalty  (src/km.cpp:162), gain = penalty + w = penalty - CD
@@ -1387,19 +1396,7 @@ int ghicp_set_from_prep(ghicp_ctx *ctx, const ghicp_prep *src, const ghicp_prep 
   int rc;
   if ((rc = use_device(c))) return rc;
   const int N = src->n_kp, M = tgt->n_kp;
-  if (N != c->N || M != c->M) {
-    c->N = N; c->M = M;
-    c->ldM = ((size_t)M + 63) / 64 * 64;
-    if ((rc = dev_alloc(c, &c->d_s, 3 * (size_t)N)) || (rc = dev_alloc(c, &c->d_t, 3 * (size_t)M)) || (rc = alloc_workspaces(c))) {
-      c->N = c->M = 0;   // half-sized workspaces must not pass for a configured context: every later call answers "keypoints not set"
-      return rc;
-    }
-    c->have_bsc = c->have_fpfh = c->fd_built = false;
-    c->have_normals = false;
-    c->have_prev = false;
-    c->last_local_nnz = -1; c->last_total_nnz = -1; c->last_max_local_nnz = -1; c->km_settled_off = false;
-    reset_loop_state(c);
-  }
+  if ((rc = resize_keypoints(c, N, M))) return rc;
   CK(c, cudaMemcpyAsync(c->d_s, src->d_kp_xyz, 3 * (size_t)N * sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
   CK(c, cudaMemcpyAsync(c->d_t, tgt->d_kp_xyz, 3 * (size_t)M * sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
   {  // centre of the FP32 filter coordinates = target centroid (scalars only; the 24 M bytes read back are not re-uploaded)

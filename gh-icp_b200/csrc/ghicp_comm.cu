@@ -91,26 +91,25 @@ void comm_destroy(Ctx *c) {
 }
 
 // The per-iteration exchange of the NN / NNR paths (and the statistics of every path).
-// what: bit 0 = partial CD sums, bit 1 = row minima/partners/FD, bit 2 = column minima
+// what: EX_STATS = partial CD sums, EX_ROWS = row minima/partners/FD, EX_COLS = column minima
 int comm_exchange(Ctx *c, int what) {
   if (c->world == 1) return GHICP_OK;
   ncclComm_t comm = (ncclComm_t)c->nccl_comm;
   cudaStream_t st = c->stream;
   const size_t sh = (size_t)c->shard;
   NCK(c, g_nccl.GroupStart());
-  if (what & 1) NCK(c, g_nccl.AllGather(c->d_xstats + 4 * c->rank, c->d_xstats, 4, ncclDouble, comm, st));
-  if (what & 2) {
+  if (what & EX_STATS) NCK(c, g_nccl.AllGather(c->d_xstats + 4 * c->rank, c->d_xstats, 4, ncclDouble, comm, st));
+  if (what & EX_ROWS) {
     NCK(c, g_nccl.AllGather(c->d_row_cd + sh * c->rank, c->d_row_cd, sh, ncclDouble, comm, st));
     NCK(c, g_nccl.AllGather(c->d_row_idx + sh * c->rank, c->d_row_idx, sh, ncclInt32, comm, st));
     NCK(c, g_nccl.AllGather(c->d_row_fd + sh * c->rank, c->d_row_fd, sh, ncclFloat32, comm, st));
   }
-  if (what & 4) {
+  if (what & EX_COLS) {
     // this rank's partial column minima sit in d_col_cd / d_col_idx
     NCK(c, g_nccl.AllGather(c->d_col_cd, c->d_colg_cd, (size_t)c->M, ncclUint64, comm, st));
     NCK(c, g_nccl.AllGather(c->d_col_idx, c->d_colg_idx, (size_t)c->M, ncclInt32, comm, st));
   }
   NCK(c, g_nccl.GroupEnd());
-  c->exchanges++;
   return GHICP_OK;
 }
 
@@ -129,7 +128,6 @@ int comm_gather_counts(Ctx *c) {
   ncclComm_t comm = (ncclComm_t)c->nccl_comm;
   const size_t sh = (size_t)c->shard;
   NCK(c, g_nccl.AllGather(c->d_cnt + sh * c->rank, c->d_cnt, sh, ncclInt32, comm, c->stream));
-  c->exchanges++;
   return GHICP_OK;
 }
 
@@ -148,7 +146,6 @@ int comm_gather_edges(Ctx *c, const long long *cut) {
     NCK(c, g_nccl.Broadcast(c->d_csr_fd + off, c->d_csr_fd + off, cnt, ncclFloat32, r, comm, st));
   }
   NCK(c, g_nccl.GroupEnd());
-  c->exchanges++;
   return GHICP_OK;
 }
 
@@ -157,7 +154,6 @@ int comm_gather_edges(Ctx *c, const long long *cut) {
 int comm_allgather_bytes(Ctx *c, const void *send, void *recv, size_t bytes) {
   if (c->world == 1) return GHICP_OK;
   NCK(c, g_nccl.AllGather(send, recv, bytes, ncclInt8, (ncclComm_t)c->nccl_comm, c->stream));
-  c->exchanges++;
   return GHICP_OK;
 }
 

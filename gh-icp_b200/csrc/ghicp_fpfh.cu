@@ -701,9 +701,9 @@ cudaError_t launch_rowsweep_mf(Ctx *c, int mode, const CostParams &cp) {
   a.iter = c->d_iter; a.cnt = c->d_cnt; a.rowptr = c->d_rowptr; a.cursor = c->d_cursor;
   a.csr_col = c->d_csr_col; a.csr_gain = c->d_csr_gain; a.csr_fd = c->d_csr_fd;
   const dim3 grid((c->nloc + TR - 1) / TR, c->n_chunks);
-  if (mode == 0) GHICP_LAUNCH(k_rowsweep_mf<0>, grid, MF_THREADS, 0, c->stream, a);
-  else if (mode == 1) GHICP_LAUNCH(k_rowsweep_mf<1>, grid, MF_THREADS, 0, c->stream, a);
-  else GHICP_LAUNCH(k_rowsweep_mf<2>, grid, MF_THREADS, 0, c->stream, a);
+  if (mode == SWEEP_ROWMIN) GHICP_LAUNCH(k_rowsweep_mf<SWEEP_ROWMIN>, grid, MF_THREADS, 0, c->stream, a);
+  else if (mode == SWEEP_COUNT) GHICP_LAUNCH(k_rowsweep_mf<SWEEP_COUNT>, grid, MF_THREADS, 0, c->stream, a);
+  else GHICP_LAUNCH(k_rowsweep_mf<SWEEP_FILL>, grid, MF_THREADS, 0, c->stream, a);
   c->launches++;
   return cudaGetLastError();
 }

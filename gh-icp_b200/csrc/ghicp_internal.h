@@ -155,8 +155,20 @@ struct XBlockHdr {
   unsigned long long pad[3];  // 64 bytes: the arrays behind it stay 16-byte aligned
 };
 
+// What the choice of an iteration's route (ghicp_capi.cu: choose_route) remembers of earlier iterations; part of the
+// context (Ctx derives from it).  Reset when the keypoints change size and by ghicp_reset.
+struct RouteHistory {
+  bool have_prev = false;             // d_row_idx / d_col_idx hold last iteration's partners
+  long long last_cands = 0;           // candidates the filter passed to exact evaluation last iteration
+  long long last_local_nnz = -1;      // KM candidate edges in this context's rows last iteration (-1: no history)
+  long long last_total_nnz = -1;      // candidate edges of the whole graph last iteration (-1: no history)
+  long long last_max_local_nnz = -1;  // largest per-rank share of them
+  bool km_settled_off = false;        // the last settled attempt overflowed: take the general route once
+  void reset() { *this = RouteHistory(); }
+};
+
 // ---- the context ----------------------------------------------------------------------------------
-struct Ctx {
+struct Ctx : RouteHistory {
   ghicp_config cfg{};
   int device = 0;
   cudaStream_t stream = nullptr;
@@ -164,7 +176,6 @@ struct Ctx {
   std::string err;
 
   int N = 0, M = 0;
-  size_t ldM = 0;  // (legacy pitch, unused by the panel-major plane)
   size_t fd_rows = 0;  // rows of the FD plane held by this context
   // coordinates, SoA doubles
   double *d_s = nullptr;  // [3][N]
@@ -176,7 +187,7 @@ struct Ctx {
   uint16_t *d_fd16 = nullptr;  // packed FD plane, fd_plane_bytes(fd_rows, M, fd_hb(bits)) bytes (allocated in 16-bit units)
   // FPFH
   float *d_fs = nullptr, *d_ft = nullptr;  // raw [N][33], [M][33]
-  float *d_fdf = nullptr;                  // [N][ldM] float FD
+  float *d_fdf = nullptr;                  // stored float FD plane, panel-major (fd_index)
   // matrix-free FPFH (ghicp_fpfh.cu): centred histograms, row-major [n][36] and transposed [36][n]; no N x M array
   bool fpfh_mf = false;
   float *d_fsc = nullptr, *d_fscT = nullptr, *d_ftc = nullptr, *d_ftcT = nullptr;
@@ -190,10 +201,9 @@ struct Ctx {
   double *d_tn = nullptr;  // target normals [3][M]
   bool have_normals = false;
   bool have_bsc = false, have_fpfh = false, fd_built = false;
-  bool fd_tensor = false;  // FD plane built by the tensor-core (wgmma) kernel
 
   // per-iteration workspaces
-  int rows_per_cta = 8, n_chunks = 1;
+  int n_chunks = 1;
   double *d_part_cd = nullptr;   // [N][n_chunks]
   int *d_part_idx = nullptr;     // [N][n_chunks]
   double *d_part_stats = nullptr;  // [grid][2]
@@ -235,9 +245,6 @@ struct Ctx {
   bool x2_ok = true;         // column-pair FP32 variant usable this iteration (feature weight exact in fp16)
   double kappa = 1.0;
   float b_eff = 0.f;
-  long long last_cands = 0;  // candidates the filter passed to exact evaluation last iteration
-  int fallbacks = 0;         // iterations that fell back to the all-double cost kernels
-  bool have_prev = false;    // d_row_idx / d_col_idx hold last iteration's partners
   double center[3] = {0, 0, 0};
   float *d_S4 = nullptr, *d_T4 = nullptr;   // float4[N], float4[M]
   StreamDev *d_sdev = nullptr;
@@ -253,7 +260,6 @@ struct Ctx {
   unsigned long long *d_emit = nullptr;     // KM edge list of the count pass
   size_t emit_cap = 0;
   bool emit_on = false;                     // this iteration's count pass appends to the list
-  long long last_local_nnz = -1;            // gate hits in this context's rows last iteration (-1: no history)
 
   // host loop state (include/ghicp_reg.h:173-202)
   int iteration = 0;
@@ -279,31 +285,33 @@ struct Ctx {
   unsigned long long *d_colg_cd = nullptr;  // [world][M] gathered column minima (ordered-double bits)
   int *d_colg_idx = nullptr;                // [world][M]
   long long *h_rowptr_cut = nullptr;        // pinned [world + 1] CSR offsets at the shard boundaries
-  int exchanges = 0;
   // settled KM iteration: one candidate block per rank, one all-gather, no host round trip inside the iteration
   size_t xcap = 0;                          // candidate edges a block can carry (allocation)
   size_t xuse = 0;                          // ... and carries this iteration: 2 x last iteration's largest share (same on every rank)
   unsigned char *d_xsend = nullptr;         // this rank's block
   unsigned char *d_xrecv = nullptr;         // [world] blocks (world > 1)
-  long long last_total_nnz = -1;            // candidate edges of the whole graph last iteration (-1: no history)
-  long long last_max_local_nnz = -1;        // largest per-rank share of them
   unsigned long long *d_xcounts = nullptr;  // [world] edges per block (device)
   unsigned long long *h_xcounts = nullptr;  // pinned copy
-  bool km_settled_off = false;              // the last settled attempt overflowed: take the general route once
-  bool km_redone = false;                   // ... and this is that repeat (reported as bit 1 of ghicp_iter_stats.exact_fallback)
-  int settled_iterations = 0;
 };
 
 struct KmResult {
   int rounds = 0, phases = 0;
 };
 
+// ---- modes the orchestration passes to the launchers --------------------------------------------------
+// launch_stream (k_stream's MODE): NN / NNR filter pass, KM count / fill pass, FP32 seed pre-pass (rows / rows + columns)
+enum StreamMode { SM_NN = 0, SM_NNR = 1, SM_COUNT = 2, SM_FILL = 3, SM_PRE = 4, SM_PRE_COLS = 5 };
+// launch_rowsweep / launch_rowsweep_mf (mode, an int holding one of these): row minima + CD statistics, KM candidate count
+// (needs the penalty in d_iter), KM fill
+enum SweepMode { SWEEP_ROWMIN = 0, SWEEP_COUNT = 1, SWEEP_FILL = 2 };
+// comm_exchange: what the grouped all-gather carries (OR of the bits)
+enum ExchangeBits { EX_STATS = 1, EX_ROWS = 2, EX_COLS = 4 };
+
 // ---- launchers (ghicp_kernels.cu) ---------------------------------------------------------------
 cudaError_t launch_pack_bsc(Ctx *c, const uint8_t *d_raw_s, const uint8_t *d_raw_t);
 cudaError_t launch_fd_bsc(Ctx *c);
 cudaError_t launch_fd_bsc_tc(Ctx *c);  // wgmma path; cudaErrorNotSupported when the shape does not fit
 cudaError_t launch_fd_fpfh(Ctx *c);
-// mode: 0 rowmin+stats, 1 count (needs penalty in d_iter), 2 fill
 cudaError_t launch_rowsweep(Ctx *c, int mode, const CostParams &cp);
 cudaError_t launch_colsweep(Ctx *c, const CostParams &cp);
 cudaError_t launch_finalize_stats(Ctx *c, const CostParams &cp, const LoopScalars &ls);
@@ -376,9 +384,9 @@ cudaError_t prep_bounds(cudaStream_t st, const float *d_xyz, int n, float mn[3],
 cudaError_t launch_stream_prep(Ctx *c, const CostParams &cp, int for_km_gate);
 cudaError_t launch_stream_gate(Ctx *c, const CostParams &cp);
 cudaError_t launch_stream_seed(Ctx *c, const CostParams &cp, bool with_cols);
-cudaError_t launch_stream(Ctx *c, const CostParams &cp, int mode, bool stats);  // 0 NN, 1 NNR, 2 count, 3 fill
+cudaError_t launch_stream(Ctx *c, const CostParams &cp, StreamMode mode, bool stats);
 cudaError_t launch_stream_resolve(Ctx *c, const CostParams &cp, bool with_cols);
-cudaError_t launch_finalize_fast(Ctx *c, const LoopScalars &ls);
+cudaError_t launch_finalize_fast(Ctx *c);
 cudaError_t launch_penalty_only(Ctx *c, const LoopScalars &ls);
 cudaError_t launch_scan_rows(Ctx *c);
 cudaError_t launch_emit_scatter(Ctx *c, const CostParams &cp, unsigned long long n_emitted);
@@ -403,13 +411,12 @@ int comm_unique_id(void *id128);
 int comm_init(Ctx *c, const void *id128, int rank, int world);
 void comm_destroy(Ctx *c);
 int comm_warmup(Ctx *c);
-int comm_exchange(Ctx *c, int what);         // bit0 stats, bit1 rows, bit2 columns
+int comm_exchange(Ctx *c, int what);         // what: OR of ExchangeBits
 int comm_gather_counts(Ctx *c);
 int comm_gather_edges(Ctx *c, const long long *cut);
 int comm_allgather_bytes(Ctx *c, const void *send, void *recv, size_t bytes);   // the one exchange of a settled KM iteration
 
 // misc
-int ensure_capacity(Ctx *c, void **ptr, size_t *cap, size_t need_bytes);
 void set_error(Ctx *c, const std::string &msg);
 
 }  // namespace ghicp_b200

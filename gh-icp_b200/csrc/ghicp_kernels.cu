@@ -870,7 +870,8 @@ cudaError_t launch_rowsweep(Ctx *c, int mode, const CostParams &cp) {
   dim3 grid((c->nloc + TR - 1) / TR, c->n_chunks);
   cudaError_t e = dispatch_ft(c->cfg.feature_type, [&](auto ft) {
     constexpr int FT = decltype(ft)::value;
-    void (*kern)(const SweepArgs) = mode == 0 ? k_rowsweep<FT, 0> : (mode == 1 ? k_rowsweep<FT, 1> : k_rowsweep<FT, 2>);
+    void (*kern)(const SweepArgs) = mode == SWEEP_ROWMIN ? k_rowsweep<FT, SWEEP_ROWMIN>
+                                    : (mode == SWEEP_COUNT ? k_rowsweep<FT, SWEEP_COUNT> : k_rowsweep<FT, SWEEP_FILL>);
     GHICP_LAUNCH(kern, grid, SWEEP_THREADS, 0, c->stream, a);
     return cudaGetLastError();
   });

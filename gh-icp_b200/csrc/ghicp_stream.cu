@@ -98,8 +98,6 @@ __device__ __forceinline__ void bulk_g2s(void *dst, const void *src, unsigned by
 
 #endif
 
-enum { SM_NN = 0, SM_NNR = 1, SM_COUNT = 2, SM_FILL = 3, SM_PRE = 4, SM_PRE_COLS = 5 };
-
 // Column pairs travel as one 64-bit value (two floats); Hopper has no packed f32x2 arithmetic, so fma2 / add2 are two scalar
 // operations with one rounding each.
 typedef unsigned long long u64;
@@ -939,9 +937,8 @@ cudaError_t launch_stream_seed(Ctx *c, const CostParams &cp, bool with_cols) {
   return cudaGetLastError();
 }
 
-// mode: 0 NN, 1 NNR, 2 KM count, 3 KM fill, 4 seed pass (rows), 5 seed pass (rows + columns);
 // stats: accumulate sum / sumsq of CD
-cudaError_t launch_stream(Ctx *c, const CostParams &cp, int mode, bool stats) {
+cudaError_t launch_stream(Ctx *c, const CostParams &cp, StreamMode mode, bool stats) {
   StreamArgs a = make_args(c, cp);
   if (mode == SM_NNR || mode == SM_PRE_COLS) a.col_thr_init = c->d_col_thr;
   const dim3 grid = stream_grid(c);
@@ -1006,8 +1003,7 @@ cudaError_t launch_stream_resolve(Ctx *c, const CostParams &cp, bool with_cols) 
   return cudaGetLastError();
 }
 
-cudaError_t launch_finalize_fast(Ctx *c, const LoopScalars &ls) {
-  (void)ls;
+cudaError_t launch_finalize_fast(Ctx *c) {
   GHICP_LAUNCH(k_finalize_fast, 1, 1024, 0, c->stream, c->d_part_stats, stream_num_parts_now(c), c->d_xstats, c->rank, c->kappa);
   c->launches++;
   return cudaGetLastError();
