@@ -75,7 +75,7 @@ EXPORTS = ["ghicp_abi_version", "ghicp_device_count", "ghicp_last_error", "ghicp
            "ghicp_bsc_extract", "ghicp_bsc_default_pattern", "ghicp_comm_unique_id", "ghicp_comm_init",
            "ghicp_prep_run", "ghicp_prep_info", "ghicp_prep_get", "ghicp_prep_destroy", "ghicp_set_from_prep",
            "ghicp_host_alloc", "ghicp_host_free", "ghicp_fpfh_extract", "ghicp_prep_fpfh", "ghicp_prep_get_fpfh",
-           "ghicp_prep_fpfh_stats"]
+           "ghicp_prep_fpfh_stats", "ghicp_sac_ia", "ghicp_prep_sac_ia", "ghicp_set_initial_transform"]
 
 
 def lib():
@@ -130,12 +130,39 @@ def lib():
     L.ghicp_prep_fpfh.argtypes = [vp, C.c_int, fpp]
     L.ghicp_prep_get_fpfh.argtypes = [vp, fpp]
     L.ghicp_prep_fpfh_stats.argtypes = [vp, C.POINTER(C.c_longlong), ip, ip, fpp]
+    L.ghicp_sac_ia.argtypes = [C.c_int, fpp, fpp, C.c_int, fpp, fpp, C.c_int, C.POINTER(SacParams), C.POINTER(SacResult)]
+    L.ghicp_prep_sac_ia.argtypes = [vp, vp, C.POINTER(SacParams), C.POINTER(SacResult)]
+    L.ghicp_set_initial_transform.argtypes = [vp, dp]
     _lib = L
     return L
 
 
 def device_count():
     return lib().ghicp_device_count()
+
+
+class SacParams(C.Structure):
+    """ghicp_sac_params (include/ghicp_b200.h): SAC-IA, DESIGN.md §3.11."""
+    _fields_ = [("max_iterations", C.c_int), ("nr_samples", C.c_int), ("k_correspondences", C.c_int),
+                ("min_sample_distance", C.c_float), ("corr_dist_threshold", C.c_float), ("reserved", C.c_int),
+                ("seed", C.c_ulonglong)]
+
+
+class SacResult(C.Structure):
+    _fields_ = [("Rt", C.c_double * 16), ("error", C.c_double), ("fitness", C.c_double), ("inliers", C.c_int),
+                ("best_hypothesis", C.c_int), ("invalid_hypotheses", C.c_int), ("reserved", C.c_int), ("stage_ms", C.c_float * 4)]
+
+
+def _sac_params(iterations, samples, k, min_sample_distance, threshold, seed):
+    return SacParams(int(iterations), int(samples), int(k), float(min_sample_distance), float(threshold), 0, int(seed))
+
+
+def _sac_out(r):
+    Rt = np.array(r.Rt).reshape(4, 4).T.copy()
+    ms = list(r.stage_ms)
+    return Rt, dict(error=r.error, fitness=r.fitness, inliers=r.inliers, best_hypothesis=r.best_hypothesis,
+                    invalid_hypotheses=r.invalid_hypotheses,
+                    stage_ms=dict(sample_knn=ms[0], estimate=ms[1], score=ms[2], pick=ms[3], total=float(sum(ms))))
 
 
 class PrepParams(C.Structure):
@@ -212,6 +239,13 @@ class Prep:
         out = np.zeros((self.n_kp, 33), np.float32)
         check(lib().ghicp_prep_get_fpfh(self.h, out.ctypes.data_as(C.POINTER(C.c_float))))
         return out
+
+    def sac_ia(self, target, iterations=1000, samples=3, k=6, min_sample_distance=0.0, threshold=100.0, seed=0):
+        """SAC-IA from this cloud's keypoints onto `target`'s (both after fpfh()), device to device: see sac_ia."""
+        r = SacResult()
+        check(lib().ghicp_prep_sac_ia(self.h, target.h, C.byref(_sac_params(iterations, samples, k, min_sample_distance, threshold,
+                                                                             seed)), C.byref(r)))
+        return _sac_out(r)
 
     def close(self):
         if getattr(self, "h", None):
@@ -366,6 +400,27 @@ def fpfh_extract(xyz, idx=None, k=20, device=0):
     check(lib().ghicp_fpfh_extract(device, xyz.ctypes.data_as(fpp), n, None if ia is None else _ip(ia), m, k,
                                    fpfh.ctypes.data_as(fpp), normals.ctypes.data_as(fpp), _ip(status)))
     return fpfh, normals, status
+
+
+def sac_ia(src_xyz, src_fpfh, tgt_xyz, tgt_fpfh, iterations=1000, samples=3, k=6, min_sample_distance=0.0, threshold=100.0,
+           seed=0, device=0):
+    """FPFHfeature::fpfhalign (include/fpfh.hpp:117-133; PCL SampleConsensusInitialAlignment) on the GPU, DESIGN.md §3.11:
+    `iterations` hypotheses of `samples` source points, each paired with one of its `k` nearest target histograms, scored by
+    the truncated error over all source points with `threshold` on SQUARED distances.  Deterministic for a given `seed`.
+    Returns (Rt 4x4 mapping the source onto the target, info: error, fitness, inliers, best_hypothesis, invalid_hypotheses,
+    stage_ms)."""
+    fpp = C.POINTER(C.c_float)
+    P = np.ascontiguousarray(src_xyz, dtype=np.float32).reshape(-1, 3)
+    Fs = np.ascontiguousarray(src_fpfh, dtype=np.float32).reshape(-1, 33)
+    Q = np.ascontiguousarray(tgt_xyz, dtype=np.float32).reshape(-1, 3)
+    Ft = np.ascontiguousarray(tgt_fpfh, dtype=np.float32).reshape(-1, 33)
+    if len(P) != len(Fs) or len(Q) != len(Ft):
+        raise GhicpError(-1, "sac_ia: one histogram per point expected")
+    r = SacResult()
+    check(lib().ghicp_sac_ia(device, P.ctypes.data_as(fpp), Fs.ctypes.data_as(fpp), len(P), Q.ctypes.data_as(fpp),
+                             Ft.ctypes.data_as(fpp), len(Q), C.byref(_sac_params(iterations, samples, k, min_sample_distance,
+                                                                                threshold, seed)), C.byref(r)))
+    return _sac_out(r)
 
 
 def rigid_fit_ex(S, T, solver=SOLVER_SVD, normals=None, weights=None, device=0):

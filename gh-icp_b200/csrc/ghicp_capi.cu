@@ -12,6 +12,14 @@
 #include <mutex>
 
 #include "ghicp_internal.h"
+#include "ghicp_sac.h"
+
+#if defined(GHICP_EMU_HOST)
+// The CPU emulation of the whole library (tests/harness/emu_library.cpp) compiles the product's .cu files as ONE translation
+// unit and lists the kernel files it includes; the SAC-IA kernels join it here, next to the entry points that call them.
+// nvcc builds ghicp_sac.cu as a translation unit of its own (Makefile SRCS).
+#include "ghicp_sac.cu"
+#endif
 
 namespace ghicp_b200 {
 
@@ -1506,6 +1514,91 @@ int ghicp_prep_fpfh_stats(const ghicp_prep *h, long long *candidates, int *queri
   if (queries) *queries = h->fpfh_stats.queries;
   if (fallbacks) *fallbacks = h->fpfh_stats.fallbacks;
   if (cell) *cell = h->fpfh_stats.cell;
+  return GHICP_OK;
+}
+
+// ---- SAC-IA coarse alignment -------------------------------------------------------------------------------------------
+static bool sac_params_ok(const ghicp_sac_params *p, const char *who) {
+  const char *why = nullptr;
+  if (!p) why = "no parameters";
+  else if (p->max_iterations < 1) why = "max_iterations must be >= 1";
+  else if (p->nr_samples < 3 || p->nr_samples > ghicp_sac::SAC_MAX_SAMPLES) why = "nr_samples must be in 3..8";
+  else if (p->k_correspondences < 1 || p->k_correspondences > ghicp_sac::SAC_KMAX) why = "k_correspondences must be in 1..32";
+  else if (!(p->min_sample_distance >= 0.f) || !std::isfinite(p->min_sample_distance)) why = "min_sample_distance must be finite and >= 0";
+  else if (!(p->corr_dist_threshold > 0.f) || !std::isfinite(p->corr_dist_threshold)) why = "corr_dist_threshold must be finite and > 0";
+  if (why) set_error(nullptr, std::string(who) + ": " + why);
+  return why == nullptr;
+}
+static int sac_status(cudaError_t e, const char *who) {
+  if (e == cudaSuccess) return GHICP_OK;
+  set_error(nullptr, std::string(who) + ": " + cudaGetErrorString(e));
+  cudaGetLastError();
+  return e == cudaErrorMemoryAllocation ? GHICP_E_NOMEM : GHICP_E_CUDA;
+}
+
+int ghicp_sac_ia(int device, const float *src_xyz, const float *src_fpfh, int n_s, const float *tgt_xyz, const float *tgt_fpfh,
+                 int n_t, const ghicp_sac_params *p, ghicp_sac_result *out) {
+  if (!src_xyz || !src_fpfh || !tgt_xyz || !tgt_fpfh || !out || n_s <= 0 || n_t <= 0) {
+    set_error(nullptr, "sac_ia: bad argument (null array or empty cloud)");
+    return GHICP_E_ARG;
+  }
+  if (!sac_params_ok(p, "sac_ia")) return GHICP_E_ARG;
+  if (ghicp_device_count() <= 0) { set_error(nullptr, "sac_ia: no CUDA device"); return GHICP_E_NODEV; }
+  if (cudaSetDevice(device) != cudaSuccess) return GHICP_E_CUDA;
+  float *d_p = nullptr, *d_fs = nullptr, *d_q = nullptr, *d_ft = nullptr;
+  cudaError_t e = cudaMallocAsync((void **)&d_p, 3 * (size_t)n_s * sizeof(float), 0);
+  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_fs, 33 * (size_t)n_s * sizeof(float), 0);
+  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_q, 3 * (size_t)n_t * sizeof(float), 0);
+  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_ft, 33 * (size_t)n_t * sizeof(float), 0);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(d_p, src_xyz, 3 * (size_t)n_s * sizeof(float), cudaMemcpyHostToDevice, 0);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(d_fs, src_fpfh, 33 * (size_t)n_s * sizeof(float), cudaMemcpyHostToDevice, 0);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(d_q, tgt_xyz, 3 * (size_t)n_t * sizeof(float), cudaMemcpyHostToDevice, 0);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(d_ft, tgt_fpfh, 33 * (size_t)n_t * sizeof(float), cudaMemcpyHostToDevice, 0);
+  if (e == cudaSuccess) e = sac_run(d_p, d_fs, n_s, d_q, d_ft, n_t, p, out, nullptr);
+  for (float *x : {d_p, d_fs, d_q, d_ft}) if (x) cudaFreeAsync(x, 0);
+  return sac_status(e, "sac_ia");
+}
+
+int ghicp_prep_sac_ia(const ghicp_prep *src, const ghicp_prep *tgt, const ghicp_sac_params *p, ghicp_sac_result *out) {
+  if (!src || !tgt || !out || src->n_kp <= 0 || tgt->n_kp <= 0 || !src->d_fpfh || !tgt->d_fpfh) {
+    set_error(nullptr, "prep_sac_ia: bad argument, a cloud without keypoints or without histograms (call ghicp_prep_fpfh first)");
+    return GHICP_E_ARG;
+  }
+  if (src->device != tgt->device) { set_error(nullptr, "prep_sac_ia: the two pipeline results live on different devices"); return GHICP_E_ARG; }
+  if (!sac_params_ok(p, "prep_sac_ia")) return GHICP_E_ARG;
+  if (cudaSetDevice(src->device) != cudaSuccess) return GHICP_E_CUDA;
+  float *d_p = nullptr, *d_q = nullptr;
+  cudaError_t e = cudaMallocAsync((void **)&d_p, 3 * (size_t)src->n_kp * sizeof(float), 0);
+  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_q, 3 * (size_t)tgt->n_kp * sizeof(float), 0);
+  if (e == cudaSuccess) e = sac_points_from_soa(src->d_kp_xyz, src->n_kp, d_p);   // exact: the doubles are widened floats
+  if (e == cudaSuccess) e = sac_points_from_soa(tgt->d_kp_xyz, tgt->n_kp, d_q);
+  if (e == cudaSuccess) e = sac_run(d_p, src->d_fpfh, src->n_kp, d_q, tgt->d_fpfh, tgt->n_kp, p, out, nullptr);
+  if (d_p) cudaFreeAsync(d_p, 0);
+  if (d_q) cudaFreeAsync(d_q, 0);
+  return sac_status(e, "prep_sac_ia");
+}
+
+int ghicp_set_initial_transform(ghicp_ctx *ctx, const double Rt[16]) {
+  Ctx *c = reinterpret_cast<Ctx *>(ctx);
+  if (!c || !Rt) { set_error(c, "set_initial_transform: bad argument"); return GHICP_E_ARG; }
+  if (c->N <= 0) { set_error(c, "set_initial_transform: keypoints not set"); return GHICP_E_ARG; }
+  if (c->iteration != 0) { set_error(c, "set_initial_transform: only before iteration 0 (after ghicp_reset, re-upload the source first)"); return GHICP_E_ARG; }
+  for (int i = 0; i < 16; ++i)
+    if (!std::isfinite(Rt[i])) { set_error(c, "set_initial_transform: non-finite matrix"); return GHICP_E_ARG; }
+  int rc;
+  if ((rc = use_device(c))) return rc;
+  // the update of every iteration (k_apply) with this transform
+  CK(c, cudaMemcpyAsync(c->d_iter->Rt, Rt, sizeof(double) * 16, cudaMemcpyHostToDevice, c->stream));
+  CK(c, launch_apply(c, false));
+  CK(c, cudaStreamSynchronize(c->stream));
+  double acc[16];   // Rt_tillnow = Rt * Rt_tillnow, as after an iteration
+  for (int col = 0; col < 4; ++col)
+    for (int row = 0; row < 4; ++row) {
+      double s = 0;
+      for (int k = 0; k < 4; ++k) s += Rt[k * 4 + row] * c->Rt_tillnow[col * 4 + k];
+      acc[col * 4 + row] = s;
+    }
+  std::memcpy(c->Rt_tillnow, acc, sizeof(acc));
   return GHICP_OK;
 }
 

@@ -1,0 +1,82 @@
+// ghicp_grid.cuh — the cell-sorted uniform point grid of the pre-processing kernels (ghicp_prep.cu: radius PCA, NMS, the
+// FPFH k-NN) and of the SAC-IA scoring (ghicp_sac.cu), which runs exact nearest-neighbour queries against the same index.
+// Points are sorted by cell key; ucell lists the occupied cells in key order and cstart their first sorted position.
+#pragma once
+#include "ghicp_internal.h"
+
+namespace ghicp_b200 {
+
+typedef unsigned long long pu64;
+
+__device__ __forceinline__ pu64 cell_key(int cx, int cy, int cz) { return ((pu64)cx << 42) | ((pu64)cy << 21) | (pu64)cz; }
+__device__ __forceinline__ int cell_coord(float v, float mn, float inv) { const int c = (int)floorf((v - mn) * inv); return c < 0 ? 0 : c; }
+inline int cell_coord_host(float v, float mn, float inv) { const float f = (v - mn) * inv; const int c = (int)floorf(f); return c < 0 ? 0 : c; }
+
+struct GridArgs {
+  const float *xyz; const int *ids;      // point of position k = xyz[ids ? ids[k] : k]
+  const int *order;                      // positions sorted by cell (ascending position inside a cell)
+  const float4 *sorted;                  // the same points in that order (x y z _): a cell's run is read with coalesced 16-byte loads
+  const pu64 *ucell; const int *cstart; int nu;
+  float mnx, mny, mnz, inv, r2;
+};
+// Per-thread neighbour walks (k_pca, k_nms_round): every thread first resolves its nine column runs, then walks them in one
+// flat loop nest, with the grid description copied into per-thread registers.  A form that walked "for dx, for dy
+// { column_run; for s }" reading the grid description straight from the kernel parameters returned neighbour counts short
+// for whole warps on hardware (its SASS re-loaded kernel parameters in per-warp uniform registers across the divergent
+// per-thread loops), while the CPU emulation of the same source passed.
+struct GridRegs {
+  const float4 *sorted; const pu64 *ucell; const int *cstart; const int *order; int nu; float r2;
+};
+__device__ __forceinline__ GridRegs grid_regs(const GridArgs &g) {
+  GridRegs r;
+  r.sorted = g.sorted; r.ucell = g.ucell; r.cstart = g.cstart; r.order = g.order; r.nu = g.nu; r.r2 = g.r2;
+  return r;
+}
+// first occupied cell with a key >= key
+__device__ __forceinline__ int lower_cell(const GridRegs &g, pu64 key) {
+  int lo = 0, hi = g.nu;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (g.ucell[mid] < key) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+// Top-k lists of the k-NN searches (k_knn, and the feature k-NN of SAC-IA): (d2, index) as one ascending u64 key.  d2 >= 0,
+// so its float bits order like the value; + 1 keeps key 0 free as the sentinel that pads the sorted list when k < K.
+__device__ __forceinline__ pu64 knn_key(float d2, int idx) { return ((pu64)(__float_as_uint(d2) + 1u) << 32) | (unsigned)idx; }
+__device__ __forceinline__ float knn_key_d2(pu64 key) { return __uint_as_float((unsigned)(key >> 32) - 1u); }
+
+// sorted insertion with static indices only (the list stays in registers): the largest key sits in the last slot
+template <int K>
+__device__ __forceinline__ void knn_insert(pu64 (&key)[K], pu64 c) {
+  if (!(c < key[K - 1])) return;
+  key[K - 1] = c;
+#pragma unroll
+  for (int j = K - 1; j > 0; --j) {
+    const pu64 lo = key[j - 1], hi = key[j];
+    const bool sw = hi < lo;
+    key[j - 1] = sw ? hi : lo; key[j] = sw ? lo : hi;
+  }
+}
+// d2 = (dx*dx + dy*dy) + dz*dz, dx = q.x - p.x, every operation rounded separately (the oracle's fpfh_d2)
+__device__ __forceinline__ float knn_d2(float qx, float qy, float qz, const float4 &p) {
+  const float dx = qx - p.x, dy = qy - p.y, dz = qz - p.z;
+  return (dx * dx + dy * dy) + dz * dz;
+}
+
+// A grid over all n points of d_xyz with the cell rule of the FPFH k-NN (k_eff neighbours wanted per query), for ring
+// searches: gx / gy / gz = the largest occupied cell coordinate per axis, slack = cells of margin for the float32 rounding
+// of cell_coord.  The arrays come from the stream-ordered pool; prep_point_grid_free returns them.
+struct PointGrid {
+  GridArgs g{};
+  int gx = 0, gy = 0, gz = 0;
+  float mx[3] = {0.f, 0.f, 0.f};         // bounding-box maximum (the minimum is g.mnx, g.mny, g.mnz)
+  double cell = 0.0, slack = 0.0;
+  int *order = nullptr, *cstart = nullptr; pu64 *ucell = nullptr; float4 *sorted = nullptr;
+};
+// cell edge = the k-NN rule times cell_scale (if > 0), at least min_cell, at least the extent / 2^20 (21-bit key fields)
+cudaError_t prep_point_grid(cudaStream_t st, const float *d_xyz, int n, int ke, float cell_scale, double min_cell, PointGrid *out);
+void prep_point_grid_free(PointGrid *g);
+
+}  // namespace ghicp_b200

@@ -375,6 +375,21 @@ cudaError_t prep_fpfh(cudaStream_t st, const float *d_xyz, int n, const int *d_i
                       float *d_fpfh, float *d_normals, int *d_status, int *d_nb_idx, float *d_nb_d2, cudaEvent_t ev_mid,
                       FpfhStats *stats);
 
+// SAC-IA coarse alignment from FPFH histograms (ghicp_sac.cu, DESIGN.md §3.11) on device arrays: source points [ns][3] and
+// histograms [ns][33], target likewise; parameters already checked.  dbg (may be null): host arrays that receive the
+// per-hypothesis intermediates (any may be null) and the scoring grid's cell edge — for tests and tools.
+struct SacDebug {
+  int *samples = nullptr;             // [H][nr_samples], -1 for an invalid hypothesis
+  int *valid = nullptr;               // [H]
+  int *corr = nullptr;                // [H][nr_samples] target indices
+  float *rt = nullptr;                // [H][12]: R row-major, then t
+  unsigned long long *err = nullptr;  // [H] error sums in units of 2^-32
+  double cell = 0.0;
+};
+cudaError_t sac_run(const float *d_P, const float *d_Fs, int ns, const float *d_Q, const float *d_Ft, int nt,
+                    const ghicp_sac_params *p, ghicp_sac_result *out, SacDebug *dbg);
+cudaError_t sac_points_from_soa(const double *d_soa, int n, float *d_xyz);   // [3][n] doubles -> [n][3] floats
+
 // glue of the device-resident pipeline (ghicp_prep_run)
 cudaError_t prep_gather_points(cudaStream_t st, const float *d_xyz, const int *d_idx, int m, float *d_out);
 cudaError_t prep_kp_coords(cudaStream_t st, const float *d_xyz, const int *d_kp, int nkp, double *d_soa);

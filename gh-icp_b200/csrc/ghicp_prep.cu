@@ -22,6 +22,7 @@
 
 #include "ghicp_internal.h"
 #include "ghicp_device.cuh"
+#include "ghicp_grid.cuh"
 
 #if !defined(GHICP_EMU_HOST)
 #include <cub/cub.cuh>
@@ -31,7 +32,6 @@ namespace ghicp_b200 {
 
 namespace {
 
-typedef unsigned long long pu64;
 constexpr int PT = 256;
 
 // ---- plumbing: device memory, sort, scan (CUB under nvcc; the C++ library under the emulation shim) -------------------
@@ -118,9 +118,6 @@ __host__ __device__ inline float ord2f(unsigned u) {
 #endif
   return f;
 }
-__device__ __forceinline__ pu64 cell_key(int cx, int cy, int cz) { return ((pu64)cx << 42) | ((pu64)cy << 21) | (pu64)cz; }
-__device__ __forceinline__ int cell_coord(float v, float mn, float inv) { const int c = (int)floorf((v - mn) * inv); return c < 0 ? 0 : c; }
-inline int cell_coord_host(float v, float mn, float inv) { const float f = (v - mn) * inv; const int c = (int)floorf(f); return c < 0 ? 0 : c; }
 
 // cyclic Jacobi on a symmetric 3x3 (float32), eigenvalues descending; c = {xx, xy, xz, yy, yz, zz}
 __device__ void sym3_eig_f32(const float c[6], float lam[3]) {
@@ -215,13 +212,6 @@ __global__ void k_cell_table(const pu64 *__restrict__ keys, const int *__restric
   if (i < n && flags[i]) { ucell[pos[i]] = keys[i]; cstart[pos[i]] = i; }
   if (i == n) cstart[pos[n]] = n;
 }
-struct GridArgs {
-  const float *xyz; const int *ids;      // point of position k = xyz[ids ? ids[k] : k]
-  const int *order;                      // positions sorted by cell (ascending position inside a cell)
-  const float4 *sorted;                  // the same points in that order (x y z _): a cell's run is read with coalesced 16-byte loads
-  const pu64 *ucell; const int *cstart; int nu;
-  float mnx, mny, mnz, inv, r2;
-};
 // The three cells (x, y, cz - 1 .. cz + 1) of a grid column have consecutive keys (z is the low field), so their points are
 // ONE contiguous run of the sorted order: one lower-bound search per column instead of three exact searches — 9 per point.
 __device__ __forceinline__ void column_run(const GridArgs &g, int x, int y, int cz, int &s0, int &s1) {
@@ -234,19 +224,6 @@ __device__ __forceinline__ void column_run(const GridArgs &g, int x, int y, int 
   int u1 = lo;
   while (u1 < g.nu && g.ucell[u1] <= khi) ++u1;   // at most three cells
   s0 = g.cstart[lo]; s1 = g.cstart[u1];            // cstart holds nu + 1 entries
-}
-// Per-thread neighbour walks (k_pca, k_nms_round): every thread first resolves its nine column runs, then walks them in one
-// flat loop nest, with the grid description copied into per-thread registers.  A form that walked "for dx, for dy
-// { column_run; for s }" reading the grid description straight from the kernel parameters returned neighbour counts short
-// for whole warps on hardware (its SASS re-loaded kernel parameters in per-warp uniform registers across the divergent
-// per-thread loops), while the CPU emulation of the same source passed.
-struct GridRegs {
-  const float4 *sorted; const pu64 *ucell; const int *cstart; const int *order; int nu; float r2;
-};
-__device__ __forceinline__ GridRegs grid_regs(const GridArgs &g) {
-  GridRegs r;
-  r.sorted = g.sorted; r.ucell = g.ucell; r.cstart = g.cstart; r.order = g.order; r.nu = g.nu; r.r2 = g.r2;
-  return r;
 }
 __device__ __forceinline__ void column_run_r(const GridRegs &g, int x, int y, int cz, int &s0, int &s1) {
   const pu64 klo = cell_key(x, y, cz > 0 ? cz - 1 : 0), khi = cell_key(x, y, cz + 1);
@@ -941,35 +918,6 @@ struct KnnArgs {
   int *fallbacks;                   // queries that took the exhaustive scan
 };
 
-// (d2, index) as one ascending u64 key.  d2 >= 0, so its float bits order like the value; + 1 keeps key 0 free as the
-// sentinel that pads the sorted list when k < FPFH_KMAX.
-__device__ __forceinline__ pu64 knn_key(float d2, int idx) { return ((pu64)(__float_as_uint(d2) + 1u) << 32) | (unsigned)idx; }
-__device__ __forceinline__ float knn_key_d2(pu64 key) { return __uint_as_float((unsigned)(key >> 32) - 1u); }
-
-// sorted insertion with static indices only (the list stays in registers): the largest key sits in the last slot
-__device__ __forceinline__ void knn_insert(pu64 (&key)[FPFH_KMAX], pu64 c) {
-  if (!(c < key[FPFH_KMAX - 1])) return;
-  key[FPFH_KMAX - 1] = c;
-#pragma unroll
-  for (int j = FPFH_KMAX - 1; j > 0; --j) {
-    const pu64 lo = key[j - 1], hi = key[j];
-    const bool sw = hi < lo;
-    key[j - 1] = sw ? hi : lo; key[j] = sw ? lo : hi;
-  }
-}
-// d2 = (dx*dx + dy*dy) + dz*dz, dx = q.x - p.x, every operation rounded separately (the oracle's fpfh_d2)
-__device__ __forceinline__ float knn_d2(float qx, float qy, float qz, const float4 &p) {
-  const float dx = qx - p.x, dy = qy - p.y, dz = qz - p.z;
-  return (dx * dx + dy * dy) + dz * dz;
-}
-__device__ __forceinline__ int lower_cell(const GridRegs &g, pu64 key) {
-  int lo = 0, hi = g.nu;
-  while (lo < hi) {
-    const int mid = (lo + hi) >> 1;
-    if (g.ucell[mid] < key) lo = mid + 1; else hi = mid;
-  }
-  return lo;
-}
 // cells (x, y, zlo .. zhi) = one run of the sorted order
 __device__ __forceinline__ void knn_column(const GridRegs &g, int x, int y, int zlo, int zhi, float qx, float qy, float qz,
                                            pu64 (&key)[FPFH_KMAX], long long &cand) {
@@ -1175,24 +1123,16 @@ __global__ void k_fpfh(const int *__restrict__ idx, int nidx, const int *__restr
 
 }  // namespace
 
-// FPFH histograms at d_idx [nidx] (all points when d_idx == nullptr) of the cloud d_xyz [n][3]; d_normals [n][3] receives
-// every point's normal, d_status [n] (may be null) 1 where fewer than 3 neighbours exist, d_nb_idx / d_nb_d2 [n][min(k, n)]
-// (may be null) the k-NN lists.  ev_mid (may be null) is recorded between the k-NN + normals and the SPFH + FPFH stages.
-// cell_scale multiplies the data-derived cell edge (test hook).
-cudaError_t prep_fpfh(cudaStream_t st, const float *d_xyz, int n, const int *d_idx, int nidx, int k, float cell_scale,
-                      float *d_fpfh, float *d_normals, int *d_status, int *d_nb_idx, float *d_nb_d2, cudaEvent_t ev_mid,
-                      FpfhStats *stats) {
+// The grid of a ring search over d_xyz [n][3] (see PointGrid).
+cudaError_t prep_point_grid(cudaStream_t st, const float *d_xyz, int n, int ke, float cell_scale, double min_cell, PointGrid *out) {
   cudaError_t err = cudaSuccess;
   GridArgs g{};
   int *order = nullptr, *cstart = nullptr; pu64 *ucell = nullptr; float4 *sorted = nullptr;
-  int *nb_idx = nullptr, *need = nullptr, *d_fb = nullptr; float *nb_d2 = nullptr, *spfh = nullptr;
-  unsigned long long *d_cand = nullptr;
-  if (stats) *stats = FpfhStats{};
-  if (n <= 0 || k < 3 || k > FPFH_KMAX) return cudaErrorInvalidValue;
+  float mn[3], mx[3];
+  *out = PointGrid();
+  if (n <= 0 || ke <= 0) return cudaErrorInvalidValue;
+  PCK(prep_bounds(st, d_xyz, n, mn, mx));
   {
-    const int ke = k < n ? k : n;
-    float mn[3], mx[3];
-    PCK(prep_bounds(st, d_xyz, n, mn, mx));
     // Cell edge from the data: a volume guess (k points per cell if the cloud filled its box), then corrected once by the
     // observed mean occupancy of the occupied cells assuming a surface (occupancy ~ edge^2), aiming at 0.4 k per cell —
     // enough for the k nearest to lie within one ring.  The results do not depend on it; the work per query does.
@@ -1211,14 +1151,47 @@ cudaError_t prep_fpfh(cudaStream_t st, const float *d_xyz, int n, const int *d_i
       pfree(order); pfree(ucell); pfree(cstart); pfree(sorted); order = cstart = nullptr; ucell = nullptr; sorted = nullptr;
     }
     if (cell_scale > 0.f) cell *= cell_scale;
+    if (cell < min_cell) cell = min_cell;
     if (cell < emax / 1048576.0) cell = emax / 1048576.0;   // cell coordinates stay below 2^20 (21-bit key fields)
     PCK(build_grid(st, d_xyz, nullptr, n, (float)cell, &g, &order, &ucell, &cstart, &sorted));
+    out->g = g;
+    out->gx = cell_coord_host(mx[0], g.mnx, g.inv); out->gy = cell_coord_host(mx[1], g.mny, g.inv); out->gz = cell_coord_host(mx[2], g.mnz, g.inv);
+    for (int a = 0; a < 3; ++a) out->mx[a] = mx[a];
+    out->cell = (double)(float)cell;
+    const int gmax = out->gx > out->gy ? (out->gx > out->gz ? out->gx : out->gz) : (out->gy > out->gz ? out->gy : out->gz);
+    out->slack = 0.01 + (gmax + 2.0) / 1048576.0;
+    out->order = order; out->ucell = ucell; out->cstart = cstart; out->sorted = sorted;
+    order = cstart = nullptr; ucell = nullptr; sorted = nullptr;
+  }
+done:
+  pfree(order); pfree(ucell); pfree(cstart); pfree(sorted);
+  return err;
+}
+void prep_point_grid_free(PointGrid *g) {
+  pfree(g->order); pfree(g->ucell); pfree(g->cstart); pfree(g->sorted);
+  *g = PointGrid();
+}
+
+// FPFH histograms at d_idx [nidx] (all points when d_idx == nullptr) of the cloud d_xyz [n][3]; d_normals [n][3] receives
+// every point's normal, d_status [n] (may be null) 1 where fewer than 3 neighbours exist, d_nb_idx / d_nb_d2 [n][min(k, n)]
+// (may be null) the k-NN lists.  ev_mid (may be null) is recorded between the k-NN + normals and the SPFH + FPFH stages.
+// cell_scale multiplies the data-derived cell edge (test hook).
+cudaError_t prep_fpfh(cudaStream_t st, const float *d_xyz, int n, const int *d_idx, int nidx, int k, float cell_scale,
+                      float *d_fpfh, float *d_normals, int *d_status, int *d_nb_idx, float *d_nb_d2, cudaEvent_t ev_mid,
+                      FpfhStats *stats) {
+  cudaError_t err = cudaSuccess;
+  PointGrid pg;
+  int *nb_idx = nullptr, *need = nullptr, *d_fb = nullptr; float *nb_d2 = nullptr, *spfh = nullptr;
+  unsigned long long *d_cand = nullptr;
+  if (stats) *stats = FpfhStats{};
+  if (n <= 0 || k < 3 || k > FPFH_KMAX) return cudaErrorInvalidValue;
+  {
+    const int ke = k < n ? k : n;
+    PCK(prep_point_grid(st, d_xyz, n, ke, cell_scale, 0.0, &pg));
     KnnArgs a{};
-    a.g = g; a.n = n; a.k = ke;
-    a.gx = cell_coord_host(mx[0], g.mnx, g.inv); a.gy = cell_coord_host(mx[1], g.mny, g.inv); a.gz = cell_coord_host(mx[2], g.mnz, g.inv);
-    a.cell = (double)(float)cell;
-    const int gmax = a.gx > a.gy ? (a.gx > a.gz ? a.gx : a.gz) : (a.gy > a.gz ? a.gy : a.gz);
-    a.slack = 0.01 + (gmax + 2.0) / 1048576.0;
+    a.g = pg.g; a.n = n; a.k = ke;
+    a.gx = pg.gx; a.gy = pg.gy; a.gz = pg.gz;
+    a.cell = pg.cell; a.slack = pg.slack;
     PCK(pmalloc(&nb_idx, (size_t)n * ke)); PCK(pmalloc(&nb_d2, (size_t)n * ke));
     PCK(pmalloc(&d_cand, 1)); PCK(pmalloc(&d_fb, 1));
     PCK(pzero(d_cand, sizeof(pu64), st)); PCK(pzero(d_fb, sizeof(int), st));
@@ -1240,14 +1213,14 @@ cudaError_t prep_fpfh(cudaStream_t st, const float *d_xyz, int n, const int *d_i
       pu64 c = 0; int fb = 0;
       PCK(pcopy(&c, d_cand, sizeof(c), P_D2H, st)); PCK(pcopy(&fb, d_fb, sizeof(fb), P_D2H, st));
       PCK(psync(st));
-      stats->candidates = (long long)c; stats->fallbacks = fb; stats->cell = (float)cell; stats->queries = n;
+      stats->candidates = (long long)c; stats->fallbacks = fb; stats->cell = (float)pg.cell; stats->queries = n;
     }
 #if !defined(GHICP_EMU_HOST)
     PCK(cudaGetLastError());
 #endif
   }
 done:
-  pfree(order); pfree(ucell); pfree(cstart); pfree(sorted);
+  prep_point_grid_free(&pg);
   pfree(nb_idx); pfree(nb_d2); pfree(need); pfree(spfh); pfree(d_cand); pfree(d_fb);
   return err;
 }

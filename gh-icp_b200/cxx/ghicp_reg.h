@@ -126,6 +126,13 @@ class GHRegistration {
     check(ghicp_set_target_normals(ctx_, normals.data()), "ghicp_set_target_normals");
   }
 
+  // Extension: start the loop from Rt (e.g. FPFHfeature::fpfhalign's getFinalTransformation), before the first iteration;
+  // ghicp_reg then returns the whole transform.
+  void set_initial_transform(const Matrix4d &Rt) {
+    check(ghicp_set_initial_transform(ctx_, Rt.data()), "ghicp_set_initial_transform");
+    check(ghicp_get_rt(ctx_, Rt_tillnow.data()), "ghicp_get_rt");
+  }
+
   // Main entrance (src/ghicp_reg.cpp:24-112)
   bool ghicp_reg(Matrix4d &Rt_final) {
     check(ghicp_build_fd(ctx_), "ghicp_build_fd");

@@ -15,6 +15,14 @@ every stage runs on the GPU and the descriptors are computed there too:
     rejects it.
 `features(target_down, target_kp_idx, source_down, source_kp_idx) -> Keypoints` attaches descriptors computed elsewhere
 instead.
+
+GH-ICP is a local method.  initial_alignment = "fpfh_sac" first runs SAC-IA (FPFHfeature::fpfhalign, include/fpfh.hpp:117-133;
+DESIGN.md §3.11) on the keypoints and their FPFH histograms — computed for this stage alone when the loop uses BSC or no
+feature — and starts the loop from its transform; the returned transform is the whole one and info["sac"] describes the
+coarse stage.  `sac` overrides the capi.sac_ia arguments (iterations, samples, k, min_sample_distance, threshold, seed); the
+default threshold is the keypoint NMS radius squared: keypoints are at least one NMS radius apart, so within that distance the
+nearest target keypoint of a moved source keypoint can only be its counterpart, and the error counts the keypoints that land
+on their counterparts.  On small keypoint sets of repetitive scenes 1000 hypotheses may not be enough (DESIGN.md §3.11).
 """
 import numpy as np
 
@@ -24,7 +32,12 @@ from .registration import Energyfunction, GHRegistration, Keypoints
 
 def register_clouds(target_xyz, source_xyz, resolution, neighborhood_radius, curvature_non_max_radius, corr_type=capi.CT_NN,
                     feature_type=capi.FT_NONE, features=None, weight_adjustment_ratio=1.1, weight_adjustment_step=0.1,
-                    dof_type=6, estimated_IoU=0.5, max_iter=0, device=0, bsc_pattern=None, fpfh_k=20, **reg_kw):
+                    dof_type=6, estimated_IoU=0.5, max_iter=0, device=0, bsc_pattern=None, fpfh_k=20, initial_alignment=None,
+                    sac=None, **reg_kw):
+    if initial_alignment not in (None, "fpfh_sac"):
+        raise capi.GhicpError(-1, f"initial_alignment must be None or 'fpfh_sac', not {initial_alignment!r}")
+    sac_kw = dict(threshold=float(curvature_non_max_radius) ** 2)
+    sac_kw.update(sac or {})
     T = np.ascontiguousarray(target_xyz, dtype=np.float32)
     S = np.ascontiguousarray(source_xyz, dtype=np.float32)
     if features is None:
@@ -38,18 +51,25 @@ def register_clouds(target_xyz, source_xyz, resolution, neighborhood_radius, cur
             for name, pr in (("target", pt), ("source", ps)):
                 if pr.n_kp == 0:
                     raise capi.GhicpError(-1, f"no keypoints in the {name} cloud: check the radii")
-            if feature_type == capi.FT_FPFH:                                             # :120-127
+            if feature_type == capi.FT_FPFH or initial_alignment == "fpfh_sac":          # :120-127
                 pt.fpfh(fpfh_k); ps.fpfh(fpfh_k)
+            Rt0, sac_info = None, None
+            if initial_alignment == "fpfh_sac":
+                Rt0, sac_info = ps.sac_ia(pt, **sac_kw)
             bbx = ps.bbx_magnitude                                                       # getCloudBound, :91-93
             Ef = Energyfunction().init(ps.n_kp, pt.n_kp, bbx)
             reg = GHRegistration((ps, pt), Ef, feature_type, corr_type, curvature_non_max_radius, weight_adjustment_ratio,
                                  weight_adjustment_step, dof_type, estimated_IoU, max_iter=max_iter, device=device, **reg_kw)
+            if Rt0 is not None:
+                reg.set_initial_transform(Rt0)
             Rt, iterations = reg.ghicp_reg()
             info = dict(iterations=iterations, n_target_down=pt.n_down, n_source_down=ps.n_down, n_target_kp=pt.n_kp,
                         n_source_kp=ps.n_kp, bbx_magnitude=bbx, cor=len(reg.pairs()[0]),
                         stage_ms=dict(target=pt.stage_ms, source=ps.stage_ms))
             if feature_type == capi.FT_FPFH:
                 info["fpfh_ms"] = dict(target=pt.fpfh_ms, source=ps.fpfh_ms)
+            if sac_info is not None:
+                info["sac"] = dict(sac_info, Rt=Rt0)
             reg.close()
         finally:
             pt.close(); ps.close()
@@ -68,9 +88,18 @@ def register_clouds(target_xyz, source_xyz, resolution, neighborhood_radius, cur
     Ef = Energyfunction().init(Kp.kps_num, Kp.kpt_num, bbx)
     reg = GHRegistration(Kp, Ef, feature_type, corr_type, curvature_non_max_radius, weight_adjustment_ratio,
                          weight_adjustment_step, dof_type, estimated_IoU, max_iter=max_iter, device=device, **reg_kw)
+    sac_info = None
+    if initial_alignment == "fpfh_sac":
+        fs, _, _ = capi.fpfh_extract(down["S"], kp_idx["S"], fpfh_k, device=device)
+        ft, _, _ = capi.fpfh_extract(down["T"], kp_idx["T"], fpfh_k, device=device)
+        Rt0, sac_info = capi.sac_ia(down["S"][kp_idx["S"]], fs, down["T"][kp_idx["T"]], ft, device=device, **sac_kw)
+        reg.set_initial_transform(Rt0)
+        sac_info = dict(sac_info, Rt=Rt0)
     Rt, iterations = reg.ghicp_reg()
     info = dict(iterations=iterations, n_target_down=len(down["T"]), n_source_down=len(down["S"]), n_target_kp=len(kp_idx["T"]),
                 n_source_kp=len(kp_idx["S"]), bbx_magnitude=bbx, cor=len(reg.pairs()[0]))
+    if sac_info is not None:
+        info["sac"] = sac_info
     reg.close()
     return Rt, info
 

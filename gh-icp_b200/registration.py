@@ -110,6 +110,13 @@ class GHRegistration:
         n = np.asfortranarray(normals, dtype=np.float64)
         capi.check(self.L.ghicp_set_target_normals(self.ctx, capi._dp(n)), self.ctx)
 
+    def set_initial_transform(self, Rt):
+        """Start the loop from Rt (4x4, source -> target), e.g. a SAC-IA result: the source keypoints are moved on the device
+        and Rt_tillnow starts at Rt, so ghicp_reg() and Rt_tillnow() return the whole transform.  Only before iteration 0."""
+        Rt = np.asarray(Rt, dtype=np.float64).reshape(4, 4)
+        cm = np.ascontiguousarray(Rt.T).reshape(16)   # column-major (Eigen::Matrix4d::data())
+        capi.check(self.L.ghicp_set_initial_transform(self.ctx, capi._dp(cm)), self.ctx)
+
     def set_solver(self, solver):
         capi.check(self.L.ghicp_set_solver(self.ctx, int(solver)), self.ctx)
 

@@ -266,6 +266,45 @@ int ghicp_prep_get_fpfh(const ghicp_prep *h, float *fpfh);
  * the exhaustive scan, grid cell edge.  Any output may be NULL. */
 int ghicp_prep_fpfh_stats(const ghicp_prep *h, long long *candidates, int *queries, int *fallbacks, float *cell);
 
+/* ---- SAC-IA coarse alignment on the GPU -------------------------------------------------------------------------------
+ * FPFHfeature::fpfhalign (include/fpfh.hpp:117-133: PCL SampleConsensusInitialAlignment, correspondence randomness 6) and
+ * CRegistration::Coarsereg_FPFHSAC (src/common_reg.cpp:393-423, randomness 15) on the canonical definition of DESIGN.md
+ * §3.11: max_iterations independent hypotheses of nr_samples source points (counter-based SplitMix64 draws from seed), each
+ * paired with one of its k_correspondences nearest target histograms, fitted by the float32 Umeyama of the loop and scored by
+ * PCL's truncated error over every source point (d2 / thr if d2 <= thr, else 1; thr applies to SQUARED distances) with exact
+ * nearest neighbours; the smallest error wins, ties to the smallest hypothesis.  Deterministic: the same inputs and seed give
+ * the same result bit for bit.  Zero-initialise ghicp_sac_params and fill it; the defaults of the definition are
+ * max_iterations 1000, nr_samples 3 (3..8), k_correspondences 6 (1..32), min_sample_distance 0, corr_dist_threshold 100,
+ * seed 0.  Out-of-range parameters return GHICP_E_ARG. */
+typedef struct ghicp_sac_params {
+  int max_iterations;          /* hypotheses H >= 1 */
+  int nr_samples;              /* 3 .. 8 */
+  int k_correspondences;       /* 1 .. 32; min(k, n_t) are used */
+  float min_sample_distance;   /* >= 0: every two samples of a hypothesis at least this far apart (float32 Euclidean) */
+  float corr_dist_threshold;   /* > 0, on squared distances */
+  int reserved;
+  unsigned long long seed;
+} ghicp_sac_params;
+typedef struct ghicp_sac_result {
+  double Rt[16];               /* column-major; the chosen float32 transform widened (identity when no hypothesis is valid) */
+  double error;                /* sum of the truncated error terms (each rounded to a multiple of 2^-32) */
+  double fitness;              /* mean squared nearest distance over the source points within the threshold (DBL_MAX: none) */
+  int inliers;                 /* source points within the threshold */
+  int best_hypothesis;         /* h* (-1: every hypothesis failed to draw its samples) */
+  int invalid_hypotheses;      /* hypotheses without nr_samples acceptable samples (3 n_s rejections in a row) */
+  int reserved;
+  float stage_ms[4];           /* CUDA events: sampling + feature k-NN, estimation, scoring (with the target grid), pick */
+} ghicp_sac_result;
+/* src_xyz [n_s][3], src_fpfh [n_s][33], tgt_xyz [n_t][3], tgt_fpfh [n_t][33] (host arrays) */
+int ghicp_sac_ia(int device, const float *src_xyz, const float *src_fpfh, int n_s, const float *tgt_xyz, const float *tgt_fpfh,
+                 int n_t, const ghicp_sac_params *p, ghicp_sac_result *out);
+/* keypoint coordinates + keypoint histograms of two pipeline results (ghicp_prep_fpfh on both), device to device */
+int ghicp_prep_sac_ia(const ghicp_prep *source, const ghicp_prep *target, const ghicp_sac_params *p, ghicp_sac_result *out);
+/* After ghicp_set_keypoints / ghicp_set_from_prep, before iteration 0: move the source keypoints by Rt on the device (the
+ * update every iteration applies, src/ghicp_reg.cpp:891-894) and compose Rt into Rt_tillnow, so that ghicp_get_rt and
+ * ghicp_run return the whole transform.  GHICP_E_ARG after iteration 0 or without keypoints. */
+int ghicp_set_initial_transform(ghicp_ctx *ctx, const double Rt[16]);
+
 /* ---- multi-GPU (one process per GPU; source rows sharded, target replicated) ---------------- */
 /* 128-byte NCCL unique id; rank 0 creates it, the host runtime broadcasts it (torch.distributed,
  * MPI, a file ...). No NCCL symbol is touched unless these are called (world == 1 → never). */
