@@ -190,6 +190,11 @@ static int alloc_workspaces(Ctx *c) {
     c->cand_cap = (int)std::min<size_t>((size_t)96 * nmax + (1u << 20), (size_t)1 << 28);
     if ((rc = dev_alloc(c, &c->d_cand[0], (size_t)c->cand_cap))) return rc;
     if (c->cfg.corr_type == GHICP_CT_NNR) { if ((rc = dev_alloc(c, &c->d_cand[1], (size_t)c->cand_cap))) return rc; }
+    // GHICP_CAND_CAP_MAX lowers the capacity the kernels see (test hook: forces the overflow -> all-double redo at any size)
+    if (const char *ov = getenv("GHICP_CAND_CAP_MAX")) {
+      const long long v = atoll(ov);
+      if (v >= 1) c->cand_cap = (int)std::min<long long>(c->cand_cap, v);
+    }
   }
   c->tile_cap = 2 * ((std::max(L, (size_t)nmax) + 1023) / 1024 + 1);
   if ((rc = dev_alloc(c, &c->d_tile_sum, c->tile_cap))) return rc;

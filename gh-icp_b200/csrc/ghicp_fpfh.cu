@@ -355,7 +355,9 @@ __device__ GHICP_NOINLINE double ff_exact_cd(const FfArgs &a, int i, int j) {
                              a.t[2 * (size_t)a.M + j], a.cp.scale);
   return cd_exact<GHICP_FT_FPFH>(ed, (double)fdf, a.cp);
 }
+// saturating like push_candidate (ghicp_stream.cu): the count stays below cap + resident threads and cannot wrap
 __device__ __forceinline__ void ff_push(const FfArgs &a, int which, int i, int j, double cd) {
+  if (*(volatile int *)&a.dev->cand_count[which] >= a.cand_cap) { a.dev->overflow = 1; return; }
   const int slot = atomicAdd(&a.dev->cand_count[which], 1);
   if (slot < a.cand_cap) {
     Cand c;

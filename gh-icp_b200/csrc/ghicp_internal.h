@@ -120,8 +120,8 @@ struct StreamDev {  // device-resident scalars of the streaming path
   unsigned r2max_bits;   // max squared centred norm of any keypoint (float bits)
   float margin;          // bound on |cd32 - cd64|
   float thr_hi;          // KM superset gate
-  int cand_count[2];     // row / column candidates
-  int overflow;
+  int cand_count[2];     // row / column candidates (saturating: at most cand_cap + resident threads)
+  int overflow;          // some candidate did not fit below cand_cap
   unsigned long long nnz_valid;
   unsigned long long emit_count;  // KM: gate hits appended to the edge list by the count pass (may exceed its capacity)
 };

@@ -239,7 +239,10 @@ __global__ void k_seed(StreamArgs a, const int *__restrict__ prev_row_idx, const
 // ---------------------------------------------------------------------------------------------
 // the streaming kernel
 // ---------------------------------------------------------------------------------------------
+// Saturating: once the count has reached the cap nobody adds to it, so it stays below cap + resident threads and cannot wrap
+// past INT_MAX into a negative slot that passes the bound (a far outlier widens the margin enough for billions of pushes).
 __device__ __forceinline__ void push_candidate(const StreamArgs &a, int which, int i, int j, double cd) {
+  if (*(volatile int *)&a.dev->cand_count[which] >= a.cand_cap) { a.dev->overflow = 1; return; }
   const int slot = atomicAdd(&a.dev->cand_count[which], 1);
   if (slot < a.cand_cap) {
     Cand c;

@@ -110,7 +110,9 @@ typedef struct ghicp_iter_stats {
   float ms_cost, ms_corr, ms_solve, ms_total; /* CUDA-event stage times on the ctx stream */
   float ms_stream;      /* CUDA-event time of ONE streaming pass over the FD plane (the dominant kernel) */
   int stream_passes;    /* passes over the FD plane this iteration (1 NN/NNR, +1 seed pass, 2-3 KM) */
-  long long candidates; /* NN/NNR: pairs the FP32 filter handed to exact FP64 evaluation */
+  long long candidates; /* NN/NNR: pairs the FP32 filter handed to exact FP64 evaluation.  Once the candidate buffer has
+                           overflowed (exact_fallback bit 0) the count stops growing near the buffer's capacity: it is then
+                           a lower bound */
 } ghicp_iter_stats;
 
 typedef struct ghicp_ctx ghicp_ctx;

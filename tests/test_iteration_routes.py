@@ -57,7 +57,8 @@ CASES = {
     "probe_bsc": ("bsc", "nn", 6, {}, {}),
     "probe_fpfh": ("fpfh", "nn", 6, {}, {}),
 }
-HOOKS = ("GHICP_KM_FILL", "GHICP_KM_GENERAL", "GHICP_KM_XUSE_MAX", "GHICP_FPFH_EXACT", "GHICP_FPFH_MATRIX_FREE", "GHICP_FD_POPC")
+HOOKS = ("GHICP_KM_FILL", "GHICP_KM_GENERAL", "GHICP_KM_XUSE_MAX", "GHICP_FPFH_EXACT", "GHICP_FPFH_MATRIX_FREE", "GHICP_FD_POPC",
+         "GHICP_CAND_CAP_MAX")
 INT_FIELDS = ("iteration", "cor", "converged", "warnings", "nnz", "km_rounds", "km_phases", "gpu_launches", "exact_fallback",
               "stream_passes", "candidates")
 DOUBLE_FIELDS = ("cd_mean", "cd_std", "penalty", "rmse", "rmse_after", "fdm", "fdstd", "iou", "para1", "para2", "km_energy",
