@@ -75,7 +75,8 @@ EXPORTS = ["ghicp_abi_version", "ghicp_device_count", "ghicp_last_error", "ghicp
            "ghicp_bsc_extract", "ghicp_bsc_default_pattern", "ghicp_comm_unique_id", "ghicp_comm_init",
            "ghicp_prep_run", "ghicp_prep_info", "ghicp_prep_get", "ghicp_prep_destroy", "ghicp_set_from_prep",
            "ghicp_host_alloc", "ghicp_host_free", "ghicp_fpfh_extract", "ghicp_prep_fpfh", "ghicp_prep_get_fpfh",
-           "ghicp_prep_fpfh_stats", "ghicp_sac_ia", "ghicp_prep_sac_ia", "ghicp_set_initial_transform"]
+           "ghicp_prep_fpfh_stats", "ghicp_sac_ia", "ghicp_prep_sac_ia", "ghicp_set_initial_transform",
+           "ghicp_fpfh_extract_radius", "ghicp_prep_fpfh_radius"]
 
 
 def lib():
@@ -133,6 +134,8 @@ def lib():
     L.ghicp_sac_ia.argtypes = [C.c_int, fpp, fpp, C.c_int, fpp, fpp, C.c_int, C.POINTER(SacParams), C.POINTER(SacResult)]
     L.ghicp_prep_sac_ia.argtypes = [vp, vp, C.POINTER(SacParams), C.POINTER(SacResult)]
     L.ghicp_set_initial_transform.argtypes = [vp, dp]
+    L.ghicp_fpfh_extract_radius.argtypes = [C.c_int, fpp, C.c_int, ip, C.c_int, C.c_float, C.c_float, fpp, fpp, ip]
+    L.ghicp_prep_fpfh_radius.argtypes = [vp, C.c_float, C.c_float, fpp, C.POINTER(C.c_longlong)]
     _lib = L
     return L
 
@@ -232,6 +235,18 @@ class Prep:
         self.fpfh_stats = dict(candidates=cand.value, queries=q.value, candidates_per_query=cand.value / max(q.value, 1),
                                fallbacks=fb.value, cell=cell.value)
         self.fpfh_ms = dict(knn_normals=float(ms[0]), spfh_fpfh=float(ms[1]), total=float(ms[2]))
+        return self.fpfh_ms
+
+    def fpfh_radius(self, normal_radius, feature_radius):
+        """fpfh() with the radius estimator (ghicp_prep_fpfh_radius; see fpfh_extract_radius): normals over `normal_radius`,
+        histograms over `feature_radius`, at the keypoints, kept on the device where fpfh() keeps them.  Returns the stage
+        times {lists, normals, spfh_fpfh, total} in ms; fpfh_work then holds {normal_entries, feature_entries, spfh_points}."""
+        ms, work = np.zeros(4, np.float32), np.zeros(3, np.int64)
+        check(lib().ghicp_prep_fpfh_radius(self.h, normal_radius, feature_radius, ms.ctypes.data_as(C.POINTER(C.c_float)),
+                                           work.ctypes.data_as(C.POINTER(C.c_longlong))))
+        self.fpfh_radii = (float(normal_radius), float(feature_radius))
+        self.fpfh_work = dict(normal_entries=int(work[0]), feature_entries=int(work[1]), spfh_points=int(work[2]))
+        self.fpfh_ms = dict(lists=float(ms[0]), normals=float(ms[1]), spfh_fpfh=float(ms[2]), total=float(ms[3]))
         return self.fpfh_ms
 
     def get_fpfh(self):
@@ -399,6 +414,27 @@ def fpfh_extract(xyz, idx=None, k=20, device=0):
     normals, status = np.zeros((n, 3), np.float32), np.zeros(n, np.int32)
     check(lib().ghicp_fpfh_extract(device, xyz.ctypes.data_as(fpp), n, None if ia is None else _ip(ia), m, k,
                                    fpfh.ctypes.data_as(fpp), normals.ctypes.data_as(fpp), _ip(status)))
+    return fpfh, normals, status
+
+
+def fpfh_extract_radius(xyz, idx=None, normal_radius=None, feature_radius=None, device=0):
+    """CRegistration::compute_fpfh_feature (src/common_reg.cpp:373-389) on the GPU: PCL's NormalEstimation and FPFHEstimation
+    with radius searches (DESIGN.md §3.10, "Radius neighbourhoods").  Normals over every point within `normal_radius`,
+    histograms over every point within `feature_radius` (strict d2 < r*r in float32).  Returns (fpfh [len(idx) or n][33]
+    float32, normals [n][3] float32, status [n] int32: 1 = NaN normal, fewer than 3 points within the radius; 2 = normal not
+    needed by the requested histograms, NaN)."""
+    if normal_radius is None or feature_radius is None:
+        raise GhicpError(-1, "fpfh_extract_radius: normal_radius and feature_radius are required")
+    xyz = np.ascontiguousarray(xyz, dtype=np.float32).reshape(-1, 3)
+    n = len(xyz)
+    fpp = C.POINTER(C.c_float)
+    ia = None if idx is None else np.ascontiguousarray(idx, dtype=np.int32).reshape(-1)
+    m = n if ia is None else len(ia)
+    fpfh = np.zeros((m, 33), np.float32)
+    normals, status = np.zeros((n, 3), np.float32), np.zeros(n, np.int32)
+    check(lib().ghicp_fpfh_extract_radius(device, xyz.ctypes.data_as(fpp), n, None if ia is None else _ip(ia), m,
+                                          float(normal_radius), float(feature_radius), fpfh.ctypes.data_as(fpp),
+                                          normals.ctypes.data_as(fpp), _ip(status)))
     return fpfh, normals, status
 
 

@@ -1522,6 +1522,92 @@ int ghicp_prep_fpfh_stats(const ghicp_prep *h, long long *candidates, int *queri
   return GHICP_OK;
 }
 
+// ---- FPFH over radius neighbourhoods -------------------------------------------------------------------------------------
+// GHICP_FPFH_NB_MAX=<entries> (test hook) lowers the neighbour-list budget, forcing the GHICP_E_NOMEM path at any size
+static long long fpfh_nb_max() {
+  const char *s = getenv("GHICP_FPFH_NB_MAX");
+  return s ? atoll(s) : 0;
+}
+static bool radii_ok(float rn, float rf, const char *who) {
+  // the lists compare against r*r in float32: a radius whose square is 0 or infinite is refused with the others
+  const bool ok = std::isfinite(rn) && std::isfinite(rf) && rn > 0.f && rf > 0.f && rn * rn > 0.f && rf * rf > 0.f &&
+                  std::isfinite(rn * rn) && std::isfinite(rf * rf);
+  if (!ok) set_error(nullptr, std::string(who) + ": normal_radius and feature_radius must be positive and finite");
+  return ok;
+}
+static int fpfh_radius_status(cudaError_t e, const FpfhRadiusStats &s, const char *who) {
+  if (e == cudaSuccess) return GHICP_OK;
+  cudaGetLastError();
+  if (e == cudaErrorMemoryAllocation && s.needed > s.budget) {
+    set_error(nullptr, std::string(who) + ": the neighbour lists need at least " + std::to_string(s.needed) + " entries, the budget is " +
+                           std::to_string(s.budget) + " entries (16 bytes each)");
+    return GHICP_E_NOMEM;
+  }
+  set_error(nullptr, std::string(who) + ": " + cudaGetErrorString(e));
+  return e == cudaErrorMemoryAllocation ? GHICP_E_NOMEM : GHICP_E_CUDA;
+}
+
+int ghicp_fpfh_extract_radius(int device, const float *xyz, int n, const int *idx, int nidx, float normal_radius,
+                              float feature_radius, float *fpfh, float *normals, int *status) {
+  if (!xyz || n <= 0 || (idx && nidx < 0) || ((idx ? nidx : n) > 0 && !fpfh)) { set_error(nullptr, "fpfh_extract_radius: bad argument"); return GHICP_E_ARG; }
+  if (!radii_ok(normal_radius, feature_radius, "fpfh_extract_radius")) return GHICP_E_ARG;
+  if (!idx) nidx = n;
+  if (idx) for (int i = 0; i < nidx; ++i) if (idx[i] < 0 || idx[i] >= n) { set_error(nullptr, "fpfh_extract_radius: index out of range"); return GHICP_E_ARG; }
+  if (ghicp_device_count() <= 0) { set_error(nullptr, "fpfh_extract_radius: no CUDA device"); return GHICP_E_NODEV; }
+  if (cudaSetDevice(device) != cudaSuccess) return GHICP_E_CUDA;
+  float *d_xyz = nullptr, *d_fpfh = nullptr, *d_nrm = nullptr; int *d_idx = nullptr, *d_status = nullptr;
+  FpfhRadiusStats s;
+  cudaError_t e = cudaMallocAsync((void **)&d_xyz, 3 * (size_t)n * sizeof(float), 0);
+  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_fpfh, ((size_t)nidx * 33 + 1) * sizeof(float), 0);
+  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_nrm, 3 * (size_t)n * sizeof(float), 0);
+  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_status, (size_t)n * sizeof(int), 0);
+  if (e == cudaSuccess && idx) e = cudaMallocAsync((void **)&d_idx, ((size_t)nidx + 1) * sizeof(int), 0);
+  if (e == cudaSuccess) e = cudaMemcpy(d_xyz, xyz, 3 * (size_t)n * sizeof(float), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess && idx && nidx > 0) e = cudaMemcpy(d_idx, idx, (size_t)nidx * sizeof(int), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = prep_fpfh_radius(0, d_xyz, n, d_idx, nidx, normal_radius, feature_radius, fpfh_nb_max(), d_fpfh, d_nrm,
+                                             d_status, nullptr, nullptr, &s);
+  if (e == cudaSuccess && nidx > 0) e = cudaMemcpy(fpfh, d_fpfh, (size_t)nidx * 33 * sizeof(float), cudaMemcpyDeviceToHost);
+  if (e == cudaSuccess && normals) e = cudaMemcpy(normals, d_nrm, 3 * (size_t)n * sizeof(float), cudaMemcpyDeviceToHost);
+  if (e == cudaSuccess && status) e = cudaMemcpy(status, d_status, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost);
+  for (void *p : {(void *)d_xyz, (void *)d_fpfh, (void *)d_nrm, (void *)d_status, (void *)d_idx}) if (p) cudaFreeAsync(p, 0);
+  return fpfh_radius_status(e, s, "fpfh_extract_radius");
+}
+
+int ghicp_prep_fpfh_radius(ghicp_prep *h, float normal_radius, float feature_radius, float stage_ms[4], long long work[3]) {
+  if (!h || h->n_kp <= 0) { set_error(nullptr, "prep_fpfh_radius: bad argument or a cloud without keypoints"); return GHICP_E_ARG; }
+  if (!radii_ok(normal_radius, feature_radius, "prep_fpfh_radius")) return GHICP_E_ARG;
+  if (cudaSetDevice(h->device) != cudaSuccess) return GHICP_E_CUDA;
+  cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
+  float *d_nrm = nullptr, *d_out = nullptr;
+  FpfhRadiusStats s;
+  cudaError_t e = cudaSuccess;
+  for (auto &x : ev) if (e == cudaSuccess) e = cudaEventCreate(&x);
+  // into a fresh buffer: histograms a failed call leaves behind are never mistaken for results
+  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_out, ((size_t)h->n_kp * 33 + 1) * sizeof(float), 0);
+  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_nrm, 3 * (size_t)h->n_down * sizeof(float), 0);
+  if (e == cudaSuccess) e = cudaEventRecord(ev[0], 0);
+  if (e == cudaSuccess) e = prep_fpfh_radius(0, h->d_down, h->n_down, h->d_kp, h->n_kp, normal_radius, feature_radius, fpfh_nb_max(),
+                                             d_out, d_nrm, nullptr, ev[1], ev[2], &s);
+  if (e == cudaSuccess) e = cudaEventRecord(ev[3], 0);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(0);
+  float ms[4] = {0.f, 0.f, 0.f, 0.f};
+  if (e == cudaSuccess) {
+    cudaEventElapsedTime(&ms[0], ev[0], ev[1]); cudaEventElapsedTime(&ms[1], ev[1], ev[2]);
+    cudaEventElapsedTime(&ms[2], ev[2], ev[3]); cudaEventElapsedTime(&ms[3], ev[0], ev[3]);
+  }
+  for (auto &x : ev) if (x) cudaEventDestroy(x);
+  if (d_nrm) cudaFreeAsync(d_nrm, 0);
+  if (e != cudaSuccess) {
+    if (d_out) cudaFreeAsync(d_out, 0);
+    return fpfh_radius_status(e, s, "prep_fpfh_radius");
+  }
+  if (h->d_fpfh) cudaFreeAsync(h->d_fpfh, 0);
+  h->d_fpfh = d_out;
+  if (stage_ms) std::memcpy(stage_ms, ms, sizeof(ms));
+  if (work) { work[0] = s.nb_n; work[1] = s.nb_f; work[2] = s.spfh_points; }
+  return GHICP_OK;
+}
+
 // ---- SAC-IA coarse alignment -------------------------------------------------------------------------------------------
 static bool sac_params_ok(const ghicp_sac_params *p, const char *who) {
   const char *why = nullptr;

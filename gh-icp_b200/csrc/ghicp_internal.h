@@ -374,6 +374,19 @@ struct FpfhStats {
 cudaError_t prep_fpfh(cudaStream_t st, const float *d_xyz, int n, const int *d_idx, int nidx, int k, float cell_scale,
                       float *d_fpfh, float *d_normals, int *d_status, int *d_nb_idx, float *d_nb_d2, cudaEvent_t ev_mid,
                       FpfhStats *stats);
+// The same estimator over radius neighbourhoods (CRegistration::compute_fpfh_feature, src/common_reg.cpp:373-389), see
+// ghicp_prep.cu
+struct FpfhRadiusStats {
+  long long nb_n = 0, nb_f = 0;   // list entries at the normal / the feature radius
+  long long needed = 0;           // entries counted (both radii); > budget: the call returned cudaErrorMemoryAllocation
+  long long budget = 0;           // entry budget of the call
+  int spfh_points = 0;            // points whose SPFH was computed
+  int rings_n = 0, rings_f = 0;   // grid rings walked per query
+  float cell = 0.f;               // grid cell edge
+};
+cudaError_t prep_fpfh_radius(cudaStream_t st, const float *d_xyz, int n, const int *d_idx, int nidx, float rn, float rf,
+                             long long nb_max, float *d_fpfh, float *d_normals, int *d_status, cudaEvent_t ev_lists,
+                             cudaEvent_t ev_normals, FpfhRadiusStats *stats);
 
 // SAC-IA coarse alignment from FPFH histograms (ghicp_sac.cu, DESIGN.md §3.11) on device arrays: source points [ns][3] and
 // histograms [ns][33], target likewise; parameters already checked.  dbg (may be null): host arrays that receive the

@@ -63,6 +63,18 @@ cudaError_t exclusive_scan(const int *in, int *out, int n, cudaStream_t) {   // 
   out[n] = run;
   return cudaSuccess;
 }
+cudaError_t exclusive_scan64(const long long *in, long long *out, int n, cudaStream_t) {   // out[n] = total
+  long long run = 0;
+  for (int i = 0; i < n; ++i) { out[i] = run; run += in[i]; }
+  out[n] = run;
+  return cudaSuccess;
+}
+// every segment [off[r], off[r + 1]) of in sorted ascending into out (keys are distinct within a segment)
+cudaError_t segmented_sort(const pu64 *in, pu64 *out, long long total, int m, const long long *off, cudaStream_t) {
+  memcpy(out, in, sizeof(pu64) * (size_t)total);
+  for (int r = 0; r < m; ++r) std::sort(out + off[r], out + off[r + 1]);
+  return cudaSuccess;
+}
 #else
 // Workspaces come from the device's stream-ordered pool (the whole pre-processing runs on one stream): a cudaMalloc /
 // cudaFree pair per temporary costs more host time than all the kernels of a 1 M-point scan together, cudaFree being a
@@ -104,6 +116,15 @@ cudaError_t exclusive_scan(const int *in, int *out, int n, cudaStream_t st) {   
   if (tmp) cudaFreeAsync(tmp, st);
   return e;
 }
+cudaError_t exclusive_scan64(const long long *in, long long *out, int n, cudaStream_t st) {   // out[n] = total (in[n] readable)
+  void *tmp = nullptr; size_t tb = 0;
+  cudaError_t e = cub::DeviceScan::ExclusiveSum(nullptr, tb, in, out, n + 1, st);
+  if (e == cudaSuccess) e = cudaMallocAsync(&tmp, tb ? tb : 1, st);
+  if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(tmp, tb, in, out, n + 1, st);
+  if (tmp) cudaFreeAsync(tmp, st);
+  return e;
+}
+cudaError_t segmented_sort(const pu64 *in, pu64 *out, long long total, int m, const long long *off, cudaStream_t st);   // below
 #endif
 
 // ---- small device helpers ---------------------------------------------------------------------------------------------
@@ -987,11 +1008,31 @@ __global__ void k_knn(const KnnArgs a) {
   if (threadIdx.x == 0) { atomicAdd(a.cand, s_cand); atomicAdd(a.fallbacks, s_fb); }
 }
 
-// NormalEstimation::computePointNormal + flipNormalTowardsViewpoint (viewpoint 0): one thread per point
-__global__ void k_normals(const float *__restrict__ xyz, const int *__restrict__ nb_idx, int n, int k, float *__restrict__ nrm,
-                          int *__restrict__ status) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
+// Neighbour lists the estimator reads.  The normal, SPFH and FPFH arithmetic below is written once, over a list accessor:
+//   FixedLists  the k-NN lists, [n][k] (k_knn)
+//   CsrLists    the radius lists (k_rad_fill + segmented sort): row[point] -> 64-bit offsets into knn_key entries
+// list(i) gives the first entry of point i's list and its length; id / dist2 read entry e.
+struct FixedLists {
+  const int *idx; const float *d2; int k;
+  __device__ __forceinline__ size_t first(size_t i) const { return i * (size_t)k; }
+  __device__ __forceinline__ int count(size_t) const { return k; }
+  __device__ __forceinline__ int id(size_t e) const { return idx[e]; }
+  __device__ __forceinline__ float dist2(size_t e) const { return d2[e]; }
+};
+struct CsrLists {
+  const pu64 *key; const long long *off; const int *row;
+  __device__ __forceinline__ size_t first(size_t i) const { return (size_t)off[row[i]]; }
+  __device__ __forceinline__ int count(size_t i) const { const int r = row[i]; return (int)(off[r + 1] - off[r]); }
+  __device__ __forceinline__ int id(size_t e) const { return (int)(unsigned)key[e]; }
+  __device__ __forceinline__ float dist2(size_t e) const { return knn_key_d2(key[e]); }
+};
+
+// NormalEstimation::computePointNormal + flipNormalTowardsViewpoint (viewpoint 0) of point i over its list
+template <class L>
+__device__ __forceinline__ void est_normal(const float *__restrict__ xyz, int i, const L &l, float *__restrict__ nrm,
+                                           int *__restrict__ status) {
+  const int k = l.count((size_t)i);
+  const size_t b = l.first((size_t)i);
   const float qx = xyz[3 * (size_t)i], qy = xyz[3 * (size_t)i + 1], qz = xyz[3 * (size_t)i + 2];
   if (k < 3) {
     const float nan = __uint_as_float(0x7fc00000u);
@@ -1000,8 +1041,8 @@ __global__ void k_normals(const float *__restrict__ xyz, const int *__restrict__
     return;
   }
   double sd[3] = {0, 0, 0}, sdd[6] = {0, 0, 0, 0, 0, 0};
-  for (int j = 0; j < k; ++j) {   // k-NN order; the sums of k_pca
-    const size_t p = (size_t)nb_idx[(size_t)i * k + j];
+  for (int j = 0; j < k; ++j) {   // list order; the sums of k_pca
+    const size_t p = (size_t)l.id(b + j);
     const float ex = xyz[3 * p] - qx, ey = xyz[3 * p + 1] - qy, ez = xyz[3 * p + 2] - qz;
     const double a = ex, b = ey, c = ez;
     sd[0] += a; sd[1] += b; sd[2] += c;
@@ -1022,6 +1063,14 @@ __global__ void k_normals(const float *__restrict__ xyz, const int *__restrict__
   if (((-qx) * nx + (-qy) * ny) + (-qz) * nz < 0.f) { nx = -nx; ny = -ny; nz = -nz; }
   nrm[3 * (size_t)i] = nx; nrm[3 * (size_t)i + 1] = ny; nrm[3 * (size_t)i + 2] = nz;
   if (status) status[i] = 0;
+}
+
+// k-NN normals: one thread per point
+__global__ void k_normals(const float *__restrict__ xyz, const int *__restrict__ nb_idx, int n, int k, float *__restrict__ nrm,
+                          int *__restrict__ status) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  est_normal(xyz, i, FixedLists{nb_idx, nullptr, k}, nrm, status);
 }
 
 // points whose SPFH a requested histogram reads: the neighbours of every requested index
@@ -1047,11 +1096,12 @@ __device__ __forceinline__ int fpfh_bin(double x) {   // x = the feature mapped 
   return h < 0 ? 0 : (h > 10 ? 10 : h);
 }
 
-// computePointSPFHSignature: one thread per needed point
-__global__ void k_spfh(const float *__restrict__ xyz, const float *__restrict__ nrm, const int *__restrict__ nb_idx, int n, int k,
-                       const int *__restrict__ need, float *__restrict__ spfh) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n || (need && !need[i])) return;
+// computePointSPFHSignature of point i over its list (the increments are all equal: the bins do not depend on list order)
+template <class L>
+__device__ __forceinline__ void est_spfh(const float *__restrict__ xyz, const float *__restrict__ nrm, int i, const L &l,
+                                         float *__restrict__ spfh) {
+  const int k = l.count((size_t)i);
+  const size_t e0 = l.first((size_t)i);
   float hist[33];
   for (int b = 0; b < 33; ++b) hist[b] = 0.f;
   const float np[3] = {nrm[3 * (size_t)i], nrm[3 * (size_t)i + 1], nrm[3 * (size_t)i + 2]};
@@ -1060,7 +1110,7 @@ __global__ void k_spfh(const float *__restrict__ xyz, const float *__restrict__ 
     const float inv2pi = 1.0f / (2.0f * 3.14159265358979323846f);
     const float p[3] = {xyz[3 * (size_t)i], xyz[3 * (size_t)i + 1], xyz[3 * (size_t)i + 2]};
     for (int j = 0; j < k; ++j) {
-      const int qi = nb_idx[(size_t)i * k + j];
+      const int qi = l.id(e0 + j);
       if (qi == i) continue;
       const float nq[3] = {nrm[3 * (size_t)qi], nrm[3 * (size_t)qi + 1], nrm[3 * (size_t)qi + 2]};
       if (nq[0] != nq[0]) continue;
@@ -1092,21 +1142,28 @@ __global__ void k_spfh(const float *__restrict__ xyz, const float *__restrict__ 
   for (int b = 0; b < 33; ++b) spfh[(size_t)i * 33 + b] = hist[b];
 }
 
-// weightPointSPFHSignature: one thread per requested index
-__global__ void k_fpfh(const int *__restrict__ idx, int nidx, const int *__restrict__ nb_idx, const float *__restrict__ nb_d2, int k,
-                       const float *__restrict__ spfh, float *__restrict__ out) {
-  const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= nidx) return;
-  const size_t p = (size_t)(idx ? idx[t] : t);
+// k-NN SPFH: one thread per needed point
+__global__ void k_spfh(const float *__restrict__ xyz, const float *__restrict__ nrm, const int *__restrict__ nb_idx, int n, int k,
+                       const int *__restrict__ need, float *__restrict__ spfh) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n || (need && !need[i])) return;
+  est_spfh(xyz, nrm, i, FixedLists{nb_idx, nullptr, k}, spfh);
+}
+
+// weightPointSPFHSignature of point p over its list into out [33]: float per-bin sums and double per-block sums in list order
+template <class L>
+__device__ __forceinline__ void est_fpfh(size_t p, const L &l, const float *__restrict__ spfh, float *__restrict__ out) {
+  const int k = l.count(p);
+  const size_t e0 = l.first(p);
   float hist[33];
   double sum[3] = {0.0, 0.0, 0.0};
 #pragma unroll
   for (int b = 0; b < 33; ++b) hist[b] = 0.f;
   for (int j = 0; j < k; ++j) {
-    const float d2 = nb_d2[p * k + j];
+    const float d2 = l.dist2(e0 + j);
     if (d2 == 0.f) continue;                       // the point itself and its duplicates
     const float wgt = 1.0f / d2;
-    const float *sq = spfh + (size_t)nb_idx[p * k + j] * 33;
+    const float *sq = spfh + (size_t)l.id(e0 + j) * 33;
 #pragma unroll
     for (int b = 0; b < 33; ++b) {
       const float val = sq[b] * wgt;
@@ -1117,9 +1174,165 @@ __global__ void k_fpfh(const int *__restrict__ idx, int nidx, const int *__restr
 #pragma unroll
   for (int b = 0; b < 33; ++b) {
     const float h = sum[b / 11] != 0.0 ? hist[b] * (float)(100.0 / sum[b / 11]) : hist[b];
-    out[(size_t)t * 33 + b] = h;
+    out[b] = h;
   }
 }
+
+// k-NN FPFH: one thread per requested index
+__global__ void k_fpfh(const int *__restrict__ idx, int nidx, const int *__restrict__ nb_idx, const float *__restrict__ nb_d2, int k,
+                       const float *__restrict__ spfh, float *__restrict__ out) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= nidx) return;
+  est_fpfh((size_t)(idx ? idx[t] : t), FixedLists{nb_idx, nb_d2, k}, spfh, out + (size_t)t * 33);
+}
+
+// ---- radius neighbourhoods (DESIGN.md §3.10, "Radius neighbourhoods") ------------------------------------------------------
+// N_r(p) = every q with d2(p, q) < r2 (knn_d2, r2 = r*r in float32), ascending (d2, index).  A query walks the columns
+// (x, y) within `rings` cells of its own, each column's z-range cz - rings .. cz + rings being one run of the cell-sorted
+// points.  rings = ceil(r / cell + slack) covers the float32 rounding of cell_coord, so the lists are exact.
+struct RadWalk {
+  GridArgs g;
+  int rings; float r2;
+};
+
+// calls f(sorted position, d2) for every point of N_r(q) in walk order (not sorted)
+template <class F>
+__device__ __forceinline__ void rad_walk(const GridRegs &r, const RadWalk &w, float qx, float qy, float qz, F &&f) {
+  const int cx = cell_coord(qx, w.g.mnx, w.g.inv), cy = cell_coord(qy, w.g.mny, w.g.inv), cz = cell_coord(qz, w.g.mnz, w.g.inv);
+  const int R = w.rings, zlo = max(cz - R, 0), zhi = cz + R;
+  for (int x = max(cx - R, 0); x <= cx + R; ++x)
+    for (int y = max(cy - R, 0); y <= cy + R; ++y) {
+      const int s0 = r.cstart[lower_cell(r, cell_key(x, y, zlo))], s1 = r.cstart[lower_cell(r, cell_key(x, y, zhi) + 1)];
+      for (int s = s0; s < s1; ++s) {
+        const float d2 = knn_d2(qx, qy, qz, r.sorted[s]);
+        if (d2 < r.r2) f(s, d2);
+      }
+    }
+}
+
+// need[q] = 1 for every q in N_r(idx[t]) (the points whose SPFH the requested histograms read)
+__global__ void k_rad_mark(const RadWalk w, const int *__restrict__ idx, int nidx, int *__restrict__ need) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= nidx) return;
+  GridRegs r = grid_regs(w.g);   // per-thread registers, see k_pca
+  r.r2 = w.r2;
+  const float *q = w.g.xyz + 3 * (size_t)idx[t];
+  rad_walk(r, w, q[0], q[1], q[2], [&](int s, float) { need[r.order[s]] = 1; });
+}
+// need[q] = 1 for every entry of the lists of rows [0, m)
+__global__ void k_list_mark(const pu64 *__restrict__ key, const long long *__restrict__ off, int m, int *__restrict__ need) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= m) return;
+  for (long long e = off[t]; e < off[t + 1]; ++e) need[(unsigned)key[e]] = 1;
+}
+// rows in cell order (warps walk the same columns): flags[s] = need[order[s]] (every point when need == nullptr), flags[n] = 0
+__global__ void k_row_flags(const int *__restrict__ order, const int *__restrict__ need, int n, int *__restrict__ flags) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s > n) return;
+  flags[s] = s < n && (!need || need[order[s]]) ? 1 : 0;
+}
+// rows[pos[s]] = order[s], row_of[order[s]] = pos[s] for the flagged positions (row_of holds -1 elsewhere)
+__global__ void k_row_emit(const int *__restrict__ order, const int *__restrict__ flags, const int *__restrict__ pos, int n,
+                           int *__restrict__ rows, int *__restrict__ row_of) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= n || !flags[s]) return;
+  rows[pos[s]] = order[s]; row_of[order[s]] = pos[s];
+}
+// |N_r(rows[t])| (cnt[m] = 0 so that the scan yields the total)
+__global__ void k_rad_count(const RadWalk w, const int *__restrict__ rows, int m, long long *__restrict__ cnt) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t > m) return;
+  if (t == m) { cnt[t] = 0; return; }
+  GridRegs r = grid_regs(w.g);
+  r.r2 = w.r2;
+  const float *q = w.g.xyz + 3 * (size_t)rows[t];
+  int c = 0;
+  rad_walk(r, w, q[0], q[1], q[2], [&](int, float) { ++c; });
+  cnt[t] = c;
+}
+// the entries knn_key(d2, q) of row t at off[t] .. off[t + 1], in walk order (the segmented sort orders them)
+__global__ void k_rad_fill(const RadWalk w, const int *__restrict__ rows, int m, const long long *__restrict__ off,
+                           pu64 *__restrict__ key) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= m) return;
+  GridRegs r = grid_regs(w.g);
+  r.r2 = w.r2;
+  const float *q = w.g.xyz + 3 * (size_t)rows[t];
+  pu64 *out = key + off[t];
+  rad_walk(r, w, q[0], q[1], q[2], [&](int s, float d2) { *out++ = knn_key(d2, r.order[s]); });
+}
+// normals of every point: over its N_rn list where one was built (row_of >= 0), NaN with status 2 elsewhere
+__global__ void k_rad_normals(const float *__restrict__ xyz, int n, const CsrLists l, float *__restrict__ nrm, int *__restrict__ status) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  if (l.row[i] >= 0) { est_normal(xyz, i, l, nrm, status); return; }
+  const float nan = __uint_as_float(0x7fc00000u);
+  nrm[3 * (size_t)i] = nan; nrm[3 * (size_t)i + 1] = nan; nrm[3 * (size_t)i + 2] = nan;
+  if (status) status[i] = 2;
+}
+// SPFH of the rows of the N_rf lists (one thread per row, rows in cell order)
+__global__ void k_rad_spfh(const float *__restrict__ xyz, const float *__restrict__ nrm, const int *__restrict__ rows, int m,
+                           const CsrLists l, float *__restrict__ spfh) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= m) return;
+  est_spfh(xyz, nrm, rows[t], l, spfh);
+}
+__global__ void k_rad_fpfh(const int *__restrict__ idx, int nidx, const CsrLists l, const float *__restrict__ spfh, float *__restrict__ out) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= nidx) return;
+  est_fpfh((size_t)(idx ? idx[t] : t), l, spfh, out + (size_t)t * 33);
+}
+// the chunks of a segmented sort: first row of chunk c = first row whose offset is >= c * chunk (bounds[nchunks] = m)
+__global__ void k_chunk_bounds(const long long *__restrict__ off, int m, long long chunk, int nchunks, int *__restrict__ bounds) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c > nchunks) return;
+  if (c == nchunks) { bounds[c] = m; return; }
+  const long long want = c * chunk;
+  int lo = 0, hi = m;
+  while (lo < hi) { const int mid = (lo + hi) >> 1; if (off[mid] < want) lo = mid + 1; else hi = mid; }
+  bounds[c] = lo;
+}
+// int offsets of rows r0 .. r1 relative to off[r0]
+__global__ void k_rel_offsets(const long long *__restrict__ off, int r0, int r1, int *__restrict__ rel) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r0 + t > r1) return;
+  rel[t] = (int)(off[r0 + t] - off[r0]);
+}
+
+#if !defined(GHICP_EMU_HOST)
+// CUB's segmented sort counts items in int: the rows are sorted in chunks of at most 2^30 entries plus one row
+cudaError_t segmented_sort(const pu64 *in, pu64 *out, long long total, int m, const long long *off, cudaStream_t st) {
+  constexpr long long CHUNK = 1ll << 30;
+  const int nch = (int)((total + CHUNK - 1) / CHUNK);
+  if (nch == 0) return cudaSuccess;
+  cudaError_t err = cudaSuccess;
+  int *d_bounds = nullptr, *rel = nullptr; void *tmp = nullptr;
+  size_t tmp_bytes = 0;
+  std::vector<int> bounds(nch + 1);
+  PCK(pmalloc(&d_bounds, (size_t)nch + 1)); PCK(pmalloc(&rel, (size_t)m + 1));
+  GHICP_LAUNCH(k_chunk_bounds, blocks(nch + 1), PT, 0, st, off, m, CHUNK, nch, d_bounds);
+  PCK(pcopy(bounds.data(), d_bounds, sizeof(int) * (nch + 1), P_D2H, st)); PCK(psync(st));
+  for (int c = 0; c < nch; ++c) {
+    const int r0 = bounds[c], r1 = bounds[c + 1];
+    if (r1 <= r0) continue;
+    long long lo = 0, hi = 0;
+    PCK(pcopy(&lo, off + r0, sizeof(lo), P_D2H, st)); PCK(pcopy(&hi, off + r1, sizeof(hi), P_D2H, st)); PCK(psync(st));
+    if (hi - lo > INT_MAX) { err = cudaErrorInvalidValue; goto done; }   // one row of more than 2^31 - 2^30 entries
+    GHICP_LAUNCH(k_rel_offsets, blocks(r1 - r0 + 1), PT, 0, st, off, r0, r1, rel);
+    size_t need = 0;
+    PCK(cub::DeviceSegmentedSort::SortKeys(nullptr, need, in + lo, out + lo, (int)(hi - lo), r1 - r0, rel, rel + 1, st));
+    if (need > tmp_bytes) {
+      if (tmp) cudaFreeAsync(tmp, st);
+      tmp = nullptr; tmp_bytes = need;
+      PCK(cudaMallocAsync(&tmp, tmp_bytes ? tmp_bytes : 1, st));
+    }
+    PCK(cub::DeviceSegmentedSort::SortKeys(tmp, need, in + lo, out + lo, (int)(hi - lo), r1 - r0, rel, rel + 1, st));
+  }
+done:
+  pfree(d_bounds); pfree(rel); if (tmp) cudaFreeAsync(tmp, st);
+  return err;
+}
+#endif
 
 }  // namespace
 
@@ -1222,6 +1435,124 @@ cudaError_t prep_fpfh(cudaStream_t st, const float *d_xyz, int n, const int *d_i
 done:
   prep_point_grid_free(&pg);
   pfree(nb_idx); pfree(nb_d2); pfree(need); pfree(spfh); pfree(d_cand); pfree(d_fb);
+  return err;
+}
+
+namespace {
+// List rows in cell order: the points flagged in need (every point when need == nullptr).  rows [m], row_of [n] (-1: no row).
+cudaError_t make_rows(cudaStream_t st, const int *order, const int *need, int n, int *flags, int *pos, int **rows, int **row_of,
+                      int *m) {
+  cudaError_t err = cudaSuccess;
+  GHICP_LAUNCH(k_row_flags, blocks(n + 1), PT, 0, st, order, need, n, flags);
+  PCK(exclusive_scan(flags, pos, n, st));
+  PCK(pcopy(m, pos + n, sizeof(int), P_D2H, st)); PCK(psync(st));
+  PCK(pmalloc(rows, (size_t)*m)); PCK(pmalloc(row_of, (size_t)n));
+  PCK(cudaMemsetAsync(*row_of, 0xff, sizeof(int) * (size_t)n, st));
+  GHICP_LAUNCH(k_row_emit, blocks(n), PT, 0, st, order, flags, pos, n, *rows, *row_of);
+done:
+  return err;
+}
+// The sorted N_r lists of rows [m]: count, 64-bit offsets, budget check (cudaErrorMemoryAllocation before the entries are
+// allocated when *total > budget), fill, segmented sort.  off [m + 1] and key [*total] are the caller's to free.
+cudaError_t build_lists(cudaStream_t st, const RadWalk &w, const int *rows, int m, long long budget, long long **off, pu64 **key,
+                        long long *total) {
+  cudaError_t err = cudaSuccess;
+  long long *cnt = nullptr; pu64 *raw = nullptr;
+  *total = 0;
+  PCK(pmalloc(&cnt, (size_t)m + 1)); PCK(pmalloc(off, (size_t)m + 1));
+  GHICP_LAUNCH(k_rad_count, blocks(m + 1), PT, 0, st, w, rows, m, cnt);
+  PCK(exclusive_scan64(cnt, *off, m, st));
+  PCK(pcopy(total, *off + m, sizeof(long long), P_D2H, st)); PCK(psync(st));
+  if (*total > budget) { err = cudaErrorMemoryAllocation; goto done; }
+  PCK(pmalloc(&raw, (size_t)*total)); PCK(pmalloc(key, (size_t)*total));
+  if (m > 0) GHICP_LAUNCH(k_rad_fill, blocks(m), PT, 0, st, w, rows, m, *off, raw);
+  PCK(segmented_sort(raw, *key, *total, m, *off, st));
+done:
+  pfree(cnt); pfree(raw);
+  return err;
+}
+}  // namespace
+
+// FPFH over radius neighbourhoods (DESIGN.md §3.10, "Radius neighbourhoods"): normals over N_rn, SPFH and FPFH over N_rf, at
+// d_idx [nidx] (every point when d_idx == nullptr) of d_xyz [n][3].  Only what the requested histograms read is computed:
+// N_rf lists of the requested points' rf-neighbours, N_rn lists and normals of every point those SPFHs touch; d_normals [n][3]
+// and d_status [n] (may be null) hold NaN / 2 at the points whose normal was not needed.  nb_max > 0 caps the list entries
+// (both radii together) below the default budget (half the free device memory at 16 bytes per entry); over the budget the call
+// returns cudaErrorMemoryAllocation with stats->needed set, before any output is written.  ev_lists / ev_normals (may be null)
+// are recorded after the lists and after the normals.
+cudaError_t prep_fpfh_radius(cudaStream_t st, const float *d_xyz, int n, const int *d_idx, int nidx, float rn, float rf,
+                             long long nb_max, float *d_fpfh, float *d_normals, int *d_status, cudaEvent_t ev_lists,
+                             cudaEvent_t ev_normals, FpfhRadiusStats *stats) {
+  cudaError_t err = cudaSuccess;
+  GridArgs g{};
+  int *order = nullptr, *cstart = nullptr; pu64 *ucell = nullptr; float4 *sorted = nullptr;
+  int *need = nullptr, *flags = nullptr, *pos = nullptr, *rows_f = nullptr, *row_of_f = nullptr, *rows_n = nullptr, *row_of_n = nullptr;
+  long long *off_f = nullptr, *off_n = nullptr; pu64 *key_f = nullptr, *key_n = nullptr;
+  float *spfh = nullptr;
+  float mn[3], mx[3];
+  FpfhRadiusStats s;
+  int m_f = 0, m_n = 0;
+  if (stats) *stats = s;
+  if (n <= 0 || !(rn * rn > 0.f) || !(rf * rf > 0.f) || !std::isfinite(rn * rn) || !std::isfinite(rf * rf)) return cudaErrorInvalidValue;
+  {
+    long long budget;
+    {
+      size_t fr = 0, tot = 0;
+      PCK(cudaMemGetInfo(&fr, &tot));
+      budget = (long long)(fr / 2 / 16);
+      if (nb_max > 0 && nb_max < budget) budget = nb_max;
+    }
+    s.budget = budget;
+    // cell edge = the larger radius, widened by 2 % so that one ring covers the rounding of cell_coord (rings = 1), at least
+    // the extent / 2^20 (21-bit key fields; more rings then)
+    PCK(prep_bounds(st, d_xyz, n, mn, mx));
+    double emax = 0.0;
+    for (int a = 0; a < 3; ++a) emax = (double)mx[a] - (double)mn[a] > emax ? (double)mx[a] - (double)mn[a] : emax;
+    double cell = 1.02 * (double)(rn > rf ? rn : rf);
+    if (cell < emax / 1048576.0) cell = emax / 1048576.0;
+    PCK(build_grid(st, d_xyz, nullptr, n, (float)cell, &g, &order, &ucell, &cstart, &sorted));
+    int gmax = 0;
+    for (int a = 0; a < 3; ++a) { const int c = cell_coord_host(mx[a], a == 0 ? g.mnx : (a == 1 ? g.mny : g.mnz), g.inv); gmax = c > gmax ? c : gmax; }
+    // two cell coordinates of points closer than r differ by at most r / cell plus twice the float32 rounding of cell_coord
+    // (< (gmax + 1) 2^-23 each); 0.01 covers the rounding of d2 against r2
+    const double slack = 0.01 + (gmax + 2.0) / 1048576.0;
+    const RadWalk wf{g, (int)ceil((double)rf * (double)g.inv + slack), rf * rf};
+    const RadWalk wn{g, (int)ceil((double)rn * (double)g.inv + slack), rn * rn};
+    s.cell = (float)cell; s.rings_f = wf.rings; s.rings_n = wn.rings;
+    PCK(pmalloc(&flags, (size_t)n + 1)); PCK(pmalloc(&pos, (size_t)n + 1));
+    if (d_idx) {   // rows of the rf lists: the requested points' rf-neighbours
+      PCK(pmalloc(&need, (size_t)n));
+      PCK(pzero(need, sizeof(int) * (size_t)n, st));
+      if (nidx > 0) GHICP_LAUNCH(k_rad_mark, blocks(nidx), PT, 0, st, wf, d_idx, nidx, need);
+    }
+    PCK(make_rows(st, order, need, n, flags, pos, &rows_f, &row_of_f, &m_f));
+    err = build_lists(st, wf, rows_f, m_f, budget, &off_f, &key_f, &s.nb_f);
+    if (err != cudaSuccess) { s.needed = s.nb_f; goto done; }
+    if (d_idx) {   // rows of the rn lists: every point the SPFHs read
+      PCK(pzero(need, sizeof(int) * (size_t)n, st));
+      if (m_f > 0) GHICP_LAUNCH(k_list_mark, blocks(m_f), PT, 0, st, key_f, off_f, m_f, need);
+    }
+    PCK(make_rows(st, order, need, n, flags, pos, &rows_n, &row_of_n, &m_n));
+    err = build_lists(st, wn, rows_n, m_n, budget - s.nb_f, &off_n, &key_n, &s.nb_n);
+    if (err != cudaSuccess) { s.needed = s.nb_f + s.nb_n; goto done; }
+    s.needed = s.nb_f + s.nb_n; s.spfh_points = m_f;
+    if (ev_lists) PCK(cudaEventRecord(ev_lists, st));
+    GHICP_LAUNCH(k_rad_normals, blocks(n), PT, 0, st, d_xyz, n, CsrLists{key_n, off_n, row_of_n}, d_normals, d_status);
+    if (ev_normals) PCK(cudaEventRecord(ev_normals, st));
+    PCK(pmalloc(&spfh, (size_t)n * 33));
+    if (m_f > 0) GHICP_LAUNCH(k_rad_spfh, blocks(m_f), PT, 0, st, d_xyz, d_normals, rows_f, m_f, CsrLists{key_f, off_f, row_of_f}, spfh);
+    const int m_a = d_idx ? nidx : n;
+    if (m_a > 0) GHICP_LAUNCH(k_rad_fpfh, blocks(m_a), PT, 0, st, d_idx, m_a, CsrLists{key_f, off_f, row_of_f}, spfh, d_fpfh);
+    PCK(psync(st));
+#if !defined(GHICP_EMU_HOST)
+    PCK(cudaGetLastError());
+#endif
+  }
+done:
+  if (stats) *stats = s;
+  pfree(order); pfree(ucell); pfree(cstart); pfree(sorted);
+  pfree(need); pfree(flags); pfree(pos); pfree(rows_f); pfree(row_of_f); pfree(rows_n); pfree(row_of_n);
+  pfree(off_f); pfree(off_n); pfree(key_f); pfree(key_n); pfree(spfh);
   return err;
 }
 

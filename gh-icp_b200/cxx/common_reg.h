@@ -1,0 +1,84 @@
+// common_reg.h — host-side mirror of the reference's CRegistration (include/common_reg.h, src/common_reg.cpp) over
+// libghicp_b200.so, with the two members the library backs:
+//   compute_fpfh_feature (src/common_reg.cpp:373-389)  normals over search_radius, FPFH over 2 search_radius on every point
+//                                                      (PCL radius searches), on the GPU by ghicp_fpfh_extract_radius with
+//                                                      the canonical definition of DESIGN.md §3.10 ("Radius neighbourhoods")
+//   Coarsereg_FPFHSAC    (src/common_reg.cpp:393-423)  both clouds' histograms, then SAC-IA with correspondence randomness 15
+//                                                      and PCL's other defaults (1000 hypotheses of 3 samples, threshold 100
+//                                                      on squared distances), by ghicp_sac_ia (DESIGN.md §3.11, seed 0)
+// Differences, deliberate: clouds are ghicp::Cloud (cloud_io.h) and fpfhFeaturePtr the stand-in of ghicp_types.h; the
+// transform is Eigen::Matrix4f when Eigen is on the include path, else the column-major ghicp::Matrix4f; the SAC-IA is the
+// deterministic one of DESIGN.md §3.11 instead of PCL's std::rand()-driven one; no CPU path (without a CUDA device both
+// members throw).  The fitness of the last Coarsereg_FPFHSAC, which the reference prints, is kept (getFitnessScore).
+// Not provided: the PCL ICP wrappers (icp_reg, ptplicp_reg, gicp_reg), transformcloud / invTransform, calOverlap,
+// LLS_4DOF / SVD_6DOF and CSTRAN_4DOF / CSTRAN_7DOF.
+#pragma once
+#include <iostream>
+#include <stdexcept>
+#include <string>
+#include <vector>
+
+#include "../../include/ghicp_b200.h"
+#include "cloud_io.h"
+#include "ghicp_types.h"
+
+namespace ghicp {
+
+template <typename PointT = void>
+class CRegistration {
+ public:
+  // :373-389 — normals over search_radius, FPFH over 2 search_radius, every point of the cloud
+  void compute_fpfh_feature(const Cloud &input_cloud, fpfhFeaturePtr &cloud_fpfh, float search_radius) {
+    const int n = (int)input_cloud.size();
+    cloud_fpfh->points.resize(n);
+    if (n <= 0) return;
+    std::vector<float> hist((size_t)n * 33);
+    if (ghicp_fpfh_extract_radius(0, input_cloud.xyz.data(), n, nullptr, n, search_radius, 2.0f * search_radius, hist.data(),
+                                  nullptr, nullptr) < 0)
+      throw std::runtime_error(std::string("CRegistration::compute_fpfh_feature: ") + ghicp_last_error(nullptr));
+    for (int i = 0; i < n; ++i)
+      for (int b = 0; b < 33; ++b) cloud_fpfh->points[i].histogram[b] = hist[(size_t)i * 33 + b];
+  }
+
+  // :393-423 — SAC-IA of SourceCloud onto TargetCloud from their radius histograms; TransformedSource = the moved source
+  void Coarsereg_FPFHSAC(const Cloud &SourceCloud, const Cloud &TargetCloud, Cloud &TransformedSource,
+                         Matrix4f &transformationS2T, float search_radius) {
+#ifdef GHICP_HAVE_PCL
+    fpfhFeaturePtr source_fpfh(new pcl::PointCloud<pcl::FPFHSignature33>), target_fpfh(new pcl::PointCloud<pcl::FPFHSignature33>);
+#else
+    fpfhFeature source_store, target_store;
+    fpfhFeaturePtr source_fpfh = &source_store, target_fpfh = &target_store;
+#endif
+    compute_fpfh_feature(SourceCloud, source_fpfh, search_radius);
+    compute_fpfh_feature(TargetCloud, target_fpfh, search_radius);
+    const int ns = (int)SourceCloud.size(), nt = (int)TargetCloud.size();
+    std::vector<float> fs((size_t)ns * 33), ft((size_t)nt * 33);
+    for (int i = 0; i < ns; ++i) for (int b = 0; b < 33; ++b) fs[(size_t)i * 33 + b] = source_fpfh->points[i].histogram[b];
+    for (int i = 0; i < nt; ++i) for (int b = 0; b < 33; ++b) ft[(size_t)i * 33 + b] = target_fpfh->points[i].histogram[b];
+    ghicp_sac_params p{};
+    p.max_iterations = 1000; p.nr_samples = 3; p.k_correspondences = 15;   // setCorrespondenceRandomness(15), :412
+    p.min_sample_distance = 0.f; p.corr_dist_threshold = 100.f; p.seed = 0;
+    if (ghicp_sac_ia(0, SourceCloud.xyz.data(), fs.data(), ns, TargetCloud.xyz.data(), ft.data(), nt, &p, &result_) < 0)
+      throw std::runtime_error(std::string("CRegistration::Coarsereg_FPFHSAC: ") + ghicp_last_error(nullptr));
+    for (int i = 0; i < 16; ++i) transformationS2T.data()[i] = (float)result_.Rt[i];
+    // pcl::transformPointCloud with the float32 matrix, as PCL's align() moves the source
+    Cloud out;
+    const float *m = transformationS2T.data();
+    for (int i = 0; i < ns; ++i) {
+      const float x = SourceCloud.xyz[3 * (size_t)i], y = SourceCloud.xyz[3 * (size_t)i + 1], z = SourceCloud.xyz[3 * (size_t)i + 2];
+      float o[3];
+      for (int r = 0; r < 3; ++r) o[r] = ((m[r] * x + m[4 + r] * y) + m[8 + r] * z) + m[12 + r];
+      out.push(o[0], o[1], o[2]);
+    }
+    TransformedSource = out;
+    std::cout << "The fitness score of this registration is " << result_.fitness << std::endl;   // :419
+  }
+
+  double getFitnessScore() const { return result_.fitness; }
+  const ghicp_sac_result &sac_result() const { return result_; }
+
+ private:
+  ghicp_sac_result result_{};
+};
+
+}  // namespace ghicp

@@ -25,6 +25,7 @@ namespace ghicp {
 #ifdef GHICP_HAVE_EIGEN
 using MatrixX3d = Eigen::MatrixX3d;   // include/ghicp_reg.h:47
 using Matrix4d = Eigen::Matrix4d;     // include/ghicp_reg.h:132
+using Matrix4f = Eigen::Matrix4f;     // include/common_reg.h:120-124
 inline Matrix4d Identity4() { return Matrix4d::Identity(); }
 #else
 // column-major N x 3 doubles: the layout of Eigen::MatrixX3d::data()
@@ -64,6 +65,14 @@ inline Matrix4d Identity4() {
   for (int i = 0; i < 16; ++i) m.v[i] = (i % 5 == 0) ? 1.0 : 0.0;
   return m;
 }
+// column-major 4 x 4 floats: the layout of Eigen::Matrix4f::data()
+struct Matrix4f {
+  float v[16];
+  float &operator()(int i, int j) { return v[j * 4 + i]; }
+  float operator()(int i, int j) const { return v[j * 4 + i]; }
+  float *data() { return v; }
+  const float *data() const { return v; }
+};
 #endif
 
 // Binary descriptor with the reference's member names (include/stereo_binary_feature.h:25-58).

@@ -23,6 +23,13 @@ coarse stage.  `sac` overrides the capi.sac_ia arguments (iterations, samples, k
 default threshold is the keypoint NMS radius squared: keypoints are at least one NMS radius apart, so within that distance the
 nearest target keypoint of a moved source keypoint can only be its counterpart, and the error counts the keypoints that land
 on their counterparts.  On small keypoint sets of repetitive scenes 1000 hypotheses may not be enough (DESIGN.md §3.11).
+
+fpfh_radius = (normal_radius, feature_radius) computes the loop's and SAC-IA's histograms with the radius estimator
+(capi.Prep.fpfh_radius, DESIGN.md §3.10) instead of k-NN with k = fpfh_k: a support of several voxels, as PCL users and the
+reference's own coarse registration compute FPFH.  The default None keeps the k-NN estimator.
+
+coarsereg_fpfh_sac(source_xyz, target_xyz, search_radius) is CRegistration::Coarsereg_FPFHSAC (src/common_reg.cpp:393-423):
+radius FPFH on every point of both clouds, then SAC-IA with correspondence randomness 15.
 """
 import numpy as np
 
@@ -33,9 +40,13 @@ from .registration import Energyfunction, GHRegistration, Keypoints
 def register_clouds(target_xyz, source_xyz, resolution, neighborhood_radius, curvature_non_max_radius, corr_type=capi.CT_NN,
                     feature_type=capi.FT_NONE, features=None, weight_adjustment_ratio=1.1, weight_adjustment_step=0.1,
                     dof_type=6, estimated_IoU=0.5, max_iter=0, device=0, bsc_pattern=None, fpfh_k=20, initial_alignment=None,
-                    sac=None, **reg_kw):
+                    sac=None, fpfh_radius=None, **reg_kw):
     if initial_alignment not in (None, "fpfh_sac"):
         raise capi.GhicpError(-1, f"initial_alignment must be None or 'fpfh_sac', not {initial_alignment!r}")
+    if fpfh_radius is not None:
+        fpfh_radius = tuple(float(r) for r in fpfh_radius)
+        if len(fpfh_radius) != 2:
+            raise capi.GhicpError(-1, "fpfh_radius must be a (normal_radius, feature_radius) pair")
     sac_kw = dict(threshold=float(curvature_non_max_radius) ** 2)
     sac_kw.update(sac or {})
     T = np.ascontiguousarray(target_xyz, dtype=np.float32)
@@ -52,7 +63,11 @@ def register_clouds(target_xyz, source_xyz, resolution, neighborhood_radius, cur
                 if pr.n_kp == 0:
                     raise capi.GhicpError(-1, f"no keypoints in the {name} cloud: check the radii")
             if feature_type == capi.FT_FPFH or initial_alignment == "fpfh_sac":          # :120-127
-                pt.fpfh(fpfh_k); ps.fpfh(fpfh_k)
+                for pr in (pt, ps):
+                    if fpfh_radius is None:
+                        pr.fpfh(fpfh_k)
+                    else:
+                        pr.fpfh_radius(*fpfh_radius)
             Rt0, sac_info = None, None
             if initial_alignment == "fpfh_sac":
                 Rt0, sac_info = ps.sac_ia(pt, **sac_kw)
@@ -90,8 +105,12 @@ def register_clouds(target_xyz, source_xyz, resolution, neighborhood_radius, cur
                          weight_adjustment_step, dof_type, estimated_IoU, max_iter=max_iter, device=device, **reg_kw)
     sac_info = None
     if initial_alignment == "fpfh_sac":
-        fs, _, _ = capi.fpfh_extract(down["S"], kp_idx["S"], fpfh_k, device=device)
-        ft, _, _ = capi.fpfh_extract(down["T"], kp_idx["T"], fpfh_k, device=device)
+        if fpfh_radius is None:
+            fs, _, _ = capi.fpfh_extract(down["S"], kp_idx["S"], fpfh_k, device=device)
+            ft, _, _ = capi.fpfh_extract(down["T"], kp_idx["T"], fpfh_k, device=device)
+        else:
+            fs, _, _ = capi.fpfh_extract_radius(down["S"], kp_idx["S"], *fpfh_radius, device=device)
+            ft, _, _ = capi.fpfh_extract_radius(down["T"], kp_idx["T"], *fpfh_radius, device=device)
         Rt0, sac_info = capi.sac_ia(down["S"][kp_idx["S"]], fs, down["T"][kp_idx["T"]], ft, device=device, **sac_kw)
         reg.set_initial_transform(Rt0)
         sac_info = dict(sac_info, Rt=Rt0)
@@ -101,6 +120,27 @@ def register_clouds(target_xyz, source_xyz, resolution, neighborhood_radius, cur
     if sac_info is not None:
         info["sac"] = sac_info
     reg.close()
+    return Rt, info
+
+
+def coarsereg_fpfh_sac(source_xyz, target_xyz, search_radius, sac=None, device=0):
+    """CRegistration::Coarsereg_FPFHSAC (src/common_reg.cpp:393-423) on the GPU: normals over `search_radius` and FPFH over
+    2 * search_radius on every point of both clouds (compute_fpfh_feature, :373-389; capi.fpfh_extract_radius), then SAC-IA
+    with correspondence randomness 15 and PCL's other defaults: 1000 hypotheses of 3 samples, threshold 100 on squared
+    distances, no minimum sample distance, seed 0 (capi.sac_ia; `sac` overrides these).  Returns (Rt 4x4 mapping the source
+    onto the target, info: the sac_ia result with its fitness, plus the histograms' stage times in ms)."""
+    import time
+    S = np.ascontiguousarray(source_xyz, dtype=np.float32).reshape(-1, 3)
+    T = np.ascontiguousarray(target_xyz, dtype=np.float32).reshape(-1, 3)
+    rn, rf = float(np.float32(search_radius)), float(np.float32(2.0 * np.float32(search_radius)))
+    t0 = time.perf_counter()
+    fs, _, _ = capi.fpfh_extract_radius(S, None, rn, rf, device=device)
+    ft, _, _ = capi.fpfh_extract_radius(T, None, rn, rf, device=device)
+    t1 = time.perf_counter()
+    kw = dict(iterations=1000, samples=3, k=15, min_sample_distance=0.0, threshold=100.0, seed=0)
+    kw.update(sac or {})
+    Rt, info = capi.sac_ia(S, fs, T, ft, device=device, **kw)
+    info = dict(info, fpfh_ms=1e3 * (t1 - t0), normal_radius=rn, feature_radius=rf)
     return Rt, info
 
 

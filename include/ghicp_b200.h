@@ -267,6 +267,21 @@ int ghicp_prep_get_fpfh(const ghicp_prep *h, float *fpfh);
 /* Work of the last ghicp_prep_fpfh: k-NN candidates examined (all queries together), queries, queries that fell back to
  * the exhaustive scan, grid cell edge.  Any output may be NULL. */
 int ghicp_prep_fpfh_stats(const ghicp_prep *h, long long *candidates, int *queries, int *fallbacks, float *cell);
+/* The same estimator over radius neighbourhoods, as CRegistration::compute_fpfh_feature (src/common_reg.cpp:373-389, PCL
+ * setRadiusSearch) computes it (DESIGN.md §3.10, "Radius neighbourhoods"): N_r(p) = every point q with d2(p, q) < r*r (float32,
+ * the query and its duplicates included) in ascending (d2, index) order; normals over N_normal_radius (NaN, status 1, with
+ * fewer than 3 points), SPFH and FPFH over N_feature_radius.  Arguments and outputs as ghicp_fpfh_extract; with idx given,
+ * only what those histograms read is computed and the other normals are NaN with status 2.  Radii must be positive and
+ * finite (GHICP_E_ARG).  The neighbour lists live in device memory: when they would exceed the budget (half the free device
+ * memory at 16 bytes per entry) the call returns GHICP_E_NOMEM, with the entry count in the message, before writing any
+ * output. */
+int ghicp_fpfh_extract_radius(int device, const float *xyz, int n, const int *idx, int nidx, float normal_radius,
+                              float feature_radius, float *fpfh, float *normals, int *status);
+/* ghicp_prep_fpfh with the radius estimator: the keypoint histograms of the down-sampled cloud, stored where ghicp_prep_fpfh
+ * stores them (ghicp_set_from_prep, ghicp_prep_get_fpfh and ghicp_prep_sac_ia read them unchanged).  stage_ms [4] = {lists,
+ * normals, SPFH + FPFH, total}; work [3] = {normal-radius list entries, feature-radius list entries, SPFH points}; both may
+ * be NULL. */
+int ghicp_prep_fpfh_radius(ghicp_prep *h, float normal_radius, float feature_radius, float stage_ms[4], long long work[3]);
 
 /* ---- SAC-IA coarse alignment on the GPU -------------------------------------------------------------------------------
  * FPFHfeature::fpfhalign (include/fpfh.hpp:117-133: PCL SampleConsensusInitialAlignment, correspondence randomness 6) and
