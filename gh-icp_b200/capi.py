@@ -76,7 +76,7 @@ EXPORTS = ["ghicp_abi_version", "ghicp_device_count", "ghicp_last_error", "ghicp
            "ghicp_prep_run", "ghicp_prep_info", "ghicp_prep_get", "ghicp_prep_destroy", "ghicp_set_from_prep",
            "ghicp_host_alloc", "ghicp_host_free", "ghicp_fpfh_extract", "ghicp_prep_fpfh", "ghicp_prep_get_fpfh",
            "ghicp_prep_fpfh_stats", "ghicp_sac_ia", "ghicp_prep_sac_ia", "ghicp_set_initial_transform",
-           "ghicp_fpfh_extract_radius", "ghicp_prep_fpfh_radius"]
+           "ghicp_fpfh_extract_radius", "ghicp_prep_fpfh_radius", "ghicp_cloud_overlap", "ghicp_prep_overlap"]
 
 
 def lib():
@@ -136,6 +136,9 @@ def lib():
     L.ghicp_set_initial_transform.argtypes = [vp, dp]
     L.ghicp_fpfh_extract_radius.argtypes = [C.c_int, fpp, C.c_int, ip, C.c_int, C.c_float, C.c_float, fpp, fpp, ip]
     L.ghicp_prep_fpfh_radius.argtypes = [vp, C.c_float, C.c_float, fpp, C.POINTER(C.c_longlong)]
+    L.ghicp_cloud_overlap.argtypes = [C.c_int, fpp, C.c_int, fpp, C.c_int, dp, C.c_float, C.c_double, C.c_int,
+                                      C.POINTER(OverlapResult), fpp]
+    L.ghicp_prep_overlap.argtypes = [vp, vp, dp, C.c_float, C.c_double, C.c_int, C.POINTER(OverlapResult)]
     _lib = L
     return L
 
@@ -166,6 +169,27 @@ def _sac_out(r):
     return Rt, dict(error=r.error, fitness=r.fitness, inliers=r.inliers, best_hypothesis=r.best_hypothesis,
                     invalid_hypotheses=r.invalid_hypotheses,
                     stage_ms=dict(sample_knn=ms[0], estimate=ms[1], score=ms[2], pick=ms[3], total=float(sum(ms))))
+
+
+class OverlapResult(C.Structure):
+    """ghicp_overlap_result (include/ghicp_b200.h): overlap and fitness on the dense clouds, DESIGN.md §3.12."""
+    _fields_ = [("n", C.c_longlong), ("overlap", C.c_longlong), ("n_fit", C.c_longlong), ("cells_visited", C.c_longlong),
+                ("candidates", C.c_longlong), ("ratio", C.c_float), ("overlap_rmse", C.c_double), ("fitness", C.c_double),
+                ("stage_ms", C.c_float * 3)]
+
+
+def _overlap_rt(Rt):
+    """4x4 row-major numpy transform -> the column-major double[16] of the ABI (None: the identity, passed as NULL)."""
+    if Rt is None:
+        return None, None
+    m = np.ascontiguousarray(np.asarray(Rt, dtype=np.float64).reshape(4, 4).T).reshape(16)
+    return m, _dp(m)
+
+
+def _overlap_out(r):
+    ms = list(r.stage_ms)
+    return dict(n=r.n, overlap=r.overlap, ratio=r.ratio, overlap_rmse=r.overlap_rmse, n_fit=r.n_fit, fitness=r.fitness,
+                cells_visited=r.cells_visited, candidates=r.candidates, stage_ms=dict(grid=ms[0], queries=ms[1], total=ms[2]))
 
 
 class PrepParams(C.Structure):
@@ -261,6 +285,17 @@ class Prep:
         check(lib().ghicp_prep_sac_ia(self.h, target.h, C.byref(_sac_params(iterations, samples, k, min_sample_distance, threshold,
                                                                              seed)), C.byref(r)))
         return _sac_out(r)
+
+    def overlap(self, target, Rt=None, thre_dis=None, max_range=float("inf"), fitness=True):
+        """cloud_overlap of this down-sampled cloud, moved by Rt, against `target`'s, device to device (ghicp_prep_overlap).
+        `target` keeps its grid for later calls (its stage_ms["grid"] is then 0)."""
+        if thre_dis is None:
+            raise GhicpError(-1, "overlap: thre_dis is required")
+        keep, rp = _overlap_rt(Rt)
+        r = OverlapResult()
+        check(lib().ghicp_prep_overlap(self.h, target.h, rp, float(thre_dis), float(max_range), int(bool(fitness)), C.byref(r)))
+        del keep
+        return _overlap_out(r)
 
     def close(self):
         if getattr(self, "h", None):
@@ -457,6 +492,29 @@ def sac_ia(src_xyz, src_fpfh, tgt_xyz, tgt_fpfh, iterations=1000, samples=3, k=6
                              Ft.ctypes.data_as(fpp), len(Q), C.byref(_sac_params(iterations, samples, k, min_sample_distance,
                                                                                 threshold, seed)), C.byref(r)))
     return _sac_out(r)
+
+
+def cloud_overlap(A, B, Rt=None, thre_dis=None, max_range=float("inf"), fitness=True, return_d2=False, device=0):
+    """Overlap and fitness of cloud A moved by Rt (4x4, None = identity) against cloud B on the GPU, DESIGN.md §3.12:
+    overlap = points of A with a B point at d2 < thre_dis^2 (CRegistration::calOverlap, src/common_reg.cpp:294-317), ratio =
+    (0.01 + overlap) / n, overlap_rmse over those points; fitness = mean d2 over the points with d2 <= max_range (PCL's
+    getFitnessScore; max_range bounds SQUARED distances), DBL_MAX when there are none.  fitness=False is the overlap-only mode
+    (n_fit 0, fitness and overlap_rmse NaN).  Returns a dict (+ "d2" [n] float32 with return_d2, fitness mode only)."""
+    if thre_dis is None:
+        raise GhicpError(-1, "cloud_overlap: thre_dis is required")
+    fpp = C.POINTER(C.c_float)
+    A = np.ascontiguousarray(A, dtype=np.float32).reshape(-1, 3)
+    B = np.ascontiguousarray(B, dtype=np.float32).reshape(-1, 3)
+    keep, rp = _overlap_rt(Rt)
+    d2 = np.zeros(len(A), np.float32) if return_d2 else None
+    r = OverlapResult()
+    check(lib().ghicp_cloud_overlap(device, A.ctypes.data_as(fpp), len(A), B.ctypes.data_as(fpp), len(B), rp, float(thre_dis),
+                                    float(max_range), int(bool(fitness)), C.byref(r), None if d2 is None else d2.ctypes.data_as(fpp)))
+    del keep
+    out = _overlap_out(r)
+    if d2 is not None:
+        out["d2"] = d2
+    return out
 
 
 def rigid_fit_ex(S, T, solver=SOLVER_SVD, normals=None, weights=None, device=0):

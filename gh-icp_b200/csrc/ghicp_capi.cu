@@ -17,8 +17,9 @@
 #if defined(GHICP_EMU_HOST)
 // The CPU emulation of the whole library (tests/harness/emu_library.cpp) compiles the product's .cu files as ONE translation
 // unit and lists the kernel files it includes; the SAC-IA kernels join it here, next to the entry points that call them.
-// nvcc builds ghicp_sac.cu as a translation unit of its own (Makefile SRCS).
+// nvcc builds ghicp_sac.cu and ghicp_overlap.cu as translation units of their own (Makefile SRCS).
 #include "ghicp_sac.cu"
+#include "ghicp_overlap.cu"
 #endif
 
 namespace ghicp_b200 {
@@ -1285,6 +1286,8 @@ struct ghicp_prep {
   float bbox_min[3] = {0, 0, 0}, bbox_max[3] = {0, 0, 0};
   float stage_ms[5] = {0, 0, 0, 0, 0};
   FpfhStats fpfh_stats;
+  OverlapTarget *ov_target = nullptr;   // the down-sampled cloud's grid as an overlap target, after ghicp_prep_overlap
+  std::mutex ov_mu;                     // guards ov_target: concurrent first calls on one target build it once
 };
 
 int ghicp_prep_destroy(ghicp_prep *h) {
@@ -1295,6 +1298,7 @@ int ghicp_prep_destroy(ghicp_prep *h) {
   if (h->d_kp_xyz) cudaFreeAsync(h->d_kp_xyz, 0);
   if (h->d_bits) cudaFreeAsync(h->d_bits, 0);
   if (h->d_fpfh) cudaFreeAsync(h->d_fpfh, 0);
+  overlap_target_free(h->ov_target);
   delete h;
   return GHICP_OK;
 }
@@ -1667,6 +1671,109 @@ int ghicp_prep_sac_ia(const ghicp_prep *src, const ghicp_prep *tgt, const ghicp_
   if (d_p) cudaFreeAsync(d_p, 0);
   if (d_q) cudaFreeAsync(d_q, 0);
   return sac_status(e, "prep_sac_ia");
+}
+
+// ---- overlap and fitness on the dense clouds ---------------------------------------------------------------------------
+static bool overlap_args_ok(float thre_dis, double max_range, const char *who) {
+  // thre_dis * thre_dis is compared in float32: a radius whose square is 0 or infinite is refused with the others
+  const bool ok = std::isfinite(thre_dis) && thre_dis > 0.f && thre_dis * thre_dis > 0.f && std::isfinite(thre_dis * thre_dis) &&
+                  max_range >= 0.0;   // false for NaN; +inf allowed (PCL's default)
+  if (!ok) set_error(nullptr, std::string(who) + ": thre_dis must be positive and finite, max_range >= 0 (+inf allowed)");
+  return ok;
+}
+static bool overlap_rt_ok(const double *Rt, const char *who) {
+  if (Rt)
+    for (int i = 0; i < 16; ++i)
+      if (!std::isfinite(Rt[i])) { set_error(nullptr, std::string(who) + ": non-finite transform"); return false; }
+  return true;
+}
+static int overlap_status(cudaError_t e, const char *who) {
+  if (e == cudaSuccess) return GHICP_OK;
+  set_error(nullptr, std::string(who) + ": " + cudaGetErrorString(e));
+  cudaGetLastError();
+  return e == cudaErrorMemoryAllocation ? GHICP_E_NOMEM : GHICP_E_CUDA;
+}
+
+int ghicp_cloud_overlap(int device, const float *a_xyz, int n_a, const float *b_xyz, int n_b, const double Rt[16],
+                        float thre_dis, double max_range, int want_fitness, ghicp_overlap_result *out, float *d2) {
+  if (!a_xyz || !b_xyz || !out || n_a <= 0 || n_b <= 0 || (d2 && !want_fitness)) {
+    set_error(nullptr, "cloud_overlap: bad argument (null array, empty cloud, or d2 without want_fitness)");
+    return GHICP_E_ARG;
+  }
+  if (!overlap_args_ok(thre_dis, max_range, "cloud_overlap") || !overlap_rt_ok(Rt, "cloud_overlap")) return GHICP_E_ARG;
+  // B's non-finite points (the NaN returns of an organised scan) are left out of the grid, as PCL's KdTreeFLANN leaves them
+  // out of its tree; they can be no one's nearest point
+  std::vector<float> b_fin;
+  long long nb_fin = n_b;
+  {
+    size_t j = 0;
+    for (; j < (size_t)n_b; ++j)
+      if (!(std::isfinite(b_xyz[3 * j]) && std::isfinite(b_xyz[3 * j + 1]) && std::isfinite(b_xyz[3 * j + 2]))) break;
+    if (j < (size_t)n_b) {
+      b_fin.reserve(3 * (size_t)n_b);
+      for (size_t i = 0; i < (size_t)n_b; ++i)
+        if (std::isfinite(b_xyz[3 * i]) && std::isfinite(b_xyz[3 * i + 1]) && std::isfinite(b_xyz[3 * i + 2]))
+          b_fin.insert(b_fin.end(), b_xyz + 3 * i, b_xyz + 3 * i + 3);
+      nb_fin = (long long)(b_fin.size() / 3);
+      b_xyz = b_fin.data();
+    }
+  }
+  if (nb_fin <= 0) { set_error(nullptr, "cloud_overlap: cloud B has no finite point"); return GHICP_E_ARG; }
+  if (ghicp_device_count() <= 0) { set_error(nullptr, "cloud_overlap: no CUDA device"); return GHICP_E_NODEV; }
+  if (cudaSetDevice(device) != cudaSuccess) return GHICP_E_CUDA;
+  cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
+  float *d_a = nullptr, *d_b = nullptr;
+  OverlapTarget *t = nullptr;
+  ghicp_overlap_result r{};
+  cudaError_t e = cudaSuccess;
+  for (auto &x : ev) if (e == cudaSuccess) e = cudaEventCreate(&x);
+  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_a, 3 * (size_t)n_a * sizeof(float), 0);
+  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_b, 3 * (size_t)nb_fin * sizeof(float), 0);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(d_a, a_xyz, 3 * (size_t)n_a * sizeof(float), cudaMemcpyHostToDevice, 0);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(d_b, b_xyz, 3 * (size_t)nb_fin * sizeof(float), cudaMemcpyHostToDevice, 0);
+  if (e == cudaSuccess) e = cudaEventRecord(ev[0], 0);
+  if (e == cudaSuccess) e = overlap_target_build(d_b, (int)nb_fin, &t);
+  if (e == cudaSuccess) e = overlap_run(d_a, n_a, t, Rt, thre_dis, max_range, want_fitness, ev[1], &r, d2);
+  if (e == cudaSuccess) e = cudaEventRecord(ev[2], 0);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(0);
+  if (e == cudaSuccess) {
+    cudaEventElapsedTime(&r.stage_ms[0], ev[0], ev[1]); cudaEventElapsedTime(&r.stage_ms[1], ev[1], ev[2]);
+    cudaEventElapsedTime(&r.stage_ms[2], ev[0], ev[2]);
+  }
+  overlap_target_free(t);
+  for (float *x : {d_a, d_b}) if (x) cudaFreeAsync(x, 0);
+  for (auto &x : ev) if (x) cudaEventDestroy(x);
+  if (e == cudaSuccess) *out = r;
+  return overlap_status(e, "cloud_overlap");
+}
+
+int ghicp_prep_overlap(const ghicp_prep *a, const ghicp_prep *b, const double Rt[16], float thre_dis, double max_range,
+                       int want_fitness, ghicp_overlap_result *out) {
+  if (!a || !b || !out || a->n_down <= 0 || b->n_down <= 0) { set_error(nullptr, "prep_overlap: bad argument or an empty cloud"); return GHICP_E_ARG; }
+  if (a->device != b->device) { set_error(nullptr, "prep_overlap: the two pipeline results live on different devices"); return GHICP_E_ARG; }
+  if (!overlap_args_ok(thre_dis, max_range, "prep_overlap") || !overlap_rt_ok(Rt, "prep_overlap")) return GHICP_E_ARG;
+  if (cudaSetDevice(a->device) != cudaSuccess) return GHICP_E_CUDA;
+  ghicp_prep *tb = const_cast<ghicp_prep *>(b);   // the grid is a cache of the target's down-sampled cloud, not its state
+  cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
+  ghicp_overlap_result r{};
+  cudaError_t e = cudaSuccess;
+  for (auto &x : ev) if (e == cudaSuccess) e = cudaEventCreate(&x);
+  if (e == cudaSuccess) e = cudaEventRecord(ev[0], 0);
+  std::unique_lock<std::mutex> lk(tb->ov_mu);   // held while the grid is read: a concurrent first call waits for the build
+  const bool cached = tb->ov_target != nullptr;
+  if (e == cudaSuccess && !cached) e = overlap_target_build(tb->d_down, tb->n_down, &tb->ov_target);
+  if (e == cudaSuccess) e = overlap_run(a->d_down, a->n_down, tb->ov_target, Rt, thre_dis, max_range, want_fitness, ev[1], &r, nullptr);
+  if (e == cudaSuccess) e = cudaEventRecord(ev[2], 0);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(0);
+  if (e == cudaSuccess) {
+    if (!cached) cudaEventElapsedTime(&r.stage_ms[0], ev[0], ev[1]);
+    cudaEventElapsedTime(&r.stage_ms[1], ev[1], ev[2]);
+    cudaEventElapsedTime(&r.stage_ms[2], ev[0], ev[2]);
+    *out = r;
+  }
+  lk.unlock();
+  for (auto &x : ev) if (x) cudaEventDestroy(x);
+  return overlap_status(e, "prep_overlap");
 }
 
 int ghicp_set_initial_transform(ghicp_ctx *ctx, const double Rt[16]) {

@@ -78,5 +78,7 @@ struct PointGrid {
 // cell edge = the k-NN rule times cell_scale (if > 0), at least min_cell, at least the extent / 2^20 (21-bit key fields)
 cudaError_t prep_point_grid(cudaStream_t st, const float *d_xyz, int n, int ke, float cell_scale, double min_cell, PointGrid *out);
 void prep_point_grid_free(PointGrid *g);
+// stable ascending sort of (keys, vals) pairs in place, on the stream (the grid builder's radix sort)
+cudaError_t prep_sort_pairs(cudaStream_t st, pu64 *keys, int *vals, int n);
 
 }  // namespace ghicp_b200

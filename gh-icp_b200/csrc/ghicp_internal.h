@@ -403,6 +403,15 @@ cudaError_t sac_run(const float *d_P, const float *d_Fs, int ns, const float *d_
                     const ghicp_sac_params *p, ghicp_sac_result *out, SacDebug *dbg);
 cudaError_t sac_points_from_soa(const double *d_soa, int n, float *d_xyz);   // [3][n] doubles -> [n][3] floats
 
+// Overlap and fitness on the dense clouds (ghicp_overlap.cu, DESIGN.md §3.12).  OverlapTarget = B's grid, independent of the
+// threshold and reusable across calls.  overlap_run fills every field of out but stage_ms; h_d2_out (host, may be null)
+// receives the per-point d2.  ev_queries (may be null) is recorded after the workspaces are allocated.
+struct OverlapTarget;
+cudaError_t overlap_target_build(const float *d_b, int n_b, OverlapTarget **out);
+void overlap_target_free(OverlapTarget *t);
+cudaError_t overlap_run(const float *d_a, int n_a, const OverlapTarget *t, const double *Rt, float thre_dis, double max_range,
+                        int want_fitness, cudaEvent_t ev_queries, ghicp_overlap_result *out, float *h_d2_out);
+
 // glue of the device-resident pipeline (ghicp_prep_run)
 cudaError_t prep_gather_points(cudaStream_t st, const float *d_xyz, const int *d_idx, int m, float *d_out);
 cudaError_t prep_kp_coords(cudaStream_t st, const float *d_xyz, const int *d_kp, int nkp, double *d_soa);

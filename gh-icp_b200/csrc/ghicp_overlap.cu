@@ -1,0 +1,308 @@
+// ghicp_overlap.cu — overlap and fitness of a registration on the dense clouds (DESIGN.md §3.12): the reference's
+// CRegistration::calOverlap (src/common_reg.cpp:294-317, the share of cloud A with a cloud-B point within thre_dis) and PCL's
+// getFitnessScore (mean squared nearest-neighbour distance within max_range), for every point of A moved by a transform.
+//   target grid   B's cell-sorted grid (prep_point_grid, the k-NN cell rule with 8 points per cell): independent of the
+//                 threshold, so one grid serves every call on the same target (ghicp_prep_overlap keeps it)
+//   k_ov_keys     (fitness mode) the moved points' clamped B-cell keys, radix-sorted into the query order
+//   k_ov_query    the hot path: one exact nearest-neighbour query per point of A, a ring walk over B's grid like SAC-IA's
+//                 sac_nn_d2, but every column is culled by a lower bound on its distance (cell extents clipped to B's box)
+//                 and the walk stops once a true lower bound on every unvisited cell passes min(best, limit).  A query
+//                 outside B's box walks only the cells that could hold a closer point.  Work counters: integer atomics.
+//   k_ov_reduce   counts and double sums over contiguous point blocks, each in a fixed tree order; k_ov_total sums the
+//   k_ov_total    blocks in a fixed order: two runs give identical bits, and no floating-point atomic is used
+#include <algorithm>
+#include <cfloat>
+#include <climits>
+#include <cmath>
+#include <cstdlib>
+#include <cstring>
+
+#include "ghicp_internal.h"
+#include "ghicp_device.cuh"
+#include "ghicp_grid.cuh"
+
+namespace ghicp_b200 {
+
+struct OverlapTarget {
+  PointGrid pg;
+  int n = 0;
+};
+
+namespace {
+
+constexpr int OV_T = 128;         // threads per query CTA
+constexpr int RED_T = 256;        // threads per reduction CTA
+constexpr int RED_CHUNK = 8192;   // points per reduction CTA
+
+struct OvGrid {   // the target grid as the query kernel reads it
+  GridArgs g;
+  int gm[3];                      // largest cell coordinate per axis
+  double mn[3], ext[3];           // box minimum; box extent in cell edges
+  double cell, slack;
+};
+struct OvArgs {
+  const float *A; long long n;
+  float rt[12];                   // R row-major, then t (float32, rounded once from the double matrix)
+  float hit;                      // overlap-only mode: stop at the first d2 < hit (r*r); fitness mode: -1
+  double lim;                     // exact up to this squared distance; beyond it the query reports +inf
+  const int *perm;                // query order (nullptr: input order)
+  float *d2;                      // [n]
+  unsigned long long *work;       // [2] cells visited, candidates examined
+};
+struct OvPart { double fit, ov; unsigned long long n_fit, n_ov; };
+
+// x' = ((R00 x + R01 y) + R02 z) + t0, float32, every operation rounded separately (SAC-IA's sac_move)
+__device__ __forceinline__ void ov_move(const float *rt, float x, float y, float z, float &ox, float &oy, float &oz) {
+  ox = ((rt[0] * x + rt[1] * y) + rt[2] * z) + rt[9];
+  oy = ((rt[3] * x + rt[4] * y) + rt[5] * z) + rt[10];
+  oz = ((rt[6] * x + rt[7] * y) + rt[8] * z) + rt[11];
+}
+// distance from u to the interval [lo, hi] (cell edges)
+__device__ __forceinline__ double ov_gap(double u, double lo, double hi) { return u < lo ? lo - u : (u > hi ? u - hi : 0.0); }
+// where the points of cells lo .. hi on one axis can lie: the cells widened by the rounding slack, clipped to B's box
+__device__ __forceinline__ double ov_cells_gap(double u, int lo, int hi, double s, double ext) {
+  return ov_gap(u, fmax((double)lo - s, 0.0), fmin((double)hi + 1.0 + s, ext));
+}
+// narrow [a, b] to the cells whose extent comes within w (cell edges) of u
+__device__ __forceinline__ void ov_window(double u, double w, double s, int &a, int &b) {
+  const double lo = u - w - 1.0 - s, hi = u + w + s;
+  if (lo > (double)a) a = lo > (double)b ? b + 1 : (int)ceil(lo);
+  if (hi < (double)b) b = hi < (double)a ? a - 1 : (int)floor(hi);
+}
+
+// Nearest squared distance (knn_d2) from q to B: exact when it is <= lim, +inf otherwise.  hit >= 0: stops at the first
+// d2 < hit and returns it (overlap-only mode).  Bounds are compared in double against (1 - 1e-5) of their value, far more
+// than the float32 rounding of knn_d2.
+__device__ float ov_nn_d2(const GridRegs &r, const OvGrid &G, float qx, float qy, float qz, double lim, float hit,
+                          unsigned long long &cells, unsigned long long &cand) {
+  // a non-finite moved point (a NaN return of an organised scan) has no nearest neighbour: +inf at once, no walk
+  if (!(isfinite(qx) && isfinite(qy) && isfinite(qz))) return INFINITY;
+  const double q[3] = {(double)qx, (double)qy, (double)qz};
+  const double s = G.slack, unit = G.cell * G.cell * (1.0 - 1e-5);
+  double u[3], bg[3];
+  int c[3];
+  for (int a = 0; a < 3; ++a) {
+    u[a] = (q[a] - G.mn[a]) / G.cell;
+    bg[a] = ov_gap(u[a], 0.0, G.ext[a]);
+    c[a] = !(u[a] > 0.0) ? 0 : (u[a] >= (double)G.gm[a] ? G.gm[a] : (int)u[a]);
+  }
+  const double bg2 = (bg[0] * bg[0] + bg[1] * bg[1]) + bg[2] * bg[2];
+  if (!(bg2 * unit <= lim)) return INFINITY;   // beyond the limit from B's box
+  int kmax = 0;
+  for (int a = 0; a < 3; ++a) kmax = max(kmax, max(c[a], G.gm[a] - c[a]));
+  float best = INFINITY;
+  for (int k = 0;; ++k) {
+    // columns of ring k: a wall column (max(|dx|, |dy|) == k) spans cz - k .. cz + k, an inner one only its floor and
+    // ceiling cell; a column whose bound passes L (squared cell edges) is skipped
+    double L = fmin((double)best, lim) / unit;
+    if (bg2 > L) break;
+    int x0 = max(c[0] - k, 0), x1 = min(c[0] + k, G.gm[0]);
+    ov_window(u[0], sqrt(L - bg[1] * bg[1] - bg[2] * bg[2]), s, x0, x1);
+    for (int x = x0; x <= x1; ++x) {
+      L = fmin((double)best, lim) / unit;
+      const double gx = ov_cells_gap(u[0], x, x, s, G.ext[0]);
+      const double wy = L - gx * gx - bg[2] * bg[2];
+      if (wy < 0.0) continue;
+      int y0 = max(c[1] - k, 0), y1 = min(c[1] + k, G.gm[1]);
+      ov_window(u[1], sqrt(wy), s, y0, y1);
+      const bool xwall = abs(x - c[0]) == k;
+      const int za = c[2] - k, zb = c[2] + k;   // the two cells of an inner column, or the run za .. zb of a wall column
+      bool inner = false;                        // can an inner column of this row hold a closer point at all?
+      if (!xwall) {
+        const double wz0 = sqrt(fmax(L - gx * gx - bg[1] * bg[1], 0.0));
+        inner = (za >= 0 && ov_cells_gap(u[2], za, za, s, G.ext[2]) <= wz0) ||
+                (zb <= G.gm[2] && ov_cells_gap(u[2], zb, zb, s, G.ext[2]) <= wz0);
+      }
+      for (int y = y0; y <= y1; ++y) {
+        const bool wall = xwall || abs(y - c[1]) == k;
+        if (!wall && !inner) { if (y < c[1] + k - 1) y = c[1] + k - 1; continue; }   // on to the far wall
+        const double gy = ov_cells_gap(u[1], y, y, s, G.ext[1]);
+        const double wz = L - gx * gx - gy * gy;
+        if (wz < 0.0) continue;
+        for (int part = 0; part < (wall ? 1 : 2); ++part) {
+          int lo, hi;
+          if (wall) { lo = max(za, 0); hi = min(zb, G.gm[2]); }
+          else { lo = hi = part == 0 ? za : zb; if (lo < 0 || lo > G.gm[2]) continue; }
+          ov_window(u[2], sqrt(wz), s, lo, hi);
+          if (lo > hi) continue;
+          cells += (unsigned long long)(hi - lo + 1);
+          const int s0 = r.cstart[lower_cell(r, cell_key(x, y, lo))], s1 = r.cstart[lower_cell(r, cell_key(x, y, hi) + 1)];
+          cand += (unsigned long long)(s1 - s0);
+          for (int p = s0; p < s1; ++p) {
+            const float d2 = knn_d2(qx, qy, qz, r.sorted[p]);
+            if (d2 < hit) return d2;
+            best = d2 < best ? d2 : best;
+          }
+        }
+      }
+    }
+    if (k >= kmax) break;
+    // a true lower bound on every cell outside the visited cube: it lies beyond ring k on some axis, and within B's box
+    // on the two others
+    L = fmin((double)best, lim) / unit;
+    double lb = INFINITY;
+    for (int a = 0; a < 3; ++a) {
+      const double b1 = bg[(a + 1) % 3], b2 = bg[(a + 2) % 3], o2 = b1 * b1 + b2 * b2;
+      if (c[a] - k - 1 >= 0) { const double d = ov_cells_gap(u[a], 0, c[a] - k - 1, s, G.ext[a]); lb = fmin(lb, d * d + o2); }
+      if (c[a] + k + 1 <= G.gm[a]) { const double d = ov_cells_gap(u[a], c[a] + k + 1, G.gm[a], s, G.ext[a]); lb = fmin(lb, d * d + o2); }
+    }
+    if (lb > L) break;
+  }
+  if (hit >= 0.f) return best < hit ? best : INFINITY;
+  return (double)best <= lim ? best : INFINITY;
+}
+
+__global__ void __launch_bounds__(OV_T) k_ov_query(const OvArgs a, const OvGrid G) {
+  const long long t = (long long)blockIdx.x * OV_T + threadIdx.x;
+  unsigned long long cells = 0ull, cand = 0ull;
+  if (t < a.n) {
+    const long long i = a.perm ? (long long)a.perm[t] : t;
+    const GridRegs r = grid_regs(G.g);   // per-thread registers, see k_pca
+    float x, y, z;
+    ov_move(a.rt, a.A[3 * i], a.A[3 * i + 1], a.A[3 * i + 2], x, y, z);
+    a.d2[i] = ov_nn_d2(r, G, x, y, z, a.lim, a.hit, cells, cand);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    cells += __shfl_xor_sync(0xffffffffu, cells, o);
+    cand += __shfl_xor_sync(0xffffffffu, cand, o);
+  }
+  if ((threadIdx.x & 31) == 0 && (cells | cand)) { atomicAdd(a.work, cells); atomicAdd(a.work + 1, cand); }
+}
+
+// clamped B-cell key of each moved point of A, with its index (the cell order of the queries)
+__global__ void k_ov_keys(const OvArgs a, const OvGrid G, pu64 *__restrict__ keys, int *__restrict__ vals) {
+  const long long t = (long long)blockIdx.x * OV_T + threadIdx.x;
+  if (t >= a.n) return;
+  float v[3];
+  ov_move(a.rt, a.A[3 * t], a.A[3 * t + 1], a.A[3 * t + 2], v[0], v[1], v[2]);
+  int c[3];
+  for (int k = 0; k < 3; ++k) {
+    const double f = floor(((double)v[k] - G.mn[k]) / G.cell);
+    c[k] = !(f > 0.0) ? 0 : (f > (double)G.gm[k] ? G.gm[k] : (int)f);
+  }
+  keys[t] = cell_key(c[0], c[1], c[2]);
+  vals[t] = (int)t;
+}
+
+__device__ __forceinline__ void ov_part_add(OvPart &x, const OvPart &y) { x.fit += y.fit; x.ov += y.ov; x.n_fit += y.n_fit; x.n_ov += y.n_ov; }
+// fixed-shape tree over the CTA's RED_T partials
+__device__ void ov_tree(OvPart *sh, OvPart v, OvPart *out) {
+  sh[threadIdx.x] = v;
+  __syncthreads();
+  for (int w = RED_T / 2; w > 0; w >>= 1) {
+    if ((int)threadIdx.x < w) ov_part_add(sh[threadIdx.x], sh[threadIdx.x + w]);
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *out = sh[0];
+}
+__global__ void __launch_bounds__(RED_T) k_ov_reduce(const float *__restrict__ d2, long long n, float r2, double max_range,
+                                                     int fitness, OvPart *__restrict__ part) {
+  __shared__ OvPart sh[RED_T];
+  const long long p0 = (long long)blockIdx.x * RED_CHUNK, p1 = min(p0 + RED_CHUNK, n);
+  OvPart v{0.0, 0.0, 0ull, 0ull};
+  for (long long p = p0 + threadIdx.x; p < p1; p += RED_T) {
+    const float d = d2[p];
+    if (d < r2) { v.ov += (double)d; ++v.n_ov; }
+    if (fitness && d != INFINITY && (double)d <= max_range) { v.fit += (double)d; ++v.n_fit; }
+  }
+  ov_tree(sh, v, part + blockIdx.x);
+}
+__global__ void __launch_bounds__(RED_T) k_ov_total(const OvPart *__restrict__ part, int nb, OvPart *__restrict__ out) {
+  __shared__ OvPart sh[RED_T];
+  OvPart v{0.0, 0.0, 0ull, 0ull};
+  for (int b = threadIdx.x; b < nb; b += RED_T) ov_part_add(v, part[b]);
+  ov_tree(sh, v, out);
+}
+
+template <typename T> cudaError_t oalloc(T **p, size_t n) { return cudaMallocAsync((void **)p, (n ? n : 1) * sizeof(T), 0); }
+template <typename T> void ofree(T *&p) { if (p) cudaFreeAsync(p, 0); p = nullptr; }
+inline int oblk(long long n, int t) { return (int)((n + t - 1) / t); }
+
+}  // namespace
+
+cudaError_t overlap_target_build(const float *d_b, int n_b, OverlapTarget **out) {
+  *out = nullptr;
+  OverlapTarget *t = new OverlapTarget();
+  t->n = n_b;
+  const cudaError_t e = prep_point_grid(0, d_b, n_b, n_b < 8 ? n_b : 8, 0.f, 0.0, &t->pg);
+  if (e != cudaSuccess) { prep_point_grid_free(&t->pg); delete t; return e; }
+  *out = t;
+  return cudaSuccess;
+}
+void overlap_target_free(OverlapTarget *t) {
+  if (!t) return;
+  prep_point_grid_free(&t->pg);
+  delete t;
+}
+
+// GHICP_OVERLAP_ORDER=cell | input (test and measurement hook) overrides the query order overlap_run picks by mode
+static int overlap_order(int dflt) {
+  const char *s = getenv("GHICP_OVERLAP_ORDER");
+  if (!s) return dflt;
+  return std::strcmp(s, "cell") == 0 ? 1 : (std::strcmp(s, "input") == 0 ? 0 : dflt);
+}
+
+#define OCK(call) do { e = (call); if (e != cudaSuccess) goto done; } while (0)
+
+cudaError_t overlap_run(const float *d_a, int n_a, const OverlapTarget *t, const double *Rt, float thre_dis, double max_range,
+                        int want_fitness, cudaEvent_t ev_queries, ghicp_overlap_result *out, float *h_d2_out) {
+  cudaError_t e = cudaSuccess;
+  const long long n = n_a;
+  const float r2 = thre_dis * thre_dis;
+  // fitness mode walks several cells per query: B-cell order keeps a warp's walks in the same cells (3 - 10x faster on an
+  // H100, DESIGN.md §3.12); the overlap-only mode mostly stops in the first cell, and the sort costs more than it saves
+  const bool cell_order = overlap_order(want_fitness ? 1 : 0) == 1;
+  OvArgs a{};
+  OvGrid G{};
+  float *d2 = nullptr; unsigned long long *work = nullptr; OvPart *part = nullptr, *tot = nullptr;
+  pu64 *keys = nullptr; int *perm = nullptr;
+  const int nb = oblk(n, RED_CHUNK);
+  unsigned long long hwork[2] = {0ull, 0ull};
+  OvPart h{};
+  // every workspace first: running out of memory returns before anything is written
+  OCK(oalloc(&d2, (size_t)n)); OCK(oalloc(&work, 2)); OCK(oalloc(&part, (size_t)nb)); OCK(oalloc(&tot, 1));
+  if (cell_order) { OCK(oalloc(&keys, (size_t)n)); OCK(oalloc(&perm, (size_t)n)); }
+  OCK(cudaMemsetAsync(work, 0, 2 * sizeof(unsigned long long), 0));
+  a.A = d_a; a.n = n; a.d2 = d2; a.work = work;
+  for (int i = 0; i < 3; ++i) {
+    for (int j = 0; j < 3; ++j) a.rt[3 * i + j] = Rt ? (float)Rt[j * 4 + i] : (i == j ? 1.f : 0.f);
+    a.rt[9 + i] = Rt ? (float)Rt[12 + i] : 0.f;
+  }
+  a.hit = want_fitness ? -1.f : r2;
+  a.lim = want_fitness ? std::max((double)r2, max_range) : (double)r2;
+  G.g = t->pg.g; G.gm[0] = t->pg.gx; G.gm[1] = t->pg.gy; G.gm[2] = t->pg.gz;
+  G.mn[0] = t->pg.g.mnx; G.mn[1] = t->pg.g.mny; G.mn[2] = t->pg.g.mnz;
+  G.cell = t->pg.cell; G.slack = t->pg.slack;
+  for (int k = 0; k < 3; ++k) G.ext[k] = ((double)t->pg.mx[k] - G.mn[k]) / G.cell;
+  if (ev_queries) OCK(cudaEventRecord(ev_queries, 0));
+  if (cell_order) {
+    GHICP_LAUNCH(k_ov_keys, oblk(n, OV_T), OV_T, 0, 0, a, G, keys, perm);
+    OCK(prep_sort_pairs(0, keys, perm, n_a));
+    a.perm = perm;
+  }
+  GHICP_LAUNCH(k_ov_query, oblk(n, OV_T), OV_T, 0, 0, a, G);
+  GHICP_LAUNCH(k_ov_reduce, nb, RED_T, 0, 0, d2, n, r2, max_range, want_fitness, part);
+  GHICP_LAUNCH(k_ov_total, 1, RED_T, 0, 0, part, nb, tot);
+#if !defined(GHICP_EMU_HOST)
+  OCK(cudaGetLastError());
+#endif
+  OCK(cudaMemcpyAsync(&h, tot, sizeof(h), cudaMemcpyDeviceToHost, 0));
+  OCK(cudaMemcpyAsync(hwork, work, sizeof(hwork), cudaMemcpyDeviceToHost, 0));
+  if (h_d2_out) OCK(cudaMemcpyAsync(h_d2_out, d2, sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost, 0));
+  OCK(cudaStreamSynchronize(0));
+  out->n = n;
+  out->overlap = (long long)h.n_ov;
+  out->ratio = (float)((0.01 + (double)h.n_ov) / (double)n);   // src/common_reg.cpp:312
+  out->overlap_rmse = (want_fitness && h.n_ov > 0) ? std::sqrt(h.ov / (double)h.n_ov) : NAN;
+  out->n_fit = want_fitness ? (long long)h.n_fit : 0;
+  out->fitness = !want_fitness ? NAN : (h.n_fit > 0 ? h.fit / (double)h.n_fit : DBL_MAX);   // PCL's getFitnessScore without a point in range
+  out->cells_visited = (long long)hwork[0];
+  out->candidates = (long long)hwork[1];
+done:
+  ofree(d2); ofree(work); ofree(part); ofree(tot); ofree(keys); ofree(perm);
+  return e;
+}
+#undef OCK
+
+}  // namespace ghicp_b200

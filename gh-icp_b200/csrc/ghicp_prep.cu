@@ -1384,6 +1384,7 @@ void prep_point_grid_free(PointGrid *g) {
   pfree(g->order); pfree(g->ucell); pfree(g->cstart); pfree(g->sorted);
   *g = PointGrid();
 }
+cudaError_t prep_sort_pairs(cudaStream_t st, pu64 *keys, int *vals, int n) { return sort_pairs(keys, vals, n, st); }
 
 // FPFH histograms at d_idx [nidx] (all points when d_idx == nullptr) of the cloud d_xyz [n][3]; d_normals [n][3] receives
 // every point's normal, d_status [n] (may be null) 1 where fewer than 3 neighbours exist, d_nb_idx / d_nb_d2 [n][min(k, n)]

@@ -1,17 +1,20 @@
 // common_reg.h — host-side mirror of the reference's CRegistration (include/common_reg.h, src/common_reg.cpp) over
-// libghicp_b200.so, with the two members the library backs:
+// libghicp_b200.so, with the members the library backs:
 //   compute_fpfh_feature (src/common_reg.cpp:373-389)  normals over search_radius, FPFH over 2 search_radius on every point
 //                                                      (PCL radius searches), on the GPU by ghicp_fpfh_extract_radius with
 //                                                      the canonical definition of DESIGN.md §3.10 ("Radius neighbourhoods")
 //   Coarsereg_FPFHSAC    (src/common_reg.cpp:393-423)  both clouds' histograms, then SAC-IA with correspondence randomness 15
 //                                                      and PCL's other defaults (1000 hypotheses of 3 samples, threshold 100
 //                                                      on squared distances), by ghicp_sac_ia (DESIGN.md §3.11, seed 0)
+//   calOverlap           (src/common_reg.cpp:294-317)  the share of Cloud1 with a Cloud2 point within thre_dis, by
+//                                                      ghicp_cloud_overlap (DESIGN.md §3.12, overlap-only mode)
+//   transformcloud       (src/common_reg.cpp:325-350)  the float32 transform of every point, ((m00 x + m01 y) + m02 z) + m03
+//   invTransform         (src/common_reg.cpp:358-370)  the reference's "not mathematically" inverse, kept as it is
 // Differences, deliberate: clouds are ghicp::Cloud (cloud_io.h) and fpfhFeaturePtr the stand-in of ghicp_types.h; the
 // transform is Eigen::Matrix4f when Eigen is on the include path, else the column-major ghicp::Matrix4f; the SAC-IA is the
 // deterministic one of DESIGN.md §3.11 instead of PCL's std::rand()-driven one; no CPU path (without a CUDA device both
 // members throw).  The fitness of the last Coarsereg_FPFHSAC, which the reference prints, is kept (getFitnessScore).
-// Not provided: the PCL ICP wrappers (icp_reg, ptplicp_reg, gicp_reg), transformcloud / invTransform, calOverlap,
-// LLS_4DOF / SVD_6DOF and CSTRAN_4DOF / CSTRAN_7DOF.
+// Not provided: the PCL ICP wrappers (icp_reg, ptplicp_reg, gicp_reg), LLS_4DOF / SVD_6DOF and CSTRAN_4DOF / CSTRAN_7DOF.
 #pragma once
 #include <iostream>
 #include <stdexcept>
@@ -72,6 +75,38 @@ class CRegistration {
     }
     TransformedSource = out;
     std::cout << "The fitness score of this registration is " << result_.fitness << std::endl;   // :419
+  }
+
+  // :294-317 — (0.01 + #{points of Cloud1 with a Cloud2 point at d2 < thre_dis^2}) / |Cloud1|, as the reference's float
+  float calOverlap(const Cloud &Cloud1, const Cloud &Cloud2, float thre_dis) {
+    ghicp_overlap_result r{};
+    if (ghicp_cloud_overlap(0, Cloud1.xyz.data(), (int)Cloud1.size(), Cloud2.xyz.data(), (int)Cloud2.size(), nullptr, thre_dis,
+                            0.0, 0, &r, nullptr) < 0)
+      throw std::runtime_error(std::string("CRegistration::calOverlap: ") + ghicp_last_error(nullptr));
+    std::cout << "The estimated approximate overlap ratio of Cloud 1 is " << r.ratio << std::endl;   // the reference logs this line
+    return r.ratio;
+  }
+
+  // :325-350 — TransformedCloud receives every point moved by the float32 matrix (the reference appends to it)
+  void transformcloud(const Cloud &CloudIn, Cloud &TransformedCloud, const Matrix4f &transformation) {
+    const Matrix4f &m = transformation;
+    for (size_t i = 0; i < CloudIn.size(); ++i) {
+      const float x = CloudIn.xyz[3 * i], y = CloudIn.xyz[3 * i + 1], z = CloudIn.xyz[3 * i + 2];
+      float o[3];
+      for (int r = 0; r < 3; ++r) o[r] = ((m(r, 0) * x + m(r, 1) * y) + m(r, 2) * z) + m(r, 3);
+      TransformedCloud.push(o[0], o[1], o[2]);
+    }
+    std::cout << "Transform done ..." << std::endl;
+  }
+
+  // :358-370 — NOT the inverse of a rigid transform: the rotation is transposed but the translation is only negated
+  // (-t instead of -R^T t).  Reproduced as the reference has it; it is the inverse only when R is the identity.
+  void invTransform(const Matrix4f &transformation, Matrix4f &invtransformation) {
+    for (int i = 0; i < 3; ++i)
+      for (int j = 0; j < 3; ++j) invtransformation(i, j) = transformation(j, i);
+    for (int i = 0; i < 3; ++i) invtransformation(i, 3) = -transformation(i, 3);
+    for (int j = 0; j < 3; ++j) invtransformation(3, j) = 0.f;
+    invtransformation(3, 3) = 1.f;
   }
 
   double getFitnessScore() const { return result_.fitness; }

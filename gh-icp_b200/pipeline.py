@@ -28,6 +28,11 @@ fpfh_radius = (normal_radius, feature_radius) computes the loop's and SAC-IA's h
 (capi.Prep.fpfh_radius, DESIGN.md §3.10) instead of k-NN with k = fpfh_k: a support of several voxels, as PCL users and the
 reference's own coarse registration compute FPFH.  The default None keeps the k-NN estimator.
 
+evaluate = {"thre_dis": r, "max_range": m} scores the result on the down-sampled clouds (capi.Prep.overlap on the device
+pipeline, capi.cloud_overlap with `features`; DESIGN.md §3.12): info["evaluation"] for the final transform and, with
+initial_alignment="fpfh_sac", info["sac"]["evaluation"] for the coarse one.  The default None leaves info as it was.
+cal_overlap and evaluate_registration score any pair of clouds.
+
 coarsereg_fpfh_sac(source_xyz, target_xyz, search_radius) is CRegistration::Coarsereg_FPFHSAC (src/common_reg.cpp:393-423):
 radius FPFH on every point of both clouds, then SAC-IA with correspondence randomness 15.
 """
@@ -40,7 +45,8 @@ from .registration import Energyfunction, GHRegistration, Keypoints
 def register_clouds(target_xyz, source_xyz, resolution, neighborhood_radius, curvature_non_max_radius, corr_type=capi.CT_NN,
                     feature_type=capi.FT_NONE, features=None, weight_adjustment_ratio=1.1, weight_adjustment_step=0.1,
                     dof_type=6, estimated_IoU=0.5, max_iter=0, device=0, bsc_pattern=None, fpfh_k=20, initial_alignment=None,
-                    sac=None, fpfh_radius=None, **reg_kw):
+                    sac=None, fpfh_radius=None, evaluate=None, **reg_kw):
+    ev_kw = _evaluate_kw(evaluate)
     if initial_alignment not in (None, "fpfh_sac"):
         raise capi.GhicpError(-1, f"initial_alignment must be None or 'fpfh_sac', not {initial_alignment!r}")
     if fpfh_radius is not None:
@@ -85,6 +91,10 @@ def register_clouds(target_xyz, source_xyz, resolution, neighborhood_radius, cur
                 info["fpfh_ms"] = dict(target=pt.fpfh_ms, source=ps.fpfh_ms)
             if sac_info is not None:
                 info["sac"] = dict(sac_info, Rt=Rt0)
+            if ev_kw is not None:
+                info["evaluation"] = ps.overlap(pt, Rt, **ev_kw)
+                if sac_info is not None:
+                    info["sac"]["evaluation"] = ps.overlap(pt, Rt0, **ev_kw)
             reg.close()
         finally:
             pt.close(); ps.close()
@@ -119,8 +129,32 @@ def register_clouds(target_xyz, source_xyz, resolution, neighborhood_radius, cur
                 n_source_kp=len(kp_idx["S"]), bbx_magnitude=bbx, cor=len(reg.pairs()[0]))
     if sac_info is not None:
         info["sac"] = sac_info
+    if ev_kw is not None:
+        info["evaluation"] = capi.cloud_overlap(down["S"], down["T"], Rt, device=device, **ev_kw)
+        if sac_info is not None:
+            info["sac"]["evaluation"] = capi.cloud_overlap(down["S"], down["T"], sac_info["Rt"], device=device, **ev_kw)
     reg.close()
     return Rt, info
+
+
+def _evaluate_kw(evaluate):
+    if evaluate is None:
+        return None
+    if not isinstance(evaluate, dict) or "thre_dis" not in evaluate or set(evaluate) - {"thre_dis", "max_range"}:
+        raise capi.GhicpError(-1, "evaluate must be a dict {thre_dis, max_range (optional)}")
+    return dict(thre_dis=float(evaluate["thre_dis"]), max_range=float(evaluate.get("max_range", float("inf"))))
+
+
+def cal_overlap(cloud1, cloud2, thre_dis, device=0):
+    """CRegistration::calOverlap (src/common_reg.cpp:294-317) on the GPU: the share of cloud1 with a cloud2 point within
+    thre_dis (d2 < thre_dis^2 in float32), as the reference's float (0.01 + overlap) / n.  Overlap-only mode (DESIGN.md §3.12)."""
+    return capi.cloud_overlap(cloud1, cloud2, None, thre_dis=thre_dis, fitness=False, device=device)["ratio"]
+
+
+def evaluate_registration(source_xyz, target_xyz, Rt, thre_dis, max_range=float("inf"), device=0):
+    """Scores Rt (4x4, the source onto the target) on the two clouds: capi.cloud_overlap's dict (overlap, ratio, overlap_rmse
+    within thre_dis; fitness = PCL's getFitnessScore over d2 <= max_range, a bound on squared distances)."""
+    return capi.cloud_overlap(source_xyz, target_xyz, Rt, thre_dis=thre_dis, max_range=max_range, device=device)
 
 
 def coarsereg_fpfh_sac(source_xyz, target_xyz, search_radius, sac=None, device=0):

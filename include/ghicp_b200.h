@@ -322,6 +322,32 @@ int ghicp_prep_sac_ia(const ghicp_prep *source, const ghicp_prep *target, const 
  * ghicp_run return the whole transform.  GHICP_E_ARG after iteration 0 or without keypoints. */
 int ghicp_set_initial_transform(ghicp_ctx *ctx, const double Rt[16]);
 
+/* ---- overlap and fitness of a registration on the dense clouds (DESIGN.md §3.12) ----------------- */
+/* Every point a_i of cloud A is moved by Rt (column-major, rounded once to float32; NULL = identity) and its squared distance
+ * d2_i to the nearest point of cloud B found (float32, exact wherever d2_i <= max(thre_dis^2, max_range), +inf beyond).
+ * overlap = #{d2_i < thre_dis * thre_dis} (CRegistration::calOverlap, src/common_reg.cpp:294-317); fitness = the mean of the
+ * finite d2_i <= max_range (PCL's getFitnessScore; max_range is a bound on SQUARED distances, +inf allowed).  Sums are in
+ * double in a fixed order: two calls give identical bits.  want_fitness = 0 is the overlap-only mode: each query stops at the
+ * first point within thre_dis; n_fit = 0 and overlap_rmse = fitness = NaN.  A point of A whose moved coordinates are not
+ * finite (the NaN returns of an organised scan) gets d2 = +inf at once; non-finite points of B are left out of B, as PCL's
+ * KdTreeFLANN leaves them out of its tree.  Argument errors (NULL, n <= 0, no finite point in B, thre_dis <= 0 or NaN,
+ * max_range < 0 or NaN, a non-finite entry of Rt, d2 without want_fitness, handles on different devices) return GHICP_E_ARG
+ * and write nothing; out of memory returns GHICP_E_NOMEM before anything is written. */
+typedef struct ghicp_overlap_result {
+  long long n, overlap, n_fit, cells_visited, candidates;   /* points of A; work: B-grid cells read, points examined */
+  float ratio;            /* (0.01 + overlap) / n, src/common_reg.cpp:312 */
+  double overlap_rmse, fitness;
+  float stage_ms[3];      /* grid (0 when cached), queries, total */
+} ghicp_overlap_result;
+/* a_xyz [n_a][3], b_xyz [n_b][3] (host arrays); d2 [n_a] (host, may be NULL) receives d2_i */
+int ghicp_cloud_overlap(int device, const float *a_xyz, int n_a, const float *b_xyz, int n_b, const double Rt[16],
+                        float thre_dis, double max_range, int want_fitness, ghicp_overlap_result *out, float *d2);
+/* the down-sampled clouds of two pipeline results, device to device; the target keeps B's grid until ghicp_prep_destroy,
+ * so a second call on the same target does not rebuild it (stage_ms[0] = 0).  Calls on one target from several host threads
+ * are serialised on it (the grid is built once); ghicp_prep_destroy must not overlap them. */
+int ghicp_prep_overlap(const ghicp_prep *a, const ghicp_prep *b, const double Rt[16], float thre_dis, double max_range,
+                       int want_fitness, ghicp_overlap_result *out);
+
 /* ---- multi-GPU (one process per GPU; source rows sharded, target replicated) ---------------- */
 /* 128-byte NCCL unique id; rank 0 creates it, the host runtime broadcasts it (torch.distributed,
  * MPI, a file ...). No NCCL symbol is touched unless these are called (world == 1 → never). */
