@@ -33,14 +33,27 @@ void set_error(Ctx *c, const std::string &msg) {
   g_last_error = msg;
 }
 
-#define CK(c, call)                                                                          \
-  do {                                                                                       \
-    cudaError_t e__ = (call);                                                                \
-    if (e__ != cudaSuccess) {                                                                \
-      set_error((c), std::string(#call) + ": " + cudaGetErrorString(e__));                   \
-      return (e__ == cudaErrorMemoryAllocation) ? GHICP_E_NOMEM : GHICP_E_CUDA;              \
-    }                                                                                        \
+// The ABI code of a CUDA call's result.  On an error: "<who>: <CUDA's message>" becomes the last error (of the context c,
+// when given, and of the process), the error is cleared from the runtime, and the code is GHICP_E_NOMEM for an allocation
+// failure, GHICP_E_CUDA otherwise.
+static int cuda_status(cudaError_t e, const char *who, Ctx *c = nullptr) {
+  if (e == cudaSuccess) return GHICP_OK;
+  set_error(c, std::string(who) + ": " + cudaGetErrorString(e));
+  cudaGetLastError();
+  return e == cudaErrorMemoryAllocation ? GHICP_E_NOMEM : GHICP_E_CUDA;
+}
+
+#define CK(c, call)                                                \
+  do {                                                             \
+    cudaError_t e__ = (call);                                      \
+    if (e__ != cudaSuccess) return cuda_status(e__, #call, (c));   \
   } while (0)
+
+// The start of every stand-alone and pipeline entry point: a device must exist (GHICP_E_NODEV otherwise) and becomes current
+static int enter_device(int device, const char *who) {
+  if (ghicp_device_count() <= 0) { set_error(nullptr, std::string(who) + ": no CUDA device"); return GHICP_E_NODEV; }
+  return cuda_status(cudaSetDevice(device), who);
+}
 
 template <typename T>
 static int dev_alloc(Ctx *c, T **p, size_t count) {
@@ -80,11 +93,7 @@ static bool is_pinned(const void *p) {
   return at.type == cudaMemoryTypeHost;
 }
 
-static int use_device(Ctx *c) {
-  cudaError_t e = cudaSetDevice(c->device);
-  if (e != cudaSuccess) { set_error(c, std::string("cudaSetDevice: ") + cudaGetErrorString(e)); return GHICP_E_CUDA; }
-  return GHICP_OK;
-}
+static int use_device(Ctx *c) { return cuda_status(cudaSetDevice(c->device), "cudaSetDevice", c); }
 
 static void free_all(Ctx *c) {
   dev_free(&c->d_s); dev_free(&c->d_t);
@@ -1130,25 +1139,31 @@ int ghicp_km_solve(int device, const double *W, int n, int sp, int tp, double ep
   return GHICP_OK;
 }
 
+// solver < 0: the loop's SVD solve (launch_solve_explicit); otherwise launch_solve_alt_explicit with that solver
+static cudaError_t rigid_fit_run(int solver, const double *s, const double *t, const double *tn, const double *w, int n,
+                                 DevIter *h) {
+  const size_t b3 = 3 * (size_t)n * sizeof(double);
+  DevBuf<double> d_s, d_t, d_n, d_w; DevBuf<DevIter> d_iter;
+  CUDA_TRY(d_s.alloc(3 * (size_t)n)); CUDA_TRY(d_t.alloc(3 * (size_t)n));
+  if (tn) CUDA_TRY(d_n.alloc(3 * (size_t)n));
+  if (w) CUDA_TRY(d_w.alloc((size_t)n));
+  CUDA_TRY(d_iter.alloc(1));
+  CUDA_TRY(cudaMemcpy(d_s.get(), s, b3, cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemcpy(d_t.get(), t, b3, cudaMemcpyHostToDevice));
+  if (tn) CUDA_TRY(cudaMemcpy(d_n.get(), tn, b3, cudaMemcpyHostToDevice));
+  if (w) CUDA_TRY(cudaMemcpy(d_w.get(), w, (size_t)n * sizeof(double), cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemset(d_iter.get(), 0, sizeof(DevIter)));
+  CUDA_TRY(solver < 0 ? launch_solve_explicit(0, d_s.get(), d_t.get(), n, d_iter.get())
+                      : launch_solve_alt_explicit(0, solver, d_s.get(), d_t.get(), d_n.get(), d_w.get(), n, d_iter.get()));
+  return cudaMemcpy(h, d_iter.get(), sizeof(DevIter), cudaMemcpyDeviceToHost);
+}
+
 int ghicp_rigid_fit(int device, const double *s, const double *t, int n, double Rt[16]) {
   if (!s || !t || !Rt || n <= 0) { set_error(nullptr, "rigid_fit: bad argument"); return GHICP_E_ARG; }
-  if (ghicp_device_count() <= 0) { set_error(nullptr, "rigid_fit: no CUDA device"); return GHICP_E_NODEV; }
-  if (cudaSetDevice(device) != cudaSuccess) return GHICP_E_CUDA;
-  double *d_s = nullptr, *d_t = nullptr;
-  DevIter *d_iter = nullptr;
+  int rc;
+  if ((rc = enter_device(device, "rigid_fit"))) return rc;
   DevIter h;
-  cudaError_t e = cudaMalloc((void **)&d_s, 3 * (size_t)n * sizeof(double));
-  if (e == cudaSuccess) e = cudaMalloc((void **)&d_t, 3 * (size_t)n * sizeof(double));
-  if (e == cudaSuccess) e = cudaMalloc((void **)&d_iter, sizeof(DevIter));
-  if (e == cudaSuccess) e = cudaMemcpy(d_s, s, 3 * (size_t)n * sizeof(double), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(d_t, t, 3 * (size_t)n * sizeof(double), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemset(d_iter, 0, sizeof(DevIter));
-  if (e == cudaSuccess) e = launch_solve_explicit(0, d_s, d_t, n, d_iter);
-  if (e == cudaSuccess) e = cudaMemcpy(&h, d_iter, sizeof(DevIter), cudaMemcpyDeviceToHost);
-  if (d_s) cudaFree(d_s);
-  if (d_t) cudaFree(d_t);
-  if (d_iter) cudaFree(d_iter);
-  if (e != cudaSuccess) { set_error(nullptr, std::string("rigid_fit: ") + cudaGetErrorString(e)); return GHICP_E_CUDA; }
+  if ((rc = cuda_status(rigid_fit_run(-1, s, t, nullptr, nullptr, n, &h), "rigid_fit"))) return rc;
   std::memcpy(Rt, h.Rt, sizeof(double) * 16);
   return GHICP_OK;
 }
@@ -1160,81 +1175,72 @@ int ghicp_rigid_fit_ex(int device, int solver, const double *s, const double *t,
     return GHICP_E_ARG;
   }
   if (solver == GHICP_SOLVER_POINT_TO_PLANE && !tn) { set_error(nullptr, "rigid_fit_ex: point-to-plane needs target normals"); return GHICP_E_ARG; }
-  if (ghicp_device_count() <= 0) { set_error(nullptr, "rigid_fit_ex: no CUDA device"); return GHICP_E_NODEV; }
-  if (cudaSetDevice(device) != cudaSuccess) return GHICP_E_CUDA;
-  double *d_s = nullptr, *d_t = nullptr, *d_n = nullptr, *d_w = nullptr;
-  DevIter *d_iter = nullptr;
+  int rc;
+  if ((rc = enter_device(device, "rigid_fit_ex"))) return rc;
   DevIter h;
-  const size_t b3 = 3 * (size_t)n * sizeof(double);
-  cudaError_t e = cudaMalloc((void **)&d_s, b3);
-  if (e == cudaSuccess) e = cudaMalloc((void **)&d_t, b3);
-  if (e == cudaSuccess && tn) e = cudaMalloc((void **)&d_n, b3);
-  if (e == cudaSuccess && w) e = cudaMalloc((void **)&d_w, (size_t)n * sizeof(double));
-  if (e == cudaSuccess) e = cudaMalloc((void **)&d_iter, sizeof(DevIter));
-  if (e == cudaSuccess) e = cudaMemcpy(d_s, s, b3, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(d_t, t, b3, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess && tn) e = cudaMemcpy(d_n, tn, b3, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess && w) e = cudaMemcpy(d_w, w, (size_t)n * sizeof(double), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemset(d_iter, 0, sizeof(DevIter));
-  if (e == cudaSuccess) e = launch_solve_alt_explicit(0, solver, d_s, d_t, d_n, d_w, n, d_iter);
-  if (e == cudaSuccess) e = cudaMemcpy(&h, d_iter, sizeof(DevIter), cudaMemcpyDeviceToHost);
-  if (d_s) cudaFree(d_s);
-  if (d_t) cudaFree(d_t);
-  if (d_n) cudaFree(d_n);
-  if (d_w) cudaFree(d_w);
-  if (d_iter) cudaFree(d_iter);
-  if (e != cudaSuccess) { set_error(nullptr, std::string("rigid_fit_ex: ") + cudaGetErrorString(e)); return GHICP_E_CUDA; }
+  if ((rc = cuda_status(rigid_fit_run(solver, s, t, tn, w, n, &h), "rigid_fit_ex"))) return rc;
   std::memcpy(Rt, h.Rt, sizeof(double) * 16);
   return h.solve_degenerate ? GHICP_W_FEW_PAIRS : GHICP_OK;
 }
 
 // ---- pre-processing ----------------------------------------------------------------------------------------------
+static cudaError_t voxel_downsample_run(const float *xyz, int n, float voxel_size, int *out_idx, int *n_out) {
+  DevBuf<float> d_xyz; DevBuf<int> d_out;
+  CUDA_TRY(d_xyz.alloc(3 * (size_t)n)); CUDA_TRY(d_out.alloc((size_t)n + 1));
+  CUDA_TRY(cudaMemcpy(d_xyz.get(), xyz, 3 * (size_t)n * sizeof(float), cudaMemcpyHostToDevice));
+  int m = 0;
+  CUDA_TRY(prep_voxel_downsample(0, d_xyz.get(), n, voxel_size, d_out.get(), &m));
+  if (m > 0) CUDA_TRY(cudaMemcpy(out_idx, d_out.get(), (size_t)m * sizeof(int), cudaMemcpyDeviceToHost));
+  *n_out = m;
+  return cudaSuccess;
+}
 int ghicp_voxel_downsample(int device, const float *xyz, int n, float voxel_size, int *out_idx, int *n_out) {
   if (!xyz || !out_idx || !n_out || n <= 0 || !(voxel_size > 0.f)) { set_error(nullptr, "voxel_downsample: bad argument"); return GHICP_E_ARG; }
-  if (ghicp_device_count() <= 0) { set_error(nullptr, "voxel_downsample: no CUDA device"); return GHICP_E_NODEV; }
-  if (cudaSetDevice(device) != cudaSuccess) return GHICP_E_CUDA;
-  float *d_xyz = nullptr; int *d_out = nullptr;
-  cudaError_t e = cudaMallocAsync((void **)&d_xyz, 3 * (size_t)n * sizeof(float), 0);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_out, ((size_t)n + 1) * sizeof(int), 0);
-  if (e == cudaSuccess) e = cudaMemcpy(d_xyz, xyz, 3 * (size_t)n * sizeof(float), cudaMemcpyHostToDevice);
-  int m = 0;
-  if (e == cudaSuccess) e = prep_voxel_downsample(0, d_xyz, n, voxel_size, d_out, &m);
-  if (e == cudaSuccess && m > 0) e = cudaMemcpy(out_idx, d_out, (size_t)m * sizeof(int), cudaMemcpyDeviceToHost);
-  if (d_xyz) cudaFreeAsync(d_xyz, 0);
-  if (d_out) cudaFreeAsync(d_out, 0);
-  if (e != cudaSuccess) { set_error(nullptr, std::string("voxel_downsample: ") + cudaGetErrorString(e)); cudaGetLastError(); return e == cudaErrorMemoryAllocation ? GHICP_E_NOMEM : GHICP_E_CUDA; }
-  *n_out = m;
-  return GHICP_OK;
+  if (int rc = enter_device(device, "voxel_downsample")) return rc;
+  return cuda_status(voxel_downsample_run(xyz, n, voxel_size, out_idx, n_out), "voxel_downsample");
 }
 
+static cudaError_t detect_keypoints_run(const float *xyz, int n, float radius, float ratio_max, int min_pts, float nms_radius,
+                                        int *kp_idx, int *n_kp, float *lam, double *curvature, int *pt_num) {
+  DevBuf<float> d_xyz, d_lam; DevBuf<double> d_curv; DevBuf<int> d_cnt, d_kp;
+  CUDA_TRY(d_xyz.alloc(3 * (size_t)n)); CUDA_TRY(d_lam.alloc(3 * (size_t)n)); CUDA_TRY(d_curv.alloc((size_t)n));
+  CUDA_TRY(d_cnt.alloc((size_t)n)); CUDA_TRY(d_kp.alloc((size_t)n));
+  CUDA_TRY(cudaMemcpy(d_xyz.get(), xyz, 3 * (size_t)n * sizeof(float), cudaMemcpyHostToDevice));
+  int m = 0, rounds = 0;
+  CUDA_TRY(prep_detect_keypoints(0, d_xyz.get(), n, radius, ratio_max, min_pts, nms_radius, d_lam.get(), d_curv.get(), d_cnt.get(),
+                                 d_kp.get(), &m, &rounds));
+  if (m > 0) CUDA_TRY(cudaMemcpy(kp_idx, d_kp.get(), (size_t)m * sizeof(int), cudaMemcpyDeviceToHost));
+  if (lam) CUDA_TRY(cudaMemcpy(lam, d_lam.get(), 3 * (size_t)n * sizeof(float), cudaMemcpyDeviceToHost));
+  if (curvature) CUDA_TRY(cudaMemcpy(curvature, d_curv.get(), (size_t)n * sizeof(double), cudaMemcpyDeviceToHost));
+  if (pt_num) CUDA_TRY(cudaMemcpy(pt_num, d_cnt.get(), (size_t)n * sizeof(int), cudaMemcpyDeviceToHost));
+  *n_kp = m;
+  return cudaSuccess;
+}
 int ghicp_detect_keypoints(int device, const float *xyz, int n, float radius, float ratio_max, int min_pts, float nms_radius,
                            int *kp_idx, int *n_kp, float *lam, double *curvature, int *pt_num) {
   if (!xyz || !kp_idx || !n_kp || n <= 0 || !(radius > 0.f) || !(nms_radius > 0.f)) { set_error(nullptr, "detect_keypoints: bad argument"); return GHICP_E_ARG; }
-  if (ghicp_device_count() <= 0) { set_error(nullptr, "detect_keypoints: no CUDA device"); return GHICP_E_NODEV; }
-  if (cudaSetDevice(device) != cudaSuccess) return GHICP_E_CUDA;
-  float *d_xyz = nullptr, *d_lam = nullptr; double *d_curv = nullptr; int *d_cnt = nullptr, *d_kp = nullptr;
-  cudaError_t e = cudaMallocAsync((void **)&d_xyz, 3 * (size_t)n * sizeof(float), 0);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_lam, 3 * (size_t)n * sizeof(float), 0);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_curv, (size_t)n * sizeof(double), 0);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_cnt, (size_t)n * sizeof(int), 0);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_kp, (size_t)n * sizeof(int), 0);
-  if (e == cudaSuccess) e = cudaMemcpy(d_xyz, xyz, 3 * (size_t)n * sizeof(float), cudaMemcpyHostToDevice);
-  int m = 0, rounds = 0;
-  if (e == cudaSuccess) e = prep_detect_keypoints(0, d_xyz, n, radius, ratio_max, min_pts, nms_radius, d_lam, d_curv, d_cnt, d_kp, &m, &rounds);
-  if (e == cudaSuccess && m > 0) e = cudaMemcpy(kp_idx, d_kp, (size_t)m * sizeof(int), cudaMemcpyDeviceToHost);
-  if (e == cudaSuccess && lam) e = cudaMemcpy(lam, d_lam, 3 * (size_t)n * sizeof(float), cudaMemcpyDeviceToHost);
-  if (e == cudaSuccess && curvature) e = cudaMemcpy(curvature, d_curv, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost);
-  if (e == cudaSuccess && pt_num) e = cudaMemcpy(pt_num, d_cnt, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost);
-  if (d_xyz) cudaFreeAsync(d_xyz, 0);
-  if (d_lam) cudaFreeAsync(d_lam, 0);
-  if (d_curv) cudaFreeAsync(d_curv, 0);
-  if (d_cnt) cudaFreeAsync(d_cnt, 0);
-  if (d_kp) cudaFreeAsync(d_kp, 0);
-  if (e != cudaSuccess) { set_error(nullptr, std::string("detect_keypoints: ") + cudaGetErrorString(e)); cudaGetLastError(); return e == cudaErrorMemoryAllocation ? GHICP_E_NOMEM : GHICP_E_CUDA; }
-  *n_kp = m;
-  return GHICP_OK;
+  if (int rc = enter_device(device, "detect_keypoints")) return rc;
+  return cuda_status(detect_keypoints_run(xyz, n, radius, ratio_max, min_pts, nms_radius, kp_idx, n_kp, lam, curvature, pt_num),
+                     "detect_keypoints");
 }
 
+static cudaError_t bsc_extract_run(const float *xyz, int n, const int *kp_idx, int nkp, float extract_radius, int side,
+                                   const int *pairs, int dof_type, unsigned char *features, float *lrf, int *status) {
+  const int V = dof_type > 4 ? 4 : (dof_type > 0 ? 2 : 1), S2 = side * side;
+  const size_t nbytes = (size_t)(9 * S2 + 7) / 8, out_bytes = (size_t)V * nkp * nbytes;
+  DevBuf<float> d_xyz, d_lrf; DevBuf<int> d_kp, d_pairs, d_status; DevBuf<unsigned char> d_bits;
+  CUDA_TRY(d_xyz.alloc(3 * (size_t)n)); CUDA_TRY(d_kp.alloc((size_t)nkp)); CUDA_TRY(d_pairs.alloc(2 * (size_t)S2));
+  CUDA_TRY(d_bits.alloc(out_bytes)); CUDA_TRY(d_lrf.alloc(12 * (size_t)nkp)); CUDA_TRY(d_status.alloc((size_t)nkp));
+  CUDA_TRY(cudaMemcpy(d_xyz.get(), xyz, 3 * (size_t)n * sizeof(float), cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemcpy(d_kp.get(), kp_idx, (size_t)nkp * sizeof(int), cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemcpy(d_pairs.get(), pairs, 2 * (size_t)S2 * sizeof(int), cudaMemcpyHostToDevice));
+  CUDA_TRY(prep_bsc_extract(0, d_xyz.get(), n, d_kp.get(), nkp, extract_radius, side, d_pairs.get(), dof_type, d_bits.get(),
+                            d_lrf.get(), d_status.get()));
+  CUDA_TRY(cudaMemcpy(features, d_bits.get(), out_bytes, cudaMemcpyDeviceToHost));
+  if (lrf) CUDA_TRY(cudaMemcpy(lrf, d_lrf.get(), 12 * (size_t)nkp * sizeof(float), cudaMemcpyDeviceToHost));
+  if (status) CUDA_TRY(cudaMemcpy(status, d_status.get(), (size_t)nkp * sizeof(int), cudaMemcpyDeviceToHost));
+  return cudaSuccess;
+}
 int ghicp_bsc_extract(int device, const float *xyz, int n, const int *kp_idx, int nkp, float extract_radius, int voxel_side_num,
                       const int *pairs, int dof_type, unsigned char *features, int *n_variants, float *lrf, int *status) {
   if (!xyz || !kp_idx || !pairs || !features || n <= 0 || nkp <= 0 || !(extract_radius > 0.f) || voxel_side_num < 1 ||
@@ -1245,32 +1251,12 @@ int ghicp_bsc_extract(int device, const float *xyz, int n, const int *kp_idx, in
   const int S2 = voxel_side_num * voxel_side_num;
   for (int i = 0; i < nkp; ++i) if (kp_idx[i] < 0 || kp_idx[i] >= n) { set_error(nullptr, "bsc_extract: keypoint index out of range"); return GHICP_E_ARG; }
   for (int i = 0; i < 2 * S2; ++i) if (pairs[i] < 0 || pairs[i] >= S2) { set_error(nullptr, "bsc_extract: sampling pair out of range"); return GHICP_E_ARG; }
-  if (ghicp_device_count() <= 0) { set_error(nullptr, "bsc_extract: no CUDA device"); return GHICP_E_NODEV; }
-  if (cudaSetDevice(device) != cudaSuccess) return GHICP_E_CUDA;
-  const int V = dof_type > 4 ? 4 : (dof_type > 0 ? 2 : 1);
-  const size_t nbytes = (size_t)(9 * S2 + 7) / 8, out_bytes = (size_t)V * nkp * nbytes;
-  float *d_xyz = nullptr, *d_lrf = nullptr; int *d_kp = nullptr, *d_pairs = nullptr, *d_status = nullptr; unsigned char *d_bits = nullptr;
-  cudaError_t e = cudaMallocAsync((void **)&d_xyz, 3 * (size_t)n * sizeof(float), 0);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_kp, (size_t)nkp * sizeof(int), 0);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_pairs, 2 * (size_t)S2 * sizeof(int), 0);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_bits, out_bytes, 0);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_lrf, 12 * (size_t)nkp * sizeof(float), 0);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_status, (size_t)nkp * sizeof(int), 0);
-  if (e == cudaSuccess) e = cudaMemcpy(d_xyz, xyz, 3 * (size_t)n * sizeof(float), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(d_kp, kp_idx, (size_t)nkp * sizeof(int), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(d_pairs, pairs, 2 * (size_t)S2 * sizeof(int), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = prep_bsc_extract(0, d_xyz, n, d_kp, nkp, extract_radius, voxel_side_num, d_pairs, dof_type, d_bits, d_lrf, d_status);
-  if (e == cudaSuccess) e = cudaMemcpy(features, d_bits, out_bytes, cudaMemcpyDeviceToHost);
-  if (e == cudaSuccess && lrf) e = cudaMemcpy(lrf, d_lrf, 12 * (size_t)nkp * sizeof(float), cudaMemcpyDeviceToHost);
-  if (e == cudaSuccess && status) e = cudaMemcpy(status, d_status, (size_t)nkp * sizeof(int), cudaMemcpyDeviceToHost);
-  if (d_xyz) cudaFreeAsync(d_xyz, 0);
-  if (d_kp) cudaFreeAsync(d_kp, 0);
-  if (d_pairs) cudaFreeAsync(d_pairs, 0);
-  if (d_bits) cudaFreeAsync(d_bits, 0);
-  if (d_lrf) cudaFreeAsync(d_lrf, 0);
-  if (d_status) cudaFreeAsync(d_status, 0);
-  if (e != cudaSuccess) { set_error(nullptr, std::string("bsc_extract: ") + cudaGetErrorString(e)); cudaGetLastError(); return e == cudaErrorMemoryAllocation ? GHICP_E_NOMEM : GHICP_E_CUDA; }
-  if (n_variants) *n_variants = V;
+  int rc;
+  if ((rc = enter_device(device, "bsc_extract"))) return rc;
+  if ((rc = cuda_status(bsc_extract_run(xyz, n, kp_idx, nkp, extract_radius, voxel_side_num, pairs, dof_type, features, lrf, status),
+                        "bsc_extract")))
+    return rc;
+  if (n_variants) *n_variants = dof_type > 4 ? 4 : (dof_type > 0 ? 2 : 1);
   return GHICP_OK;
 }
 
@@ -1278,11 +1264,11 @@ int ghicp_bsc_extract(int device, const float *xyz, int n, const int *kp_idx, in
 struct ghicp_prep {
   int device = 0;
   int n = 0, n_down = 0, n_kp = 0, V = 0, side = 0, nbytes = 0;
-  float *d_down = nullptr;          // [n_down][3]
-  int *d_kp = nullptr;              // [n_kp] indices into d_down
-  double *d_kp_xyz = nullptr;       // [3][n_kp]
-  unsigned char *d_bits = nullptr;  // [V][n_kp][nbytes]
-  float *d_fpfh = nullptr;          // [n_kp][33] after ghicp_prep_fpfh
+  DevBuf<float> d_down;           // [n_down][3]
+  DevBuf<int> d_kp;               // [n_kp] indices into d_down
+  DevBuf<double> d_kp_xyz;        // [3][n_kp]
+  DevBuf<unsigned char> d_bits;   // [V][n_kp][nbytes]
+  DevBuf<float> d_fpfh;           // [n_kp][33] after ghicp_prep_fpfh
   float bbox_min[3] = {0, 0, 0}, bbox_max[3] = {0, 0, 0};
   float stage_ms[5] = {0, 0, 0, 0, 0};
   FpfhStats fpfh_stats;
@@ -1293,16 +1279,57 @@ struct ghicp_prep {
 int ghicp_prep_destroy(ghicp_prep *h) {
   if (!h) return GHICP_OK;
   cudaSetDevice(h->device);
-  if (h->d_down) cudaFreeAsync(h->d_down, 0);
-  if (h->d_kp) cudaFreeAsync(h->d_kp, 0);
-  if (h->d_kp_xyz) cudaFreeAsync(h->d_kp_xyz, 0);
-  if (h->d_bits) cudaFreeAsync(h->d_bits, 0);
-  if (h->d_fpfh) cudaFreeAsync(h->d_fpfh, 0);
   overlap_target_free(h->ov_target);
   delete h;
   return GHICP_OK;
 }
 
+static cudaError_t prep_run_stages(const float *xyz, int n, const ghicp_prep_params *p, const int *bsc_pairs, bool want_bsc,
+                                   ghicp_prep *h) {
+  const int side = h->side;
+  StageEvents<5> ev;
+  DevBuf<float> d_xyz, d_lam, d_lrf; DevBuf<double> d_curv;
+  DevBuf<int> d_keep, d_cnt, d_kpbuf, d_pairs, d_status;
+  CUDA_TRY(ev.create());
+  CUDA_TRY(d_xyz.alloc(3 * (size_t)n)); CUDA_TRY(d_keep.alloc((size_t)n + 1));
+  CUDA_TRY(cudaEventRecord(ev[0], 0));
+  CUDA_TRY(cudaMemcpyAsync(d_xyz.get(), xyz, 3 * (size_t)n * sizeof(float), cudaMemcpyHostToDevice, 0));
+  CUDA_TRY(cudaEventRecord(ev[1], 0));
+  int n_down = 0, n_kp = 0, rounds = 0;
+  CUDA_TRY(prep_voxel_downsample(0, d_xyz.get(), n, p->voxel_size, d_keep.get(), &n_down));
+  if (n_down <= 0) return cudaErrorInvalidValue;
+  CUDA_TRY(h->d_down.alloc(3 * (size_t)n_down));
+  CUDA_TRY(prep_gather_points(0, d_xyz.get(), d_keep.get(), n_down, h->d_down.get()));
+  CUDA_TRY(cudaEventRecord(ev[2], 0));
+  d_xyz.reset(); d_keep.reset();
+  CUDA_TRY(prep_bounds(0, h->d_down.get(), n_down, h->bbox_min, h->bbox_max));
+  CUDA_TRY(d_lam.alloc(3 * (size_t)n_down)); CUDA_TRY(d_curv.alloc((size_t)n_down));
+  CUDA_TRY(d_cnt.alloc((size_t)n_down)); CUDA_TRY(d_kpbuf.alloc((size_t)n_down));
+  CUDA_TRY(prep_detect_keypoints(0, h->d_down.get(), n_down, p->neighborhood_radius, p->ratio_max, p->min_pts, p->nms_radius,
+                                 d_lam.get(), d_curv.get(), d_cnt.get(), d_kpbuf.get(), &n_kp, &rounds));
+  CUDA_TRY(cudaEventRecord(ev[3], 0));
+  h->n_down = n_down; h->n_kp = n_kp;
+  if (n_kp > 0) {
+    CUDA_TRY(h->d_kp.alloc((size_t)n_kp));
+    CUDA_TRY(cudaMemcpyAsync(h->d_kp.get(), d_kpbuf.get(), (size_t)n_kp * sizeof(int), cudaMemcpyDeviceToDevice, 0));
+    CUDA_TRY(h->d_kp_xyz.alloc(3 * (size_t)n_kp));
+    CUDA_TRY(prep_kp_coords(0, h->d_down.get(), h->d_kp.get(), n_kp, h->d_kp_xyz.get()));
+    if (want_bsc) {
+      h->V = p->dof_type > 4 ? 4 : (p->dof_type > 0 ? 2 : 1);
+      h->nbytes = (9 * side * side + 7) / 8;
+      CUDA_TRY(h->d_bits.alloc((size_t)h->V * n_kp * h->nbytes));
+      CUDA_TRY(d_pairs.alloc(2 * (size_t)side * side)); CUDA_TRY(d_lrf.alloc(12 * (size_t)n_kp)); CUDA_TRY(d_status.alloc((size_t)n_kp));
+      CUDA_TRY(cudaMemcpyAsync(d_pairs.get(), bsc_pairs, 2 * (size_t)side * side * sizeof(int), cudaMemcpyHostToDevice, 0));
+      CUDA_TRY(prep_bsc_extract(0, h->d_down.get(), n_down, h->d_kp.get(), n_kp, p->bsc_radius, side, d_pairs.get(), p->dof_type,
+                                h->d_bits.get(), d_lrf.get(), d_status.get()));
+    }
+  }
+  CUDA_TRY(cudaEventRecord(ev[4], 0));
+  CUDA_TRY(cudaStreamSynchronize(0));
+  for (int k = 0; k < 4; ++k) h->stage_ms[k] = ev.ms(k, k + 1);
+  h->stage_ms[4] = ev.ms(0, 4);
+  return cudaSuccess;
+}
 int ghicp_prep_run(int device, const float *xyz, int n, const ghicp_prep_params *p, const int *bsc_pairs, ghicp_prep **out) {
   if (!xyz || !p || !out || n <= 0 || !(p->voxel_size > 0.f) || !(p->neighborhood_radius > 0.f) || !(p->nms_radius > 0.f)) {
     set_error(nullptr, "prep_run: bad argument");
@@ -1312,73 +1339,11 @@ int ghicp_prep_run(int device, const float *xyz, int n, const ghicp_prep_params 
   const int side = p->bsc_side > 0 ? p->bsc_side : 7;
   if (want_bsc && (!bsc_pairs || side > 9)) { set_error(nullptr, "prep_run: BSC needs the sampling pattern and voxel_side_num <= 9"); return GHICP_E_ARG; }
   if (want_bsc) for (int i = 0; i < 2 * side * side; ++i) if (bsc_pairs[i] < 0 || bsc_pairs[i] >= side * side) { set_error(nullptr, "prep_run: sampling pair out of range"); return GHICP_E_ARG; }
-  if (ghicp_device_count() <= 0) { set_error(nullptr, "prep_run: no CUDA device"); return GHICP_E_NODEV; }
-  if (cudaSetDevice(device) != cudaSuccess) return GHICP_E_CUDA;
+  int rc;
+  if ((rc = enter_device(device, "prep_run"))) return rc;
   ghicp_prep *h = new ghicp_prep();
   h->device = device; h->n = n; h->side = side;
-  cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-  float *d_xyz = nullptr, *d_lam = nullptr, *d_lrf = nullptr; double *d_curv = nullptr;
-  int *d_keep = nullptr, *d_cnt = nullptr, *d_kpbuf = nullptr, *d_pairs = nullptr, *d_status = nullptr;
-  cudaError_t e = cudaSuccess;
-  auto fail = [&](const char *what) {
-    set_error(nullptr, std::string("prep_run: ") + what + ": " + cudaGetErrorString(e));
-    cudaGetLastError();
-  };
-  for (auto &x : ev) if (e == cudaSuccess) e = cudaEventCreate(&x);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_xyz, 3 * (size_t)n * sizeof(float), 0);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_keep, ((size_t)n + 1) * sizeof(int), 0);
-  if (e == cudaSuccess) e = cudaEventRecord(ev[0], 0);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(d_xyz, xyz, 3 * (size_t)n * sizeof(float), cudaMemcpyHostToDevice, 0);
-  if (e == cudaSuccess) e = cudaEventRecord(ev[1], 0);
-  int n_down = 0, n_kp = 0, rounds = 0;
-  if (e == cudaSuccess) e = prep_voxel_downsample(0, d_xyz, n, p->voxel_size, d_keep, &n_down);
-  if (e == cudaSuccess && n_down <= 0) e = cudaErrorInvalidValue;
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&h->d_down, 3 * (size_t)n_down * sizeof(float), 0);
-  if (e == cudaSuccess) e = prep_gather_points(0, d_xyz, d_keep, n_down, h->d_down);
-  if (e == cudaSuccess) e = cudaEventRecord(ev[2], 0);
-  if (e == cudaSuccess) { cudaFreeAsync(d_xyz, 0); d_xyz = nullptr; cudaFreeAsync(d_keep, 0); d_keep = nullptr; }
-  if (e == cudaSuccess) e = prep_bounds(0, h->d_down, n_down, h->bbox_min, h->bbox_max);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_lam, 3 * (size_t)n_down * sizeof(float), 0);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_curv, (size_t)n_down * sizeof(double), 0);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_cnt, (size_t)n_down * sizeof(int), 0);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_kpbuf, (size_t)n_down * sizeof(int), 0);
-  if (e == cudaSuccess) e = prep_detect_keypoints(0, h->d_down, n_down, p->neighborhood_radius, p->ratio_max, p->min_pts, p->nms_radius,
-                                                  d_lam, d_curv, d_cnt, d_kpbuf, &n_kp, &rounds);
-  if (e == cudaSuccess) e = cudaEventRecord(ev[3], 0);
-  h->n_down = n_down; h->n_kp = n_kp;
-  if (e == cudaSuccess && n_kp > 0) {
-    e = cudaMallocAsync((void **)&h->d_kp, (size_t)n_kp * sizeof(int), 0);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(h->d_kp, d_kpbuf, (size_t)n_kp * sizeof(int), cudaMemcpyDeviceToDevice, 0);
-    if (e == cudaSuccess) e = cudaMallocAsync((void **)&h->d_kp_xyz, 3 * (size_t)n_kp * sizeof(double), 0);
-    if (e == cudaSuccess) e = prep_kp_coords(0, h->d_down, h->d_kp, n_kp, h->d_kp_xyz);
-    if (e == cudaSuccess && want_bsc) {
-      h->V = p->dof_type > 4 ? 4 : (p->dof_type > 0 ? 2 : 1);
-      h->nbytes = (9 * side * side + 7) / 8;
-      e = cudaMallocAsync((void **)&h->d_bits, (size_t)h->V * n_kp * h->nbytes, 0);
-      if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_pairs, 2 * (size_t)side * side * sizeof(int), 0);
-      if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_lrf, 12 * (size_t)n_kp * sizeof(float), 0);
-      if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_status, (size_t)n_kp * sizeof(int), 0);
-      if (e == cudaSuccess) e = cudaMemcpyAsync(d_pairs, bsc_pairs, 2 * (size_t)side * side * sizeof(int), cudaMemcpyHostToDevice, 0);
-      if (e == cudaSuccess) e = prep_bsc_extract(0, h->d_down, n_down, h->d_kp, n_kp, p->bsc_radius, side, d_pairs, p->dof_type, h->d_bits, d_lrf, d_status);
-    }
-  }
-  if (e == cudaSuccess) e = cudaEventRecord(ev[4], 0);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(0);
-  if (e == cudaSuccess) {
-    for (int k = 0; k < 4; ++k) cudaEventElapsedTime(&h->stage_ms[k], ev[k], ev[k + 1]);
-    cudaEventElapsedTime(&h->stage_ms[4], ev[0], ev[4]);
-  }
-  for (auto &x : ev) if (x) cudaEventDestroy(x);
-  if (d_xyz) cudaFreeAsync(d_xyz, 0);
-  if (d_keep) cudaFreeAsync(d_keep, 0);
-  if (d_lam) cudaFreeAsync(d_lam, 0);
-  if (d_curv) cudaFreeAsync(d_curv, 0);
-  if (d_cnt) cudaFreeAsync(d_cnt, 0);
-  if (d_kpbuf) cudaFreeAsync(d_kpbuf, 0);
-  if (d_pairs) cudaFreeAsync(d_pairs, 0);
-  if (d_lrf) cudaFreeAsync(d_lrf, 0);
-  if (d_status) cudaFreeAsync(d_status, 0);
-  if (e != cudaSuccess) { fail("pipeline"); ghicp_prep_destroy(h); return e == cudaErrorMemoryAllocation ? GHICP_E_NOMEM : GHICP_E_CUDA; }
+  if ((rc = cuda_status(prep_run_stages(xyz, n, p, bsc_pairs, want_bsc, h), "prep_run"))) { ghicp_prep_destroy(h); return rc; }
   *out = h;
   return GHICP_OK;
 }
@@ -1394,16 +1359,17 @@ int ghicp_prep_info(const ghicp_prep *h, int *n_down, int *n_kp, int *n_variants
   return GHICP_OK;
 }
 
+static cudaError_t prep_get_run(const ghicp_prep *h, float *down_xyz, int *kp_idx, double *kp_xyz, unsigned char *bsc_bits) {
+  if (down_xyz && h->n_down > 0) CUDA_TRY(cudaMemcpy(down_xyz, h->d_down.get(), 3 * (size_t)h->n_down * sizeof(float), cudaMemcpyDeviceToHost));
+  if (kp_idx && h->n_kp > 0) CUDA_TRY(cudaMemcpy(kp_idx, h->d_kp.get(), (size_t)h->n_kp * sizeof(int), cudaMemcpyDeviceToHost));
+  if (kp_xyz && h->n_kp > 0) CUDA_TRY(cudaMemcpy(kp_xyz, h->d_kp_xyz.get(), 3 * (size_t)h->n_kp * sizeof(double), cudaMemcpyDeviceToHost));
+  if (bsc_bits && h->d_bits.get()) CUDA_TRY(cudaMemcpy(bsc_bits, h->d_bits.get(), (size_t)h->V * h->n_kp * h->nbytes, cudaMemcpyDeviceToHost));
+  return cudaSuccess;
+}
 int ghicp_prep_get(const ghicp_prep *h, float *down_xyz, int *kp_idx, double *kp_xyz, unsigned char *bsc_bits) {
   if (!h) return GHICP_E_ARG;
-  if (cudaSetDevice(h->device) != cudaSuccess) return GHICP_E_CUDA;
-  cudaError_t e = cudaSuccess;
-  if (down_xyz && h->n_down > 0) e = cudaMemcpy(down_xyz, h->d_down, 3 * (size_t)h->n_down * sizeof(float), cudaMemcpyDeviceToHost);
-  if (e == cudaSuccess && kp_idx && h->n_kp > 0) e = cudaMemcpy(kp_idx, h->d_kp, (size_t)h->n_kp * sizeof(int), cudaMemcpyDeviceToHost);
-  if (e == cudaSuccess && kp_xyz && h->n_kp > 0) e = cudaMemcpy(kp_xyz, h->d_kp_xyz, 3 * (size_t)h->n_kp * sizeof(double), cudaMemcpyDeviceToHost);
-  if (e == cudaSuccess && bsc_bits && h->d_bits) e = cudaMemcpy(bsc_bits, h->d_bits, (size_t)h->V * h->n_kp * h->nbytes, cudaMemcpyDeviceToHost);
-  if (e != cudaSuccess) { set_error(nullptr, std::string("prep_get: ") + cudaGetErrorString(e)); return GHICP_E_CUDA; }
-  return GHICP_OK;
+  if (int rc = enter_device(h->device, "prep_get")) return rc;
+  return cuda_status(prep_get_run(h, down_xyz, kp_idx, kp_xyz, bsc_bits), "prep_get");
 }
 
 int ghicp_set_from_prep(ghicp_ctx *ctx, const ghicp_prep *src, const ghicp_prep *tgt) {
@@ -1414,11 +1380,11 @@ int ghicp_set_from_prep(ghicp_ctx *ctx, const ghicp_prep *src, const ghicp_prep 
   if ((rc = use_device(c))) return rc;
   const int N = src->n_kp, M = tgt->n_kp;
   if ((rc = resize_keypoints(c, N, M))) return rc;
-  CK(c, cudaMemcpyAsync(c->d_s, src->d_kp_xyz, 3 * (size_t)N * sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
-  CK(c, cudaMemcpyAsync(c->d_t, tgt->d_kp_xyz, 3 * (size_t)M * sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
+  CK(c, cudaMemcpyAsync(c->d_s, src->d_kp_xyz.get(), 3 * (size_t)N * sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
+  CK(c, cudaMemcpyAsync(c->d_t, tgt->d_kp_xyz.get(), 3 * (size_t)M * sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
   {  // centre of the FP32 filter coordinates = target centroid (scalars only; the 24 M bytes read back are not re-uploaded)
     std::vector<double> ht(3 * (size_t)M);
-    CK(c, cudaMemcpyAsync(ht.data(), tgt->d_kp_xyz, 3 * (size_t)M * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    CK(c, cudaMemcpyAsync(ht.data(), tgt->d_kp_xyz.get(), 3 * (size_t)M * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
     CK(c, cudaStreamSynchronize(c->stream));
     double cx = 0, cy = 0, cz = 0;
     for (int j = 0; j < M; ++j) { cx += ht[j]; cy += ht[(size_t)M + j]; cz += ht[2 * (size_t)M + j]; }
@@ -1426,7 +1392,7 @@ int ghicp_set_from_prep(ghicp_ctx *ctx, const ghicp_prep *src, const ghicp_prep 
   }
   if (c->cfg.feature_type == GHICP_FT_BSC) {
     const int Vneed = (c->cfg.dof == 6) ? 4 : 2;
-    if (!src->d_bits || !tgt->d_bits || src->V < Vneed || src->nbytes != tgt->nbytes) {
+    if (!src->d_bits.get() || !tgt->d_bits.get() || src->V < Vneed || src->nbytes != tgt->nbytes) {
       set_error(c, "set_from_prep: BSC context needs descriptors (source with the context's dof variants, same length)");
       return GHICP_E_ARG;
     }
@@ -1436,13 +1402,13 @@ int ghicp_set_from_prep(ghicp_ctx *ctx, const ghicp_prep *src, const ghicp_prep 
     c->W64 = (c->Bbytes + 7) / 8;
     if ((rc = dev_alloc(c, &c->d_bs, (size_t)c->V * c->W64 * c->N))) return rc;
     if ((rc = dev_alloc(c, &c->d_bt, (size_t)c->W64 * c->M))) return rc;
-    CK(c, launch_pack_bsc(c, src->d_bits, tgt->d_bits));   // the target's variant 0 = its first [M][B] block
+    CK(c, launch_pack_bsc(c, src->d_bits.get(), tgt->d_bits.get()));   // the target's variant 0 = its first [M][B] block
     CK(c, cudaStreamSynchronize(c->stream));
     c->have_bsc = true;
     c->fd_built = false;
   }
-  if (c->cfg.feature_type == GHICP_FT_FPFH && src->d_fpfh && tgt->d_fpfh) {
-    if ((rc = set_fpfh_from(c, src->d_fpfh, tgt->d_fpfh, cudaMemcpyDeviceToDevice))) return rc;
+  if (c->cfg.feature_type == GHICP_FT_FPFH && src->d_fpfh.get() && tgt->d_fpfh.get()) {
+    if ((rc = set_fpfh_from(c, src->d_fpfh.get(), tgt->d_fpfh.get(), cudaMemcpyDeviceToDevice))) return rc;
   }
   return GHICP_OK;
 }
@@ -1455,70 +1421,64 @@ static float fpfh_cell_scale() {
   return v > 0.f ? v : 1.f;
 }
 
+static cudaError_t fpfh_extract_run(const float *xyz, int n, const int *idx, int nidx, int k, float *fpfh, float *normals, int *status) {
+  DevBuf<float> d_xyz, d_fpfh, d_nrm; DevBuf<int> d_status, d_idx;
+  CUDA_TRY(d_xyz.alloc(3 * (size_t)n)); CUDA_TRY(d_fpfh.alloc((size_t)nidx * 33 + 1)); CUDA_TRY(d_nrm.alloc(3 * (size_t)n));
+  CUDA_TRY(d_status.alloc((size_t)n));
+  if (idx) CUDA_TRY(d_idx.alloc((size_t)nidx + 1));
+  CUDA_TRY(cudaMemcpy(d_xyz.get(), xyz, 3 * (size_t)n * sizeof(float), cudaMemcpyHostToDevice));
+  if (idx && nidx > 0) CUDA_TRY(cudaMemcpy(d_idx.get(), idx, (size_t)nidx * sizeof(int), cudaMemcpyHostToDevice));
+  CUDA_TRY(prep_fpfh(0, d_xyz.get(), n, d_idx.get(), nidx, k, fpfh_cell_scale(), d_fpfh.get(), d_nrm.get(), d_status.get(), nullptr,
+                     nullptr, nullptr, nullptr));
+  if (nidx > 0) CUDA_TRY(cudaMemcpy(fpfh, d_fpfh.get(), (size_t)nidx * 33 * sizeof(float), cudaMemcpyDeviceToHost));
+  if (normals) CUDA_TRY(cudaMemcpy(normals, d_nrm.get(), 3 * (size_t)n * sizeof(float), cudaMemcpyDeviceToHost));
+  if (status) CUDA_TRY(cudaMemcpy(status, d_status.get(), (size_t)n * sizeof(int), cudaMemcpyDeviceToHost));
+  return cudaSuccess;
+}
 int ghicp_fpfh_extract(int device, const float *xyz, int n, const int *idx, int nidx, int k, float *fpfh, float *normals, int *status) {
   if (!xyz || n <= 0 || k < 3 || k > 32 || (idx && nidx < 0) || (nidx > 0 && !fpfh)) { set_error(nullptr, "fpfh_extract: bad argument"); return GHICP_E_ARG; }
   if (!idx) nidx = n;
   if (idx) for (int i = 0; i < nidx; ++i) if (idx[i] < 0 || idx[i] >= n) { set_error(nullptr, "fpfh_extract: index out of range"); return GHICP_E_ARG; }
-  if (ghicp_device_count() <= 0) { set_error(nullptr, "fpfh_extract: no CUDA device"); return GHICP_E_NODEV; }
-  if (cudaSetDevice(device) != cudaSuccess) return GHICP_E_CUDA;
-  float *d_xyz = nullptr, *d_fpfh = nullptr, *d_nrm = nullptr; int *d_idx = nullptr, *d_status = nullptr;
-  cudaError_t e = cudaMallocAsync((void **)&d_xyz, 3 * (size_t)n * sizeof(float), 0);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_fpfh, ((size_t)nidx * 33 + 1) * sizeof(float), 0);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_nrm, 3 * (size_t)n * sizeof(float), 0);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_status, (size_t)n * sizeof(int), 0);
-  if (e == cudaSuccess && idx) e = cudaMallocAsync((void **)&d_idx, ((size_t)nidx + 1) * sizeof(int), 0);
-  if (e == cudaSuccess) e = cudaMemcpy(d_xyz, xyz, 3 * (size_t)n * sizeof(float), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess && idx && nidx > 0) e = cudaMemcpy(d_idx, idx, (size_t)nidx * sizeof(int), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = prep_fpfh(0, d_xyz, n, d_idx, nidx, k, fpfh_cell_scale(), d_fpfh, d_nrm, d_status, nullptr, nullptr, nullptr, nullptr);
-  if (e == cudaSuccess && nidx > 0) e = cudaMemcpy(fpfh, d_fpfh, (size_t)nidx * 33 * sizeof(float), cudaMemcpyDeviceToHost);
-  if (e == cudaSuccess && normals) e = cudaMemcpy(normals, d_nrm, 3 * (size_t)n * sizeof(float), cudaMemcpyDeviceToHost);
-  if (e == cudaSuccess && status) e = cudaMemcpy(status, d_status, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost);
-  if (d_xyz) cudaFreeAsync(d_xyz, 0);
-  if (d_fpfh) cudaFreeAsync(d_fpfh, 0);
-  if (d_nrm) cudaFreeAsync(d_nrm, 0);
-  if (d_status) cudaFreeAsync(d_status, 0);
-  if (d_idx) cudaFreeAsync(d_idx, 0);
-  if (e != cudaSuccess) { set_error(nullptr, std::string("fpfh_extract: ") + cudaGetErrorString(e)); cudaGetLastError(); return e == cudaErrorMemoryAllocation ? GHICP_E_NOMEM : GHICP_E_CUDA; }
-  return GHICP_OK;
+  if (int rc = enter_device(device, "fpfh_extract")) return rc;
+  return cuda_status(fpfh_extract_run(xyz, n, idx, nidx, k, fpfh, normals, status), "fpfh_extract");
 }
 
+static cudaError_t prep_fpfh_run(ghicp_prep *h, int k, float ms[3]) {
+  StageEvents<3> ev;
+  DevBuf<float> d_nrm;
+  CUDA_TRY(ev.create());
+  if (!h->d_fpfh.get()) CUDA_TRY(h->d_fpfh.alloc((size_t)h->n_kp * 33 + 1));
+  CUDA_TRY(d_nrm.alloc(3 * (size_t)h->n_down));
+  CUDA_TRY(cudaEventRecord(ev[0], 0));
+  CUDA_TRY(prep_fpfh(0, h->d_down.get(), h->n_down, h->d_kp.get(), h->n_kp, k, fpfh_cell_scale(), h->d_fpfh.get(), d_nrm.get(), nullptr,
+                     nullptr, nullptr, ev[1], &h->fpfh_stats));
+  CUDA_TRY(cudaEventRecord(ev[2], 0));
+  CUDA_TRY(cudaStreamSynchronize(0));
+  ms[0] = ev.ms(0, 1); ms[1] = ev.ms(1, 2); ms[2] = ev.ms(0, 2);
+  return cudaSuccess;
+}
 int ghicp_prep_fpfh(ghicp_prep *h, int k, float stage_ms[3]) {
   if (!h || k < 3 || k > 32 || h->n_kp <= 0) { set_error(nullptr, "prep_fpfh: bad argument or a cloud without keypoints"); return GHICP_E_ARG; }
-  if (cudaSetDevice(h->device) != cudaSuccess) return GHICP_E_CUDA;
-  cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
-  float *d_nrm = nullptr;
-  cudaError_t e = cudaSuccess;
-  for (auto &x : ev) if (e == cudaSuccess) e = cudaEventCreate(&x);
-  if (e == cudaSuccess && !h->d_fpfh) e = cudaMallocAsync((void **)&h->d_fpfh, ((size_t)h->n_kp * 33 + 1) * sizeof(float), 0);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_nrm, 3 * (size_t)h->n_down * sizeof(float), 0);
-  if (e == cudaSuccess) e = cudaEventRecord(ev[0], 0);
-  if (e == cudaSuccess) e = prep_fpfh(0, h->d_down, h->n_down, h->d_kp, h->n_kp, k, fpfh_cell_scale(), h->d_fpfh, d_nrm, nullptr, nullptr, nullptr, ev[1], &h->fpfh_stats);
-  if (e == cudaSuccess) e = cudaEventRecord(ev[2], 0);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(0);
+  int rc;
+  if ((rc = enter_device(h->device, "prep_fpfh"))) return rc;
   float ms[3] = {0.f, 0.f, 0.f};
-  if (e == cudaSuccess) { cudaEventElapsedTime(&ms[0], ev[0], ev[1]); cudaEventElapsedTime(&ms[1], ev[1], ev[2]); cudaEventElapsedTime(&ms[2], ev[0], ev[2]); }
-  for (auto &x : ev) if (x) cudaEventDestroy(x);
-  if (d_nrm) cudaFreeAsync(d_nrm, 0);
-  if (e != cudaSuccess) {
-    set_error(nullptr, std::string("prep_fpfh: ") + cudaGetErrorString(e)); cudaGetLastError();
-    if (h->d_fpfh) { cudaFreeAsync(h->d_fpfh, 0); h->d_fpfh = nullptr; }
-    return e == cudaErrorMemoryAllocation ? GHICP_E_NOMEM : GHICP_E_CUDA;
+  if ((rc = cuda_status(prep_fpfh_run(h, k, ms), "prep_fpfh"))) {
+    h->d_fpfh.reset();   // a failed call leaves no histograms behind
+    return rc;
   }
   if (stage_ms) std::memcpy(stage_ms, ms, sizeof(ms));
   return GHICP_OK;
 }
 
 int ghicp_prep_get_fpfh(const ghicp_prep *h, float *fpfh) {
-  if (!h || !fpfh || !h->d_fpfh) { set_error(nullptr, "prep_get_fpfh: no histograms (call ghicp_prep_fpfh first)"); return GHICP_E_ARG; }
-  if (cudaSetDevice(h->device) != cudaSuccess) return GHICP_E_CUDA;
+  if (!h || !fpfh || !h->d_fpfh.get()) { set_error(nullptr, "prep_get_fpfh: no histograms (call ghicp_prep_fpfh first)"); return GHICP_E_ARG; }
+  if (int rc = enter_device(h->device, "prep_get_fpfh")) return rc;
   if (h->n_kp <= 0) return GHICP_OK;
-  const cudaError_t e = cudaMemcpy(fpfh, h->d_fpfh, (size_t)h->n_kp * 33 * sizeof(float), cudaMemcpyDeviceToHost);
-  if (e != cudaSuccess) { set_error(nullptr, std::string("prep_get_fpfh: ") + cudaGetErrorString(e)); return GHICP_E_CUDA; }
-  return GHICP_OK;
+  return cuda_status(cudaMemcpy(fpfh, h->d_fpfh.get(), (size_t)h->n_kp * 33 * sizeof(float), cudaMemcpyDeviceToHost), "prep_get_fpfh");
 }
 
 int ghicp_prep_fpfh_stats(const ghicp_prep *h, long long *candidates, int *queries, int *fallbacks, float *cell) {
-  if (!h || !h->d_fpfh) { set_error(nullptr, "prep_fpfh_stats: no histograms (call ghicp_prep_fpfh first)"); return GHICP_E_ARG; }
+  if (!h || !h->d_fpfh.get()) { set_error(nullptr, "prep_fpfh_stats: no histograms (call ghicp_prep_fpfh first)"); return GHICP_E_ARG; }
   if (candidates) *candidates = h->fpfh_stats.candidates;
   if (queries) *queries = h->fpfh_stats.queries;
   if (fallbacks) *fallbacks = h->fpfh_stats.fallbacks;
@@ -1540,73 +1500,66 @@ static bool radii_ok(float rn, float rf, const char *who) {
   return ok;
 }
 static int fpfh_radius_status(cudaError_t e, const FpfhRadiusStats &s, const char *who) {
-  if (e == cudaSuccess) return GHICP_OK;
-  cudaGetLastError();
   if (e == cudaErrorMemoryAllocation && s.needed > s.budget) {
+    cudaGetLastError();
     set_error(nullptr, std::string(who) + ": the neighbour lists need at least " + std::to_string(s.needed) + " entries, the budget is " +
                            std::to_string(s.budget) + " entries (16 bytes each)");
     return GHICP_E_NOMEM;
   }
-  set_error(nullptr, std::string(who) + ": " + cudaGetErrorString(e));
-  return e == cudaErrorMemoryAllocation ? GHICP_E_NOMEM : GHICP_E_CUDA;
+  return cuda_status(e, who);
 }
 
+static cudaError_t fpfh_extract_radius_run(const float *xyz, int n, const int *idx, int nidx, float rn, float rf, float *fpfh,
+                                           float *normals, int *status, FpfhRadiusStats *s) {
+  DevBuf<float> d_xyz, d_fpfh, d_nrm; DevBuf<int> d_status, d_idx;
+  CUDA_TRY(d_xyz.alloc(3 * (size_t)n)); CUDA_TRY(d_fpfh.alloc((size_t)nidx * 33 + 1)); CUDA_TRY(d_nrm.alloc(3 * (size_t)n));
+  CUDA_TRY(d_status.alloc((size_t)n));
+  if (idx) CUDA_TRY(d_idx.alloc((size_t)nidx + 1));
+  CUDA_TRY(cudaMemcpy(d_xyz.get(), xyz, 3 * (size_t)n * sizeof(float), cudaMemcpyHostToDevice));
+  if (idx && nidx > 0) CUDA_TRY(cudaMemcpy(d_idx.get(), idx, (size_t)nidx * sizeof(int), cudaMemcpyHostToDevice));
+  CUDA_TRY(prep_fpfh_radius(0, d_xyz.get(), n, d_idx.get(), nidx, rn, rf, fpfh_nb_max(), d_fpfh.get(), d_nrm.get(), d_status.get(),
+                            nullptr, nullptr, s));
+  if (nidx > 0) CUDA_TRY(cudaMemcpy(fpfh, d_fpfh.get(), (size_t)nidx * 33 * sizeof(float), cudaMemcpyDeviceToHost));
+  if (normals) CUDA_TRY(cudaMemcpy(normals, d_nrm.get(), 3 * (size_t)n * sizeof(float), cudaMemcpyDeviceToHost));
+  if (status) CUDA_TRY(cudaMemcpy(status, d_status.get(), (size_t)n * sizeof(int), cudaMemcpyDeviceToHost));
+  return cudaSuccess;
+}
 int ghicp_fpfh_extract_radius(int device, const float *xyz, int n, const int *idx, int nidx, float normal_radius,
                               float feature_radius, float *fpfh, float *normals, int *status) {
   if (!xyz || n <= 0 || (idx && nidx < 0) || ((idx ? nidx : n) > 0 && !fpfh)) { set_error(nullptr, "fpfh_extract_radius: bad argument"); return GHICP_E_ARG; }
   if (!radii_ok(normal_radius, feature_radius, "fpfh_extract_radius")) return GHICP_E_ARG;
   if (!idx) nidx = n;
   if (idx) for (int i = 0; i < nidx; ++i) if (idx[i] < 0 || idx[i] >= n) { set_error(nullptr, "fpfh_extract_radius: index out of range"); return GHICP_E_ARG; }
-  if (ghicp_device_count() <= 0) { set_error(nullptr, "fpfh_extract_radius: no CUDA device"); return GHICP_E_NODEV; }
-  if (cudaSetDevice(device) != cudaSuccess) return GHICP_E_CUDA;
-  float *d_xyz = nullptr, *d_fpfh = nullptr, *d_nrm = nullptr; int *d_idx = nullptr, *d_status = nullptr;
+  if (int rc = enter_device(device, "fpfh_extract_radius")) return rc;
   FpfhRadiusStats s;
-  cudaError_t e = cudaMallocAsync((void **)&d_xyz, 3 * (size_t)n * sizeof(float), 0);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_fpfh, ((size_t)nidx * 33 + 1) * sizeof(float), 0);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_nrm, 3 * (size_t)n * sizeof(float), 0);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_status, (size_t)n * sizeof(int), 0);
-  if (e == cudaSuccess && idx) e = cudaMallocAsync((void **)&d_idx, ((size_t)nidx + 1) * sizeof(int), 0);
-  if (e == cudaSuccess) e = cudaMemcpy(d_xyz, xyz, 3 * (size_t)n * sizeof(float), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess && idx && nidx > 0) e = cudaMemcpy(d_idx, idx, (size_t)nidx * sizeof(int), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = prep_fpfh_radius(0, d_xyz, n, d_idx, nidx, normal_radius, feature_radius, fpfh_nb_max(), d_fpfh, d_nrm,
-                                             d_status, nullptr, nullptr, &s);
-  if (e == cudaSuccess && nidx > 0) e = cudaMemcpy(fpfh, d_fpfh, (size_t)nidx * 33 * sizeof(float), cudaMemcpyDeviceToHost);
-  if (e == cudaSuccess && normals) e = cudaMemcpy(normals, d_nrm, 3 * (size_t)n * sizeof(float), cudaMemcpyDeviceToHost);
-  if (e == cudaSuccess && status) e = cudaMemcpy(status, d_status, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost);
-  for (void *p : {(void *)d_xyz, (void *)d_fpfh, (void *)d_nrm, (void *)d_status, (void *)d_idx}) if (p) cudaFreeAsync(p, 0);
+  const cudaError_t e = fpfh_extract_radius_run(xyz, n, idx, nidx, normal_radius, feature_radius, fpfh, normals, status, &s);
   return fpfh_radius_status(e, s, "fpfh_extract_radius");
 }
 
+static cudaError_t prep_fpfh_radius_run(ghicp_prep *h, float rn, float rf, float ms[4], FpfhRadiusStats *s) {
+  StageEvents<4> ev;
+  DevBuf<float> d_nrm, d_out;
+  CUDA_TRY(ev.create());
+  // into a fresh buffer: histograms a failed call leaves behind are never mistaken for results
+  CUDA_TRY(d_out.alloc((size_t)h->n_kp * 33 + 1));
+  CUDA_TRY(d_nrm.alloc(3 * (size_t)h->n_down));
+  CUDA_TRY(cudaEventRecord(ev[0], 0));
+  CUDA_TRY(prep_fpfh_radius(0, h->d_down.get(), h->n_down, h->d_kp.get(), h->n_kp, rn, rf, fpfh_nb_max(), d_out.get(), d_nrm.get(),
+                            nullptr, ev[1], ev[2], s));
+  CUDA_TRY(cudaEventRecord(ev[3], 0));
+  CUDA_TRY(cudaStreamSynchronize(0));
+  ms[0] = ev.ms(0, 1); ms[1] = ev.ms(1, 2); ms[2] = ev.ms(2, 3); ms[3] = ev.ms(0, 3);
+  h->d_fpfh = std::move(d_out);
+  return cudaSuccess;
+}
 int ghicp_prep_fpfh_radius(ghicp_prep *h, float normal_radius, float feature_radius, float stage_ms[4], long long work[3]) {
   if (!h || h->n_kp <= 0) { set_error(nullptr, "prep_fpfh_radius: bad argument or a cloud without keypoints"); return GHICP_E_ARG; }
   if (!radii_ok(normal_radius, feature_radius, "prep_fpfh_radius")) return GHICP_E_ARG;
-  if (cudaSetDevice(h->device) != cudaSuccess) return GHICP_E_CUDA;
-  cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
-  float *d_nrm = nullptr, *d_out = nullptr;
+  int rc;
+  if ((rc = enter_device(h->device, "prep_fpfh_radius"))) return rc;
   FpfhRadiusStats s;
-  cudaError_t e = cudaSuccess;
-  for (auto &x : ev) if (e == cudaSuccess) e = cudaEventCreate(&x);
-  // into a fresh buffer: histograms a failed call leaves behind are never mistaken for results
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_out, ((size_t)h->n_kp * 33 + 1) * sizeof(float), 0);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_nrm, 3 * (size_t)h->n_down * sizeof(float), 0);
-  if (e == cudaSuccess) e = cudaEventRecord(ev[0], 0);
-  if (e == cudaSuccess) e = prep_fpfh_radius(0, h->d_down, h->n_down, h->d_kp, h->n_kp, normal_radius, feature_radius, fpfh_nb_max(),
-                                             d_out, d_nrm, nullptr, ev[1], ev[2], &s);
-  if (e == cudaSuccess) e = cudaEventRecord(ev[3], 0);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(0);
   float ms[4] = {0.f, 0.f, 0.f, 0.f};
-  if (e == cudaSuccess) {
-    cudaEventElapsedTime(&ms[0], ev[0], ev[1]); cudaEventElapsedTime(&ms[1], ev[1], ev[2]);
-    cudaEventElapsedTime(&ms[2], ev[2], ev[3]); cudaEventElapsedTime(&ms[3], ev[0], ev[3]);
-  }
-  for (auto &x : ev) if (x) cudaEventDestroy(x);
-  if (d_nrm) cudaFreeAsync(d_nrm, 0);
-  if (e != cudaSuccess) {
-    if (d_out) cudaFreeAsync(d_out, 0);
-    return fpfh_radius_status(e, s, "prep_fpfh_radius");
-  }
-  if (h->d_fpfh) cudaFreeAsync(h->d_fpfh, 0);
-  h->d_fpfh = d_out;
+  if ((rc = fpfh_radius_status(prep_fpfh_radius_run(h, normal_radius, feature_radius, ms, &s), s, "prep_fpfh_radius"))) return rc;
   if (stage_ms) std::memcpy(stage_ms, ms, sizeof(ms));
   if (work) { work[0] = s.nb_n; work[1] = s.nb_f; work[2] = s.spfh_points; }
   return GHICP_OK;
@@ -1624,13 +1577,18 @@ static bool sac_params_ok(const ghicp_sac_params *p, const char *who) {
   if (why) set_error(nullptr, std::string(who) + ": " + why);
   return why == nullptr;
 }
-static int sac_status(cudaError_t e, const char *who) {
-  if (e == cudaSuccess) return GHICP_OK;
-  set_error(nullptr, std::string(who) + ": " + cudaGetErrorString(e));
-  cudaGetLastError();
-  return e == cudaErrorMemoryAllocation ? GHICP_E_NOMEM : GHICP_E_CUDA;
-}
 
+static cudaError_t sac_ia_run(const float *src_xyz, const float *src_fpfh, int n_s, const float *tgt_xyz, const float *tgt_fpfh,
+                              int n_t, const ghicp_sac_params *p, ghicp_sac_result *out) {
+  DevBuf<float> d_p, d_fs, d_q, d_ft;
+  CUDA_TRY(d_p.alloc(3 * (size_t)n_s)); CUDA_TRY(d_fs.alloc(33 * (size_t)n_s));
+  CUDA_TRY(d_q.alloc(3 * (size_t)n_t)); CUDA_TRY(d_ft.alloc(33 * (size_t)n_t));
+  CUDA_TRY(cudaMemcpyAsync(d_p.get(), src_xyz, 3 * (size_t)n_s * sizeof(float), cudaMemcpyHostToDevice, 0));
+  CUDA_TRY(cudaMemcpyAsync(d_fs.get(), src_fpfh, 33 * (size_t)n_s * sizeof(float), cudaMemcpyHostToDevice, 0));
+  CUDA_TRY(cudaMemcpyAsync(d_q.get(), tgt_xyz, 3 * (size_t)n_t * sizeof(float), cudaMemcpyHostToDevice, 0));
+  CUDA_TRY(cudaMemcpyAsync(d_ft.get(), tgt_fpfh, 33 * (size_t)n_t * sizeof(float), cudaMemcpyHostToDevice, 0));
+  return sac_run(d_p.get(), d_fs.get(), n_s, d_q.get(), d_ft.get(), n_t, p, out, nullptr);
+}
 int ghicp_sac_ia(int device, const float *src_xyz, const float *src_fpfh, int n_s, const float *tgt_xyz, const float *tgt_fpfh,
                  int n_t, const ghicp_sac_params *p, ghicp_sac_result *out) {
   if (!src_xyz || !src_fpfh || !tgt_xyz || !tgt_fpfh || !out || n_s <= 0 || n_t <= 0) {
@@ -1638,39 +1596,26 @@ int ghicp_sac_ia(int device, const float *src_xyz, const float *src_fpfh, int n_
     return GHICP_E_ARG;
   }
   if (!sac_params_ok(p, "sac_ia")) return GHICP_E_ARG;
-  if (ghicp_device_count() <= 0) { set_error(nullptr, "sac_ia: no CUDA device"); return GHICP_E_NODEV; }
-  if (cudaSetDevice(device) != cudaSuccess) return GHICP_E_CUDA;
-  float *d_p = nullptr, *d_fs = nullptr, *d_q = nullptr, *d_ft = nullptr;
-  cudaError_t e = cudaMallocAsync((void **)&d_p, 3 * (size_t)n_s * sizeof(float), 0);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_fs, 33 * (size_t)n_s * sizeof(float), 0);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_q, 3 * (size_t)n_t * sizeof(float), 0);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_ft, 33 * (size_t)n_t * sizeof(float), 0);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(d_p, src_xyz, 3 * (size_t)n_s * sizeof(float), cudaMemcpyHostToDevice, 0);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(d_fs, src_fpfh, 33 * (size_t)n_s * sizeof(float), cudaMemcpyHostToDevice, 0);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(d_q, tgt_xyz, 3 * (size_t)n_t * sizeof(float), cudaMemcpyHostToDevice, 0);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(d_ft, tgt_fpfh, 33 * (size_t)n_t * sizeof(float), cudaMemcpyHostToDevice, 0);
-  if (e == cudaSuccess) e = sac_run(d_p, d_fs, n_s, d_q, d_ft, n_t, p, out, nullptr);
-  for (float *x : {d_p, d_fs, d_q, d_ft}) if (x) cudaFreeAsync(x, 0);
-  return sac_status(e, "sac_ia");
+  if (int rc = enter_device(device, "sac_ia")) return rc;
+  return cuda_status(sac_ia_run(src_xyz, src_fpfh, n_s, tgt_xyz, tgt_fpfh, n_t, p, out), "sac_ia");
 }
 
+static cudaError_t prep_sac_ia_run(const ghicp_prep *src, const ghicp_prep *tgt, const ghicp_sac_params *p, ghicp_sac_result *out) {
+  DevBuf<float> d_p, d_q;
+  CUDA_TRY(d_p.alloc(3 * (size_t)src->n_kp)); CUDA_TRY(d_q.alloc(3 * (size_t)tgt->n_kp));
+  CUDA_TRY(sac_points_from_soa(src->d_kp_xyz.get(), src->n_kp, d_p.get()));   // exact: the doubles are widened floats
+  CUDA_TRY(sac_points_from_soa(tgt->d_kp_xyz.get(), tgt->n_kp, d_q.get()));
+  return sac_run(d_p.get(), src->d_fpfh.get(), src->n_kp, d_q.get(), tgt->d_fpfh.get(), tgt->n_kp, p, out, nullptr);
+}
 int ghicp_prep_sac_ia(const ghicp_prep *src, const ghicp_prep *tgt, const ghicp_sac_params *p, ghicp_sac_result *out) {
-  if (!src || !tgt || !out || src->n_kp <= 0 || tgt->n_kp <= 0 || !src->d_fpfh || !tgt->d_fpfh) {
+  if (!src || !tgt || !out || src->n_kp <= 0 || tgt->n_kp <= 0 || !src->d_fpfh.get() || !tgt->d_fpfh.get()) {
     set_error(nullptr, "prep_sac_ia: bad argument, a cloud without keypoints or without histograms (call ghicp_prep_fpfh first)");
     return GHICP_E_ARG;
   }
   if (src->device != tgt->device) { set_error(nullptr, "prep_sac_ia: the two pipeline results live on different devices"); return GHICP_E_ARG; }
   if (!sac_params_ok(p, "prep_sac_ia")) return GHICP_E_ARG;
-  if (cudaSetDevice(src->device) != cudaSuccess) return GHICP_E_CUDA;
-  float *d_p = nullptr, *d_q = nullptr;
-  cudaError_t e = cudaMallocAsync((void **)&d_p, 3 * (size_t)src->n_kp * sizeof(float), 0);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_q, 3 * (size_t)tgt->n_kp * sizeof(float), 0);
-  if (e == cudaSuccess) e = sac_points_from_soa(src->d_kp_xyz, src->n_kp, d_p);   // exact: the doubles are widened floats
-  if (e == cudaSuccess) e = sac_points_from_soa(tgt->d_kp_xyz, tgt->n_kp, d_q);
-  if (e == cudaSuccess) e = sac_run(d_p, src->d_fpfh, src->n_kp, d_q, tgt->d_fpfh, tgt->n_kp, p, out, nullptr);
-  if (d_p) cudaFreeAsync(d_p, 0);
-  if (d_q) cudaFreeAsync(d_q, 0);
-  return sac_status(e, "prep_sac_ia");
+  if (int rc = enter_device(src->device, "prep_sac_ia")) return rc;
+  return cuda_status(prep_sac_ia_run(src, tgt, p, out), "prep_sac_ia");
 }
 
 // ---- overlap and fitness on the dense clouds ---------------------------------------------------------------------------
@@ -1687,13 +1632,29 @@ static bool overlap_rt_ok(const double *Rt, const char *who) {
       if (!std::isfinite(Rt[i])) { set_error(nullptr, std::string(who) + ": non-finite transform"); return false; }
   return true;
 }
-static int overlap_status(cudaError_t e, const char *who) {
-  if (e == cudaSuccess) return GHICP_OK;
-  set_error(nullptr, std::string(who) + ": " + cudaGetErrorString(e));
-  cudaGetLastError();
-  return e == cudaErrorMemoryAllocation ? GHICP_E_NOMEM : GHICP_E_CUDA;
-}
 
+// Both overlap entries write *out (and d2) only once every stage succeeded.
+static cudaError_t cloud_overlap_run(const float *a_xyz, int n_a, const float *b_xyz, int n_b, const double *Rt, float thre_dis,
+                                     double max_range, int want_fitness, ghicp_overlap_result *out, float *d2) {
+  StageEvents<3> ev;
+  DevBuf<float> d_a, d_b;
+  ghicp_overlap_result r{};
+  CUDA_TRY(ev.create());
+  CUDA_TRY(d_a.alloc(3 * (size_t)n_a)); CUDA_TRY(d_b.alloc(3 * (size_t)n_b));
+  CUDA_TRY(cudaMemcpyAsync(d_a.get(), a_xyz, 3 * (size_t)n_a * sizeof(float), cudaMemcpyHostToDevice, 0));
+  CUDA_TRY(cudaMemcpyAsync(d_b.get(), b_xyz, 3 * (size_t)n_b * sizeof(float), cudaMemcpyHostToDevice, 0));
+  CUDA_TRY(cudaEventRecord(ev[0], 0));
+  OverlapTarget *t = nullptr;
+  CUDA_TRY(overlap_target_build(d_b.get(), n_b, &t));
+  const cudaError_t e = overlap_run(d_a.get(), n_a, t, Rt, thre_dis, max_range, want_fitness, ev[1], &r, d2);
+  overlap_target_free(t);
+  CUDA_TRY(e);
+  CUDA_TRY(cudaEventRecord(ev[2], 0));
+  CUDA_TRY(cudaStreamSynchronize(0));
+  r.stage_ms[0] = ev.ms(0, 1); r.stage_ms[1] = ev.ms(1, 2); r.stage_ms[2] = ev.ms(0, 2);
+  *out = r;
+  return cudaSuccess;
+}
 int ghicp_cloud_overlap(int device, const float *a_xyz, int n_a, const float *b_xyz, int n_b, const double Rt[16],
                         float thre_dis, double max_range, int want_fitness, ghicp_overlap_result *out, float *d2) {
   if (!a_xyz || !b_xyz || !out || n_a <= 0 || n_b <= 0 || (d2 && !want_fitness)) {
@@ -1719,61 +1680,35 @@ int ghicp_cloud_overlap(int device, const float *a_xyz, int n_a, const float *b_
     }
   }
   if (nb_fin <= 0) { set_error(nullptr, "cloud_overlap: cloud B has no finite point"); return GHICP_E_ARG; }
-  if (ghicp_device_count() <= 0) { set_error(nullptr, "cloud_overlap: no CUDA device"); return GHICP_E_NODEV; }
-  if (cudaSetDevice(device) != cudaSuccess) return GHICP_E_CUDA;
-  cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
-  float *d_a = nullptr, *d_b = nullptr;
-  OverlapTarget *t = nullptr;
-  ghicp_overlap_result r{};
-  cudaError_t e = cudaSuccess;
-  for (auto &x : ev) if (e == cudaSuccess) e = cudaEventCreate(&x);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_a, 3 * (size_t)n_a * sizeof(float), 0);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_b, 3 * (size_t)nb_fin * sizeof(float), 0);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(d_a, a_xyz, 3 * (size_t)n_a * sizeof(float), cudaMemcpyHostToDevice, 0);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(d_b, b_xyz, 3 * (size_t)nb_fin * sizeof(float), cudaMemcpyHostToDevice, 0);
-  if (e == cudaSuccess) e = cudaEventRecord(ev[0], 0);
-  if (e == cudaSuccess) e = overlap_target_build(d_b, (int)nb_fin, &t);
-  if (e == cudaSuccess) e = overlap_run(d_a, n_a, t, Rt, thre_dis, max_range, want_fitness, ev[1], &r, d2);
-  if (e == cudaSuccess) e = cudaEventRecord(ev[2], 0);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(0);
-  if (e == cudaSuccess) {
-    cudaEventElapsedTime(&r.stage_ms[0], ev[0], ev[1]); cudaEventElapsedTime(&r.stage_ms[1], ev[1], ev[2]);
-    cudaEventElapsedTime(&r.stage_ms[2], ev[0], ev[2]);
-  }
-  overlap_target_free(t);
-  for (float *x : {d_a, d_b}) if (x) cudaFreeAsync(x, 0);
-  for (auto &x : ev) if (x) cudaEventDestroy(x);
-  if (e == cudaSuccess) *out = r;
-  return overlap_status(e, "cloud_overlap");
+  if (int rc = enter_device(device, "cloud_overlap")) return rc;
+  return cuda_status(cloud_overlap_run(a_xyz, n_a, b_xyz, (int)nb_fin, Rt, thre_dis, max_range, want_fitness, out, d2), "cloud_overlap");
 }
 
+static cudaError_t prep_overlap_run(const ghicp_prep *a, ghicp_prep *tb, const double *Rt, float thre_dis, double max_range,
+                                    int want_fitness, ghicp_overlap_result *out) {
+  StageEvents<3> ev;
+  ghicp_overlap_result r{};
+  CUDA_TRY(ev.create());
+  CUDA_TRY(cudaEventRecord(ev[0], 0));
+  std::lock_guard<std::mutex> lk(tb->ov_mu);   // held while the grid is read: a concurrent first call waits for the build
+  const bool cached = tb->ov_target != nullptr;
+  if (!cached) CUDA_TRY(overlap_target_build(tb->d_down.get(), tb->n_down, &tb->ov_target));
+  CUDA_TRY(overlap_run(a->d_down.get(), a->n_down, tb->ov_target, Rt, thre_dis, max_range, want_fitness, ev[1], &r, nullptr));
+  CUDA_TRY(cudaEventRecord(ev[2], 0));
+  CUDA_TRY(cudaStreamSynchronize(0));
+  if (!cached) r.stage_ms[0] = ev.ms(0, 1);
+  r.stage_ms[1] = ev.ms(1, 2); r.stage_ms[2] = ev.ms(0, 2);
+  *out = r;
+  return cudaSuccess;
+}
 int ghicp_prep_overlap(const ghicp_prep *a, const ghicp_prep *b, const double Rt[16], float thre_dis, double max_range,
                        int want_fitness, ghicp_overlap_result *out) {
   if (!a || !b || !out || a->n_down <= 0 || b->n_down <= 0) { set_error(nullptr, "prep_overlap: bad argument or an empty cloud"); return GHICP_E_ARG; }
   if (a->device != b->device) { set_error(nullptr, "prep_overlap: the two pipeline results live on different devices"); return GHICP_E_ARG; }
   if (!overlap_args_ok(thre_dis, max_range, "prep_overlap") || !overlap_rt_ok(Rt, "prep_overlap")) return GHICP_E_ARG;
-  if (cudaSetDevice(a->device) != cudaSuccess) return GHICP_E_CUDA;
+  if (int rc = enter_device(a->device, "prep_overlap")) return rc;
   ghicp_prep *tb = const_cast<ghicp_prep *>(b);   // the grid is a cache of the target's down-sampled cloud, not its state
-  cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
-  ghicp_overlap_result r{};
-  cudaError_t e = cudaSuccess;
-  for (auto &x : ev) if (e == cudaSuccess) e = cudaEventCreate(&x);
-  if (e == cudaSuccess) e = cudaEventRecord(ev[0], 0);
-  std::unique_lock<std::mutex> lk(tb->ov_mu);   // held while the grid is read: a concurrent first call waits for the build
-  const bool cached = tb->ov_target != nullptr;
-  if (e == cudaSuccess && !cached) e = overlap_target_build(tb->d_down, tb->n_down, &tb->ov_target);
-  if (e == cudaSuccess) e = overlap_run(a->d_down, a->n_down, tb->ov_target, Rt, thre_dis, max_range, want_fitness, ev[1], &r, nullptr);
-  if (e == cudaSuccess) e = cudaEventRecord(ev[2], 0);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(0);
-  if (e == cudaSuccess) {
-    if (!cached) cudaEventElapsedTime(&r.stage_ms[0], ev[0], ev[1]);
-    cudaEventElapsedTime(&r.stage_ms[1], ev[1], ev[2]);
-    cudaEventElapsedTime(&r.stage_ms[2], ev[0], ev[2]);
-    *out = r;
-  }
-  lk.unlock();
-  for (auto &x : ev) if (x) cudaEventDestroy(x);
-  return overlap_status(e, "prep_overlap");
+  return cuda_status(prep_overlap_run(a, tb, Rt, thre_dis, max_range, want_fitness, out), "prep_overlap");
 }
 
 int ghicp_set_initial_transform(ghicp_ctx *ctx, const double Rt[16]) {

@@ -331,29 +331,27 @@ cudaError_t launch_fd_bsc_tc(Ctx *c) {
     if ((size_t)cand * KP + ring_bytes <= smem_max) { TN = cand; break; }
   if (TN == 0) return cudaErrorNotSupported;
   const size_t smem = (size_t)TN * KP + ring_bytes;
-  int8_t *T8 = nullptr, *S8 = nullptr;
-  cudaError_t e;
+  DevBuf<int8_t> T8, S8;
   const int src_per_tile = TN / V;
   const int grid = (c->nloc + src_per_tile - 1) / src_per_tile;
   const int n_ttiles = (c->M + TC_TM - 1) / TC_TM;
   const size_t t_bytes = (size_t)n_ttiles * TC_TM * KP, s_bytes = (size_t)grid * TN * KP;
-  if ((e = cudaMallocAsync((void **)&T8, t_bytes, c->stream)) != cudaSuccess) return e;
-  if ((e = cudaMallocAsync((void **)&S8, s_bytes, c->stream)) != cudaSuccess) { cudaFreeAsync(T8, c->stream); return e; }
+  CUDA_TRY(T8.alloc(t_bytes, c->stream));
+  CUDA_TRY(S8.alloc(s_bytes, c->stream));
   {
     const long long tot = (long long)(t_bytes / 16);
-    GHICP_LAUNCH(k_unpack_pm1, (unsigned)((tot + 255) / 256), 256, 0, c->stream, c->d_bt, 1, c->M, c->W64, c->bits, KP, TC_TM, 0, c->M, T8);
+    GHICP_LAUNCH(k_unpack_pm1, (unsigned)((tot + 255) / 256), 256, 0, c->stream, c->d_bt, 1, c->M, c->W64, c->bits, KP, TC_TM, 0, c->M, T8.get());
     const long long tos = (long long)(s_bytes / 16);
     GHICP_LAUNCH(k_unpack_pm1, (unsigned)((tos + 255) / 256), 256, 0, c->stream, c->d_bs, V, c->N, c->W64, c->bits, KP, TN, c->r0,
-                 c->nloc * V, S8);
+                 c->nloc * V, S8.get());
     c->launches += 2;
   }
   // the high-bit count of the plane is a template parameter, so the epilogue's bit positions are shifts by constants
   const int hb = fd_hb(c->bits);
-  if (V == 4) e = launch_tc_hb<4>(c, T8, S8, KP, grid, smem, TN, hb);
-  else e = launch_tc_hb<2>(c, T8, S8, KP, grid, smem, TN, hb);
+  cudaError_t e;
+  if (V == 4) e = launch_tc_hb<4>(c, T8.get(), S8.get(), KP, grid, smem, TN, hb);
+  else e = launch_tc_hb<2>(c, T8.get(), S8.get(), KP, grid, smem, TN, hb);
   c->launches++;
-  cudaFreeAsync(T8, c->stream);
-  cudaFreeAsync(S8, c->stream);
   return e;
 }
 

@@ -67,17 +67,19 @@ __device__ __forceinline__ float knn_d2(float qx, float qy, float qz, const floa
 
 // A grid over all n points of d_xyz with the cell rule of the FPFH k-NN (k_eff neighbours wanted per query), for ring
 // searches: gx / gy / gz = the largest occupied cell coordinate per axis, slack = cells of margin for the float32 rounding
-// of cell_coord.  The arrays come from the stream-ordered pool; prep_point_grid_free returns them.
+// of cell_coord.
+struct GridBufs {   // the device arrays GridArgs points into
+  DevBuf<int> order, cstart; DevBuf<pu64> ucell; DevBuf<float4> sorted;
+};
 struct PointGrid {
   GridArgs g{};
   int gx = 0, gy = 0, gz = 0;
   float mx[3] = {0.f, 0.f, 0.f};         // bounding-box maximum (the minimum is g.mnx, g.mny, g.mnz)
   double cell = 0.0, slack = 0.0;
-  int *order = nullptr, *cstart = nullptr; pu64 *ucell = nullptr; float4 *sorted = nullptr;
+  GridBufs buf;
 };
 // cell edge = the k-NN rule times cell_scale (if > 0), at least min_cell, at least the extent / 2^20 (21-bit key fields)
 cudaError_t prep_point_grid(cudaStream_t st, const float *d_xyz, int n, int ke, float cell_scale, double min_cell, PointGrid *out);
-void prep_point_grid_free(PointGrid *g);
 // stable ascending sort of (keys, vals) pairs in place, on the stream (the grid builder's radix sort)
 cudaError_t prep_sort_pairs(cudaStream_t st, pu64 *keys, int *vals, int n);
 

@@ -25,6 +25,91 @@ namespace ghicp_b200 {
 // launches that must match the device query cudaDevAttrMultiProcessorCount instead.
 constexpr int GHICP_SMS = 132;
 
+// ---- host plumbing of the stages around the loop: temporary device memory, events, early return on error ----------------
+// Return the error of a cudaError_t call from the enclosing function (which returns cudaError_t); the DevBufs in scope free
+// their arrays on the way out.
+#define CUDA_TRY(call)                                      \
+  do {                                                      \
+    const cudaError_t e__ = (call);                         \
+    if (e__ != cudaSuccess) return e__;                     \
+  } while (0)
+
+// The pool keeps what it has handed out once (release threshold = unlimited), so the second scan of a pair allocates
+// nothing new.  Set once per process, for the device current at the first DevBuf allocation.
+inline void pool_init() {
+#if !defined(GHICP_EMU_HOST)
+  static const bool done = [] {
+    int dev = 0;
+    cudaMemPool_t pool;
+    if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetDefaultMemPool(&pool, dev) == cudaSuccess) {
+      unsigned long long thr = ~0ull;
+      cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &thr);
+    }
+    return true;
+  }();
+  (void)done;
+#endif
+}
+
+// A temporary device array from the device's stream-ordered pool, freed (stream-ordered, on the stream it was allocated on)
+// when it goes out of scope or at reset().  A cudaMalloc / cudaFree pair per temporary costs more host time than all the
+// kernels of a 1 M-point scan together, cudaFree being a device-wide synchronisation.  Move-only.
+template <typename T>
+class DevBuf {
+ public:
+  DevBuf() = default;
+  DevBuf(const DevBuf &) = delete;
+  DevBuf &operator=(const DevBuf &) = delete;
+  DevBuf(DevBuf &&o) noexcept : p_(o.p_), st_(o.st_) { o.p_ = nullptr; }
+  DevBuf &operator=(DevBuf &&o) noexcept {
+    if (this != &o) { reset(); p_ = o.p_; st_ = o.st_; o.p_ = nullptr; }
+    return *this;
+  }
+  ~DevBuf() { reset(); }
+
+  // n elements (one when n = 0, so that an empty array still has an address); frees what the buffer held first
+  cudaError_t alloc(size_t n, cudaStream_t st = 0) {
+    reset();
+    pool_init();
+    st_ = st;
+    const cudaError_t e = cudaMallocAsync((void **)&p_, (n ? n : 1) * sizeof(T), st);
+    if (e != cudaSuccess) p_ = nullptr;
+    return e;
+  }
+  T *get() const { return p_; }
+  void reset() {
+    if (p_) cudaFreeAsync(p_, st_);
+    p_ = nullptr;
+  }
+
+ private:
+  T *p_ = nullptr;
+  cudaStream_t st_ = 0;
+};
+
+// The events that time the stages of one call, destroyed with it
+template <int N>
+struct StageEvents {
+  cudaEvent_t ev[N] = {};
+  StageEvents() = default;
+  StageEvents(const StageEvents &) = delete;
+  StageEvents &operator=(const StageEvents &) = delete;
+  ~StageEvents() {
+    for (cudaEvent_t e : ev)
+      if (e) cudaEventDestroy(e);
+  }
+  cudaError_t create() {
+    for (cudaEvent_t &e : ev) CUDA_TRY(cudaEventCreate(&e));
+    return cudaSuccess;
+  }
+  cudaEvent_t operator[](int i) const { return ev[i]; }
+  float ms(int from, int to) const {   // elapsed time between two recorded events
+    float t = 0.f;
+    cudaEventElapsedTime(&t, ev[from], ev[to]);
+    return t;
+  }
+};
+
 // Feature-distance plane layout: PANEL-MAJOR.  The N x M plane is stored as ceil(M/256) column panels, each
 // a dense row-major [rows][256] block, so the 256-column panel a warp sweeps down the source rows is one
 // perfectly sequential HBM stream instead of short reads at a row stride.  fd_index / fd_elems address the

@@ -841,17 +841,14 @@ cudaError_t launch_fd_bsc(Ctx *c) {
 }
 
 cudaError_t launch_fd_fpfh(Ctx *c) {
-  float *sc = nullptr, *tc = nullptr;
-  cudaError_t e;
-  if ((e = cudaMallocAsync(&sc, (size_t)c->N * 36 * sizeof(float), c->stream)) != cudaSuccess) return e;
-  if ((e = cudaMallocAsync(&tc, (size_t)c->M * 36 * sizeof(float), c->stream)) != cudaSuccess) return e;
-  GHICP_LAUNCH(k_fpfh_center, (c->N + 127) / 128, 128, 0, c->stream, c->d_fs, sc, c->N);
-  GHICP_LAUNCH(k_fpfh_center, (c->M + 127) / 128, 128, 0, c->stream, c->d_ft, tc, c->M);
+  DevBuf<float> sc, tc;
+  CUDA_TRY(sc.alloc((size_t)c->N * 36, c->stream));
+  CUDA_TRY(tc.alloc((size_t)c->M * 36, c->stream));
+  GHICP_LAUNCH(k_fpfh_center, (c->N + 127) / 128, 128, 0, c->stream, c->d_fs, sc.get(), c->N);
+  GHICP_LAUNCH(k_fpfh_center, (c->M + 127) / 128, 128, 0, c->stream, c->d_ft, tc.get(), c->M);
   dim3 grid((c->M + FPT - 1) / FPT, (c->nloc + FPT - 1) / FPT);
-  GHICP_LAUNCH(k_fd_fpfh, grid, FPT * FPT, 0, c->stream, sc, tc, c->d_fdf, c->N, c->M, c->fd_rows, c->r0, c->nloc);
+  GHICP_LAUNCH(k_fd_fpfh, grid, FPT * FPT, 0, c->stream, sc.get(), tc.get(), c->d_fdf, c->N, c->M, c->fd_rows, c->r0, c->nloc);
   c->launches += 3;
-  cudaFreeAsync(sc, c->stream);
-  cudaFreeAsync(tc, c->stream);
   return cudaGetLastError();
 }
 

@@ -215,8 +215,6 @@ __global__ void __launch_bounds__(RED_T) k_ov_total(const OvPart *__restrict__ p
   ov_tree(sh, v, out);
 }
 
-template <typename T> cudaError_t oalloc(T **p, size_t n) { return cudaMallocAsync((void **)p, (n ? n : 1) * sizeof(T), 0); }
-template <typename T> void ofree(T *&p) { if (p) cudaFreeAsync(p, 0); p = nullptr; }
 inline int oblk(long long n, int t) { return (int)((n + t - 1) / t); }
 
 }  // namespace
@@ -226,15 +224,11 @@ cudaError_t overlap_target_build(const float *d_b, int n_b, OverlapTarget **out)
   OverlapTarget *t = new OverlapTarget();
   t->n = n_b;
   const cudaError_t e = prep_point_grid(0, d_b, n_b, n_b < 8 ? n_b : 8, 0.f, 0.0, &t->pg);
-  if (e != cudaSuccess) { prep_point_grid_free(&t->pg); delete t; return e; }
+  if (e != cudaSuccess) { delete t; return e; }
   *out = t;
   return cudaSuccess;
 }
-void overlap_target_free(OverlapTarget *t) {
-  if (!t) return;
-  prep_point_grid_free(&t->pg);
-  delete t;
-}
+void overlap_target_free(OverlapTarget *t) { delete t; }
 
 // GHICP_OVERLAP_ORDER=cell | input (test and measurement hook) overrides the query order overlap_run picks by mode
 static int overlap_order(int dflt) {
@@ -243,11 +237,8 @@ static int overlap_order(int dflt) {
   return std::strcmp(s, "cell") == 0 ? 1 : (std::strcmp(s, "input") == 0 ? 0 : dflt);
 }
 
-#define OCK(call) do { e = (call); if (e != cudaSuccess) goto done; } while (0)
-
 cudaError_t overlap_run(const float *d_a, int n_a, const OverlapTarget *t, const double *Rt, float thre_dis, double max_range,
                         int want_fitness, cudaEvent_t ev_queries, ghicp_overlap_result *out, float *h_d2_out) {
-  cudaError_t e = cudaSuccess;
   const long long n = n_a;
   const float r2 = thre_dis * thre_dis;
   // fitness mode walks several cells per query: B-cell order keeps a warp's walks in the same cells (3 - 10x faster on an
@@ -255,16 +246,16 @@ cudaError_t overlap_run(const float *d_a, int n_a, const OverlapTarget *t, const
   const bool cell_order = overlap_order(want_fitness ? 1 : 0) == 1;
   OvArgs a{};
   OvGrid G{};
-  float *d2 = nullptr; unsigned long long *work = nullptr; OvPart *part = nullptr, *tot = nullptr;
-  pu64 *keys = nullptr; int *perm = nullptr;
+  DevBuf<float> d2; DevBuf<unsigned long long> work; DevBuf<OvPart> part, tot;
+  DevBuf<pu64> keys; DevBuf<int> perm;
   const int nb = oblk(n, RED_CHUNK);
   unsigned long long hwork[2] = {0ull, 0ull};
   OvPart h{};
   // every workspace first: running out of memory returns before anything is written
-  OCK(oalloc(&d2, (size_t)n)); OCK(oalloc(&work, 2)); OCK(oalloc(&part, (size_t)nb)); OCK(oalloc(&tot, 1));
-  if (cell_order) { OCK(oalloc(&keys, (size_t)n)); OCK(oalloc(&perm, (size_t)n)); }
-  OCK(cudaMemsetAsync(work, 0, 2 * sizeof(unsigned long long), 0));
-  a.A = d_a; a.n = n; a.d2 = d2; a.work = work;
+  CUDA_TRY(d2.alloc((size_t)n)); CUDA_TRY(work.alloc(2)); CUDA_TRY(part.alloc((size_t)nb)); CUDA_TRY(tot.alloc(1));
+  if (cell_order) { CUDA_TRY(keys.alloc((size_t)n)); CUDA_TRY(perm.alloc((size_t)n)); }
+  CUDA_TRY(cudaMemsetAsync(work.get(), 0, 2 * sizeof(unsigned long long), 0));
+  a.A = d_a; a.n = n; a.d2 = d2.get(); a.work = work.get();
   for (int i = 0; i < 3; ++i) {
     for (int j = 0; j < 3; ++j) a.rt[3 * i + j] = Rt ? (float)Rt[j * 4 + i] : (i == j ? 1.f : 0.f);
     a.rt[9 + i] = Rt ? (float)Rt[12 + i] : 0.f;
@@ -275,22 +266,20 @@ cudaError_t overlap_run(const float *d_a, int n_a, const OverlapTarget *t, const
   G.mn[0] = t->pg.g.mnx; G.mn[1] = t->pg.g.mny; G.mn[2] = t->pg.g.mnz;
   G.cell = t->pg.cell; G.slack = t->pg.slack;
   for (int k = 0; k < 3; ++k) G.ext[k] = ((double)t->pg.mx[k] - G.mn[k]) / G.cell;
-  if (ev_queries) OCK(cudaEventRecord(ev_queries, 0));
+  if (ev_queries) CUDA_TRY(cudaEventRecord(ev_queries, 0));
   if (cell_order) {
-    GHICP_LAUNCH(k_ov_keys, oblk(n, OV_T), OV_T, 0, 0, a, G, keys, perm);
-    OCK(prep_sort_pairs(0, keys, perm, n_a));
-    a.perm = perm;
+    GHICP_LAUNCH(k_ov_keys, oblk(n, OV_T), OV_T, 0, 0, a, G, keys.get(), perm.get());
+    CUDA_TRY(prep_sort_pairs(0, keys.get(), perm.get(), n_a));
+    a.perm = perm.get();
   }
   GHICP_LAUNCH(k_ov_query, oblk(n, OV_T), OV_T, 0, 0, a, G);
-  GHICP_LAUNCH(k_ov_reduce, nb, RED_T, 0, 0, d2, n, r2, max_range, want_fitness, part);
-  GHICP_LAUNCH(k_ov_total, 1, RED_T, 0, 0, part, nb, tot);
-#if !defined(GHICP_EMU_HOST)
-  OCK(cudaGetLastError());
-#endif
-  OCK(cudaMemcpyAsync(&h, tot, sizeof(h), cudaMemcpyDeviceToHost, 0));
-  OCK(cudaMemcpyAsync(hwork, work, sizeof(hwork), cudaMemcpyDeviceToHost, 0));
-  if (h_d2_out) OCK(cudaMemcpyAsync(h_d2_out, d2, sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost, 0));
-  OCK(cudaStreamSynchronize(0));
+  GHICP_LAUNCH(k_ov_reduce, nb, RED_T, 0, 0, d2.get(), n, r2, max_range, want_fitness, part.get());
+  GHICP_LAUNCH(k_ov_total, 1, RED_T, 0, 0, part.get(), nb, tot.get());
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaMemcpyAsync(&h, tot.get(), sizeof(h), cudaMemcpyDeviceToHost, 0));
+  CUDA_TRY(cudaMemcpyAsync(hwork, work.get(), sizeof(hwork), cudaMemcpyDeviceToHost, 0));
+  if (h_d2_out) CUDA_TRY(cudaMemcpyAsync(h_d2_out, d2.get(), sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost, 0));
+  CUDA_TRY(cudaStreamSynchronize(0));
   out->n = n;
   out->overlap = (long long)h.n_ov;
   out->ratio = (float)((0.01 + (double)h.n_ov) / (double)n);   // src/common_reg.cpp:312
@@ -299,10 +288,7 @@ cudaError_t overlap_run(const float *d_a, int n_a, const OverlapTarget *t, const
   out->fitness = !want_fitness ? NAN : (h.n_fit > 0 ? h.fit / (double)h.n_fit : DBL_MAX);   // PCL's getFitnessScore without a point in range
   out->cells_visited = (long long)hwork[0];
   out->candidates = (long long)hwork[1];
-done:
-  ofree(d2); ofree(work); ofree(part); ofree(tot); ofree(keys); ofree(perm);
-  return e;
+  return cudaSuccess;
 }
-#undef OCK
 
 }  // namespace ghicp_b200

@@ -34,14 +34,9 @@ namespace {
 
 constexpr int PT = 256;
 
-// ---- plumbing: device memory, sort, scan (CUB under nvcc; the C++ library under the emulation shim) -------------------
+// ---- plumbing: sort, scan (CUB under nvcc; the C++ library under the emulation shim) ----------------------------------
+// Workspaces are DevBufs on stream 0 (the whole pre-processing runs on one stream), CUB's temporaries on the sort's stream.
 #if defined(GHICP_EMU_HOST)
-template <typename T> cudaError_t pmalloc(T **p, size_t n) { *p = (T *)emu_poisoned((n ? n : 1) * sizeof(T)); return *p ? cudaSuccess : cudaErrorMemoryAllocation; }
-template <typename T> void pfree(T *p) { free(p); }
-inline cudaError_t pcopy(void *dst, const void *src, size_t bytes, int, cudaStream_t) { memcpy(dst, src, bytes); return cudaSuccess; }
-inline cudaError_t pzero(void *p, size_t bytes, cudaStream_t) { memset(p, 0, bytes); return cudaSuccess; }
-inline cudaError_t psync(cudaStream_t) { return cudaSuccess; }
-enum { P_H2D = 1, P_D2H = 2, P_D2D = 3 };
 }  // namespace
 }  // namespace ghicp_b200
 #include <algorithm>
@@ -76,53 +71,28 @@ cudaError_t segmented_sort(const pu64 *in, pu64 *out, long long total, int m, co
   return cudaSuccess;
 }
 #else
-// Workspaces come from the device's stream-ordered pool (the whole pre-processing runs on one stream): a cudaMalloc /
-// cudaFree pair per temporary costs more host time than all the kernels of a 1 M-point scan together, cudaFree being a
-// device-wide synchronisation.  The pool keeps what it
-// has handed out once (release threshold = unlimited), so the second scan of a pair allocates nothing new.
-inline void ppool_init() {
-  static bool done = false;   // per process; set for the current device on first use
-  if (done) return;
-  int dev = 0; cudaMemPool_t pool;
-  if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetDefaultMemPool(&pool, dev) == cudaSuccess) {
-    unsigned long long thr = ~0ull;
-    cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &thr);
-  }
-  done = true;
-}
-template <typename T> cudaError_t pmalloc(T **p, size_t n) { ppool_init(); return cudaMallocAsync((void **)p, (n ? n : 1) * sizeof(T), 0); }
-template <typename T> void pfree(T *p) { if (p) cudaFreeAsync(p, 0); }
-enum { P_H2D = cudaMemcpyHostToDevice, P_D2H = cudaMemcpyDeviceToHost, P_D2D = cudaMemcpyDeviceToDevice };
-inline cudaError_t pcopy(void *dst, const void *src, size_t bytes, int kind, cudaStream_t st) { return cudaMemcpyAsync(dst, src, bytes, (cudaMemcpyKind)kind, st); }
-inline cudaError_t pzero(void *p, size_t bytes, cudaStream_t st) { return cudaMemsetAsync(p, 0, bytes, st); }
-inline cudaError_t psync(cudaStream_t st) { return cudaStreamSynchronize(st); }
 cudaError_t sort_pairs(pu64 *keys, int *vals, int n, cudaStream_t st) {   // stable LSD radix sort, ascending keys
-  pu64 *k2 = nullptr; int *v2 = nullptr; void *tmp = nullptr; size_t tb = 0;
-  cudaError_t e = pmalloc(&k2, (size_t)n);
-  if (e == cudaSuccess) e = pmalloc(&v2, (size_t)n);
-  if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(nullptr, tb, keys, k2, vals, v2, n, 0, 64, st);
-  if (e == cudaSuccess) e = cudaMallocAsync(&tmp, tb ? tb : 1, st);
-  if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(tmp, tb, keys, k2, vals, v2, n, 0, 64, st);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(keys, k2, sizeof(pu64) * (size_t)n, cudaMemcpyDeviceToDevice, st);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(vals, v2, sizeof(int) * (size_t)n, cudaMemcpyDeviceToDevice, st);
-  pfree(k2); pfree(v2); if (tmp) cudaFreeAsync(tmp, st);   // stream-ordered: no host synchronisation needed
-  return e;
+  DevBuf<pu64> k2; DevBuf<int> v2; DevBuf<unsigned char> tmp; size_t tb = 0;
+  CUDA_TRY(k2.alloc((size_t)n));
+  CUDA_TRY(v2.alloc((size_t)n));
+  CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, keys, k2.get(), vals, v2.get(), n, 0, 64, st));
+  CUDA_TRY(tmp.alloc(tb, st));
+  CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp.get(), tb, keys, k2.get(), vals, v2.get(), n, 0, 64, st));
+  CUDA_TRY(cudaMemcpyAsync(keys, k2.get(), sizeof(pu64) * (size_t)n, cudaMemcpyDeviceToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(vals, v2.get(), sizeof(int) * (size_t)n, cudaMemcpyDeviceToDevice, st));
+  return cudaSuccess;   // stream-ordered frees: no host synchronisation needed
 }
 cudaError_t exclusive_scan(const int *in, int *out, int n, cudaStream_t st) {   // out[n] = total (in[n] must be readable)
-  void *tmp = nullptr; size_t tb = 0;
-  cudaError_t e = cub::DeviceScan::ExclusiveSum(nullptr, tb, in, out, n + 1, st);
-  if (e == cudaSuccess) e = cudaMallocAsync(&tmp, tb ? tb : 1, st);
-  if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(tmp, tb, in, out, n + 1, st);
-  if (tmp) cudaFreeAsync(tmp, st);
-  return e;
+  DevBuf<unsigned char> tmp; size_t tb = 0;
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tb, in, out, n + 1, st));
+  CUDA_TRY(tmp.alloc(tb, st));
+  return cub::DeviceScan::ExclusiveSum(tmp.get(), tb, in, out, n + 1, st);
 }
 cudaError_t exclusive_scan64(const long long *in, long long *out, int n, cudaStream_t st) {   // out[n] = total (in[n] readable)
-  void *tmp = nullptr; size_t tb = 0;
-  cudaError_t e = cub::DeviceScan::ExclusiveSum(nullptr, tb, in, out, n + 1, st);
-  if (e == cudaSuccess) e = cudaMallocAsync(&tmp, tb ? tb : 1, st);
-  if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(tmp, tb, in, out, n + 1, st);
-  if (tmp) cudaFreeAsync(tmp, st);
-  return e;
+  DevBuf<unsigned char> tmp; size_t tb = 0;
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tb, in, out, n + 1, st));
+  CUDA_TRY(tmp.alloc(tb, st));
+  return cub::DeviceScan::ExclusiveSum(tmp.get(), tb, in, out, n + 1, st);
 }
 cudaError_t segmented_sort(const pu64 *in, pu64 *out, long long total, int m, const long long *off, cudaStream_t st);   // below
 #endif
@@ -378,127 +348,111 @@ __global__ void k_gather_sorted(const float *__restrict__ xyz, const int *__rest
   sorted[s] = make_float4(xyz[3 * (size_t)k], xyz[3 * (size_t)k + 1], xyz[3 * (size_t)k + 2], 0.f);
 }
 
-#define PCK(call) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) { err = e__; goto done; } } while (0)
 inline int blocks(int n) { return (n + PT - 1) / PT; }
 
-// uniform grid over the points ids[k] (k < n): returns device arrays (order, ucell, cstart) the caller frees
-cudaError_t build_grid(cudaStream_t st, const float *d_xyz, const int *d_ids, int n, float cell, GridArgs *g, int **o_order,
-                       pu64 **o_ucell, int **o_cstart, float4 **o_sorted) {
-  cudaError_t err = cudaSuccess;
-  unsigned *d_box = nullptr; unsigned h_box[6];
-  pu64 *d_keys = nullptr, *d_ucell = nullptr; int *d_order = nullptr, *d_flags = nullptr, *d_pos = nullptr, *d_cstart = nullptr;
-  float4 *d_sorted = nullptr;
+// uniform grid over the points ids[k] (k < n); *out receives the device arrays g points into
+cudaError_t build_grid(cudaStream_t st, const float *d_xyz, const int *d_ids, int n, float cell, GridArgs *g, GridBufs *out) {
+  DevBuf<unsigned> d_box; unsigned h_box[6];
+  DevBuf<pu64> d_keys; DevBuf<int> d_flags, d_pos;
+  GridBufs b;
   int nu = 0;
-  PCK(pmalloc(&d_box, 6));
-  { const unsigned init[6] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u}; PCK(pcopy(d_box, init, sizeof(init), P_H2D, st)); }
-  GHICP_LAUNCH(k_bbox, n < GHICP_SMS * 8 * PT ? blocks(n) : GHICP_SMS * 8, PT, 0, st, d_xyz, d_ids, n, d_box, d_box + 3);
-  PCK(pcopy(h_box, d_box, sizeof(h_box), P_D2H, st)); PCK(psync(st));
+  CUDA_TRY(d_box.alloc(6));
+  const unsigned init[6] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u};
+  CUDA_TRY(cudaMemcpyAsync(d_box.get(), init, sizeof(init), cudaMemcpyHostToDevice, st));
+  GHICP_LAUNCH(k_bbox, n < GHICP_SMS * 8 * PT ? blocks(n) : GHICP_SMS * 8, PT, 0, st, d_xyz, d_ids, n, d_box.get(), d_box.get() + 3);
+  CUDA_TRY(cudaMemcpyAsync(h_box, d_box.get(), sizeof(h_box), cudaMemcpyDeviceToHost, st)); CUDA_TRY(cudaStreamSynchronize(st));
   g->mnx = ord2f(h_box[0]); g->mny = ord2f(h_box[1]); g->mnz = ord2f(h_box[2]);
   g->inv = 1.0f / cell; g->r2 = cell * cell;
-  PCK(pmalloc(&d_keys, (size_t)n)); PCK(pmalloc(&d_order, (size_t)n)); PCK(pmalloc(&d_flags, (size_t)n + 1)); PCK(pmalloc(&d_pos, (size_t)n + 1));
-  GHICP_LAUNCH(k_cell_keys, blocks(n), PT, 0, st, d_xyz, d_ids, n, g->mnx, g->mny, g->mnz, g->inv, d_keys, d_order);
-  PCK(sort_pairs(d_keys, d_order, n, st));
-  GHICP_LAUNCH(k_run_heads, blocks(n + 1), PT, 0, st, d_keys, n, 0, d_flags);
-  PCK(exclusive_scan(d_flags, d_pos, n, st));
-  PCK(pcopy(&nu, d_pos + n, sizeof(int), P_D2H, st)); PCK(psync(st));
-  PCK(pmalloc(&d_ucell, (size_t)nu)); PCK(pmalloc(&d_cstart, (size_t)nu + 1));
-  GHICP_LAUNCH(k_cell_table, blocks(n + 1), PT, 0, st, d_keys, d_flags, d_pos, n, d_ucell, d_cstart);
-  PCK(pmalloc(&d_sorted, (size_t)n));
-  GHICP_LAUNCH(k_gather_sorted, blocks(n), PT, 0, st, d_xyz, d_ids, d_order, n, d_sorted);
-  g->xyz = d_xyz; g->ids = d_ids; g->order = d_order; g->sorted = d_sorted; g->ucell = d_ucell; g->cstart = d_cstart; g->nu = nu;
-  *o_order = d_order; *o_ucell = d_ucell; *o_cstart = d_cstart; *o_sorted = d_sorted;
-  d_order = nullptr; d_ucell = nullptr; d_cstart = nullptr; d_sorted = nullptr;
-done:
-  pfree(d_box); pfree(d_keys); pfree(d_flags); pfree(d_pos); pfree(d_order); pfree(d_ucell); pfree(d_cstart); pfree(d_sorted);
-  return err;
+  CUDA_TRY(d_keys.alloc((size_t)n)); CUDA_TRY(b.order.alloc((size_t)n)); CUDA_TRY(d_flags.alloc((size_t)n + 1)); CUDA_TRY(d_pos.alloc((size_t)n + 1));
+  GHICP_LAUNCH(k_cell_keys, blocks(n), PT, 0, st, d_xyz, d_ids, n, g->mnx, g->mny, g->mnz, g->inv, d_keys.get(), b.order.get());
+  CUDA_TRY(sort_pairs(d_keys.get(), b.order.get(), n, st));
+  GHICP_LAUNCH(k_run_heads, blocks(n + 1), PT, 0, st, d_keys.get(), n, 0, d_flags.get());
+  CUDA_TRY(exclusive_scan(d_flags.get(), d_pos.get(), n, st));
+  CUDA_TRY(cudaMemcpyAsync(&nu, d_pos.get() + n, sizeof(int), cudaMemcpyDeviceToHost, st)); CUDA_TRY(cudaStreamSynchronize(st));
+  CUDA_TRY(b.ucell.alloc((size_t)nu)); CUDA_TRY(b.cstart.alloc((size_t)nu + 1));
+  GHICP_LAUNCH(k_cell_table, blocks(n + 1), PT, 0, st, d_keys.get(), d_flags.get(), d_pos.get(), n, b.ucell.get(), b.cstart.get());
+  CUDA_TRY(b.sorted.alloc((size_t)n));
+  GHICP_LAUNCH(k_gather_sorted, blocks(n), PT, 0, st, d_xyz, d_ids, b.order.get(), n, b.sorted.get());
+  g->xyz = d_xyz; g->ids = d_ids; g->order = b.order.get(); g->sorted = b.sorted.get(); g->ucell = b.ucell.get();
+  g->cstart = b.cstart.get(); g->nu = nu;
+  *out = std::move(b);
+  return cudaSuccess;
 }
 
 }  // namespace
 
 // CFilter::voxelfilter on device arrays: d_out (capacity n + 1) receives the kept indices in output order
 cudaError_t prep_voxel_downsample(cudaStream_t st, const float *d_xyz, int n, float voxel_size, int *d_out, int *n_out) {
-  cudaError_t err = cudaSuccess;
-  unsigned *d_box = nullptr; unsigned h_box[6];
-  pu64 *d_keys = nullptr; int *d_vals = nullptr, *d_flags = nullptr, *d_pos = nullptr;
+  DevBuf<unsigned> d_box; unsigned h_box[6];
+  DevBuf<pu64> d_keys; DevBuf<int> d_vals, d_flags, d_pos;
   *n_out = 0;
   if (n <= 0) return cudaSuccess;
-  {
-    PCK(pmalloc(&d_box, 6));
-    const unsigned init[6] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u};
-    PCK(pcopy(d_box, init, sizeof(init), P_H2D, st));
-    GHICP_LAUNCH(k_bbox, n < GHICP_SMS * 8 * PT ? blocks(n) : GHICP_SMS * 8, PT, 0, st, d_xyz, (const int *)nullptr, n, d_box, d_box + 3);
-    PCK(pcopy(h_box, d_box, sizeof(h_box), P_D2H, st)); PCK(psync(st));
-    const float mn[3] = {ord2f(h_box[0]), ord2f(h_box[1]), ord2f(h_box[2])}, mx[3] = {ord2f(h_box[3]), ord2f(h_box[4]), ord2f(h_box[5])};
-    const float inv = 1.0f / voxel_size;                                   // include/filter.hpp:30
-    const float gy = mx[1] - mn[1], gz = mx[2] - mn[2];                    // :36
-    const pu64 max_vy = (pu64)(ceilf(gy * inv) + 1), max_vz = (pu64)(ceilf(gz * inv) + 1);   // :39-40
-    const pu64 mul_vx = max_vy * max_vz, mul_vy = max_vz;                  // :48-49
-    PCK(pmalloc(&d_keys, (size_t)n)); PCK(pmalloc(&d_vals, (size_t)n)); PCK(pmalloc(&d_flags, (size_t)n + 1)); PCK(pmalloc(&d_pos, (size_t)n + 1));
-    GHICP_LAUNCH(k_voxel_keys, blocks(n), PT, 0, st, d_xyz, n, mn[0], mn[1], mn[2], inv, mul_vx, mul_vy, d_keys, d_vals);
-    PCK(sort_pairs(d_keys, d_vals, n, st));          // stable: ascending index inside a voxel
-    // the reference's phantom entries {voxel 0, index 0} (:52) put point 0 first and absorb the real voxel-0 run
-    GHICP_LAUNCH(k_run_heads, blocks(n + 1), PT, 0, st, d_keys, n, 1, d_flags);
-    PCK(exclusive_scan(d_flags, d_pos, n, st));
-    int runs = 0;
-    PCK(pcopy(&runs, d_pos + n, sizeof(int), P_D2H, st)); PCK(psync(st));
-    GHICP_LAUNCH(k_voxel_emit, blocks(n), PT, 0, st, d_vals, d_flags, d_pos, n, 1, d_out);
-    PCK(psync(st));
-    *n_out = runs + 1;
-  }
-done:
-  pfree(d_box); pfree(d_keys); pfree(d_vals); pfree(d_flags); pfree(d_pos);
-  return err;
+  CUDA_TRY(d_box.alloc(6));
+  const unsigned init[6] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u};
+  CUDA_TRY(cudaMemcpyAsync(d_box.get(), init, sizeof(init), cudaMemcpyHostToDevice, st));
+  GHICP_LAUNCH(k_bbox, n < GHICP_SMS * 8 * PT ? blocks(n) : GHICP_SMS * 8, PT, 0, st, d_xyz, (const int *)nullptr, n, d_box.get(), d_box.get() + 3);
+  CUDA_TRY(cudaMemcpyAsync(h_box, d_box.get(), sizeof(h_box), cudaMemcpyDeviceToHost, st)); CUDA_TRY(cudaStreamSynchronize(st));
+  const float mn[3] = {ord2f(h_box[0]), ord2f(h_box[1]), ord2f(h_box[2])}, mx[3] = {ord2f(h_box[3]), ord2f(h_box[4]), ord2f(h_box[5])};
+  const float inv = 1.0f / voxel_size;                                   // include/filter.hpp:30
+  const float gy = mx[1] - mn[1], gz = mx[2] - mn[2];                    // :36
+  const pu64 max_vy = (pu64)(ceilf(gy * inv) + 1), max_vz = (pu64)(ceilf(gz * inv) + 1);   // :39-40
+  const pu64 mul_vx = max_vy * max_vz, mul_vy = max_vz;                  // :48-49
+  CUDA_TRY(d_keys.alloc((size_t)n)); CUDA_TRY(d_vals.alloc((size_t)n)); CUDA_TRY(d_flags.alloc((size_t)n + 1)); CUDA_TRY(d_pos.alloc((size_t)n + 1));
+  GHICP_LAUNCH(k_voxel_keys, blocks(n), PT, 0, st, d_xyz, n, mn[0], mn[1], mn[2], inv, mul_vx, mul_vy, d_keys.get(), d_vals.get());
+  CUDA_TRY(sort_pairs(d_keys.get(), d_vals.get(), n, st));          // stable: ascending index inside a voxel
+  // the reference's phantom entries {voxel 0, index 0} (:52) put point 0 first and absorb the real voxel-0 run
+  GHICP_LAUNCH(k_run_heads, blocks(n + 1), PT, 0, st, d_keys.get(), n, 1, d_flags.get());
+  CUDA_TRY(exclusive_scan(d_flags.get(), d_pos.get(), n, st));
+  int runs = 0;
+  CUDA_TRY(cudaMemcpyAsync(&runs, d_pos.get() + n, sizeof(int), cudaMemcpyDeviceToHost, st)); CUDA_TRY(cudaStreamSynchronize(st));
+  GHICP_LAUNCH(k_voxel_emit, blocks(n), PT, 0, st, d_vals.get(), d_flags.get(), d_pos.get(), n, 1, d_out);
+  CUDA_TRY(cudaStreamSynchronize(st));
+  *n_out = runs + 1;
+  return cudaSuccess;
 }
 
 // keypointDetectionBasedOnCurvature on device arrays.  d_lam [n][3], d_curv [n], d_cnt [n], d_kp (capacity n).
 cudaError_t prep_detect_keypoints(cudaStream_t st, const float *d_xyz, int n, float radius, float ratio_max, int min_pts,
                                   float nms_radius, float *d_lam, double *d_curv, int *d_cnt, int *d_kp, int *n_kp,
                                   int *nms_rounds) {
-  cudaError_t err = cudaSuccess;
   GridArgs g{}, g2{};
-  int *order = nullptr, *cstart = nullptr, *order2 = nullptr, *cstart2 = nullptr; pu64 *ucell = nullptr, *ucell2 = nullptr;
-  float4 *sorted = nullptr, *sorted2 = nullptr;
-  int *d_flags = nullptr, *d_pos = nullptr, *d_cand = nullptr, *d_state = nullptr, *d_und = nullptr; pu64 *d_keys = nullptr;
+  GridBufs grid, grid2;
+  DevBuf<int> d_flags, d_pos, d_cand, d_state, d_und; DevBuf<pu64> d_keys;
   int m = 0, rounds = 0;
   *n_kp = 0;
   if (nms_rounds) *nms_rounds = 0;
   if (n <= 0) return cudaSuccess;
-  {
-    PCK(build_grid(st, d_xyz, nullptr, n, radius, &g, &order, &ucell, &cstart, &sorted));
-    GHICP_LAUNCH(k_pca, blocks(n), PT, 0, st, g, n, d_lam, d_curv, d_cnt);
-    PCK(pmalloc(&d_flags, (size_t)n + 1)); PCK(pmalloc(&d_pos, (size_t)n + 1));
-    GHICP_LAUNCH(k_prune, blocks(n + 1), PT, 0, st, d_lam, d_cnt, n, ratio_max, min_pts, d_flags);
-    PCK(exclusive_scan(d_flags, d_pos, n, st));
-    PCK(pcopy(&m, d_pos + n, sizeof(int), P_D2H, st)); PCK(psync(st));
-    if (m == 0) goto done;
-    PCK(pmalloc(&d_cand, (size_t)m)); PCK(pmalloc(&d_keys, (size_t)m));
-    GHICP_LAUNCH(k_cand_emit, blocks(n), PT, 0, st, d_flags, d_pos, d_curv, n, d_keys, d_cand);
-    PCK(sort_pairs(d_keys, d_cand, m, st));   // rank order: descending curvature, ties by ascending index (stable)
-    PCK(build_grid(st, d_xyz, d_cand, m, nms_radius, &g2, &order2, &ucell2, &cstart2, &sorted2));
-    PCK(pmalloc(&d_state, (size_t)m)); PCK(pmalloc(&d_und, 1));
-    PCK(pzero(d_state, sizeof(int) * (size_t)m, st));
-    for (;;) {
-      int und = 0;
-      PCK(pzero(d_und, sizeof(int), st));
-      GHICP_LAUNCH(k_nms_round, blocks(m), PT, 0, st, g2, m, d_state, d_und);
-      PCK(pcopy(&und, d_und, sizeof(int), P_D2H, st)); PCK(psync(st));
-      ++rounds;
-      if (und == 0) break;
-      if (rounds > m + 1) { err = cudaErrorInvalidValue; goto done; }   // cannot happen: the best undecided rank decides every round
-    }
-    pfree(d_flags); pfree(d_pos); d_flags = d_pos = nullptr;
-    PCK(pmalloc(&d_flags, (size_t)m + 1)); PCK(pmalloc(&d_pos, (size_t)m + 1));
-    GHICP_LAUNCH(k_kept_flags, blocks(m + 1), PT, 0, st, d_state, m, d_flags);
-    PCK(exclusive_scan(d_flags, d_pos, m, st));
-    PCK(pcopy(n_kp, d_pos + m, sizeof(int), P_D2H, st)); PCK(psync(st));
-    GHICP_LAUNCH(k_kp_emit, blocks(m), PT, 0, st, d_flags, d_pos, d_cand, m, d_kp);
-    PCK(psync(st));
-    if (nms_rounds) *nms_rounds = rounds;
+  CUDA_TRY(build_grid(st, d_xyz, nullptr, n, radius, &g, &grid));
+  GHICP_LAUNCH(k_pca, blocks(n), PT, 0, st, g, n, d_lam, d_curv, d_cnt);
+  CUDA_TRY(d_flags.alloc((size_t)n + 1)); CUDA_TRY(d_pos.alloc((size_t)n + 1));
+  GHICP_LAUNCH(k_prune, blocks(n + 1), PT, 0, st, d_lam, d_cnt, n, ratio_max, min_pts, d_flags.get());
+  CUDA_TRY(exclusive_scan(d_flags.get(), d_pos.get(), n, st));
+  CUDA_TRY(cudaMemcpyAsync(&m, d_pos.get() + n, sizeof(int), cudaMemcpyDeviceToHost, st)); CUDA_TRY(cudaStreamSynchronize(st));
+  if (m == 0) return cudaSuccess;
+  CUDA_TRY(d_cand.alloc((size_t)m)); CUDA_TRY(d_keys.alloc((size_t)m));
+  GHICP_LAUNCH(k_cand_emit, blocks(n), PT, 0, st, d_flags.get(), d_pos.get(), d_curv, n, d_keys.get(), d_cand.get());
+  CUDA_TRY(sort_pairs(d_keys.get(), d_cand.get(), m, st));   // rank order: descending curvature, ties by ascending index (stable)
+  CUDA_TRY(build_grid(st, d_xyz, d_cand.get(), m, nms_radius, &g2, &grid2));
+  CUDA_TRY(d_state.alloc((size_t)m)); CUDA_TRY(d_und.alloc(1));
+  CUDA_TRY(cudaMemsetAsync(d_state.get(), 0, sizeof(int) * (size_t)m, st));
+  for (;;) {
+    int und = 0;
+    CUDA_TRY(cudaMemsetAsync(d_und.get(), 0, sizeof(int), st));
+    GHICP_LAUNCH(k_nms_round, blocks(m), PT, 0, st, g2, m, d_state.get(), d_und.get());
+    CUDA_TRY(cudaMemcpyAsync(&und, d_und.get(), sizeof(int), cudaMemcpyDeviceToHost, st)); CUDA_TRY(cudaStreamSynchronize(st));
+    ++rounds;
+    if (und == 0) break;
+    if (rounds > m + 1) return cudaErrorInvalidValue;   // cannot happen: the best undecided rank decides every round
   }
-done:
-  pfree(order); pfree(ucell); pfree(cstart); pfree(order2); pfree(ucell2); pfree(cstart2); pfree(sorted); pfree(sorted2);
-  pfree(d_flags); pfree(d_pos); pfree(d_cand); pfree(d_state); pfree(d_und); pfree(d_keys);
-  return err;
+  d_flags.reset(); d_pos.reset();
+  CUDA_TRY(d_flags.alloc((size_t)m + 1)); CUDA_TRY(d_pos.alloc((size_t)m + 1));
+  GHICP_LAUNCH(k_kept_flags, blocks(m + 1), PT, 0, st, d_state.get(), m, d_flags.get());
+  CUDA_TRY(exclusive_scan(d_flags.get(), d_pos.get(), m, st));
+  CUDA_TRY(cudaMemcpyAsync(n_kp, d_pos.get() + m, sizeof(int), cudaMemcpyDeviceToHost, st)); CUDA_TRY(cudaStreamSynchronize(st));
+  GHICP_LAUNCH(k_kp_emit, blocks(m), PT, 0, st, d_flags.get(), d_pos.get(), d_cand.get(), m, d_kp);
+  CUDA_TRY(cudaStreamSynchronize(st));
+  if (nms_rounds) *nms_rounds = rounds;
+  return cudaSuccess;
 }
 
 
@@ -530,20 +484,15 @@ cudaError_t prep_kp_coords(cudaStream_t st, const float *d_xyz, const int *d_kp,
 }
 // pcl::getMinMax3D of a device cloud (the bounding box the driver takes its bbx_magnitude from, test/ghicp_main.cpp:91-93)
 cudaError_t prep_bounds(cudaStream_t st, const float *d_xyz, int n, float mn[3], float mx[3]) {
-  cudaError_t err = cudaSuccess;
-  unsigned *d_box = nullptr; unsigned h_box[6];
+  DevBuf<unsigned> d_box; unsigned h_box[6];
   if (n <= 0) return cudaErrorInvalidValue;
-  {
-    PCK(pmalloc(&d_box, 6));
-    const unsigned init[6] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u};
-    PCK(pcopy(d_box, init, sizeof(init), P_H2D, st));
-    GHICP_LAUNCH(k_bbox, n < GHICP_SMS * 8 * PT ? blocks(n) : GHICP_SMS * 8, PT, 0, st, d_xyz, (const int *)nullptr, n, d_box, d_box + 3);
-    PCK(pcopy(h_box, d_box, sizeof(h_box), P_D2H, st)); PCK(psync(st));
-    for (int a = 0; a < 3; ++a) { mn[a] = ord2f(h_box[a]); mx[a] = ord2f(h_box[3 + a]); }
-  }
-done:
-  pfree(d_box);
-  return err;
+  CUDA_TRY(d_box.alloc(6));
+  const unsigned init[6] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u};
+  CUDA_TRY(cudaMemcpyAsync(d_box.get(), init, sizeof(init), cudaMemcpyHostToDevice, st));
+  GHICP_LAUNCH(k_bbox, n < GHICP_SMS * 8 * PT ? blocks(n) : GHICP_SMS * 8, PT, 0, st, d_xyz, (const int *)nullptr, n, d_box.get(), d_box.get() + 3);
+  CUDA_TRY(cudaMemcpyAsync(h_box, d_box.get(), sizeof(h_box), cudaMemcpyDeviceToHost, st)); CUDA_TRY(cudaStreamSynchronize(st));
+  for (int a = 0; a < 3; ++a) { mn[a] = ord2f(h_box[a]); mx[a] = ord2f(h_box[3 + a]); }
+  return cudaSuccess;
 }
 
 // =====================================================================================================================
@@ -889,27 +838,19 @@ __global__ void __launch_bounds__(BSC_T) k_bsc(const BscArgs a) {
 // d_bits [V][nkp][ceil(9 side^2 / 8)] with V = 1 (dof_type 0), 2 (1..4), 4 (> 4); d_lrf [nkp][12] and d_status [nkp] may be null.
 cudaError_t prep_bsc_extract(cudaStream_t st, const float *d_xyz, int n, const int *d_kp, int nkp, float R, int side,
                              const int *d_pairs, int dof_type, unsigned char *d_bits, float *d_lrf, int *d_status) {
-  cudaError_t err = cudaSuccess;
   GridArgs g{};
-  int *order = nullptr, *cstart = nullptr; pu64 *ucell = nullptr; float4 *sorted = nullptr;
+  GridBufs grid;
   if (n <= 0 || nkp <= 0) return cudaSuccess;
   if (side < 1 || side > BSC_MAX_SIDE) return cudaErrorInvalidValue;
-  {
-    const float search = (float)(sqrt(3.0) * (double)R);            // :643; squared in float32 like the radius of S4
-    PCK(build_grid(st, d_xyz, nullptr, n, search, &g, &order, &ucell, &cstart, &sorted));
-    BscArgs a{};
-    a.g = g; a.kp = d_kp; a.nkp = nkp; a.R = R; a.side = side; a.pairs = d_pairs;
-    a.V = dof_type > 4 ? 4 : (dof_type > 0 ? 2 : 1);
-    a.bits = d_bits; a.nbytes = (9 * side * side + 7) / 8; a.lrf = d_lrf; a.status = d_status;
-    GHICP_LAUNCH(k_bsc, nkp, BSC_T, 0, st, a);
-    PCK(psync(st));
-#if !defined(GHICP_EMU_HOST)
-    PCK(cudaGetLastError());
-#endif
-  }
-done:
-  pfree(order); pfree(ucell); pfree(cstart); pfree(sorted);
-  return err;
+  const float search = (float)(sqrt(3.0) * (double)R);            // :643; squared in float32 like the radius of S4
+  CUDA_TRY(build_grid(st, d_xyz, nullptr, n, search, &g, &grid));
+  BscArgs a{};
+  a.g = g; a.kp = d_kp; a.nkp = nkp; a.R = R; a.side = side; a.pairs = d_pairs;
+  a.V = dof_type > 4 ? 4 : (dof_type > 0 ? 2 : 1);
+  a.bits = d_bits; a.nbytes = (9 * side * side + 7) / 8; a.lrf = d_lrf; a.status = d_status;
+  GHICP_LAUNCH(k_bsc, nkp, BSC_T, 0, st, a);
+  CUDA_TRY(cudaStreamSynchronize(st));
+  return cudaGetLastError();
 }
 
 // =====================================================================================================================
@@ -1305,32 +1246,30 @@ cudaError_t segmented_sort(const pu64 *in, pu64 *out, long long total, int m, co
   constexpr long long CHUNK = 1ll << 30;
   const int nch = (int)((total + CHUNK - 1) / CHUNK);
   if (nch == 0) return cudaSuccess;
-  cudaError_t err = cudaSuccess;
-  int *d_bounds = nullptr, *rel = nullptr; void *tmp = nullptr;
+  DevBuf<int> d_bounds, rel; DevBuf<unsigned char> tmp;
   size_t tmp_bytes = 0;
   std::vector<int> bounds(nch + 1);
-  PCK(pmalloc(&d_bounds, (size_t)nch + 1)); PCK(pmalloc(&rel, (size_t)m + 1));
-  GHICP_LAUNCH(k_chunk_bounds, blocks(nch + 1), PT, 0, st, off, m, CHUNK, nch, d_bounds);
-  PCK(pcopy(bounds.data(), d_bounds, sizeof(int) * (nch + 1), P_D2H, st)); PCK(psync(st));
+  CUDA_TRY(d_bounds.alloc((size_t)nch + 1)); CUDA_TRY(rel.alloc((size_t)m + 1));
+  GHICP_LAUNCH(k_chunk_bounds, blocks(nch + 1), PT, 0, st, off, m, CHUNK, nch, d_bounds.get());
+  CUDA_TRY(cudaMemcpyAsync(bounds.data(), d_bounds.get(), sizeof(int) * (nch + 1), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
   for (int c = 0; c < nch; ++c) {
     const int r0 = bounds[c], r1 = bounds[c + 1];
     if (r1 <= r0) continue;
     long long lo = 0, hi = 0;
-    PCK(pcopy(&lo, off + r0, sizeof(lo), P_D2H, st)); PCK(pcopy(&hi, off + r1, sizeof(hi), P_D2H, st)); PCK(psync(st));
-    if (hi - lo > INT_MAX) { err = cudaErrorInvalidValue; goto done; }   // one row of more than 2^31 - 2^30 entries
-    GHICP_LAUNCH(k_rel_offsets, blocks(r1 - r0 + 1), PT, 0, st, off, r0, r1, rel);
+    CUDA_TRY(cudaMemcpyAsync(&lo, off + r0, sizeof(lo), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(&hi, off + r1, sizeof(hi), cudaMemcpyDeviceToHost, st)); CUDA_TRY(cudaStreamSynchronize(st));
+    if (hi - lo > INT_MAX) return cudaErrorInvalidValue;   // one row of more than 2^31 - 2^30 entries
+    GHICP_LAUNCH(k_rel_offsets, blocks(r1 - r0 + 1), PT, 0, st, off, r0, r1, rel.get());
     size_t need = 0;
-    PCK(cub::DeviceSegmentedSort::SortKeys(nullptr, need, in + lo, out + lo, (int)(hi - lo), r1 - r0, rel, rel + 1, st));
+    CUDA_TRY(cub::DeviceSegmentedSort::SortKeys(nullptr, need, in + lo, out + lo, (int)(hi - lo), r1 - r0, rel.get(), rel.get() + 1, st));
     if (need > tmp_bytes) {
-      if (tmp) cudaFreeAsync(tmp, st);
-      tmp = nullptr; tmp_bytes = need;
-      PCK(cudaMallocAsync(&tmp, tmp_bytes ? tmp_bytes : 1, st));
+      tmp_bytes = need;
+      CUDA_TRY(tmp.alloc(tmp_bytes, st));
     }
-    PCK(cub::DeviceSegmentedSort::SortKeys(tmp, need, in + lo, out + lo, (int)(hi - lo), r1 - r0, rel, rel + 1, st));
+    CUDA_TRY(cub::DeviceSegmentedSort::SortKeys(tmp.get(), need, in + lo, out + lo, (int)(hi - lo), r1 - r0, rel.get(), rel.get() + 1, st));
   }
-done:
-  pfree(d_bounds); pfree(rel); if (tmp) cudaFreeAsync(tmp, st);
-  return err;
+  return cudaSuccess;
 }
 #endif
 
@@ -1338,51 +1277,40 @@ done:
 
 // The grid of a ring search over d_xyz [n][3] (see PointGrid).
 cudaError_t prep_point_grid(cudaStream_t st, const float *d_xyz, int n, int ke, float cell_scale, double min_cell, PointGrid *out) {
-  cudaError_t err = cudaSuccess;
   GridArgs g{};
-  int *order = nullptr, *cstart = nullptr; pu64 *ucell = nullptr; float4 *sorted = nullptr;
+  GridBufs grid;
   float mn[3], mx[3];
   *out = PointGrid();
   if (n <= 0 || ke <= 0) return cudaErrorInvalidValue;
-  PCK(prep_bounds(st, d_xyz, n, mn, mx));
-  {
-    // Cell edge from the data: a volume guess (k points per cell if the cloud filled its box), then corrected once by the
-    // observed mean occupancy of the occupied cells assuming a surface (occupancy ~ edge^2), aiming at 0.4 k per cell —
-    // enough for the k nearest to lie within one ring.  The results do not depend on it; the work per query does.
-    double ext[3], emax = 0.0;
-    for (int a = 0; a < 3; ++a) { ext[a] = (double)mx[a] - (double)mn[a]; emax = ext[a] > emax ? ext[a] : emax; }
-    double cell = 1.0;
-    if (emax > 0.0) {
-      double vol = 1.0;
-      for (int a = 0; a < 3; ++a) vol *= ext[a] > 1e-3 * emax ? ext[a] : 1e-3 * emax;
-      cell = cbrt(vol * ke / n);
-      PCK(build_grid(st, d_xyz, nullptr, n, (float)cell, &g, &order, &ucell, &cstart, &sorted));
-      const double occ = (double)n / g.nu;
-      double f = sqrt(0.4 * ke / occ);
-      f = f < 1.0 / 16 ? 1.0 / 16 : (f > 16.0 ? 16.0 : f);
-      cell *= f;
-      pfree(order); pfree(ucell); pfree(cstart); pfree(sorted); order = cstart = nullptr; ucell = nullptr; sorted = nullptr;
-    }
-    if (cell_scale > 0.f) cell *= cell_scale;
-    if (cell < min_cell) cell = min_cell;
-    if (cell < emax / 1048576.0) cell = emax / 1048576.0;   // cell coordinates stay below 2^20 (21-bit key fields)
-    PCK(build_grid(st, d_xyz, nullptr, n, (float)cell, &g, &order, &ucell, &cstart, &sorted));
-    out->g = g;
-    out->gx = cell_coord_host(mx[0], g.mnx, g.inv); out->gy = cell_coord_host(mx[1], g.mny, g.inv); out->gz = cell_coord_host(mx[2], g.mnz, g.inv);
-    for (int a = 0; a < 3; ++a) out->mx[a] = mx[a];
-    out->cell = (double)(float)cell;
-    const int gmax = out->gx > out->gy ? (out->gx > out->gz ? out->gx : out->gz) : (out->gy > out->gz ? out->gy : out->gz);
-    out->slack = 0.01 + (gmax + 2.0) / 1048576.0;
-    out->order = order; out->ucell = ucell; out->cstart = cstart; out->sorted = sorted;
-    order = cstart = nullptr; ucell = nullptr; sorted = nullptr;
+  CUDA_TRY(prep_bounds(st, d_xyz, n, mn, mx));
+  // Cell edge from the data: a volume guess (k points per cell if the cloud filled its box), then corrected once by the
+  // observed mean occupancy of the occupied cells assuming a surface (occupancy ~ edge^2), aiming at 0.4 k per cell —
+  // enough for the k nearest to lie within one ring.  The results do not depend on it; the work per query does.
+  double ext[3], emax = 0.0;
+  for (int a = 0; a < 3; ++a) { ext[a] = (double)mx[a] - (double)mn[a]; emax = ext[a] > emax ? ext[a] : emax; }
+  double cell = 1.0;
+  if (emax > 0.0) {
+    double vol = 1.0;
+    for (int a = 0; a < 3; ++a) vol *= ext[a] > 1e-3 * emax ? ext[a] : 1e-3 * emax;
+    cell = cbrt(vol * ke / n);
+    CUDA_TRY(build_grid(st, d_xyz, nullptr, n, (float)cell, &g, &grid));
+    const double occ = (double)n / g.nu;
+    double f = sqrt(0.4 * ke / occ);
+    f = f < 1.0 / 16 ? 1.0 / 16 : (f > 16.0 ? 16.0 : f);
+    cell *= f;
+    grid = GridBufs();
   }
-done:
-  pfree(order); pfree(ucell); pfree(cstart); pfree(sorted);
-  return err;
-}
-void prep_point_grid_free(PointGrid *g) {
-  pfree(g->order); pfree(g->ucell); pfree(g->cstart); pfree(g->sorted);
-  *g = PointGrid();
+  if (cell_scale > 0.f) cell *= cell_scale;
+  if (cell < min_cell) cell = min_cell;
+  if (cell < emax / 1048576.0) cell = emax / 1048576.0;   // cell coordinates stay below 2^20 (21-bit key fields)
+  CUDA_TRY(build_grid(st, d_xyz, nullptr, n, (float)cell, &g, &out->buf));
+  out->g = g;
+  out->gx = cell_coord_host(mx[0], g.mnx, g.inv); out->gy = cell_coord_host(mx[1], g.mny, g.inv); out->gz = cell_coord_host(mx[2], g.mnz, g.inv);
+  for (int a = 0; a < 3; ++a) out->mx[a] = mx[a];
+  out->cell = (double)(float)cell;
+  const int gmax = out->gx > out->gy ? (out->gx > out->gz ? out->gx : out->gz) : (out->gy > out->gz ? out->gy : out->gz);
+  out->slack = 0.01 + (gmax + 2.0) / 1048576.0;
+  return cudaSuccess;
 }
 cudaError_t prep_sort_pairs(cudaStream_t st, pu64 *keys, int *vals, int n) { return sort_pairs(keys, vals, n, st); }
 
@@ -1393,84 +1321,133 @@ cudaError_t prep_sort_pairs(cudaStream_t st, pu64 *keys, int *vals, int n) { ret
 cudaError_t prep_fpfh(cudaStream_t st, const float *d_xyz, int n, const int *d_idx, int nidx, int k, float cell_scale,
                       float *d_fpfh, float *d_normals, int *d_status, int *d_nb_idx, float *d_nb_d2, cudaEvent_t ev_mid,
                       FpfhStats *stats) {
-  cudaError_t err = cudaSuccess;
   PointGrid pg;
-  int *nb_idx = nullptr, *need = nullptr, *d_fb = nullptr; float *nb_d2 = nullptr, *spfh = nullptr;
-  unsigned long long *d_cand = nullptr;
+  DevBuf<int> nb_idx, need, d_fb; DevBuf<float> nb_d2, spfh; DevBuf<pu64> d_cand;
   if (stats) *stats = FpfhStats{};
   if (n <= 0 || k < 3 || k > FPFH_KMAX) return cudaErrorInvalidValue;
-  {
-    const int ke = k < n ? k : n;
-    PCK(prep_point_grid(st, d_xyz, n, ke, cell_scale, 0.0, &pg));
-    KnnArgs a{};
-    a.g = pg.g; a.n = n; a.k = ke;
-    a.gx = pg.gx; a.gy = pg.gy; a.gz = pg.gz;
-    a.cell = pg.cell; a.slack = pg.slack;
-    PCK(pmalloc(&nb_idx, (size_t)n * ke)); PCK(pmalloc(&nb_d2, (size_t)n * ke));
-    PCK(pmalloc(&d_cand, 1)); PCK(pmalloc(&d_fb, 1));
-    PCK(pzero(d_cand, sizeof(pu64), st)); PCK(pzero(d_fb, sizeof(int), st));
-    a.nb_idx = nb_idx; a.nb_d2 = nb_d2; a.cand = d_cand; a.fallbacks = d_fb;
-    GHICP_LAUNCH(k_knn, blocks(n), PT, 0, st, a);
-    GHICP_LAUNCH(k_normals, blocks(n), PT, 0, st, d_xyz, nb_idx, n, ke, d_normals, d_status);
-    if (d_nb_idx) PCK(pcopy(d_nb_idx, nb_idx, sizeof(int) * (size_t)n * ke, P_D2D, st));
-    if (d_nb_d2) PCK(pcopy(d_nb_d2, nb_d2, sizeof(float) * (size_t)n * ke, P_D2D, st));
-    if (ev_mid) PCK(cudaEventRecord(ev_mid, st));
-    PCK(pmalloc(&spfh, (size_t)n * 33));
-    if (d_idx) {
-      PCK(pmalloc(&need, (size_t)n));
-      PCK(pzero(need, sizeof(int) * (size_t)n, st));
-      if (nidx > 0) GHICP_LAUNCH(k_fpfh_mark, blocks(nidx), PT, 0, st, d_idx, nidx, nb_idx, ke, need);
-    }
-    GHICP_LAUNCH(k_spfh, blocks(n), PT, 0, st, d_xyz, d_normals, nb_idx, n, ke, need, spfh);
-    if (nidx > 0) GHICP_LAUNCH(k_fpfh, blocks(nidx), PT, 0, st, d_idx, nidx, nb_idx, nb_d2, ke, spfh, d_fpfh);
-    if (stats) {
-      pu64 c = 0; int fb = 0;
-      PCK(pcopy(&c, d_cand, sizeof(c), P_D2H, st)); PCK(pcopy(&fb, d_fb, sizeof(fb), P_D2H, st));
-      PCK(psync(st));
-      stats->candidates = (long long)c; stats->fallbacks = fb; stats->cell = (float)pg.cell; stats->queries = n;
-    }
-#if !defined(GHICP_EMU_HOST)
-    PCK(cudaGetLastError());
-#endif
+  const int ke = k < n ? k : n;
+  CUDA_TRY(prep_point_grid(st, d_xyz, n, ke, cell_scale, 0.0, &pg));
+  KnnArgs a{};
+  a.g = pg.g; a.n = n; a.k = ke;
+  a.gx = pg.gx; a.gy = pg.gy; a.gz = pg.gz;
+  a.cell = pg.cell; a.slack = pg.slack;
+  CUDA_TRY(nb_idx.alloc((size_t)n * ke)); CUDA_TRY(nb_d2.alloc((size_t)n * ke));
+  CUDA_TRY(d_cand.alloc(1)); CUDA_TRY(d_fb.alloc(1));
+  CUDA_TRY(cudaMemsetAsync(d_cand.get(), 0, sizeof(pu64), st)); CUDA_TRY(cudaMemsetAsync(d_fb.get(), 0, sizeof(int), st));
+  a.nb_idx = nb_idx.get(); a.nb_d2 = nb_d2.get(); a.cand = d_cand.get(); a.fallbacks = d_fb.get();
+  GHICP_LAUNCH(k_knn, blocks(n), PT, 0, st, a);
+  GHICP_LAUNCH(k_normals, blocks(n), PT, 0, st, d_xyz, nb_idx.get(), n, ke, d_normals, d_status);
+  if (d_nb_idx) CUDA_TRY(cudaMemcpyAsync(d_nb_idx, nb_idx.get(), sizeof(int) * (size_t)n * ke, cudaMemcpyDeviceToDevice, st));
+  if (d_nb_d2) CUDA_TRY(cudaMemcpyAsync(d_nb_d2, nb_d2.get(), sizeof(float) * (size_t)n * ke, cudaMemcpyDeviceToDevice, st));
+  if (ev_mid) CUDA_TRY(cudaEventRecord(ev_mid, st));
+  CUDA_TRY(spfh.alloc((size_t)n * 33));
+  if (d_idx) {
+    CUDA_TRY(need.alloc((size_t)n));
+    CUDA_TRY(cudaMemsetAsync(need.get(), 0, sizeof(int) * (size_t)n, st));
+    if (nidx > 0) GHICP_LAUNCH(k_fpfh_mark, blocks(nidx), PT, 0, st, d_idx, nidx, nb_idx.get(), ke, need.get());
   }
-done:
-  prep_point_grid_free(&pg);
-  pfree(nb_idx); pfree(nb_d2); pfree(need); pfree(spfh); pfree(d_cand); pfree(d_fb);
-  return err;
+  GHICP_LAUNCH(k_spfh, blocks(n), PT, 0, st, d_xyz, d_normals, nb_idx.get(), n, ke, need.get(), spfh.get());
+  if (nidx > 0) GHICP_LAUNCH(k_fpfh, blocks(nidx), PT, 0, st, d_idx, nidx, nb_idx.get(), nb_d2.get(), ke, spfh.get(), d_fpfh);
+  if (stats) {
+    pu64 c = 0; int fb = 0;
+    CUDA_TRY(cudaMemcpyAsync(&c, d_cand.get(), sizeof(c), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(&fb, d_fb.get(), sizeof(fb), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    stats->candidates = (long long)c; stats->fallbacks = fb; stats->cell = (float)pg.cell; stats->queries = n;
+  }
+  return cudaGetLastError();
 }
 
 namespace {
 // List rows in cell order: the points flagged in need (every point when need == nullptr).  rows [m], row_of [n] (-1: no row).
-cudaError_t make_rows(cudaStream_t st, const int *order, const int *need, int n, int *flags, int *pos, int **rows, int **row_of,
-                      int *m) {
-  cudaError_t err = cudaSuccess;
+cudaError_t make_rows(cudaStream_t st, const int *order, const int *need, int n, int *flags, int *pos, DevBuf<int> *rows,
+                      DevBuf<int> *row_of, int *m) {
   GHICP_LAUNCH(k_row_flags, blocks(n + 1), PT, 0, st, order, need, n, flags);
-  PCK(exclusive_scan(flags, pos, n, st));
-  PCK(pcopy(m, pos + n, sizeof(int), P_D2H, st)); PCK(psync(st));
-  PCK(pmalloc(rows, (size_t)*m)); PCK(pmalloc(row_of, (size_t)n));
-  PCK(cudaMemsetAsync(*row_of, 0xff, sizeof(int) * (size_t)n, st));
-  GHICP_LAUNCH(k_row_emit, blocks(n), PT, 0, st, order, flags, pos, n, *rows, *row_of);
-done:
-  return err;
+  CUDA_TRY(exclusive_scan(flags, pos, n, st));
+  CUDA_TRY(cudaMemcpyAsync(m, pos + n, sizeof(int), cudaMemcpyDeviceToHost, st)); CUDA_TRY(cudaStreamSynchronize(st));
+  CUDA_TRY(rows->alloc((size_t)*m)); CUDA_TRY(row_of->alloc((size_t)n));
+  CUDA_TRY(cudaMemsetAsync(row_of->get(), 0xff, sizeof(int) * (size_t)n, st));
+  GHICP_LAUNCH(k_row_emit, blocks(n), PT, 0, st, order, flags, pos, n, rows->get(), row_of->get());
+  return cudaSuccess;
 }
 // The sorted N_r lists of rows [m]: count, 64-bit offsets, budget check (cudaErrorMemoryAllocation before the entries are
-// allocated when *total > budget), fill, segmented sort.  off [m + 1] and key [*total] are the caller's to free.
-cudaError_t build_lists(cudaStream_t st, const RadWalk &w, const int *rows, int m, long long budget, long long **off, pu64 **key,
-                        long long *total) {
-  cudaError_t err = cudaSuccess;
-  long long *cnt = nullptr; pu64 *raw = nullptr;
+// allocated when *total > budget), fill, segmented sort into off [m + 1] and key [*total].
+cudaError_t build_lists(cudaStream_t st, const RadWalk &w, const int *rows, int m, long long budget, DevBuf<long long> *off,
+                        DevBuf<pu64> *key, long long *total) {
+  DevBuf<long long> cnt; DevBuf<pu64> raw;
   *total = 0;
-  PCK(pmalloc(&cnt, (size_t)m + 1)); PCK(pmalloc(off, (size_t)m + 1));
-  GHICP_LAUNCH(k_rad_count, blocks(m + 1), PT, 0, st, w, rows, m, cnt);
-  PCK(exclusive_scan64(cnt, *off, m, st));
-  PCK(pcopy(total, *off + m, sizeof(long long), P_D2H, st)); PCK(psync(st));
-  if (*total > budget) { err = cudaErrorMemoryAllocation; goto done; }
-  PCK(pmalloc(&raw, (size_t)*total)); PCK(pmalloc(key, (size_t)*total));
-  if (m > 0) GHICP_LAUNCH(k_rad_fill, blocks(m), PT, 0, st, w, rows, m, *off, raw);
-  PCK(segmented_sort(raw, *key, *total, m, *off, st));
-done:
-  pfree(cnt); pfree(raw);
-  return err;
+  CUDA_TRY(cnt.alloc((size_t)m + 1)); CUDA_TRY(off->alloc((size_t)m + 1));
+  GHICP_LAUNCH(k_rad_count, blocks(m + 1), PT, 0, st, w, rows, m, cnt.get());
+  CUDA_TRY(exclusive_scan64(cnt.get(), off->get(), m, st));
+  CUDA_TRY(cudaMemcpyAsync(total, off->get() + m, sizeof(long long), cudaMemcpyDeviceToHost, st)); CUDA_TRY(cudaStreamSynchronize(st));
+  if (*total > budget) return cudaErrorMemoryAllocation;
+  CUDA_TRY(raw.alloc((size_t)*total)); CUDA_TRY(key->alloc((size_t)*total));
+  if (m > 0) GHICP_LAUNCH(k_rad_fill, blocks(m), PT, 0, st, w, rows, m, off->get(), raw.get());
+  return segmented_sort(raw.get(), key->get(), *total, m, off->get(), st);
+}
+// prep_fpfh_radius after the argument checks; *s receives the statistics as far as the call got
+cudaError_t fpfh_radius_run(cudaStream_t st, const float *d_xyz, int n, const int *d_idx, int nidx, float rn, float rf,
+                            long long nb_max, float *d_fpfh, float *d_normals, int *d_status, cudaEvent_t ev_lists,
+                            cudaEvent_t ev_normals, FpfhRadiusStats *s) {
+  GridArgs g{};
+  GridBufs grid;
+  DevBuf<int> need, flags, pos, rows_f, row_of_f, rows_n, row_of_n;
+  DevBuf<long long> off_f, off_n; DevBuf<pu64> key_f, key_n;
+  DevBuf<float> spfh;
+  float mn[3], mx[3];
+  int m_f = 0, m_n = 0;
+  long long budget;
+  {
+    size_t fr = 0, tot = 0;
+    CUDA_TRY(cudaMemGetInfo(&fr, &tot));
+    budget = (long long)(fr / 2 / 16);
+    if (nb_max > 0 && nb_max < budget) budget = nb_max;
+  }
+  s->budget = budget;
+  // cell edge = the larger radius, widened by 2 % so that one ring covers the rounding of cell_coord (rings = 1), at least
+  // the extent / 2^20 (21-bit key fields; more rings then)
+  CUDA_TRY(prep_bounds(st, d_xyz, n, mn, mx));
+  double emax = 0.0;
+  for (int a = 0; a < 3; ++a) emax = (double)mx[a] - (double)mn[a] > emax ? (double)mx[a] - (double)mn[a] : emax;
+  double cell = 1.02 * (double)(rn > rf ? rn : rf);
+  if (cell < emax / 1048576.0) cell = emax / 1048576.0;
+  CUDA_TRY(build_grid(st, d_xyz, nullptr, n, (float)cell, &g, &grid));
+  int gmax = 0;
+  for (int a = 0; a < 3; ++a) { const int c = cell_coord_host(mx[a], a == 0 ? g.mnx : (a == 1 ? g.mny : g.mnz), g.inv); gmax = c > gmax ? c : gmax; }
+  // two cell coordinates of points closer than r differ by at most r / cell plus twice the float32 rounding of cell_coord
+  // (< (gmax + 1) 2^-23 each); 0.01 covers the rounding of d2 against r2
+  const double slack = 0.01 + (gmax + 2.0) / 1048576.0;
+  const RadWalk wf{g, (int)ceil((double)rf * (double)g.inv + slack), rf * rf};
+  const RadWalk wn{g, (int)ceil((double)rn * (double)g.inv + slack), rn * rn};
+  s->cell = (float)cell; s->rings_f = wf.rings; s->rings_n = wn.rings;
+  CUDA_TRY(flags.alloc((size_t)n + 1)); CUDA_TRY(pos.alloc((size_t)n + 1));
+  if (d_idx) {   // rows of the rf lists: the requested points' rf-neighbours
+    CUDA_TRY(need.alloc((size_t)n));
+    CUDA_TRY(cudaMemsetAsync(need.get(), 0, sizeof(int) * (size_t)n, st));
+    if (nidx > 0) GHICP_LAUNCH(k_rad_mark, blocks(nidx), PT, 0, st, wf, d_idx, nidx, need.get());
+  }
+  const int *order = grid.order.get();
+  CUDA_TRY(make_rows(st, order, need.get(), n, flags.get(), pos.get(), &rows_f, &row_of_f, &m_f));
+  if (const cudaError_t e = build_lists(st, wf, rows_f.get(), m_f, budget, &off_f, &key_f, &s->nb_f)) { s->needed = s->nb_f; return e; }
+  if (d_idx) {   // rows of the rn lists: every point the SPFHs read
+    CUDA_TRY(cudaMemsetAsync(need.get(), 0, sizeof(int) * (size_t)n, st));
+    if (m_f > 0) GHICP_LAUNCH(k_list_mark, blocks(m_f), PT, 0, st, key_f.get(), off_f.get(), m_f, need.get());
+  }
+  CUDA_TRY(make_rows(st, order, need.get(), n, flags.get(), pos.get(), &rows_n, &row_of_n, &m_n));
+  const cudaError_t en = build_lists(st, wn, rows_n.get(), m_n, budget - s->nb_f, &off_n, &key_n, &s->nb_n);
+  s->needed = s->nb_f + s->nb_n;
+  CUDA_TRY(en);
+  s->spfh_points = m_f;
+  if (ev_lists) CUDA_TRY(cudaEventRecord(ev_lists, st));
+  const CsrLists lf{key_f.get(), off_f.get(), row_of_f.get()}, ln{key_n.get(), off_n.get(), row_of_n.get()};
+  GHICP_LAUNCH(k_rad_normals, blocks(n), PT, 0, st, d_xyz, n, ln, d_normals, d_status);
+  if (ev_normals) CUDA_TRY(cudaEventRecord(ev_normals, st));
+  CUDA_TRY(spfh.alloc((size_t)n * 33));
+  if (m_f > 0) GHICP_LAUNCH(k_rad_spfh, blocks(m_f), PT, 0, st, d_xyz, d_normals, rows_f.get(), m_f, lf, spfh.get());
+  const int m_a = d_idx ? nidx : n;
+  if (m_a > 0) GHICP_LAUNCH(k_rad_fpfh, blocks(m_a), PT, 0, st, d_idx, m_a, lf, spfh.get(), d_fpfh);
+  CUDA_TRY(cudaStreamSynchronize(st));
+  return cudaGetLastError();
 }
 }  // namespace
 
@@ -1484,77 +1461,13 @@ done:
 cudaError_t prep_fpfh_radius(cudaStream_t st, const float *d_xyz, int n, const int *d_idx, int nidx, float rn, float rf,
                              long long nb_max, float *d_fpfh, float *d_normals, int *d_status, cudaEvent_t ev_lists,
                              cudaEvent_t ev_normals, FpfhRadiusStats *stats) {
-  cudaError_t err = cudaSuccess;
-  GridArgs g{};
-  int *order = nullptr, *cstart = nullptr; pu64 *ucell = nullptr; float4 *sorted = nullptr;
-  int *need = nullptr, *flags = nullptr, *pos = nullptr, *rows_f = nullptr, *row_of_f = nullptr, *rows_n = nullptr, *row_of_n = nullptr;
-  long long *off_f = nullptr, *off_n = nullptr; pu64 *key_f = nullptr, *key_n = nullptr;
-  float *spfh = nullptr;
-  float mn[3], mx[3];
   FpfhRadiusStats s;
-  int m_f = 0, m_n = 0;
   if (stats) *stats = s;
   if (n <= 0 || !(rn * rn > 0.f) || !(rf * rf > 0.f) || !std::isfinite(rn * rn) || !std::isfinite(rf * rf)) return cudaErrorInvalidValue;
-  {
-    long long budget;
-    {
-      size_t fr = 0, tot = 0;
-      PCK(cudaMemGetInfo(&fr, &tot));
-      budget = (long long)(fr / 2 / 16);
-      if (nb_max > 0 && nb_max < budget) budget = nb_max;
-    }
-    s.budget = budget;
-    // cell edge = the larger radius, widened by 2 % so that one ring covers the rounding of cell_coord (rings = 1), at least
-    // the extent / 2^20 (21-bit key fields; more rings then)
-    PCK(prep_bounds(st, d_xyz, n, mn, mx));
-    double emax = 0.0;
-    for (int a = 0; a < 3; ++a) emax = (double)mx[a] - (double)mn[a] > emax ? (double)mx[a] - (double)mn[a] : emax;
-    double cell = 1.02 * (double)(rn > rf ? rn : rf);
-    if (cell < emax / 1048576.0) cell = emax / 1048576.0;
-    PCK(build_grid(st, d_xyz, nullptr, n, (float)cell, &g, &order, &ucell, &cstart, &sorted));
-    int gmax = 0;
-    for (int a = 0; a < 3; ++a) { const int c = cell_coord_host(mx[a], a == 0 ? g.mnx : (a == 1 ? g.mny : g.mnz), g.inv); gmax = c > gmax ? c : gmax; }
-    // two cell coordinates of points closer than r differ by at most r / cell plus twice the float32 rounding of cell_coord
-    // (< (gmax + 1) 2^-23 each); 0.01 covers the rounding of d2 against r2
-    const double slack = 0.01 + (gmax + 2.0) / 1048576.0;
-    const RadWalk wf{g, (int)ceil((double)rf * (double)g.inv + slack), rf * rf};
-    const RadWalk wn{g, (int)ceil((double)rn * (double)g.inv + slack), rn * rn};
-    s.cell = (float)cell; s.rings_f = wf.rings; s.rings_n = wn.rings;
-    PCK(pmalloc(&flags, (size_t)n + 1)); PCK(pmalloc(&pos, (size_t)n + 1));
-    if (d_idx) {   // rows of the rf lists: the requested points' rf-neighbours
-      PCK(pmalloc(&need, (size_t)n));
-      PCK(pzero(need, sizeof(int) * (size_t)n, st));
-      if (nidx > 0) GHICP_LAUNCH(k_rad_mark, blocks(nidx), PT, 0, st, wf, d_idx, nidx, need);
-    }
-    PCK(make_rows(st, order, need, n, flags, pos, &rows_f, &row_of_f, &m_f));
-    err = build_lists(st, wf, rows_f, m_f, budget, &off_f, &key_f, &s.nb_f);
-    if (err != cudaSuccess) { s.needed = s.nb_f; goto done; }
-    if (d_idx) {   // rows of the rn lists: every point the SPFHs read
-      PCK(pzero(need, sizeof(int) * (size_t)n, st));
-      if (m_f > 0) GHICP_LAUNCH(k_list_mark, blocks(m_f), PT, 0, st, key_f, off_f, m_f, need);
-    }
-    PCK(make_rows(st, order, need, n, flags, pos, &rows_n, &row_of_n, &m_n));
-    err = build_lists(st, wn, rows_n, m_n, budget - s.nb_f, &off_n, &key_n, &s.nb_n);
-    if (err != cudaSuccess) { s.needed = s.nb_f + s.nb_n; goto done; }
-    s.needed = s.nb_f + s.nb_n; s.spfh_points = m_f;
-    if (ev_lists) PCK(cudaEventRecord(ev_lists, st));
-    GHICP_LAUNCH(k_rad_normals, blocks(n), PT, 0, st, d_xyz, n, CsrLists{key_n, off_n, row_of_n}, d_normals, d_status);
-    if (ev_normals) PCK(cudaEventRecord(ev_normals, st));
-    PCK(pmalloc(&spfh, (size_t)n * 33));
-    if (m_f > 0) GHICP_LAUNCH(k_rad_spfh, blocks(m_f), PT, 0, st, d_xyz, d_normals, rows_f, m_f, CsrLists{key_f, off_f, row_of_f}, spfh);
-    const int m_a = d_idx ? nidx : n;
-    if (m_a > 0) GHICP_LAUNCH(k_rad_fpfh, blocks(m_a), PT, 0, st, d_idx, m_a, CsrLists{key_f, off_f, row_of_f}, spfh, d_fpfh);
-    PCK(psync(st));
-#if !defined(GHICP_EMU_HOST)
-    PCK(cudaGetLastError());
-#endif
-  }
-done:
+  const cudaError_t e = fpfh_radius_run(st, d_xyz, n, d_idx, nidx, rn, rf, nb_max, d_fpfh, d_normals, d_status, ev_lists,
+                                        ev_normals, &s);
   if (stats) *stats = s;
-  pfree(order); pfree(ucell); pfree(cstart); pfree(sorted);
-  pfree(need); pfree(flags); pfree(pos); pfree(rows_f); pfree(row_of_f); pfree(rows_n); pfree(row_of_n);
-  pfree(off_f); pfree(off_n); pfree(key_f); pfree(key_n); pfree(spfh);
-  return err;
+  return e;
 }
 
 }  // namespace ghicp_b200

@@ -299,8 +299,6 @@ __global__ void k_sac_soa_to_aos(const double *__restrict__ soa, int n, float *_
   for (int k = 0; k < 3; ++k) out[3 * (size_t)i + k] = (float)soa[(size_t)k * n + i];
 }
 
-template <typename T> cudaError_t salloc(T **p, size_t n) { return cudaMallocAsync((void **)p, (n ? n : 1) * sizeof(T), 0); }
-template <typename T> void sfree(T *&p) { if (p) cudaFreeAsync(p, 0); p = nullptr; }
 inline int nblk(long long n, int t) { return (int)((n + t - 1) / t); }
 
 }  // namespace
@@ -310,15 +308,13 @@ cudaError_t sac_points_from_soa(const double *d_soa, int n, float *d_xyz) {
   return cudaGetLastError();
 }
 
-#define SCK(call) do { e = (call); if (e != cudaSuccess) goto done; } while (0)
-
 cudaError_t sac_run(const float *d_P, const float *d_Fs, int ns, const float *d_Q, const float *d_Ft, int nt,
                     const ghicp_sac_params *p, ghicp_sac_result *out, SacDebug *dbg) {
-  cudaError_t e = cudaSuccess;
   SacArgs a{};
   PointGrid pg;
-  cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-  int *d_pick = nullptr; float *d_d2 = nullptr;
+  StageEvents<5> ev;
+  DevBuf<int> samp, valid, need, slot, list, nlist, knn, corr, d_pick; DevBuf<unsigned> dnext;
+  DevBuf<float> rts, d_d2; DevBuf<unsigned long long> err;
   int pick[2] = {-1, 0};
   Rt12 rt{};
   const int H = p->max_iterations;
@@ -327,85 +323,76 @@ cudaError_t sac_run(const float *d_P, const float *d_Fs, int ns, const float *d_
   a.H = H; a.nsamp = p->nr_samples; a.ke = p->k_correspondences < nt ? p->k_correspondences : nt;
   a.msd = p->min_sample_distance; a.thr = p->corr_dist_threshold; a.seed = p->seed;
   const long long maxq = std::min((long long)ns, (long long)H * p->nr_samples);
-  for (auto &x : ev) if (e == cudaSuccess) e = cudaEventCreate(&x);
-  if (e != cudaSuccess) goto done;
-  SCK(salloc(&a.samp, (size_t)H * a.nsamp)); SCK(salloc(&a.valid, (size_t)H)); SCK(salloc(&a.dnext, (size_t)H));
-  SCK(salloc(&a.need, (size_t)ns)); SCK(salloc(&a.slot, (size_t)ns)); SCK(salloc(&a.list, (size_t)maxq)); SCK(salloc(&a.nlist, 1));
-  SCK(salloc(&a.knn, (size_t)maxq * a.ke)); SCK(salloc(&a.corr, (size_t)H * a.nsamp)); SCK(salloc(&a.rt, (size_t)H * 12));
-  SCK(salloc(&a.err, (size_t)H)); SCK(salloc(&d_pick, 2)); SCK(salloc(&d_d2, (size_t)ns));
-  SCK(cudaMemsetAsync(a.need, 0, sizeof(int) * (size_t)ns, 0)); SCK(cudaMemsetAsync(a.nlist, 0, sizeof(int), 0));
-  SCK(cudaMemsetAsync(a.err, 0, sizeof(unsigned long long) * (size_t)H, 0));
-  SCK(cudaMemsetAsync(a.rt, 0, sizeof(float) * 12 * (size_t)H, 0));
-  SCK(cudaMemsetAsync(a.corr, 0xff, sizeof(int) * (size_t)H * a.nsamp, 0));
-  SCK(cudaEventRecord(ev[0], 0));
+  CUDA_TRY(ev.create());
+  CUDA_TRY(samp.alloc((size_t)H * a.nsamp)); CUDA_TRY(valid.alloc((size_t)H)); CUDA_TRY(dnext.alloc((size_t)H));
+  CUDA_TRY(need.alloc((size_t)ns)); CUDA_TRY(slot.alloc((size_t)ns)); CUDA_TRY(list.alloc((size_t)maxq)); CUDA_TRY(nlist.alloc(1));
+  CUDA_TRY(knn.alloc((size_t)maxq * a.ke)); CUDA_TRY(corr.alloc((size_t)H * a.nsamp)); CUDA_TRY(rts.alloc((size_t)H * 12));
+  CUDA_TRY(err.alloc((size_t)H)); CUDA_TRY(d_pick.alloc(2)); CUDA_TRY(d_d2.alloc((size_t)ns));
+  a.samp = samp.get(); a.valid = valid.get(); a.dnext = dnext.get(); a.need = need.get(); a.slot = slot.get();
+  a.list = list.get(); a.nlist = nlist.get(); a.knn = knn.get(); a.corr = corr.get(); a.rt = rts.get(); a.err = err.get();
+  CUDA_TRY(cudaMemsetAsync(a.need, 0, sizeof(int) * (size_t)ns, 0)); CUDA_TRY(cudaMemsetAsync(a.nlist, 0, sizeof(int), 0));
+  CUDA_TRY(cudaMemsetAsync(a.err, 0, sizeof(unsigned long long) * (size_t)H, 0));
+  CUDA_TRY(cudaMemsetAsync(a.rt, 0, sizeof(float) * 12 * (size_t)H, 0));
+  CUDA_TRY(cudaMemsetAsync(a.corr, 0xff, sizeof(int) * (size_t)H * a.nsamp, 0));
+  CUDA_TRY(cudaEventRecord(ev[0], 0));
   GHICP_LAUNCH(k_sac_sample, nblk(H, SAC_T), SAC_T, 0, 0, a);
   GHICP_LAUNCH(k_sac_compact, nblk(ns, SAC_T), SAC_T, 0, 0, a);
   if (maxq > 0) GHICP_LAUNCH(k_sac_feat_knn, nblk(maxq, FEAT_T), FEAT_T, 0, 0, a);
-  SCK(cudaEventRecord(ev[1], 0));
+  CUDA_TRY(cudaEventRecord(ev[1], 0));
   GHICP_LAUNCH(k_sac_estimate, nblk(H, SAC_T), SAC_T, 0, 0, a, d_Q);
-  SCK(cudaEventRecord(ev[2], 0));
-  {
-    // Target grid: the k-NN cell rule (a few points per cell), but no finer than sqrt(thr) / 4, so that a query stops within
-    // about five rings once no point can come within the threshold.  The result does not depend on the cell edge.
-    const int kcell = nt < 8 ? nt : 8;
-    SCK(prep_point_grid(0, d_Q, nt, kcell, 0.f, std::sqrt((double)a.thr) / 4.0, &pg));
-    SacGrid G{};
-    G.g = pg.g; G.gx = pg.gx; G.gy = pg.gy; G.gz = pg.gz; G.mxx = pg.mx[0]; G.mxy = pg.mx[1]; G.mxz = pg.mx[2];
-    G.cell = pg.cell; G.slack = pg.slack;
-    dim3 grid((unsigned)nblk(H, SCORE_HB), (unsigned)nblk(ns, SCORE_CHUNK));
-    GHICP_LAUNCH(k_sac_score, grid, SCORE_T, 0, 0, a, G);
-    SCK(cudaEventRecord(ev[3], 0));
-    GHICP_LAUNCH(k_sac_pick, 1, PICK_T, 0, 0, a, d_pick);
-    SCK(cudaEventRecord(ev[4], 0));
-    SCK(cudaMemcpyAsync(pick, d_pick, sizeof(pick), cudaMemcpyDeviceToHost, 0));
-    SCK(cudaStreamSynchronize(0));
-    if (pick[0] >= 0) {
-      SCK(cudaMemcpy(rt.v, a.rt + 12 * (size_t)pick[0], sizeof(rt.v), cudaMemcpyDeviceToHost));
-    } else {   // no valid hypothesis: the identity, scored like any transform
-      rt.v[0] = rt.v[4] = rt.v[8] = 1.f;
-    }
-    GHICP_LAUNCH(k_sac_fit, nblk(ns, SAC_T), SAC_T, 0, 0, a, G, rt, d_d2);
-#if !defined(GHICP_EMU_HOST)
-    SCK(cudaGetLastError());
-#endif
-    std::vector<float> d2((size_t)ns);
-    SCK(cudaMemcpyAsync(d2.data(), d_d2, sizeof(float) * (size_t)ns, cudaMemcpyDeviceToHost, 0));
-    SCK(cudaStreamSynchronize(0));
-    unsigned long long fx = 0ull;
-    double fit = 0.0;
-    int inl = 0;
-    for (int i = 0; i < ns; ++i) {   // point order: the fitness sum is fixed
-      fx += ghicp_sac::sac_term_fx(d2[i], a.thr);
-      if (d2[i] <= a.thr) { fit += (double)d2[i]; ++inl; }
-    }
-    for (int i = 0; i < 16; ++i) out->Rt[i] = 0.0;
-    for (int i = 0; i < 3; ++i) {
-      for (int j = 0; j < 3; ++j) out->Rt[j * 4 + i] = (double)rt.v[3 * i + j];
-      out->Rt[12 + i] = (double)rt.v[9 + i];
-    }
-    out->Rt[15] = 1.0;
-    out->error = (double)fx / ghicp_sac::SAC_FX_ONE;
-    out->fitness = inl > 0 ? fit / inl : DBL_MAX;   // PCL's getFitnessScore without a point in range
-    out->inliers = inl;
-    out->best_hypothesis = pick[0];
-    out->invalid_hypotheses = pick[1];
-    for (int k = 0; k < 4; ++k) cudaEventElapsedTime(&out->stage_ms[k], ev[k], ev[k + 1]);
+  CUDA_TRY(cudaEventRecord(ev[2], 0));
+  // Target grid: the k-NN cell rule (a few points per cell), but no finer than sqrt(thr) / 4, so that a query stops within
+  // about five rings once no point can come within the threshold.  The result does not depend on the cell edge.
+  const int kcell = nt < 8 ? nt : 8;
+  CUDA_TRY(prep_point_grid(0, d_Q, nt, kcell, 0.f, std::sqrt((double)a.thr) / 4.0, &pg));
+  SacGrid G{};
+  G.g = pg.g; G.gx = pg.gx; G.gy = pg.gy; G.gz = pg.gz; G.mxx = pg.mx[0]; G.mxy = pg.mx[1]; G.mxz = pg.mx[2];
+  G.cell = pg.cell; G.slack = pg.slack;
+  dim3 grid((unsigned)nblk(H, SCORE_HB), (unsigned)nblk(ns, SCORE_CHUNK));
+  GHICP_LAUNCH(k_sac_score, grid, SCORE_T, 0, 0, a, G);
+  CUDA_TRY(cudaEventRecord(ev[3], 0));
+  GHICP_LAUNCH(k_sac_pick, 1, PICK_T, 0, 0, a, d_pick.get());
+  CUDA_TRY(cudaEventRecord(ev[4], 0));
+  CUDA_TRY(cudaMemcpyAsync(pick, d_pick.get(), sizeof(pick), cudaMemcpyDeviceToHost, 0));
+  CUDA_TRY(cudaStreamSynchronize(0));
+  if (pick[0] >= 0) {
+    CUDA_TRY(cudaMemcpy(rt.v, a.rt + 12 * (size_t)pick[0], sizeof(rt.v), cudaMemcpyDeviceToHost));
+  } else {   // no valid hypothesis: the identity, scored like any transform
+    rt.v[0] = rt.v[4] = rt.v[8] = 1.f;
   }
+  GHICP_LAUNCH(k_sac_fit, nblk(ns, SAC_T), SAC_T, 0, 0, a, G, rt, d_d2.get());
+  CUDA_TRY(cudaGetLastError());
+  std::vector<float> d2((size_t)ns);
+  CUDA_TRY(cudaMemcpyAsync(d2.data(), d_d2.get(), sizeof(float) * (size_t)ns, cudaMemcpyDeviceToHost, 0));
+  CUDA_TRY(cudaStreamSynchronize(0));
+  unsigned long long fx = 0ull;
+  double fit = 0.0;
+  int inl = 0;
+  for (int i = 0; i < ns; ++i) {   // point order: the fitness sum is fixed
+    fx += ghicp_sac::sac_term_fx(d2[i], a.thr);
+    if (d2[i] <= a.thr) { fit += (double)d2[i]; ++inl; }
+  }
+  for (int i = 0; i < 16; ++i) out->Rt[i] = 0.0;
+  for (int i = 0; i < 3; ++i) {
+    for (int j = 0; j < 3; ++j) out->Rt[j * 4 + i] = (double)rt.v[3 * i + j];
+    out->Rt[12 + i] = (double)rt.v[9 + i];
+  }
+  out->Rt[15] = 1.0;
+  out->error = (double)fx / ghicp_sac::SAC_FX_ONE;
+  out->fitness = inl > 0 ? fit / inl : DBL_MAX;   // PCL's getFitnessScore without a point in range
+  out->inliers = inl;
+  out->best_hypothesis = pick[0];
+  out->invalid_hypotheses = pick[1];
+  for (int k = 0; k < 4; ++k) out->stage_ms[k] = ev.ms(k, k + 1);
   if (dbg) {
-    if (dbg->samples) SCK(cudaMemcpy(dbg->samples, a.samp, sizeof(int) * (size_t)H * a.nsamp, cudaMemcpyDeviceToHost));
-    if (dbg->valid) SCK(cudaMemcpy(dbg->valid, a.valid, sizeof(int) * (size_t)H, cudaMemcpyDeviceToHost));
-    if (dbg->corr) SCK(cudaMemcpy(dbg->corr, a.corr, sizeof(int) * (size_t)H * a.nsamp, cudaMemcpyDeviceToHost));
-    if (dbg->rt) SCK(cudaMemcpy(dbg->rt, a.rt, sizeof(float) * 12 * (size_t)H, cudaMemcpyDeviceToHost));
-    if (dbg->err) SCK(cudaMemcpy(dbg->err, a.err, sizeof(unsigned long long) * (size_t)H, cudaMemcpyDeviceToHost));
+    if (dbg->samples) CUDA_TRY(cudaMemcpy(dbg->samples, a.samp, sizeof(int) * (size_t)H * a.nsamp, cudaMemcpyDeviceToHost));
+    if (dbg->valid) CUDA_TRY(cudaMemcpy(dbg->valid, a.valid, sizeof(int) * (size_t)H, cudaMemcpyDeviceToHost));
+    if (dbg->corr) CUDA_TRY(cudaMemcpy(dbg->corr, a.corr, sizeof(int) * (size_t)H * a.nsamp, cudaMemcpyDeviceToHost));
+    if (dbg->rt) CUDA_TRY(cudaMemcpy(dbg->rt, a.rt, sizeof(float) * 12 * (size_t)H, cudaMemcpyDeviceToHost));
+    if (dbg->err) CUDA_TRY(cudaMemcpy(dbg->err, a.err, sizeof(unsigned long long) * (size_t)H, cudaMemcpyDeviceToHost));
     dbg->cell = pg.cell;
   }
-done:
-  prep_point_grid_free(&pg);
-  sfree(a.samp); sfree(a.valid); sfree(a.dnext); sfree(a.need); sfree(a.slot); sfree(a.list); sfree(a.nlist);
-  sfree(a.knn); sfree(a.corr); sfree(a.rt); sfree(a.err); sfree(d_pick); sfree(d_d2);
-  for (auto &x : ev) if (x) cudaEventDestroy(x);
-  return e;
+  return cudaSuccess;
 }
-#undef SCK
 
 }  // namespace ghicp_b200

@@ -38,16 +38,30 @@ template <typename T> inline void __stcg(T *p, T v) { *p = v; }
 // fresh "device" memory is POISONED (0xCD bytes: huge negative ints, -6.2e66 doubles): a kernel that reads what nobody wrote
 // produces garbage here instead of the zeros a fresh page usually holds
 inline void *emu_poisoned(size_t bytes) { void *q = malloc(bytes ? bytes : 1); if (q) memset(q, 0xCD, bytes ? bytes : 1); return q; }
-template <typename T> inline cudaError_t cudaMallocAsync(T **p, size_t bytes, cudaStream_t) { *p = (T *)emu_poisoned(bytes); return *p ? cudaSuccess : cudaErrorMemoryAllocation; }
-inline cudaError_t cudaFreeAsync(void *p, cudaStream_t) { free(p); return cudaSuccess; }
+// Test controls of the device allocations (tests/test_alloc_failures.py, through tests/harness/emu_library.cpp): the number of
+// live ones, and a countdown that makes the k-th allocation from now fail (-1: none fails)
+inline long long emu_live_allocs = 0;
+inline long long emu_fail_countdown = -1;
+inline void *emu_device_alloc(size_t bytes) {
+  if (emu_fail_countdown >= 0 && emu_fail_countdown-- == 0) return nullptr;
+  void *q = emu_poisoned(bytes);
+  if (q) ++emu_live_allocs;
+  return q;
+}
+inline void emu_device_free(void *p) {
+  if (p) --emu_live_allocs;
+  free(p);
+}
+template <typename T> inline cudaError_t cudaMallocAsync(T **p, size_t bytes, cudaStream_t) { *p = (T *)emu_device_alloc(bytes); return *p ? cudaSuccess : cudaErrorMemoryAllocation; }
+inline cudaError_t cudaFreeAsync(void *p, cudaStream_t) { emu_device_free(p); return cudaSuccess; }
 inline const char *cudaGetErrorString(cudaError_t e) { return e == cudaErrorNotSupported ? "operation not supported (emulation)" : "emulated"; }
 // ---- the host-side runtime calls of ghicp_capi.cu (tests/harness/emu_library.cpp): device memory = the heap, one "device",
 // streams and events are tokens, everything is synchronous
 enum { cudaStreamNonBlocking = 1 };
 inline cudaError_t cudaGetDeviceCount(int *n) { *n = 1; return cudaSuccess; }
 inline cudaError_t cudaSetDevice(int d) { return d == 0 ? cudaSuccess : cudaErrorInvalidValue; }
-inline cudaError_t cudaMalloc(void **p, size_t bytes) { *p = emu_poisoned(bytes); return *p ? cudaSuccess : cudaErrorMemoryAllocation; }
-inline cudaError_t cudaFree(void *p) { free(p); return cudaSuccess; }
+inline cudaError_t cudaMalloc(void **p, size_t bytes) { *p = emu_device_alloc(bytes); return *p ? cudaSuccess : cudaErrorMemoryAllocation; }
+inline cudaError_t cudaFree(void *p) { emu_device_free(p); return cudaSuccess; }
 template <typename T> inline cudaError_t cudaMallocHost(T **p, size_t bytes) { *p = (T *)emu_poisoned(bytes); return *p ? cudaSuccess : cudaErrorMemoryAllocation; }
 inline cudaError_t cudaFreeHost(void *p) { free(p); return cudaSuccess; }
 // every host pointer is "pageable" here: the library's staging path is the one exercised

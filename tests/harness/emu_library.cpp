@@ -19,3 +19,7 @@
 #include "../../gh-icp_b200/csrc/ghicp_fdtc.cu"
 
 #include "../../gh-icp_b200/csrc/ghicp_capi.cu"
+
+// test controls of the shim's device allocations (tests/test_alloc_failures.py)
+extern "C" long long ghicp_emu_live_allocations(void) { return emu_live_allocs; }
+extern "C" void ghicp_emu_fail_allocation(long long k) { emu_fail_countdown = k; }   // the k-th allocation from now fails; -1: none
