@@ -76,7 +76,8 @@ EXPORTS = ["ghicp_abi_version", "ghicp_device_count", "ghicp_last_error", "ghicp
            "ghicp_prep_run", "ghicp_prep_info", "ghicp_prep_get", "ghicp_prep_destroy", "ghicp_set_from_prep",
            "ghicp_host_alloc", "ghicp_host_free", "ghicp_fpfh_extract", "ghicp_prep_fpfh", "ghicp_prep_get_fpfh",
            "ghicp_prep_fpfh_stats", "ghicp_sac_ia", "ghicp_prep_sac_ia", "ghicp_set_initial_transform",
-           "ghicp_fpfh_extract_radius", "ghicp_prep_fpfh_radius", "ghicp_cloud_overlap", "ghicp_prep_overlap"]
+           "ghicp_fpfh_extract_radius", "ghicp_prep_fpfh_radius", "ghicp_cloud_overlap", "ghicp_prep_overlap",
+           "ghicp_cloud_icp", "ghicp_prep_icp"]
 
 
 def lib():
@@ -139,6 +140,8 @@ def lib():
     L.ghicp_cloud_overlap.argtypes = [C.c_int, fpp, C.c_int, fpp, C.c_int, dp, C.c_float, C.c_double, C.c_int,
                                       C.POINTER(OverlapResult), fpp]
     L.ghicp_prep_overlap.argtypes = [vp, vp, dp, C.c_float, C.c_double, C.c_int, C.POINTER(OverlapResult)]
+    L.ghicp_cloud_icp.argtypes = [C.c_int, fpp, C.c_int, fpp, C.c_int, dp, C.POINTER(IcpParams), C.POINTER(IcpResult), fpp, ip, dp]
+    L.ghicp_prep_icp.argtypes = [vp, vp, dp, C.POINTER(IcpParams), C.POINTER(IcpResult)]
     _lib = L
     return L
 
@@ -190,6 +193,34 @@ def _overlap_out(r):
     ms = list(r.stage_ms)
     return dict(n=r.n, overlap=r.overlap, ratio=r.ratio, overlap_rmse=r.overlap_rmse, n_fit=r.n_fit, fitness=r.fitness,
                 cells_visited=r.cells_visited, candidates=r.candidates, stage_ms=dict(grid=ms[0], queries=ms[1], total=ms[2]))
+
+
+class IcpParams(C.Structure):
+    """ghicp_icp_params (include/ghicp_b200.h): point-to-point ICP, DESIGN.md §3.13."""
+    _fields_ = [("max_iterations", C.c_int), ("reciprocal", C.c_int), ("trim_ratio", C.c_float),
+                ("transformation_epsilon", C.c_double), ("fitness_epsilon", C.c_double), ("reserved", C.c_int * 4)]
+
+
+class IcpResult(C.Structure):
+    _fields_ = [("Rt", C.c_double * 16), ("mse", C.c_double), ("fitness", C.c_double), ("iterations", C.c_int),
+                ("converged", C.c_int), ("state", C.c_int), ("cor", C.c_int), ("cells_visited", C.c_longlong),
+                ("candidates", C.c_longlong), ("stage_ms", C.c_float * 4)]
+
+
+ICP_STATES = {1: "ITERATIONS", 2: "TRANSFORM", 3: "ABS_MSE", 4: "REL_MSE", 5: "NO_CORRESPONDENCES"}   # ghicp_icp_state
+
+
+def _icp_params(max_iterations, reciprocal, trim_ratio, transformation_epsilon, fitness_epsilon):
+    return IcpParams(int(max_iterations), int(bool(reciprocal)), float(trim_ratio), float(transformation_epsilon),
+                     float(fitness_epsilon))
+
+
+def _icp_out(r, rc):
+    Rt = np.array(r.Rt).reshape(4, 4).T.copy()
+    ms = list(r.stage_ms)
+    return Rt, dict(iterations=r.iterations, converged=bool(r.converged), state=ICP_STATES.get(r.state, r.state), cor=r.cor,
+                    mse=r.mse, fitness=r.fitness, warnings=rc, cells_visited=r.cells_visited, candidates=r.candidates,
+                    stage_ms=dict(grid=ms[0], iterations=ms[1], fitness=ms[2], total=ms[3]))
 
 
 class PrepParams(C.Structure):
@@ -296,6 +327,18 @@ class Prep:
         check(lib().ghicp_prep_overlap(self.h, target.h, rp, float(thre_dis), float(max_range), int(bool(fitness)), C.byref(r)))
         del keep
         return _overlap_out(r)
+
+    def icp(self, target, guess=None, max_iterations=50, reciprocal=False, trim_ratio=0.0, transformation_epsilon=1e-8,
+            fitness_epsilon=1e-5):
+        """cloud_icp of this down-sampled cloud onto `target`'s, device to device (ghicp_prep_icp).  The target's grid is the one
+        overlap() keeps (its stage_ms["grid"] is 0 once either has built it).  Returns (Rt, info) as cloud_icp."""
+        keep, gp = _overlap_rt(guess)
+        r = IcpResult()
+        rc = check(lib().ghicp_prep_icp(self.h, target.h, gp, C.byref(_icp_params(max_iterations, reciprocal, trim_ratio,
+                                                                                   transformation_epsilon, fitness_epsilon)),
+                                        C.byref(r)))
+        del keep
+        return _icp_out(r, rc)
 
     def close(self):
         if getattr(self, "h", None):
@@ -515,6 +558,37 @@ def cloud_overlap(A, B, Rt=None, thre_dis=None, max_range=float("inf"), fitness=
     if d2 is not None:
         out["d2"] = d2
     return out
+
+
+def cloud_icp(S, T, guess=None, max_iterations=50, reciprocal=False, trim_ratio=0.0, transformation_epsilon=1e-8,
+              fitness_epsilon=1e-5, return_moved=False, trace=False, device=0):
+    """Point-to-point ICP of source S onto target T on the GPU, DESIGN.md §3.13: PCL's IterativeClosestPoint as
+    CRegistration::icp_reg configures it (src/common_reg.cpp:44-107), starting from `guess` (4x4, None = identity).
+    reciprocal = setUseReciprocalCorrespondences; trim_ratio > 0 adds CorrespondenceRejectorTrimmed with that overlap ratio.
+    Returns (Rt 4x4 mapping S onto T, info: iterations, converged, state (ITERATIONS, TRANSFORM, ABS_MSE, REL_MSE or
+    NO_CORRESPONDENCES), cor and mse of the last iteration, fitness = PCL's getFitnessScore, warnings (GHICP_W_FEW_PAIRS when
+    fewer than 3 pairs were left), work counters, stage_ms); + "moved" (S moved by Rt) with return_moved, + "cor_trace" /
+    "mse_trace" per iteration with trace."""
+    fpp = C.POINTER(C.c_float)
+    S = np.ascontiguousarray(S, dtype=np.float32).reshape(-1, 3)
+    T = np.ascontiguousarray(T, dtype=np.float32).reshape(-1, 3)
+    keep, gp = _overlap_rt(guess)
+    K = max(int(max_iterations), 1)
+    moved = np.zeros_like(S) if return_moved else None
+    cor_tr, mse_tr = (np.zeros(K, np.int32), np.zeros(K)) if trace else (None, None)
+    r = IcpResult()
+    rc = check(lib().ghicp_cloud_icp(device, S.ctypes.data_as(fpp), len(S), T.ctypes.data_as(fpp), len(T), gp,
+                                     C.byref(_icp_params(max_iterations, reciprocal, trim_ratio, transformation_epsilon,
+                                                         fitness_epsilon)), C.byref(r),
+                                     None if moved is None else moved.ctypes.data_as(fpp), None if cor_tr is None else _ip(cor_tr),
+                                     None if mse_tr is None else _dp(mse_tr)))
+    del keep
+    Rt, info = _icp_out(r, rc)
+    if moved is not None:
+        info["moved"] = moved
+    if trace:
+        info["cor_trace"], info["mse_trace"] = cor_tr[:r.iterations].copy(), mse_tr[:r.iterations].copy()
+    return Rt, info
 
 
 def rigid_fit_ex(S, T, solver=SOLVER_SVD, normals=None, weights=None, device=0):

@@ -17,9 +17,10 @@
 #if defined(GHICP_EMU_HOST)
 // The CPU emulation of the whole library (tests/harness/emu_library.cpp) compiles the product's .cu files as ONE translation
 // unit and lists the kernel files it includes; the SAC-IA kernels join it here, next to the entry points that call them.
-// nvcc builds ghicp_sac.cu and ghicp_overlap.cu as translation units of their own (Makefile SRCS).
+// nvcc builds ghicp_sac.cu, ghicp_overlap.cu and ghicp_icp.cu as translation units of their own (Makefile SRCS).
 #include "ghicp_sac.cu"
 #include "ghicp_overlap.cu"
+#include "ghicp_icp.cu"
 #endif
 
 namespace ghicp_b200 {
@@ -1619,6 +1620,19 @@ int ghicp_prep_sac_ia(const ghicp_prep *src, const ghicp_prep *tgt, const ghicp_
 }
 
 // ---- overlap and fitness on the dense clouds ---------------------------------------------------------------------------
+static bool finite_point(const float *p) { return std::isfinite(p[0]) && std::isfinite(p[1]) && std::isfinite(p[2]); }
+// the finite points of xyz [n][3]: xyz itself when every point is finite, else a copy in *store
+static const float *finite_points(const float *xyz, int n, std::vector<float> *store, int *n_out) {
+  int j = 0;
+  while (j < n && finite_point(xyz + 3 * (size_t)j)) ++j;
+  *n_out = n;
+  if (j == n) return xyz;
+  store->reserve(3 * (size_t)n);
+  for (int i = 0; i < n; ++i)
+    if (finite_point(xyz + 3 * (size_t)i)) store->insert(store->end(), xyz + 3 * (size_t)i, xyz + 3 * (size_t)i + 3);
+  *n_out = (int)(store->size() / 3);
+  return store->data();
+}
 static bool overlap_args_ok(float thre_dis, double max_range, const char *who) {
   // thre_dis * thre_dis is compared in float32: a radius whose square is 0 or infinite is refused with the others
   const bool ok = std::isfinite(thre_dis) && thre_dis > 0.f && thre_dis * thre_dis > 0.f && std::isfinite(thre_dis * thre_dis) &&
@@ -1664,24 +1678,12 @@ int ghicp_cloud_overlap(int device, const float *a_xyz, int n_a, const float *b_
   if (!overlap_args_ok(thre_dis, max_range, "cloud_overlap") || !overlap_rt_ok(Rt, "cloud_overlap")) return GHICP_E_ARG;
   // B's non-finite points (the NaN returns of an organised scan) are left out of the grid, as PCL's KdTreeFLANN leaves them
   // out of its tree; they can be no one's nearest point
-  std::vector<float> b_fin;
-  long long nb_fin = n_b;
-  {
-    size_t j = 0;
-    for (; j < (size_t)n_b; ++j)
-      if (!(std::isfinite(b_xyz[3 * j]) && std::isfinite(b_xyz[3 * j + 1]) && std::isfinite(b_xyz[3 * j + 2]))) break;
-    if (j < (size_t)n_b) {
-      b_fin.reserve(3 * (size_t)n_b);
-      for (size_t i = 0; i < (size_t)n_b; ++i)
-        if (std::isfinite(b_xyz[3 * i]) && std::isfinite(b_xyz[3 * i + 1]) && std::isfinite(b_xyz[3 * i + 2]))
-          b_fin.insert(b_fin.end(), b_xyz + 3 * i, b_xyz + 3 * i + 3);
-      nb_fin = (long long)(b_fin.size() / 3);
-      b_xyz = b_fin.data();
-    }
-  }
+  std::vector<float> b_store;
+  int nb_fin = 0;
+  b_xyz = finite_points(b_xyz, n_b, &b_store, &nb_fin);
   if (nb_fin <= 0) { set_error(nullptr, "cloud_overlap: cloud B has no finite point"); return GHICP_E_ARG; }
   if (int rc = enter_device(device, "cloud_overlap")) return rc;
-  return cuda_status(cloud_overlap_run(a_xyz, n_a, b_xyz, (int)nb_fin, Rt, thre_dis, max_range, want_fitness, out, d2), "cloud_overlap");
+  return cuda_status(cloud_overlap_run(a_xyz, n_a, b_xyz, nb_fin, Rt, thre_dis, max_range, want_fitness, out, d2), "cloud_overlap");
 }
 
 static cudaError_t prep_overlap_run(const ghicp_prep *a, ghicp_prep *tb, const double *Rt, float thre_dis, double max_range,
@@ -1709,6 +1711,99 @@ int ghicp_prep_overlap(const ghicp_prep *a, const ghicp_prep *b, const double Rt
   if (int rc = enter_device(a->device, "prep_overlap")) return rc;
   ghicp_prep *tb = const_cast<ghicp_prep *>(b);   // the grid is a cache of the target's down-sampled cloud, not its state
   return cuda_status(prep_overlap_run(a, tb, Rt, thre_dis, max_range, want_fitness, out), "prep_overlap");
+}
+
+// ---- point-to-point ICP on the dense clouds --------------------------------------------------------------------------------
+static bool icp_params_ok(const ghicp_icp_params *p, const double *guess, const char *who) {
+  const bool ok = p && p->max_iterations >= 1 && p->trim_ratio >= 0.f && p->trim_ratio <= 1.f &&   // false for NaN
+                  p->transformation_epsilon >= 0.0 && p->fitness_epsilon >= 0.0;
+  if (!ok) {
+    set_error(nullptr, std::string(who) + ": max_iterations must be >= 1, trim_ratio in [0, 1], the epsilons >= 0");
+    return false;
+  }
+  return overlap_rt_ok(guess, who);
+}
+
+// Both ICP entries write *out, moved and the traces only once every stage succeeded.
+static cudaError_t cloud_icp_run(const float *src, int n_s, const float *src_fin, int ns_fin, const float *tgt, int n_t,
+                                 const double *guess, const ghicp_icp_params *p, ghicp_icp_result *out, float *moved, int *cor_trace,
+                                 double *mse_trace) {
+  StageEvents<4> ev;
+  DevBuf<float> d_all, d_fin, d_t;
+  ghicp_icp_result r{};
+  CUDA_TRY(ev.create());
+  CUDA_TRY(d_all.alloc(3 * (size_t)n_s)); CUDA_TRY(d_t.alloc(3 * (size_t)n_t));
+  if (src_fin != src) CUDA_TRY(d_fin.alloc(3 * (size_t)ns_fin));
+  CUDA_TRY(cudaMemcpyAsync(d_all.get(), src, 3 * (size_t)n_s * sizeof(float), cudaMemcpyHostToDevice, 0));
+  if (src_fin != src) CUDA_TRY(cudaMemcpyAsync(d_fin.get(), src_fin, 3 * (size_t)ns_fin * sizeof(float), cudaMemcpyHostToDevice, 0));
+  CUDA_TRY(cudaMemcpyAsync(d_t.get(), tgt, 3 * (size_t)n_t * sizeof(float), cudaMemcpyHostToDevice, 0));
+  CUDA_TRY(cudaEventRecord(ev[0], 0));
+  OverlapTarget *t = nullptr;
+  CUDA_TRY(overlap_target_build(d_t.get(), n_t, &t));
+  std::vector<int> cor(cor_trace ? p->max_iterations : 0);
+  std::vector<double> mse(mse_trace ? p->max_iterations : 0);
+  const cudaError_t e = icp_run(src_fin != src ? d_fin.get() : d_all.get(), ns_fin, d_all.get(), n_s, t, d_t.get(), guess, p, ev[1],
+                                ev[2], &r, moved, cor_trace ? cor.data() : nullptr, mse_trace ? mse.data() : nullptr);
+  overlap_target_free(t);
+  CUDA_TRY(e);
+  CUDA_TRY(cudaEventRecord(ev[3], 0));
+  CUDA_TRY(cudaStreamSynchronize(0));
+  r.stage_ms[0] = ev.ms(0, 1); r.stage_ms[1] = ev.ms(1, 2); r.stage_ms[2] = ev.ms(2, 3); r.stage_ms[3] = ev.ms(0, 3);
+  *out = r;
+  if (cor_trace) std::copy(cor.begin(), cor.begin() + r.iterations, cor_trace);
+  if (mse_trace) std::copy(mse.begin(), mse.begin() + r.iterations, mse_trace);
+  return cudaSuccess;
+}
+int ghicp_cloud_icp(int device, const float *src_xyz, int n_s, const float *tgt_xyz, int n_t, const double guess[16],
+                    const ghicp_icp_params *p, ghicp_icp_result *out, float *moved, int *cor_trace, double *mse_trace) {
+  if (!src_xyz || !tgt_xyz || !out || n_s <= 0 || n_t <= 0) {
+    set_error(nullptr, "cloud_icp: bad argument (null array or empty cloud)");
+    return GHICP_E_ARG;
+  }
+  if (!icp_params_ok(p, guess, "cloud_icp")) return GHICP_E_ARG;
+  // non-finite points take no part (PCL's KdTreeFLANN leaves them out of its tree; their moved copies find no neighbour)
+  std::vector<float> s_store, t_store;
+  int ns_fin = 0, nt_fin = 0;
+  const float *s_fin = finite_points(src_xyz, n_s, &s_store, &ns_fin);
+  const float *t_fin = finite_points(tgt_xyz, n_t, &t_store, &nt_fin);
+  if (ns_fin <= 0 || nt_fin <= 0) { set_error(nullptr, "cloud_icp: the source or the target has no finite point"); return GHICP_E_ARG; }
+  if (int rc = enter_device(device, "cloud_icp")) return rc;
+  if (int rc = cuda_status(cloud_icp_run(src_xyz, n_s, s_fin, ns_fin, t_fin, nt_fin, guess, p, out, moved, cor_trace, mse_trace),
+                           "cloud_icp"))
+    return rc;
+  return out->converged ? GHICP_OK : GHICP_W_FEW_PAIRS;
+}
+
+static cudaError_t prep_icp_run(const ghicp_prep *s, ghicp_prep *tb, const double *guess, const ghicp_icp_params *p,
+                                ghicp_icp_result *out) {
+  StageEvents<4> ev;
+  ghicp_icp_result r{};
+  CUDA_TRY(ev.create());
+  CUDA_TRY(cudaEventRecord(ev[0], 0));
+  std::lock_guard<std::mutex> lk(tb->ov_mu);   // the grid ghicp_prep_overlap keeps, under its lock
+  const bool cached = tb->ov_target != nullptr;
+  if (!cached) CUDA_TRY(overlap_target_build(tb->d_down.get(), tb->n_down, &tb->ov_target));
+  CUDA_TRY(icp_run(s->d_down.get(), s->n_down, s->d_down.get(), s->n_down, tb->ov_target, tb->d_down.get(), guess, p, ev[1], ev[2],
+                   &r, nullptr, nullptr, nullptr));
+  CUDA_TRY(cudaEventRecord(ev[3], 0));
+  CUDA_TRY(cudaStreamSynchronize(0));
+  if (!cached) r.stage_ms[0] = ev.ms(0, 1);
+  r.stage_ms[1] = ev.ms(1, 2); r.stage_ms[2] = ev.ms(2, 3); r.stage_ms[3] = ev.ms(0, 3);
+  *out = r;
+  return cudaSuccess;
+}
+int ghicp_prep_icp(const ghicp_prep *source, const ghicp_prep *target, const double guess[16], const ghicp_icp_params *p,
+                   ghicp_icp_result *out) {
+  if (!source || !target || !out || source->n_down <= 0 || target->n_down <= 0) {
+    set_error(nullptr, "prep_icp: bad argument or an empty cloud");
+    return GHICP_E_ARG;
+  }
+  if (source->device != target->device) { set_error(nullptr, "prep_icp: the two pipeline results live on different devices"); return GHICP_E_ARG; }
+  if (!icp_params_ok(p, guess, "prep_icp")) return GHICP_E_ARG;
+  if (int rc = enter_device(source->device, "prep_icp")) return rc;
+  ghicp_prep *tb = const_cast<ghicp_prep *>(target);   // the grid is a cache of the target's down-sampled cloud, not its state
+  if (int rc = cuda_status(prep_icp_run(source, tb, guess, p, out), "prep_icp")) return rc;
+  return out->converged ? GHICP_OK : GHICP_W_FEW_PAIRS;
 }
 
 int ghicp_set_initial_transform(ghicp_ctx *ctx, const double Rt[16]) {

@@ -1,0 +1,340 @@
+// ghicp_icp.cu — point-to-point ICP on the dense clouds (DESIGN.md §3.13): the reference's CRegistration::icp_reg
+// (src/common_reg.cpp:44-107), PCL's IterativeClosestPoint with its two options, reciprocal correspondences and the trimmed
+// rejector.  Every stage of an iteration runs on the device; the host reads one small struct per iteration (pair count,
+// convergence state, accumulated transform, work counters) to decide whether to go on.
+//   k_icp_keys + sort   the working copy W's clamped target-cell keys, radix-sorted into the query order (the fitness-mode
+//                       query order of ghicp_overlap.cu, redone every iteration because W moves)
+//   k_icp_query         the hot path: the exact nearest target point of every W_i with its index, in (d2, index) order
+//                       (ov_nearest<true> over the target grid ghicp_prep_overlap also keeps)
+//   reciprocal          k_icp_mark / k_icp_compact the distinct targets j(i), a grid over W (prep_point_grid), k_icp_rev
+//                       queries from those targets into W, k_icp_recip keeps (i, j) when j's nearest point of W is i
+//   trimmed             k_icp_trim_keys: the u64 key (d2 bits, i) of every pair (non-negative float bits order like their
+//                       values), radix sort, k_icp_trim_thr: the first key past floor(rho c), k_icp_trim_apply drops the rest
+//   k_icp_sum<1, 2>     two-pass FP64 moments of the kept pairs over fixed point blocks and a fixed tree (means first, then
+//   k_icp_total         the demeaned cross-covariance), as k_ov_reduce / k_ov_total: no floating-point atomic
+//   k_icp_solve         one thread: the float32 Umeyama of the loop, F <- T F, DefaultConvergenceCriteria
+//   k_icp_move          W <- T W (sac_move's formula)
+#include <algorithm>
+#include <cfloat>
+#include <cmath>
+#include <cstring>
+#include <vector>
+
+#include "ghicp_internal.h"
+#include "ghicp_device.cuh"
+#include "ghicp_grid.cuh"
+#include "ghicp_ovwalk.cuh"
+
+namespace ghicp_b200 {
+namespace {
+
+constexpr int IC_T = 128;            // threads per query / per-point CTA
+constexpr int IC_RED_T = 256;        // threads per reduction CTA
+constexpr int IC_RED_CHUNK = 8192;   // points per reduction CTA
+
+struct IcpHead {                     // what the host reads after every iteration
+  int state, cor;                    // ghicp_icp_state (0: running); kept pairs
+  double mse;
+  float F[16];                       // accumulated transform, row-major float32
+  unsigned long long work[2];        // cells visited, candidates examined (every query so far)
+};
+struct IcpDev {
+  IcpHead h;
+  float T[16];                       // this iteration's transform, row-major float32
+  double prev_mse;
+  unsigned long long thr;            // trimmed: the smallest dropped (d2, i) key (~0: none dropped)
+  int n_rev;                         // reciprocal: distinct targets to query
+};
+struct IcpSum { double v[9]; unsigned long long n; };   // pass 1: s, q, sum d; pass 2: sum (q - mu_q)(s - mu_s)^T
+
+__device__ __forceinline__ void icp_move(const float *m, float x, float y, float z, float *o) {
+  o[0] = ((m[0] * x + m[1] * y) + m[2] * z) + m[3];
+  o[1] = ((m[4] * x + m[5] * y) + m[6] * z) + m[7];
+  o[2] = ((m[8] * x + m[9] * y) + m[10] * z) + m[11];
+}
+// dst = src moved by the row-major float32 matrix m (device memory: the loop's T or F); dst may be src
+__global__ void k_icp_move(const float *src, float *dst, long long n, const float *m) {
+  const long long i = (long long)blockIdx.x * IC_T + threadIdx.x;
+  if (i >= n) return;
+  float o[3];
+  icp_move(m, src[3 * i], src[3 * i + 1], src[3 * i + 2], o);
+  dst[3 * i] = o[0]; dst[3 * i + 1] = o[1]; dst[3 * i + 2] = o[2];
+}
+
+// clamped target-cell key of each W_i, with its index (the cell order of the queries)
+__global__ void k_icp_keys(const float *__restrict__ W, long long n, const OvGrid G, pu64 *__restrict__ keys, int *__restrict__ vals) {
+  const long long t = (long long)blockIdx.x * IC_T + threadIdx.x;
+  if (t >= n) return;
+  int c[3];
+  for (int k = 0; k < 3; ++k) {
+    const double f = floor(((double)W[3 * t + k] - G.mn[k]) / G.cell);
+    c[k] = !(f > 0.0) ? 0 : (f > (double)G.gm[k] ? G.gm[k] : (int)f);
+  }
+  keys[t] = cell_key(c[0], c[1], c[2]);
+  vals[t] = (int)t;
+}
+
+// warp-reduced integer work counters (every lane of the warp must call it)
+__device__ __forceinline__ void icp_add_work(unsigned long long cells, unsigned long long cand, unsigned long long *work) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    cells += __shfl_xor_sync(0xffffffffu, cells, o);
+    cand += __shfl_xor_sync(0xffffffffu, cand, o);
+  }
+  if ((threadIdx.x & 31) == 0 && (cells | cand)) { atomicAdd(work, cells); atomicAdd(work + 1, cand); }
+}
+
+// j(i) and d_i: the nearest target point of W_i in (d2, index) order, -1 / +inf for a non-finite W_i
+__global__ void __launch_bounds__(IC_T) k_icp_query(const float *__restrict__ W, long long n, const int *__restrict__ perm,
+                                                    const OvGrid G, int *__restrict__ corr, float *__restrict__ d2, IcpDev *dev) {
+  const long long t = (long long)blockIdx.x * IC_T + threadIdx.x;
+  unsigned long long cells = 0ull, cand = 0ull;
+  if (t < n) {
+    const long long i = perm[t];
+    const GridRegs r = grid_regs(G.g);   // per-thread registers, see k_pca
+    int j = -1;
+    d2[i] = ov_nearest<true>(r, G, W[3 * i], W[3 * i + 1], W[3 * i + 2], (double)INFINITY, -1.f, cells, cand, j);
+    corr[i] = j;
+  }
+  icp_add_work(cells, cand, dev->h.work);
+}
+
+// reciprocal: the distinct targets of the pairs, compacted into list[0 .. n_rev) (any order: results are stored per target)
+__global__ void k_icp_mark(const int *__restrict__ corr, long long n, unsigned char *__restrict__ flag) {
+  const long long i = (long long)blockIdx.x * IC_T + threadIdx.x;
+  if (i < n && corr[i] >= 0) flag[corr[i]] = 1;
+}
+__global__ void k_icp_compact(const unsigned char *__restrict__ flag, long long nt, int *__restrict__ list, IcpDev *dev) {
+  const long long j = (long long)blockIdx.x * IC_T + threadIdx.x;
+  const bool f = j < nt && flag[j];
+  const unsigned m = __ballot_sync(0xffffffffu, f);
+  const int lane = threadIdx.x & 31;
+  int base = 0;
+  if (lane == 0 && m) base = atomicAdd(&dev->n_rev, __popc(m));
+  base = __shfl_sync(0xffffffffu, base, 0);
+  if (f) list[base + __popc(m & ((1u << lane) - 1u))] = (int)j;
+}
+// rev[j] = the nearest point of W to Q_j in (d2, index) order, for the listed targets
+__global__ void __launch_bounds__(IC_T) k_icp_rev(const float *__restrict__ Q, const int *__restrict__ list, const OvGrid Gw,
+                                                  int *__restrict__ rev, IcpDev *dev) {
+  const long long t = (long long)blockIdx.x * IC_T + threadIdx.x;
+  unsigned long long cells = 0ull, cand = 0ull;
+  if (t < dev->n_rev) {
+    const int j = list[t];
+    const GridRegs r = grid_regs(Gw.g);
+    int i = -1;
+    ov_nearest<true>(r, Gw, Q[3 * (size_t)j], Q[3 * (size_t)j + 1], Q[3 * (size_t)j + 2], (double)INFINITY, -1.f, cells, cand, i);
+    rev[j] = i;
+  }
+  icp_add_work(cells, cand, dev->h.work);
+}
+__global__ void k_icp_recip(int *__restrict__ corr, long long n, const int *__restrict__ rev) {
+  const long long i = (long long)blockIdx.x * IC_T + threadIdx.x;
+  if (i >= n) return;
+  const int j = corr[i];
+  if (j >= 0 && rev[j] != (int)i) corr[i] = -1;
+}
+
+// trimmed: (d2 bits, i) of every pair; ~0 for a point without one
+__device__ __forceinline__ pu64 icp_trim_key(float d2, long long i) { return ((pu64)__float_as_uint(d2) << 32) | (pu64)(unsigned)i; }
+__global__ void k_icp_trim_keys(const int *__restrict__ corr, const float *__restrict__ d2, long long n, pu64 *__restrict__ keys,
+                                int *__restrict__ vals) {
+  const long long i = (long long)blockIdx.x * IC_T + threadIdx.x;
+  if (i >= n) return;
+  keys[i] = corr[i] >= 0 ? icp_trim_key(d2[i], i) : ~0ull;
+  vals[i] = (int)i;
+}
+// one thread: c = the pairs (sorted keys below ~0), keep = floor(rho * (float)c); thr = the first dropped key
+__global__ void k_icp_trim_thr(const pu64 *__restrict__ sorted, long long n, float rho, IcpDev *dev) {
+  long long lo = 0, hi = n;
+  while (lo < hi) {
+    const long long mid = (lo + hi) >> 1;
+    if (sorted[mid] != ~0ull) lo = mid + 1; else hi = mid;
+  }
+  const long long c = lo, keep = (long long)floorf(rho * (float)c);
+  dev->thr = keep >= c ? ~0ull : sorted[keep];
+}
+__global__ void k_icp_trim_apply(int *__restrict__ corr, const float *__restrict__ d2, long long n, const IcpDev *dev) {
+  const long long i = (long long)blockIdx.x * IC_T + threadIdx.x;
+  if (i >= n) return;
+  if (corr[i] >= 0 && icp_trim_key(d2[i], i) >= dev->thr) corr[i] = -1;
+}
+
+// moments of the kept pairs: thread t of block b sums the kept points b*CHUNK + t, + t + T, ... in that order, then a fixed
+// halving tree over the block's threads; k_icp_total does the same over the blocks (tests/harness/icp_oracle.cpp restates it)
+__device__ __forceinline__ void icp_sum_add(IcpSum &x, const IcpSum &y) {
+  for (int k = 0; k < 9; ++k) x.v[k] += y.v[k];
+  x.n += y.n;
+}
+__device__ void icp_tree(IcpSum *sh, const IcpSum &v, IcpSum *out) {
+  sh[threadIdx.x] = v;
+  __syncthreads();
+  for (int w = IC_RED_T / 2; w > 0; w >>= 1) {
+    if ((int)threadIdx.x < w) icp_sum_add(sh[threadIdx.x], sh[threadIdx.x + w]);
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *out = sh[0];
+}
+template <int PASS>
+__global__ void __launch_bounds__(IC_RED_T) k_icp_sum(const float *__restrict__ W, const float *__restrict__ Q, const int *__restrict__ corr,
+                                                      const float *__restrict__ d2, long long n, const IcpSum *__restrict__ m1,
+                                                      IcpSum *__restrict__ part) {
+  __shared__ IcpSum sh[IC_RED_T];
+  const long long p0 = (long long)blockIdx.x * IC_RED_CHUNK, p1 = min(p0 + IC_RED_CHUNK, n);
+  IcpSum v{};
+  double mus[3] = {0, 0, 0}, mud[3] = {0, 0, 0};
+  if (PASS == 2)
+    for (int k = 0; k < 3; ++k) { mus[k] = m1->v[k] / (double)m1->n; mud[k] = m1->v[3 + k] / (double)m1->n; }
+  for (long long p = p0 + threadIdx.x; p < p1; p += IC_RED_T) {
+    const int j = corr[p];
+    if (j < 0) continue;
+    const double s[3] = {(double)W[3 * p], (double)W[3 * p + 1], (double)W[3 * p + 2]};
+    const double q[3] = {(double)Q[3 * (size_t)j], (double)Q[3 * (size_t)j + 1], (double)Q[3 * (size_t)j + 2]};
+    if (PASS == 1) {
+      for (int k = 0; k < 3; ++k) { v.v[k] += s[k]; v.v[3 + k] += q[k]; }
+      v.v[6] += (double)d2[p];
+      ++v.n;
+    } else {
+      const double ds[3] = {s[0] - mus[0], s[1] - mus[1], s[2] - mus[2]};
+      const double dd[3] = {q[0] - mud[0], q[1] - mud[1], q[2] - mud[2]};
+      for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) v.v[r * 3 + c] += dd[r] * ds[c];
+    }
+  }
+  icp_tree(sh, v, part + blockIdx.x);
+}
+__global__ void __launch_bounds__(IC_RED_T) k_icp_total(const IcpSum *__restrict__ part, int nb, IcpSum *__restrict__ out) {
+  __shared__ IcpSum sh[IC_RED_T];
+  IcpSum v{};
+  for (int b = threadIdx.x; b < nb; b += IC_RED_T) icp_sum_add(v, part[b]);
+  icp_tree(sh, v, out);
+}
+
+// one thread: T_k from the moments, F <- T_k F, and DefaultConvergenceCriteria with max_iterations_similar_transforms = 0
+__global__ void k_icp_solve(IcpDev *dev, const IcpSum *__restrict__ m1, const IcpSum *__restrict__ m2, int k, int max_it,
+                            double eps_t, double eps_f) {
+  IcpHead &h = dev->h;
+  const unsigned long long c = m1->n;
+  h.cor = (int)c;
+  h.mse = c > 0 ? m1->v[6] / (double)c : (double)NAN;   // the distances found before T_k is applied, as PCL has it
+  for (int i = 0; i < 16; ++i) dev->T[i] = (i % 5 == 0) ? 1.f : 0.f;
+  if (c < 3) { h.state = GHICP_ICP_NO_CORRESPONDENCES; return; }
+  float mu_s[3], mu_d[3], sigma[9];
+  for (int a = 0; a < 3; ++a) { mu_s[a] = (float)(m1->v[a] / (double)c); mu_d[a] = (float)(m1->v[3 + a] / (double)c); }
+  for (int a = 0; a < 9; ++a) sigma[a] = (float)(m2->v[a] / (double)c);
+  double Rt[16];
+  umeyama_from_moments_f32(mu_s, mu_d, sigma, Rt);
+  float T[16], F[16];
+  for (int r = 0; r < 4; ++r)
+    for (int cc = 0; cc < 4; ++cc) T[r * 4 + cc] = (float)Rt[cc * 4 + r];
+  for (int r = 0; r < 4; ++r)
+    for (int cc = 0; cc < 4; ++cc)
+      F[r * 4 + cc] = ((T[r * 4] * h.F[cc] + T[r * 4 + 1] * h.F[4 + cc]) + T[r * 4 + 2] * h.F[8 + cc]) + T[r * 4 + 3] * h.F[12 + cc];
+  for (int i = 0; i < 16; ++i) { dev->T[i] = T[i]; h.F[i] = F[i]; }
+  if (k >= max_it) { h.state = GHICP_ICP_ITERATIONS; return; }
+  const double cosa = 0.5 * ((((double)T[0] + (double)T[5]) + (double)T[10]) - 1.0);
+  const double t2 = ((double)T[3] * (double)T[3] + (double)T[7] * (double)T[7]) + (double)T[11] * (double)T[11];
+  if (cosa >= 1.0 - eps_t && t2 <= eps_t) { h.state = GHICP_ICP_TRANSFORM; return; }
+  const double d = fabs(h.mse - dev->prev_mse);
+  if (d < 1e-12) { h.state = GHICP_ICP_ABS_MSE; return; }
+  if (d / dev->prev_mse < eps_f) { h.state = GHICP_ICP_REL_MSE; return; }
+  dev->prev_mse = h.mse;
+}
+
+inline int iblk(long long n, int t) { return (int)((n + t - 1) / t); }
+
+}  // namespace
+
+cudaError_t icp_run(const float *d_src, int n_src, const float *d_all, int n_all, const OverlapTarget *t, const float *d_tgt,
+                    const double *guess, const ghicp_icp_params *p, cudaEvent_t ev_iter, cudaEvent_t ev_fit, ghicp_icp_result *out,
+                    float *h_moved, int *h_cor, double *h_mse) {
+  const long long n = n_src, nt = t->n;
+  const bool recip = p->reciprocal != 0, trim = p->trim_ratio > 0.f;
+  const int nb = iblk(n, IC_RED_CHUNK);
+  DevBuf<float> W, d2, moved; DevBuf<int> corr, perm, rev, list; DevBuf<pu64> keys; DevBuf<unsigned char> flag;
+  DevBuf<IcpDev> dev; DevBuf<IcpSum> part, tot;
+  // every workspace of the loop first: running out of memory returns before anything is written (the reciprocal option's
+  // grid over W is the exception: prep_point_grid allocates it every iteration, from the same pool)
+  CUDA_TRY(W.alloc(3 * (size_t)n)); CUDA_TRY(d2.alloc((size_t)n)); CUDA_TRY(corr.alloc((size_t)n));
+  CUDA_TRY(perm.alloc((size_t)n)); CUDA_TRY(keys.alloc((size_t)n));
+  CUDA_TRY(dev.alloc(1)); CUDA_TRY(part.alloc((size_t)nb)); CUDA_TRY(tot.alloc(2));
+  if (recip) { CUDA_TRY(rev.alloc((size_t)nt)); CUDA_TRY(list.alloc((size_t)nt)); CUDA_TRY(flag.alloc((size_t)nt)); }
+  if (h_moved) CUDA_TRY(moved.alloc(3 * (size_t)n_all));
+  IcpDev h0{};
+  for (int r = 0; r < 4; ++r)
+    for (int c = 0; c < 4; ++c) h0.h.F[r * 4 + c] = guess ? (float)guess[c * 4 + r] : (r == c ? 1.f : 0.f);
+  h0.prev_mse = DBL_MAX;
+  CUDA_TRY(cudaMemcpyAsync(dev.get(), &h0, sizeof(h0), cudaMemcpyHostToDevice, 0));
+  IcpDev *D = dev.get();
+  const OvGrid G = ov_grid_of(t->pg);
+  if (ev_iter) CUDA_TRY(cudaEventRecord(ev_iter, 0));
+  GHICP_LAUNCH(k_icp_move, iblk(n, IC_T), IC_T, 0, 0, d_src, W.get(), n, D->h.F);   // W = P moved by the guess
+  IcpHead hh{};
+  std::vector<int> cor_tr;
+  std::vector<double> mse_tr;
+  int k = 1;
+  for (;; ++k) {
+    GHICP_LAUNCH(k_icp_keys, iblk(n, IC_T), IC_T, 0, 0, W.get(), n, G, keys.get(), perm.get());
+    CUDA_TRY(prep_sort_pairs(0, keys.get(), perm.get(), n_src));
+    GHICP_LAUNCH(k_icp_query, iblk(n, IC_T), IC_T, 0, 0, W.get(), n, perm.get(), G, corr.get(), d2.get(), D);
+    if (recip) {
+      CUDA_TRY(cudaMemsetAsync(flag.get(), 0, (size_t)nt, 0));
+      CUDA_TRY(cudaMemsetAsync(&D->n_rev, 0, sizeof(int), 0));
+      GHICP_LAUNCH(k_icp_mark, iblk(n, IC_T), IC_T, 0, 0, corr.get(), n, flag.get());
+      GHICP_LAUNCH(k_icp_compact, iblk(nt, IC_T), IC_T, 0, 0, flag.get(), nt, list.get(), D);
+      PointGrid pw;
+      CUDA_TRY(prep_point_grid(0, W.get(), n_src, n_src < 8 ? n_src : 8, 0.f, 0.0, &pw));
+      GHICP_LAUNCH(k_icp_rev, iblk(nt, IC_T), IC_T, 0, 0, d_tgt, list.get(), ov_grid_of(pw), rev.get(), D);
+      GHICP_LAUNCH(k_icp_recip, iblk(n, IC_T), IC_T, 0, 0, corr.get(), n, rev.get());
+    }
+    if (trim) {
+      GHICP_LAUNCH(k_icp_trim_keys, iblk(n, IC_T), IC_T, 0, 0, corr.get(), d2.get(), n, keys.get(), perm.get());
+      CUDA_TRY(prep_sort_pairs(0, keys.get(), perm.get(), n_src));
+      GHICP_LAUNCH(k_icp_trim_thr, 1, 1, 0, 0, keys.get(), n, p->trim_ratio, D);
+      GHICP_LAUNCH(k_icp_trim_apply, iblk(n, IC_T), IC_T, 0, 0, corr.get(), d2.get(), n, D);
+    }
+    GHICP_LAUNCH(k_icp_sum<1>, nb, IC_RED_T, 0, 0, W.get(), d_tgt, corr.get(), d2.get(), n, nullptr, part.get());
+    GHICP_LAUNCH(k_icp_total, 1, IC_RED_T, 0, 0, part.get(), nb, tot.get());
+    GHICP_LAUNCH(k_icp_sum<2>, nb, IC_RED_T, 0, 0, W.get(), d_tgt, corr.get(), d2.get(), n, tot.get(), part.get());
+    GHICP_LAUNCH(k_icp_total, 1, IC_RED_T, 0, 0, part.get(), nb, tot.get() + 1);
+    GHICP_LAUNCH(k_icp_solve, 1, 1, 0, 0, D, tot.get(), tot.get() + 1, k, p->max_iterations, p->transformation_epsilon,
+                 p->fitness_epsilon);
+    GHICP_LAUNCH(k_icp_move, iblk(n, IC_T), IC_T, 0, 0, W.get(), W.get(), n, D->T);
+    CUDA_TRY(cudaGetLastError());
+    // the one read-back of an iteration
+    CUDA_TRY(cudaMemcpyAsync(&hh, &D->h, sizeof(hh), cudaMemcpyDeviceToHost, 0));
+    CUDA_TRY(cudaStreamSynchronize(0));
+    cor_tr.push_back(hh.cor);
+    mse_tr.push_back(hh.mse);
+    if (hh.state != 0) break;
+  }
+  if (ev_fit) CUDA_TRY(cudaEventRecord(ev_fit, 0));
+  double Rt[16];
+  for (int r = 0; r < 4; ++r)
+    for (int c = 0; c < 4; ++c) Rt[c * 4 + r] = (double)hh.F[r * 4 + c];
+  // PCL's getFitnessScore after align: the §3.12 fitness of the whole source moved by F, max_range = +inf
+  ghicp_overlap_result ov{};
+  CUDA_TRY(overlap_run(d_all, n_all, t, Rt, 1.f, (double)INFINITY, 1, nullptr, &ov, nullptr));
+  if (h_moved) {
+    GHICP_LAUNCH(k_icp_move, iblk(n_all, IC_T), IC_T, 0, 0, d_all, moved.get(), (long long)n_all, D->h.F);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaMemcpyAsync(h_moved, moved.get(), 3 * sizeof(float) * (size_t)n_all, cudaMemcpyDeviceToHost, 0));
+  }
+  CUDA_TRY(cudaStreamSynchronize(0));
+  ghicp_icp_result r{};
+  std::memcpy(r.Rt, Rt, sizeof(Rt));
+  r.mse = hh.mse;
+  r.fitness = ov.fitness;
+  r.iterations = k;
+  r.state = hh.state;
+  r.converged = hh.state != GHICP_ICP_NO_CORRESPONDENCES;
+  r.cor = hh.cor;
+  r.cells_visited = (long long)hh.work[0];
+  r.candidates = (long long)hh.work[1];
+  *out = r;
+  if (h_cor) std::copy(cor_tr.begin(), cor_tr.end(), h_cor);
+  if (h_mse) std::copy(mse_tr.begin(), mse_tr.end(), h_mse);
+  return cudaSuccess;
+}
+
+}  // namespace ghicp_b200

@@ -20,13 +20,9 @@
 #include "ghicp_internal.h"
 #include "ghicp_device.cuh"
 #include "ghicp_grid.cuh"
+#include "ghicp_ovwalk.cuh"
 
 namespace ghicp_b200 {
-
-struct OverlapTarget {
-  PointGrid pg;
-  int n = 0;
-};
 
 namespace {
 
@@ -34,12 +30,6 @@ constexpr int OV_T = 128;         // threads per query CTA
 constexpr int RED_T = 256;        // threads per reduction CTA
 constexpr int RED_CHUNK = 8192;   // points per reduction CTA
 
-struct OvGrid {   // the target grid as the query kernel reads it
-  GridArgs g;
-  int gm[3];                      // largest cell coordinate per axis
-  double mn[3], ext[3];           // box minimum; box extent in cell edges
-  double cell, slack;
-};
 struct OvArgs {
   const float *A; long long n;
   float rt[12];                   // R row-major, then t (float32, rounded once from the double matrix)
@@ -51,105 +41,11 @@ struct OvArgs {
 };
 struct OvPart { double fit, ov; unsigned long long n_fit, n_ov; };
 
-// x' = ((R00 x + R01 y) + R02 z) + t0, float32, every operation rounded separately (SAC-IA's sac_move)
-__device__ __forceinline__ void ov_move(const float *rt, float x, float y, float z, float &ox, float &oy, float &oz) {
-  ox = ((rt[0] * x + rt[1] * y) + rt[2] * z) + rt[9];
-  oy = ((rt[3] * x + rt[4] * y) + rt[5] * z) + rt[10];
-  oz = ((rt[6] * x + rt[7] * y) + rt[8] * z) + rt[11];
-}
-// distance from u to the interval [lo, hi] (cell edges)
-__device__ __forceinline__ double ov_gap(double u, double lo, double hi) { return u < lo ? lo - u : (u > hi ? u - hi : 0.0); }
-// where the points of cells lo .. hi on one axis can lie: the cells widened by the rounding slack, clipped to B's box
-__device__ __forceinline__ double ov_cells_gap(double u, int lo, int hi, double s, double ext) {
-  return ov_gap(u, fmax((double)lo - s, 0.0), fmin((double)hi + 1.0 + s, ext));
-}
-// narrow [a, b] to the cells whose extent comes within w (cell edges) of u
-__device__ __forceinline__ void ov_window(double u, double w, double s, int &a, int &b) {
-  const double lo = u - w - 1.0 - s, hi = u + w + s;
-  if (lo > (double)a) a = lo > (double)b ? b + 1 : (int)ceil(lo);
-  if (hi < (double)b) b = hi < (double)a ? a - 1 : (int)floor(hi);
-}
-
-// Nearest squared distance (knn_d2) from q to B: exact when it is <= lim, +inf otherwise.  hit >= 0: stops at the first
-// d2 < hit and returns it (overlap-only mode).  Bounds are compared in double against (1 - 1e-5) of their value, far more
-// than the float32 rounding of knn_d2.
+// Nearest squared distance from q to B (ov_nearest of ghicp_ovwalk.cuh without the index)
 __device__ float ov_nn_d2(const GridRegs &r, const OvGrid &G, float qx, float qy, float qz, double lim, float hit,
                           unsigned long long &cells, unsigned long long &cand) {
-  // a non-finite moved point (a NaN return of an organised scan) has no nearest neighbour: +inf at once, no walk
-  if (!(isfinite(qx) && isfinite(qy) && isfinite(qz))) return INFINITY;
-  const double q[3] = {(double)qx, (double)qy, (double)qz};
-  const double s = G.slack, unit = G.cell * G.cell * (1.0 - 1e-5);
-  double u[3], bg[3];
-  int c[3];
-  for (int a = 0; a < 3; ++a) {
-    u[a] = (q[a] - G.mn[a]) / G.cell;
-    bg[a] = ov_gap(u[a], 0.0, G.ext[a]);
-    c[a] = !(u[a] > 0.0) ? 0 : (u[a] >= (double)G.gm[a] ? G.gm[a] : (int)u[a]);
-  }
-  const double bg2 = (bg[0] * bg[0] + bg[1] * bg[1]) + bg[2] * bg[2];
-  if (!(bg2 * unit <= lim)) return INFINITY;   // beyond the limit from B's box
-  int kmax = 0;
-  for (int a = 0; a < 3; ++a) kmax = max(kmax, max(c[a], G.gm[a] - c[a]));
-  float best = INFINITY;
-  for (int k = 0;; ++k) {
-    // columns of ring k: a wall column (max(|dx|, |dy|) == k) spans cz - k .. cz + k, an inner one only its floor and
-    // ceiling cell; a column whose bound passes L (squared cell edges) is skipped
-    double L = fmin((double)best, lim) / unit;
-    if (bg2 > L) break;
-    int x0 = max(c[0] - k, 0), x1 = min(c[0] + k, G.gm[0]);
-    ov_window(u[0], sqrt(L - bg[1] * bg[1] - bg[2] * bg[2]), s, x0, x1);
-    for (int x = x0; x <= x1; ++x) {
-      L = fmin((double)best, lim) / unit;
-      const double gx = ov_cells_gap(u[0], x, x, s, G.ext[0]);
-      const double wy = L - gx * gx - bg[2] * bg[2];
-      if (wy < 0.0) continue;
-      int y0 = max(c[1] - k, 0), y1 = min(c[1] + k, G.gm[1]);
-      ov_window(u[1], sqrt(wy), s, y0, y1);
-      const bool xwall = abs(x - c[0]) == k;
-      const int za = c[2] - k, zb = c[2] + k;   // the two cells of an inner column, or the run za .. zb of a wall column
-      bool inner = false;                        // can an inner column of this row hold a closer point at all?
-      if (!xwall) {
-        const double wz0 = sqrt(fmax(L - gx * gx - bg[1] * bg[1], 0.0));
-        inner = (za >= 0 && ov_cells_gap(u[2], za, za, s, G.ext[2]) <= wz0) ||
-                (zb <= G.gm[2] && ov_cells_gap(u[2], zb, zb, s, G.ext[2]) <= wz0);
-      }
-      for (int y = y0; y <= y1; ++y) {
-        const bool wall = xwall || abs(y - c[1]) == k;
-        if (!wall && !inner) { if (y < c[1] + k - 1) y = c[1] + k - 1; continue; }   // on to the far wall
-        const double gy = ov_cells_gap(u[1], y, y, s, G.ext[1]);
-        const double wz = L - gx * gx - gy * gy;
-        if (wz < 0.0) continue;
-        for (int part = 0; part < (wall ? 1 : 2); ++part) {
-          int lo, hi;
-          if (wall) { lo = max(za, 0); hi = min(zb, G.gm[2]); }
-          else { lo = hi = part == 0 ? za : zb; if (lo < 0 || lo > G.gm[2]) continue; }
-          ov_window(u[2], sqrt(wz), s, lo, hi);
-          if (lo > hi) continue;
-          cells += (unsigned long long)(hi - lo + 1);
-          const int s0 = r.cstart[lower_cell(r, cell_key(x, y, lo))], s1 = r.cstart[lower_cell(r, cell_key(x, y, hi) + 1)];
-          cand += (unsigned long long)(s1 - s0);
-          for (int p = s0; p < s1; ++p) {
-            const float d2 = knn_d2(qx, qy, qz, r.sorted[p]);
-            if (d2 < hit) return d2;
-            best = d2 < best ? d2 : best;
-          }
-        }
-      }
-    }
-    if (k >= kmax) break;
-    // a true lower bound on every cell outside the visited cube: it lies beyond ring k on some axis, and within B's box
-    // on the two others
-    L = fmin((double)best, lim) / unit;
-    double lb = INFINITY;
-    for (int a = 0; a < 3; ++a) {
-      const double b1 = bg[(a + 1) % 3], b2 = bg[(a + 2) % 3], o2 = b1 * b1 + b2 * b2;
-      if (c[a] - k - 1 >= 0) { const double d = ov_cells_gap(u[a], 0, c[a] - k - 1, s, G.ext[a]); lb = fmin(lb, d * d + o2); }
-      if (c[a] + k + 1 <= G.gm[a]) { const double d = ov_cells_gap(u[a], c[a] + k + 1, G.gm[a], s, G.ext[a]); lb = fmin(lb, d * d + o2); }
-    }
-    if (lb > L) break;
-  }
-  if (hit >= 0.f) return best < hit ? best : INFINITY;
-  return (double)best <= lim ? best : INFINITY;
+  int unused = -1;
+  return ov_nearest<false>(r, G, qx, qy, qz, lim, hit, cells, cand, unused);
 }
 
 __global__ void __launch_bounds__(OV_T) k_ov_query(const OvArgs a, const OvGrid G) {
@@ -262,10 +158,7 @@ cudaError_t overlap_run(const float *d_a, int n_a, const OverlapTarget *t, const
   }
   a.hit = want_fitness ? -1.f : r2;
   a.lim = want_fitness ? std::max((double)r2, max_range) : (double)r2;
-  G.g = t->pg.g; G.gm[0] = t->pg.gx; G.gm[1] = t->pg.gy; G.gm[2] = t->pg.gz;
-  G.mn[0] = t->pg.g.mnx; G.mn[1] = t->pg.g.mny; G.mn[2] = t->pg.g.mnz;
-  G.cell = t->pg.cell; G.slack = t->pg.slack;
-  for (int k = 0; k < 3; ++k) G.ext[k] = ((double)t->pg.mx[k] - G.mn[k]) / G.cell;
+  G = ov_grid_of(t->pg);
   if (ev_queries) CUDA_TRY(cudaEventRecord(ev_queries, 0));
   if (cell_order) {
     GHICP_LAUNCH(k_ov_keys, oblk(n, OV_T), OV_T, 0, 0, a, G, keys.get(), perm.get());

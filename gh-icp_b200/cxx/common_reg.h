@@ -10,12 +10,17 @@
 //                                                      ghicp_cloud_overlap (DESIGN.md §3.12, overlap-only mode)
 //   transformcloud       (src/common_reg.cpp:325-350)  the float32 transform of every point, ((m00 x + m01 y) + m02 z) + m03
 //   invTransform         (src/common_reg.cpp:358-370)  the reference's "not mathematically" inverse, kept as it is
+//   icp_reg              (src/common_reg.cpp:44-107)   PCL's point-to-point IterativeClosestPoint from the identity, with the
+//                                                      reciprocal and trimmed options, by ghicp_cloud_icp (DESIGN.md §3.13)
 // Differences, deliberate: clouds are ghicp::Cloud (cloud_io.h) and fpfhFeaturePtr the stand-in of ghicp_types.h; the
 // transform is Eigen::Matrix4f when Eigen is on the include path, else the column-major ghicp::Matrix4f; the SAC-IA is the
 // deterministic one of DESIGN.md §3.11 instead of PCL's std::rand()-driven one; no CPU path (without a CUDA device both
-// members throw).  The fitness of the last Coarsereg_FPFHSAC, which the reference prints, is kept (getFitnessScore).
-// Not provided: the PCL ICP wrappers (icp_reg, ptplicp_reg, gicp_reg), LLS_4DOF / SVD_6DOF and CSTRAN_4DOF / CSTRAN_7DOF.
+// members throw).  The fitness of the last Coarsereg_FPFHSAC or icp_reg, which the reference prints, is kept
+// (getFitnessScore).  icp_reg prints its lines to std::cout only (the reference also logs them through glog).
+// Not provided: the other PCL ICP wrappers (ptplicp_reg, gicp_reg), LLS_4DOF / SVD_6DOF and CSTRAN_4DOF / CSTRAN_7DOF.
 #pragma once
+#include <algorithm>
+#include <ctime>
 #include <iostream>
 #include <stdexcept>
 #include <string>
@@ -74,7 +79,47 @@ class CRegistration {
       out.push(o[0], o[1], o[2]);
     }
     TransformedSource = out;
+    fitness_ = result_.fitness;
     std::cout << "The fitness score of this registration is " << result_.fitness << std::endl;   // :419
+  }
+
+  // :44-107 — point-to-point ICP of SourceCloud onto TargetCloud from the identity (transformation epsilon 1e-8, fitness
+  // epsilon 1e-5); with use_trimmed_rejector the rejector's ratio is calOverlap(SourceCloud, TargetCloud, thre_dis), and the
+  // call returns false without registering when that ratio is below min_overlap_for_reg.  TransformedSource = the moved source.
+  bool icp_reg(const Cloud &SourceCloud, const Cloud &TargetCloud, Cloud &TransformedSource, Matrix4f &transformationS2T,
+               int max_iter, bool use_reciprocal_correspondence, bool use_trimmed_rejector, float thre_dis,
+               float min_overlap_for_reg) {
+    const clock_t t0 = clock();
+    ghicp_icp_params p{};
+    p.max_iterations = max_iter; p.reciprocal = use_reciprocal_correspondence ? 1 : 0;
+    p.transformation_epsilon = 1e-8; p.fitness_epsilon = 1e-5;   // :86, :88
+    if (use_trimmed_rejector) {
+      const float overlap_ratio = calOverlap(SourceCloud, TargetCloud, thre_dis);
+      if (overlap_ratio < min_overlap_for_reg) {
+        std::cout << "The overlap ratio is too small. This registration would not be done." << std::endl;
+        return false;
+      }
+      p.trim_ratio = std::min(1.0f, overlap_ratio);   // setOverlapRatio clamps to [0, 1]
+    }
+    const int n = (int)SourceCloud.size();
+    std::vector<float> moved(3 * (size_t)n);
+    ghicp_icp_result r{};
+    if (ghicp_cloud_icp(0, SourceCloud.xyz.data(), n, TargetCloud.xyz.data(), (int)TargetCloud.size(), nullptr, &p, &r, moved.data(),
+                        nullptr, nullptr) < 0)
+      throw std::runtime_error(std::string("CRegistration::icp_reg: ") + ghicp_last_error(nullptr));
+    for (int i = 0; i < 16; ++i) transformationS2T.data()[i] = (float)r.Rt[i];
+    TransformedSource.xyz = moved;
+    fitness_ = r.fitness;
+    icp_result_ = r;
+    const clock_t t1 = clock();
+    std::cout << "Point-to-Point ICP done in " << float(t1 - t0) / CLOCKS_PER_SEC << " s" << std::endl;
+    for (int i = 0; i < 4; ++i) {
+      for (int j = 0; j < 4; ++j) std::cout << (j ? " " : "") << transformationS2T(i, j);
+      std::cout << std::endl;
+    }
+    std::cout << "The fitness score of this registration is " << fitness_ << std::endl;
+    std::cout << "-----------------------------------------------------------------------------" << std::endl;
+    return true;
   }
 
   // :294-317 — (0.01 + #{points of Cloud1 with a Cloud2 point at d2 < thre_dis^2}) / |Cloud1|, as the reference's float
@@ -109,11 +154,14 @@ class CRegistration {
     invtransformation(3, 3) = 1.f;
   }
 
-  double getFitnessScore() const { return result_.fitness; }
+  double getFitnessScore() const { return fitness_; }
   const ghicp_sac_result &sac_result() const { return result_; }
+  const ghicp_icp_result &icp_result() const { return icp_result_; }
 
  private:
   ghicp_sac_result result_{};
+  ghicp_icp_result icp_result_{};
+  double fitness_ = 0.0;   // of the last Coarsereg_FPFHSAC or icp_reg
 };
 
 }  // namespace ghicp

@@ -33,6 +33,13 @@ pipeline, capi.cloud_overlap with `features`; DESIGN.md §3.12): info["evaluatio
 initial_alignment="fpfh_sac", info["sac"]["evaluation"] for the coarse one.  The default None leaves info as it was.
 cal_overlap and evaluate_registration score any pair of clouds.
 
+refine = {"max_iter": m, "reciprocal": b, "trimmed_thre_dis": r (optional)} refines the GH-ICP transform on the down-sampled
+clouds with point-to-point ICP (capi.Prep.icp / capi.cloud_icp with `features`; DESIGN.md §3.13), started from that
+transform, and returns the refined one; info["icp"] describes the refinement and keeps the GH-ICP transform as "Rt_before".
+With "trimmed_thre_dis" the trimmed rejector's ratio is calOverlap at that start pose, where the reference's icp_reg measures
+it on the unmoved source (it starts from the identity); with `evaluate`, info["evaluation"] scores the refined transform.
+The default None leaves the result and info as they were.  icp_reg(source, target, ...) is CRegistration::icp_reg itself.
+
 coarsereg_fpfh_sac(source_xyz, target_xyz, search_radius) is CRegistration::Coarsereg_FPFHSAC (src/common_reg.cpp:393-423):
 radius FPFH on every point of both clouds, then SAC-IA with correspondence randomness 15.
 """
@@ -45,8 +52,9 @@ from .registration import Energyfunction, GHRegistration, Keypoints
 def register_clouds(target_xyz, source_xyz, resolution, neighborhood_radius, curvature_non_max_radius, corr_type=capi.CT_NN,
                     feature_type=capi.FT_NONE, features=None, weight_adjustment_ratio=1.1, weight_adjustment_step=0.1,
                     dof_type=6, estimated_IoU=0.5, max_iter=0, device=0, bsc_pattern=None, fpfh_k=20, initial_alignment=None,
-                    sac=None, fpfh_radius=None, evaluate=None, **reg_kw):
+                    sac=None, fpfh_radius=None, evaluate=None, refine=None, **reg_kw):
     ev_kw = _evaluate_kw(evaluate)
+    icp_kw = _refine_kw(refine)
     if initial_alignment not in (None, "fpfh_sac"):
         raise capi.GhicpError(-1, f"initial_alignment must be None or 'fpfh_sac', not {initial_alignment!r}")
     if fpfh_radius is not None:
@@ -91,6 +99,9 @@ def register_clouds(target_xyz, source_xyz, resolution, neighborhood_radius, cur
                 info["fpfh_ms"] = dict(target=pt.fpfh_ms, source=ps.fpfh_ms)
             if sac_info is not None:
                 info["sac"] = dict(sac_info, Rt=Rt0)
+            if icp_kw is not None:
+                Rt = _refine(Rt, icp_kw, info, lambda G, thr: ps.overlap(pt, G, thre_dis=thr, fitness=False)["ratio"],
+                             lambda G, **kw: ps.icp(pt, G, **kw))
             if ev_kw is not None:
                 info["evaluation"] = ps.overlap(pt, Rt, **ev_kw)
                 if sac_info is not None:
@@ -129,6 +140,10 @@ def register_clouds(target_xyz, source_xyz, resolution, neighborhood_radius, cur
                 n_source_kp=len(kp_idx["S"]), bbx_magnitude=bbx, cor=len(reg.pairs()[0]))
     if sac_info is not None:
         info["sac"] = sac_info
+    if icp_kw is not None:
+        Rt = _refine(Rt, icp_kw, info,
+                     lambda G, thr: capi.cloud_overlap(down["S"], down["T"], G, thre_dis=thr, fitness=False, device=device)["ratio"],
+                     lambda G, **kw: capi.cloud_icp(down["S"], down["T"], G, device=device, **kw))
     if ev_kw is not None:
         info["evaluation"] = capi.cloud_overlap(down["S"], down["T"], Rt, device=device, **ev_kw)
         if sac_info is not None:
@@ -143,6 +158,45 @@ def _evaluate_kw(evaluate):
     if not isinstance(evaluate, dict) or "thre_dis" not in evaluate or set(evaluate) - {"thre_dis", "max_range"}:
         raise capi.GhicpError(-1, "evaluate must be a dict {thre_dis, max_range (optional)}")
     return dict(thre_dis=float(evaluate["thre_dis"]), max_range=float(evaluate.get("max_range", float("inf"))))
+
+
+def _refine_kw(refine):
+    if refine is None:
+        return None
+    if not isinstance(refine, dict) or "max_iter" not in refine or set(refine) - {"max_iter", "reciprocal", "trimmed_thre_dis"}:
+        raise capi.GhicpError(-1, "refine must be a dict {max_iter, reciprocal (optional), trimmed_thre_dis (optional)}")
+    return dict(max_iter=int(refine["max_iter"]), reciprocal=bool(refine.get("reciprocal", False)),
+                thre_dis=refine.get("trimmed_thre_dis"))
+
+
+def _refine(Rt, kw, info, ratio_at, icp_from):
+    """ICP from Rt (icp_from(guess, **cloud_icp options)); the trimmed ratio is calOverlap at Rt (ratio_at(Rt, thre_dis))."""
+    rho = 0.0 if kw["thre_dis"] is None else float(ratio_at(Rt, float(kw["thre_dis"])))
+    Rt_icp, icp_info = icp_from(Rt, max_iterations=kw["max_iter"], reciprocal=kw["reciprocal"], trim_ratio=min(rho, 1.0))
+    info["icp"] = dict(icp_info, Rt_before=Rt, trim_ratio=rho)
+    return Rt_icp
+
+
+def icp_reg(source_xyz, target_xyz, max_iter, use_reciprocal_correspondence, use_trimmed_rejector, thre_dis,
+            min_overlap_for_reg=0.0, device=0):
+    """CRegistration::icp_reg (src/common_reg.cpp:44-107) on the GPU: point-to-point ICP of the source onto the target from
+    the identity, transformation epsilon 1e-8 and fitness epsilon 1e-5 as :86-88 set them (capi.cloud_icp, DESIGN.md §3.13).
+    With use_trimmed_rejector the trimmed rejector's ratio is calOverlap(source, target, thre_dis) of the unmoved source, and
+    the call returns None when that ratio is below min_overlap_for_reg (the reference returns false).  Returns (Rt 4x4, info
+    with the transformed source under "moved"; info["overlap_ratio"] when trimmed)."""
+    S = np.ascontiguousarray(source_xyz, dtype=np.float32).reshape(-1, 3)
+    T = np.ascontiguousarray(target_xyz, dtype=np.float32).reshape(-1, 3)
+    rho = 0.0
+    if use_trimmed_rejector:
+        rho = cal_overlap(S, T, thre_dis, device=device)
+        if rho < min_overlap_for_reg:
+            return None
+    Rt, info = capi.cloud_icp(S, T, None, max_iterations=max_iter, reciprocal=use_reciprocal_correspondence,
+                              trim_ratio=min(rho, 1.0), transformation_epsilon=1e-8, fitness_epsilon=1e-5, return_moved=True,
+                              device=device)
+    if use_trimmed_rejector:
+        info["overlap_ratio"] = rho
+    return Rt, info
 
 
 def cal_overlap(cloud1, cloud2, thre_dis, device=0):

@@ -348,6 +348,51 @@ int ghicp_cloud_overlap(int device, const float *a_xyz, int n_a, const float *b_
 int ghicp_prep_overlap(const ghicp_prep *a, const ghicp_prep *b, const double Rt[16], float thre_dis, double max_range,
                        int want_fitness, ghicp_overlap_result *out);
 
+/* ---- point-to-point ICP on the dense clouds (DESIGN.md §3.13) ------------------------------------------------------------
+ * CRegistration::icp_reg (src/common_reg.cpp:44-107): PCL's IterativeClosestPoint<PointXYZ, PointXYZ> with
+ * DefaultConvergenceCriteria, on the canonical definition of DESIGN.md §3.13.  Every iteration pairs each source point, moved
+ * by the transform so far, with its exact nearest target point ((d2, index) order), optionally keeps only reciprocal pairs
+ * and then the floor(trim_ratio * pairs) closest ones, fits the float32 Umeyama of the loop to FP64 two-pass moments of the
+ * kept pairs, and stops on the first of: max_iterations, a transform within transformation_epsilon of the identity, an
+ * absolute (1e-12) or relative (fitness_epsilon) change of the pairs' mean squared distance, or fewer than 3 pairs.  Sums are
+ * in double in a fixed order: two calls give identical bits.  Non-finite source and target points take no part. */
+enum ghicp_icp_state {   /* PCL's DefaultConvergenceCriteria::ConvergenceState values */
+  GHICP_ICP_ITERATIONS = 1,
+  GHICP_ICP_TRANSFORM = 2,
+  GHICP_ICP_ABS_MSE = 3,
+  GHICP_ICP_REL_MSE = 4,
+  GHICP_ICP_NO_CORRESPONDENCES = 5
+};
+typedef struct ghicp_icp_params {
+  int max_iterations;              /* >= 1 (icp_reg's max_iter) */
+  int reciprocal;                  /* setUseReciprocalCorrespondences */
+  float trim_ratio;                /* CorrespondenceRejectorTrimmed::setOverlapRatio, 0 = no rejector, else (0, 1] */
+  double transformation_epsilon;   /* >= 0; icp_reg: 1e-8 */
+  double fitness_epsilon;          /* >= 0; icp_reg: 1e-5 */
+  int reserved[4];
+} ghicp_icp_params;
+typedef struct ghicp_icp_result {
+  double Rt[16];                   /* column-major: the float32 accumulated transform widened (the guess when no step ran) */
+  double mse;                      /* mean squared distance of the last iteration's kept pairs (NaN without a pair) */
+  double fitness;                  /* PCL's getFitnessScore: §3.12 fitness of the source moved by Rt, max_range = +inf */
+  int iterations, converged, state, cor;          /* state: ghicp_icp_state; cor: the last iteration's kept pairs */
+  long long cells_visited, candidates;            /* work of every nearest-neighbour query of every iteration */
+  float stage_ms[4];                              /* target grid (0 when cached), iterations, fitness, total */
+} ghicp_icp_result;
+/* src_xyz [n_s][3], tgt_xyz [n_t][3] (host arrays); guess column-major (NULL = identity), rounded once to float32; moved [n_s][3]
+ * (may be NULL) receives the source moved by Rt (PCL's align output); cor_trace / mse_trace [max_iterations] (may be NULL)
+ * receive each iteration's kept pairs and mean squared distance (entries past `iterations` are left as they are).  Fewer than
+ * 3 pairs returns GHICP_W_FEW_PAIRS with the result filled in (converged = 0, Rt = the transform so far).  Argument errors
+ * (NULL, n <= 0, no finite source or target point, max_iterations < 1, trim_ratio outside [0, 1] or NaN, a negative or NaN
+ * epsilon, a non-finite guess, handles on different devices) return GHICP_E_ARG and write nothing; out of memory returns
+ * GHICP_E_NOMEM and writes nothing. */
+int ghicp_cloud_icp(int device, const float *src_xyz, int n_s, const float *tgt_xyz, int n_t, const double guess[16],
+                    const ghicp_icp_params *p, ghicp_icp_result *out, float *moved, int *cor_trace, double *mse_trace);
+/* the down-sampled clouds of two pipeline results, device to device; the target's grid is the one ghicp_prep_overlap keeps
+ * (built by whichever call comes first, stage_ms[0] = 0 when it already exists) */
+int ghicp_prep_icp(const ghicp_prep *source, const ghicp_prep *target, const double guess[16], const ghicp_icp_params *p,
+                   ghicp_icp_result *out);
+
 /* ---- multi-GPU (one process per GPU; source rows sharded, target replicated) ---------------- */
 /* 128-byte NCCL unique id; rank 0 creates it, the host runtime broadcasts it (torch.distributed,
  * MPI, a file ...). No NCCL symbol is touched unless these are called (world == 1 → never). */
