@@ -19,4 +19,6 @@ from .registration import GHRegistration, Keypoints, Energyfunction  # noqa: F40
 from . import synth  # noqa: F401
 from . import capi  # noqa: F401
 from . import pipeline  # noqa: F401
-from .pipeline import register_clouds, transform_cloud, coarsereg_fpfh_sac, cal_overlap, evaluate_registration, icp_reg  # noqa: F401
+from .pipeline import (  # noqa: F401
+    register_clouds, transform_cloud, coarsereg_fpfh_sac, cal_overlap, evaluate_registration, icp_reg, ptplicp_reg,
+)

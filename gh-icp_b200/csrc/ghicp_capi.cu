@@ -1274,7 +1274,9 @@ struct ghicp_prep {
   float stage_ms[5] = {0, 0, 0, 0, 0};
   FpfhStats fpfh_stats;
   OverlapTarget *ov_target = nullptr;   // the down-sampled cloud's grid as an overlap target, after ghicp_prep_overlap
-  std::mutex ov_mu;                     // guards ov_target: concurrent first calls on one target build it once
+  DevBuf<float> icp_nrm;                // [n_down][3] k-NN normals of point-to-plane ICP, after ghicp_prep_icp with metric 1
+  int icp_nrm_k = 0;                    // their k (0: none)
+  std::mutex ov_mu;                     // guards ov_target and the normals: concurrent first calls on one target build once
 };
 
 int ghicp_prep_destroy(ghicp_prep *h) {
@@ -1713,7 +1715,7 @@ int ghicp_prep_overlap(const ghicp_prep *a, const ghicp_prep *b, const double Rt
   return cuda_status(prep_overlap_run(a, tb, Rt, thre_dis, max_range, want_fitness, out), "prep_overlap");
 }
 
-// ---- point-to-point ICP on the dense clouds --------------------------------------------------------------------------------
+// ---- point-to-point and point-to-plane ICP on the dense clouds -------------------------------------------------------------
 static bool icp_params_ok(const ghicp_icp_params *p, const double *guess, const char *who) {
   const bool ok = p && p->max_iterations >= 1 && p->trim_ratio >= 0.f && p->trim_ratio <= 1.f &&   // false for NaN
                   p->transformation_epsilon >= 0.0 && p->fitness_epsilon >= 0.0;
@@ -1721,7 +1723,15 @@ static bool icp_params_ok(const ghicp_icp_params *p, const double *guess, const 
     set_error(nullptr, std::string(who) + ": max_iterations must be >= 1, trim_ratio in [0, 1], the epsilons >= 0");
     return false;
   }
+  if (p->metric != 0 && !(p->metric == 1 && p->normal_k >= 3 && p->normal_k <= 32)) {
+    set_error(nullptr, std::string(who) + ": metric must be 0 (point-to-point) or 1 (point-to-plane, with normal_k in 3..32)");
+    return false;
+  }
   return overlap_rt_ok(guess, who);
+}
+// the status of a finished ICP call: its warning bit, if any
+static int icp_warnings(const ghicp_icp_result *r) {
+  return r->state == GHICP_ICP_NO_CORRESPONDENCES ? GHICP_W_FEW_PAIRS : (r->state == GHICP_ICP_SINGULAR ? GHICP_W_SINGULAR : GHICP_OK);
 }
 
 // Both ICP entries write *out, moved and the traces only once every stage succeeded.
@@ -1729,11 +1739,12 @@ static cudaError_t cloud_icp_run(const float *src, int n_s, const float *src_fin
                                  const double *guess, const ghicp_icp_params *p, ghicp_icp_result *out, float *moved, int *cor_trace,
                                  double *mse_trace) {
   StageEvents<4> ev;
-  DevBuf<float> d_all, d_fin, d_t;
+  DevBuf<float> d_all, d_fin, d_t, d_nrm;
   ghicp_icp_result r{};
   CUDA_TRY(ev.create());
   CUDA_TRY(d_all.alloc(3 * (size_t)n_s)); CUDA_TRY(d_t.alloc(3 * (size_t)n_t));
   if (src_fin != src) CUDA_TRY(d_fin.alloc(3 * (size_t)ns_fin));
+  if (p->metric == 1) CUDA_TRY(d_nrm.alloc(3 * (size_t)n_t));
   CUDA_TRY(cudaMemcpyAsync(d_all.get(), src, 3 * (size_t)n_s * sizeof(float), cudaMemcpyHostToDevice, 0));
   if (src_fin != src) CUDA_TRY(cudaMemcpyAsync(d_fin.get(), src_fin, 3 * (size_t)ns_fin * sizeof(float), cudaMemcpyHostToDevice, 0));
   CUDA_TRY(cudaMemcpyAsync(d_t.get(), tgt, 3 * (size_t)n_t * sizeof(float), cudaMemcpyHostToDevice, 0));
@@ -1742,8 +1753,10 @@ static cudaError_t cloud_icp_run(const float *src, int n_s, const float *src_fin
   CUDA_TRY(overlap_target_build(d_t.get(), n_t, &t));
   std::vector<int> cor(cor_trace ? p->max_iterations : 0);
   std::vector<double> mse(mse_trace ? p->max_iterations : 0);
-  const cudaError_t e = icp_run(src_fin != src ? d_fin.get() : d_all.get(), ns_fin, d_all.get(), n_s, t, d_t.get(), guess, p, ev[1],
-                                ev[2], &r, moved, cor_trace ? cor.data() : nullptr, mse_trace ? mse.data() : nullptr);
+  cudaError_t e = p->metric == 1 ? prep_knn_normals(0, d_t.get(), n_t, p->normal_k, d_nrm.get()) : cudaSuccess;
+  if (e == cudaSuccess)
+    e = icp_run(src_fin != src ? d_fin.get() : d_all.get(), ns_fin, d_all.get(), n_s, t, d_t.get(), d_nrm.get(), guess, p, ev[1],
+                ev[2], &r, moved, cor_trace ? cor.data() : nullptr, mse_trace ? mse.data() : nullptr);
   overlap_target_free(t);
   CUDA_TRY(e);
   CUDA_TRY(cudaEventRecord(ev[3], 0));
@@ -1771,7 +1784,7 @@ int ghicp_cloud_icp(int device, const float *src_xyz, int n_s, const float *tgt_
   if (int rc = cuda_status(cloud_icp_run(src_xyz, n_s, s_fin, ns_fin, t_fin, nt_fin, guess, p, out, moved, cor_trace, mse_trace),
                            "cloud_icp"))
     return rc;
-  return out->converged ? GHICP_OK : GHICP_W_FEW_PAIRS;
+  return icp_warnings(out);
 }
 
 static cudaError_t prep_icp_run(const ghicp_prep *s, ghicp_prep *tb, const double *guess, const ghicp_icp_params *p,
@@ -1780,11 +1793,20 @@ static cudaError_t prep_icp_run(const ghicp_prep *s, ghicp_prep *tb, const doubl
   ghicp_icp_result r{};
   CUDA_TRY(ev.create());
   CUDA_TRY(cudaEventRecord(ev[0], 0));
-  std::lock_guard<std::mutex> lk(tb->ov_mu);   // the grid ghicp_prep_overlap keeps, under its lock
-  const bool cached = tb->ov_target != nullptr;
+  std::lock_guard<std::mutex> lk(tb->ov_mu);   // the grid ghicp_prep_overlap keeps, and the normals, under its lock
+  bool cached = tb->ov_target != nullptr;
   if (!cached) CUDA_TRY(overlap_target_build(tb->d_down.get(), tb->n_down, &tb->ov_target));
-  CUDA_TRY(icp_run(s->d_down.get(), s->n_down, s->d_down.get(), s->n_down, tb->ov_target, tb->d_down.get(), guess, p, ev[1], ev[2],
-                   &r, nullptr, nullptr, nullptr));
+  if (p->metric == 1 && tb->icp_nrm_k != p->normal_k) {
+    // into a fresh buffer: the cache changes only once the new normals exist
+    DevBuf<float> nrm;
+    CUDA_TRY(nrm.alloc(3 * (size_t)tb->n_down));
+    CUDA_TRY(prep_knn_normals(0, tb->d_down.get(), tb->n_down, p->normal_k, nrm.get()));
+    tb->icp_nrm = std::move(nrm);
+    tb->icp_nrm_k = p->normal_k;
+    cached = false;
+  }
+  CUDA_TRY(icp_run(s->d_down.get(), s->n_down, s->d_down.get(), s->n_down, tb->ov_target, tb->d_down.get(), tb->icp_nrm.get(), guess,
+                   p, ev[1], ev[2], &r, nullptr, nullptr, nullptr));
   CUDA_TRY(cudaEventRecord(ev[3], 0));
   CUDA_TRY(cudaStreamSynchronize(0));
   if (!cached) r.stage_ms[0] = ev.ms(0, 1);
@@ -1803,7 +1825,7 @@ int ghicp_prep_icp(const ghicp_prep *source, const ghicp_prep *target, const dou
   if (int rc = enter_device(source->device, "prep_icp")) return rc;
   ghicp_prep *tb = const_cast<ghicp_prep *>(target);   // the grid is a cache of the target's down-sampled cloud, not its state
   if (int rc = cuda_status(prep_icp_run(source, tb, guess, p, out), "prep_icp")) return rc;
-  return out->converged ? GHICP_OK : GHICP_W_FEW_PAIRS;
+  return icp_warnings(out);
 }
 
 int ghicp_set_initial_transform(ghicp_ctx *ctx, const double Rt[16]) {

@@ -14,6 +14,14 @@
 //   k_icp_total         the demeaned cross-covariance), as k_ov_reduce / k_ov_total: no floating-point atomic
 //   k_icp_solve         one thread: the float32 Umeyama of the loop, F <- T F, DefaultConvergenceCriteria
 //   k_icp_move          W <- T W (sac_move's formula)
+// Point-to-plane (metric 1, DESIGN.md §3.14: the reference's CRegistration::ptplicp_reg, src/common_reg.cpp:123-199, PCL's
+// IterativeClosestPointWithNormals with TransformationEstimationPointToPlaneLLS) keeps every stage above but the estimate:
+//   k_icp_sum<1>        as above: the kept pairs' count, sum s (-> the centre m), sum d
+//   k_icp_sum_pl        the 21 + 6 FP64 sums of the centred normal equations, rows [(s - m) x n_j, n_j], rhs n_j.(q_j - s),
+//   k_icp_total_pl      over the same point blocks and thread tree as k_icp_sum, one component at a time
+//   k_icp_solve_pl      one thread: chol_solve<6>, t = t' - omega x m, det_sincos, PCL's constructTransformationMatrix in double
+//                       rounded once to float32, then k_icp_solve's F <- T F and convergence; a singular system stops the loop
+// The target's normals (prep_knn_normals) are computed once per call, or kept on a pipeline result.
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
@@ -24,6 +32,7 @@
 #include "ghicp_device.cuh"
 #include "ghicp_grid.cuh"
 #include "ghicp_ovwalk.cuh"
+#include "ghicp_solvers_math.h"
 
 namespace ghicp_b200 {
 namespace {
@@ -46,6 +55,7 @@ struct IcpDev {
   int n_rev;                         // reciprocal: distinct targets to query
 };
 struct IcpSum { double v[9]; unsigned long long n; };   // pass 1: s, q, sum d; pass 2: sum (q - mu_q)(s - mu_s)^T
+constexpr int IC_PL = 27;            // point-to-plane sums: the upper triangle of sum r r^T (row order), then sum r b
 
 __device__ __forceinline__ void icp_move(const float *m, float x, float y, float z, float *o) {
   o[0] = ((m[0] * x + m[1] * y) + m[2] * z) + m[3];
@@ -210,23 +220,75 @@ __global__ void __launch_bounds__(IC_RED_T) k_icp_total(const IcpSum *__restrict
   icp_tree(sh, v, out);
 }
 
-// one thread: T_k from the moments, F <- T_k F, and DefaultConvergenceCriteria with max_iterations_similar_transforms = 0
-__global__ void k_icp_solve(IcpDev *dev, const IcpSum *__restrict__ m1, const IcpSum *__restrict__ m2, int k, int max_it,
-                            double eps_t, double eps_f) {
+// point-to-plane pass 2: the 27 sums of the kept pairs' centred rows (m = the kept source mean of pass 1), the same point
+// blocks and per-thread order as k_icp_sum; each of the 27 components then goes through k_icp_sum's halving tree in turn
+// (one 2 KB shared array instead of 55 KB for all of them at once; tests/harness/icp_oracle.cpp restates it)
+__device__ void icp_tree_pl(double *sh, const double (&v)[IC_PL], double *out) {
+#pragma unroll
+  for (int c = 0; c < IC_PL; ++c) {
+    sh[threadIdx.x] = v[c];
+    __syncthreads();
+    for (int w = IC_RED_T / 2; w > 0; w >>= 1) {
+      if ((int)threadIdx.x < w) sh[threadIdx.x] += sh[threadIdx.x + w];
+      __syncthreads();
+    }
+    if (threadIdx.x == 0) out[c] = sh[0];
+    __syncthreads();
+  }
+}
+__global__ void __launch_bounds__(IC_RED_T) k_icp_sum_pl(const float *__restrict__ W, const float *__restrict__ Q,
+                                                         const float *__restrict__ N, const int *__restrict__ corr, long long n,
+                                                         const IcpSum *__restrict__ m1, double *__restrict__ part) {
+  __shared__ double sh[IC_RED_T];
+  const long long p0 = (long long)blockIdx.x * IC_RED_CHUNK, p1 = min(p0 + IC_RED_CHUNK, n);
+  double v[IC_PL];
+#pragma unroll
+  for (int c = 0; c < IC_PL; ++c) v[c] = 0.0;
+  double m[3];
+  for (int k = 0; k < 3; ++k) m[k] = m1->v[k] / (double)m1->n;
+  for (long long p = p0 + threadIdx.x; p < p1; p += IC_RED_T) {
+    const int j = corr[p];
+    if (j < 0) continue;
+    const double s[3] = {(double)W[3 * p], (double)W[3 * p + 1], (double)W[3 * p + 2]};
+    const double q[3] = {(double)Q[3 * (size_t)j], (double)Q[3 * (size_t)j + 1], (double)Q[3 * (size_t)j + 2]};
+    const double nn[3] = {(double)N[3 * (size_t)j], (double)N[3 * (size_t)j + 1], (double)N[3 * (size_t)j + 2]};
+    const double u[3] = {s[0] - m[0], s[1] - m[1], s[2] - m[2]};
+    const double r[6] = {u[1] * nn[2] - u[2] * nn[1], u[2] * nn[0] - u[0] * nn[2], u[0] * nn[1] - u[1] * nn[0], nn[0], nn[1], nn[2]};
+    const double b = (nn[0] * (q[0] - s[0]) + nn[1] * (q[1] - s[1])) + nn[2] * (q[2] - s[2]);
+    int e = 0;
+#pragma unroll
+    for (int a = 0; a < 6; ++a)
+#pragma unroll
+      for (int c = a; c < 6; ++c) v[e++] += r[a] * r[c];
+#pragma unroll
+    for (int a = 0; a < 6; ++a) v[21 + a] += r[a] * b;
+  }
+  icp_tree_pl(sh, v, part + (size_t)IC_PL * blockIdx.x);
+}
+__global__ void __launch_bounds__(IC_RED_T) k_icp_total_pl(const double *__restrict__ part, int nb, double *__restrict__ out) {
+  __shared__ double sh[IC_RED_T];
+  double v[IC_PL];
+#pragma unroll
+  for (int c = 0; c < IC_PL; ++c) v[c] = 0.0;
+  for (int b = threadIdx.x; b < nb; b += IC_RED_T)
+#pragma unroll
+    for (int c = 0; c < IC_PL; ++c) v[c] += part[(size_t)IC_PL * b + c];
+  icp_tree_pl(sh, v, out);
+}
+
+// the start of every solve: this iteration's pairs and mean squared distance, T_k = the identity; returns the pair count
+__device__ unsigned long long icp_begin(IcpDev *dev, const IcpSum *__restrict__ m1) {
   IcpHead &h = dev->h;
   const unsigned long long c = m1->n;
   h.cor = (int)c;
   h.mse = c > 0 ? m1->v[6] / (double)c : (double)NAN;   // the distances found before T_k is applied, as PCL has it
   for (int i = 0; i < 16; ++i) dev->T[i] = (i % 5 == 0) ? 1.f : 0.f;
-  if (c < 3) { h.state = GHICP_ICP_NO_CORRESPONDENCES; return; }
-  float mu_s[3], mu_d[3], sigma[9];
-  for (int a = 0; a < 3; ++a) { mu_s[a] = (float)(m1->v[a] / (double)c); mu_d[a] = (float)(m1->v[3 + a] / (double)c); }
-  for (int a = 0; a < 9; ++a) sigma[a] = (float)(m2->v[a] / (double)c);
-  double Rt[16];
-  umeyama_from_moments_f32(mu_s, mu_d, sigma, Rt);
-  float T[16], F[16];
-  for (int r = 0; r < 4; ++r)
-    for (int cc = 0; cc < 4; ++cc) T[r * 4 + cc] = (float)Rt[cc * 4 + r];
+  return c;
+}
+// F <- T_k F, and DefaultConvergenceCriteria with max_iterations_similar_transforms = 0
+__device__ void icp_step(IcpDev *dev, const float (&T)[16], int k, int max_it, double eps_t, double eps_f) {
+  IcpHead &h = dev->h;
+  float F[16];
   for (int r = 0; r < 4; ++r)
     for (int cc = 0; cc < 4; ++cc)
       F[r * 4 + cc] = ((T[r * 4] * h.F[cc] + T[r * 4 + 1] * h.F[4 + cc]) + T[r * 4 + 2] * h.F[8 + cc]) + T[r * 4 + 3] * h.F[12 + cc];
@@ -241,23 +303,67 @@ __global__ void k_icp_solve(IcpDev *dev, const IcpSum *__restrict__ m1, const Ic
   dev->prev_mse = h.mse;
 }
 
+// one thread: T_k from the moments (the float32 Umeyama of the loop), then icp_step
+__global__ void k_icp_solve(IcpDev *dev, const IcpSum *__restrict__ m1, const IcpSum *__restrict__ m2, int k, int max_it,
+                            double eps_t, double eps_f) {
+  const unsigned long long c = icp_begin(dev, m1);
+  if (c < 3) { dev->h.state = GHICP_ICP_NO_CORRESPONDENCES; return; }
+  float mu_s[3], mu_d[3], sigma[9];
+  for (int a = 0; a < 3; ++a) { mu_s[a] = (float)(m1->v[a] / (double)c); mu_d[a] = (float)(m1->v[3 + a] / (double)c); }
+  for (int a = 0; a < 9; ++a) sigma[a] = (float)(m2->v[a] / (double)c);
+  double Rt[16];
+  umeyama_from_moments_f32(mu_s, mu_d, sigma, Rt);
+  float T[16];
+  for (int r = 0; r < 4; ++r)
+    for (int cc = 0; cc < 4; ++cc) T[r * 4 + cc] = (float)Rt[cc * 4 + r];
+  icp_step(dev, T, k, max_it, eps_t, eps_f);
+}
+
+// one thread: T_k from the point-to-plane sums, then icp_step.  The normal equations are centred on the kept source mean m
+// (x = (alpha, beta, gamma, t')), PCL's translation is t = t' - omega x m; a system chol_solve<6> refuses, or angles beyond
+// det_sincos's range, stop the loop (GHICP_ICP_SINGULAR) with F unchanged
+__global__ void k_icp_solve_pl(IcpDev *dev, const IcpSum *__restrict__ m1, const double *__restrict__ acc, int k, int max_it,
+                               double eps_t, double eps_f) {
+  const unsigned long long c = icp_begin(dev, m1);
+  if (c < 3) { dev->h.state = GHICP_ICP_NO_CORRESPONDENCES; return; }
+  double A[6][6], b[6], x[6] = {0, 0, 0, 0, 0, 0};
+  int e = 0;
+  for (int i = 0; i < 6; ++i)
+    for (int j = i; j < 6; ++j) { A[i][j] = acc[e]; A[j][i] = acc[e]; ++e; }
+  for (int i = 0; i < 6; ++i) b[i] = acc[21 + i];
+  const double m[3] = {m1->v[0] / (double)c, m1->v[1] / (double)c, m1->v[2] / (double)c};
+  bool ok = chol_solve<6>(A, b, x);
+  const double al = x[0], be = x[1], ga = x[2];
+  const double t[3] = {x[3] - (be * m[2] - ga * m[1]), x[4] - (ga * m[0] - al * m[2]), x[5] - (al * m[1] - be * m[0])};
+  for (int i = 0; i < 3; ++i) ok = ok && fabs(x[i]) <= 1048576.0 && fabs(t[i]) <= DBL_MAX;   // false for NaN
+  if (!ok) { dev->h.state = GHICP_ICP_SINGULAR; return; }
+  double sa, ca, sb, cb, sg, cg;
+  det_sincos(al, sa, ca); det_sincos(be, sb, cb); det_sincos(ga, sg, cg);
+  const float T[16] = {(float)(cg * cb), (float)((-sg) * ca + (cg * sb) * sa), (float)(sg * sa + (cg * sb) * ca), (float)t[0],
+                       (float)(sg * cb), (float)(cg * ca + (sg * sb) * sa), (float)((-cg) * sa + (sg * sb) * ca), (float)t[1],
+                       (float)(-sb), (float)(cb * sa), (float)(cb * ca), (float)t[2],
+                       0.f, 0.f, 0.f, 1.f};
+  icp_step(dev, T, k, max_it, eps_t, eps_f);
+}
+
 inline int iblk(long long n, int t) { return (int)((n + t - 1) / t); }
 
 }  // namespace
 
 cudaError_t icp_run(const float *d_src, int n_src, const float *d_all, int n_all, const OverlapTarget *t, const float *d_tgt,
-                    const double *guess, const ghicp_icp_params *p, cudaEvent_t ev_iter, cudaEvent_t ev_fit, ghicp_icp_result *out,
-                    float *h_moved, int *h_cor, double *h_mse) {
+                    const float *d_nrm, const double *guess, const ghicp_icp_params *p, cudaEvent_t ev_iter, cudaEvent_t ev_fit,
+                    ghicp_icp_result *out, float *h_moved, int *h_cor, double *h_mse) {
   const long long n = n_src, nt = t->n;
-  const bool recip = p->reciprocal != 0, trim = p->trim_ratio > 0.f;
+  const bool recip = p->reciprocal != 0, trim = p->trim_ratio > 0.f, plane = p->metric == 1;
   const int nb = iblk(n, IC_RED_CHUNK);
   DevBuf<float> W, d2, moved; DevBuf<int> corr, perm, rev, list; DevBuf<pu64> keys; DevBuf<unsigned char> flag;
-  DevBuf<IcpDev> dev; DevBuf<IcpSum> part, tot;
+  DevBuf<IcpDev> dev; DevBuf<IcpSum> part, tot; DevBuf<double> part_pl, tot_pl;
   // every workspace of the loop first: running out of memory returns before anything is written (the reciprocal option's
   // grid over W is the exception: prep_point_grid allocates it every iteration, from the same pool)
   CUDA_TRY(W.alloc(3 * (size_t)n)); CUDA_TRY(d2.alloc((size_t)n)); CUDA_TRY(corr.alloc((size_t)n));
   CUDA_TRY(perm.alloc((size_t)n)); CUDA_TRY(keys.alloc((size_t)n));
   CUDA_TRY(dev.alloc(1)); CUDA_TRY(part.alloc((size_t)nb)); CUDA_TRY(tot.alloc(2));
+  if (plane) { CUDA_TRY(part_pl.alloc((size_t)IC_PL * nb)); CUDA_TRY(tot_pl.alloc(IC_PL)); }
   if (recip) { CUDA_TRY(rev.alloc((size_t)nt)); CUDA_TRY(list.alloc((size_t)nt)); CUDA_TRY(flag.alloc((size_t)nt)); }
   if (h_moved) CUDA_TRY(moved.alloc(3 * (size_t)n_all));
   IcpDev h0{};
@@ -295,10 +401,17 @@ cudaError_t icp_run(const float *d_src, int n_src, const float *d_all, int n_all
     }
     GHICP_LAUNCH(k_icp_sum<1>, nb, IC_RED_T, 0, 0, W.get(), d_tgt, corr.get(), d2.get(), n, nullptr, part.get());
     GHICP_LAUNCH(k_icp_total, 1, IC_RED_T, 0, 0, part.get(), nb, tot.get());
-    GHICP_LAUNCH(k_icp_sum<2>, nb, IC_RED_T, 0, 0, W.get(), d_tgt, corr.get(), d2.get(), n, tot.get(), part.get());
-    GHICP_LAUNCH(k_icp_total, 1, IC_RED_T, 0, 0, part.get(), nb, tot.get() + 1);
-    GHICP_LAUNCH(k_icp_solve, 1, 1, 0, 0, D, tot.get(), tot.get() + 1, k, p->max_iterations, p->transformation_epsilon,
-                 p->fitness_epsilon);
+    if (plane) {
+      GHICP_LAUNCH(k_icp_sum_pl, nb, IC_RED_T, 0, 0, W.get(), d_tgt, d_nrm, corr.get(), n, tot.get(), part_pl.get());
+      GHICP_LAUNCH(k_icp_total_pl, 1, IC_RED_T, 0, 0, part_pl.get(), nb, tot_pl.get());
+      GHICP_LAUNCH(k_icp_solve_pl, 1, 1, 0, 0, D, tot.get(), tot_pl.get(), k, p->max_iterations, p->transformation_epsilon,
+                   p->fitness_epsilon);
+    } else {
+      GHICP_LAUNCH(k_icp_sum<2>, nb, IC_RED_T, 0, 0, W.get(), d_tgt, corr.get(), d2.get(), n, tot.get(), part.get());
+      GHICP_LAUNCH(k_icp_total, 1, IC_RED_T, 0, 0, part.get(), nb, tot.get() + 1);
+      GHICP_LAUNCH(k_icp_solve, 1, 1, 0, 0, D, tot.get(), tot.get() + 1, k, p->max_iterations, p->transformation_epsilon,
+                   p->fitness_epsilon);
+    }
     GHICP_LAUNCH(k_icp_move, iblk(n, IC_T), IC_T, 0, 0, W.get(), W.get(), n, D->T);
     CUDA_TRY(cudaGetLastError());
     // the one read-back of an iteration
@@ -327,7 +440,7 @@ cudaError_t icp_run(const float *d_src, int n_src, const float *d_all, int n_all
   r.fitness = ov.fitness;
   r.iterations = k;
   r.state = hh.state;
-  r.converged = hh.state != GHICP_ICP_NO_CORRESPONDENCES;
+  r.converged = hh.state != GHICP_ICP_NO_CORRESPONDENCES && hh.state != GHICP_ICP_SINGULAR;
   r.cor = hh.cor;
   r.cells_visited = (long long)hh.work[0];
   r.candidates = (long long)hh.work[1];

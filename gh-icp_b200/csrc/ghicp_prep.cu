@@ -1318,6 +1318,43 @@ cudaError_t prep_sort_pairs(cudaStream_t st, pu64 *keys, int *vals, int n) { ret
 // every point's normal, d_status [n] (may be null) 1 where fewer than 3 neighbours exist, d_nb_idx / d_nb_d2 [n][min(k, n)]
 // (may be null) the k-NN lists.  ev_mid (may be null) is recorded between the k-NN + normals and the SPFH + FPFH stages.
 // cell_scale multiplies the data-derived cell edge (test hook).
+namespace {
+// The k-NN stage of the FPFH estimator: the grid, the k_eff-NN lists of every point (nb_idx / nb_d2 [n][ke]) and their work
+// counters (cand, fb), all allocated before the first launch; then k_knn and k_normals.
+cudaError_t knn_normals(cudaStream_t st, const float *d_xyz, int n, int ke, float cell_scale, PointGrid *pg, DevBuf<int> *nb_idx,
+                        DevBuf<float> *nb_d2, DevBuf<pu64> *cand, DevBuf<int> *fb, float *d_normals, int *d_status) {
+  CUDA_TRY(prep_point_grid(st, d_xyz, n, ke, cell_scale, 0.0, pg));
+  KnnArgs a{};
+  a.g = pg->g; a.n = n; a.k = ke;
+  a.gx = pg->gx; a.gy = pg->gy; a.gz = pg->gz;
+  a.cell = pg->cell; a.slack = pg->slack;
+  CUDA_TRY(nb_idx->alloc((size_t)n * ke)); CUDA_TRY(nb_d2->alloc((size_t)n * ke));
+  CUDA_TRY(cand->alloc(1)); CUDA_TRY(fb->alloc(1));
+  CUDA_TRY(cudaMemsetAsync(cand->get(), 0, sizeof(pu64), st)); CUDA_TRY(cudaMemsetAsync(fb->get(), 0, sizeof(int), st));
+  a.nb_idx = nb_idx->get(); a.nb_d2 = nb_d2->get(); a.cand = cand->get(); a.fallbacks = fb->get();
+  GHICP_LAUNCH(k_knn, blocks(n), PT, 0, st, a);
+  GHICP_LAUNCH(k_normals, blocks(n), PT, 0, st, d_xyz, nb_idx->get(), n, ke, d_normals, d_status);
+  return cudaSuccess;
+}
+
+// PrincipleComponentAnalysis::CheckNormals (include/pca.h:258-271): a non-finite normal becomes (0.577, 0.577, 0.577)
+__global__ void k_check_normals(float *__restrict__ nrm, int n) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  float *v = nrm + 3 * (size_t)i;
+  if (!(isfinite(v[0]) && isfinite(v[1]) && isfinite(v[2]))) { v[0] = 0.577f; v[1] = 0.577f; v[2] = 0.577f; }
+}
+}  // namespace
+
+cudaError_t prep_knn_normals(cudaStream_t st, const float *d_xyz, int n, int k, float *d_normals) {
+  PointGrid pg;
+  DevBuf<int> nb_idx, d_fb; DevBuf<float> nb_d2; DevBuf<pu64> d_cand;
+  if (n <= 0 || k < 3 || k > FPFH_KMAX) return cudaErrorInvalidValue;
+  CUDA_TRY(knn_normals(st, d_xyz, n, k < n ? k : n, 0.f, &pg, &nb_idx, &nb_d2, &d_cand, &d_fb, d_normals, nullptr));
+  GHICP_LAUNCH(k_check_normals, blocks(n), PT, 0, st, d_normals, n);
+  return cudaGetLastError();
+}
+
 cudaError_t prep_fpfh(cudaStream_t st, const float *d_xyz, int n, const int *d_idx, int nidx, int k, float cell_scale,
                       float *d_fpfh, float *d_normals, int *d_status, int *d_nb_idx, float *d_nb_d2, cudaEvent_t ev_mid,
                       FpfhStats *stats) {
@@ -1326,17 +1363,7 @@ cudaError_t prep_fpfh(cudaStream_t st, const float *d_xyz, int n, const int *d_i
   if (stats) *stats = FpfhStats{};
   if (n <= 0 || k < 3 || k > FPFH_KMAX) return cudaErrorInvalidValue;
   const int ke = k < n ? k : n;
-  CUDA_TRY(prep_point_grid(st, d_xyz, n, ke, cell_scale, 0.0, &pg));
-  KnnArgs a{};
-  a.g = pg.g; a.n = n; a.k = ke;
-  a.gx = pg.gx; a.gy = pg.gy; a.gz = pg.gz;
-  a.cell = pg.cell; a.slack = pg.slack;
-  CUDA_TRY(nb_idx.alloc((size_t)n * ke)); CUDA_TRY(nb_d2.alloc((size_t)n * ke));
-  CUDA_TRY(d_cand.alloc(1)); CUDA_TRY(d_fb.alloc(1));
-  CUDA_TRY(cudaMemsetAsync(d_cand.get(), 0, sizeof(pu64), st)); CUDA_TRY(cudaMemsetAsync(d_fb.get(), 0, sizeof(int), st));
-  a.nb_idx = nb_idx.get(); a.nb_d2 = nb_d2.get(); a.cand = d_cand.get(); a.fallbacks = d_fb.get();
-  GHICP_LAUNCH(k_knn, blocks(n), PT, 0, st, a);
-  GHICP_LAUNCH(k_normals, blocks(n), PT, 0, st, d_xyz, nb_idx.get(), n, ke, d_normals, d_status);
+  CUDA_TRY(knn_normals(st, d_xyz, n, ke, cell_scale, &pg, &nb_idx, &nb_d2, &d_cand, &d_fb, d_normals, d_status));
   if (d_nb_idx) CUDA_TRY(cudaMemcpyAsync(d_nb_idx, nb_idx.get(), sizeof(int) * (size_t)n * ke, cudaMemcpyDeviceToDevice, st));
   if (d_nb_d2) CUDA_TRY(cudaMemcpyAsync(d_nb_d2, nb_d2.get(), sizeof(float) * (size_t)n * ke, cudaMemcpyDeviceToDevice, st));
   if (ev_mid) CUDA_TRY(cudaEventRecord(ev_mid, st));

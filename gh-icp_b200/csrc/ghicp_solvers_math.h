@@ -69,6 +69,78 @@ GHICP_HD inline bool pt2pl_from_normal_equations(const double acc[27], double Rt
   return true;
 }
 
+// Deterministic double sine and cosine for |x| <= 2^20 (NaN beyond, and for a non-finite x): the same bits on the host and
+// the device, because they use only correctly rounded + - * / in a fixed order (build without FMA contraction: nvcc
+// --fmad=false, g++ -ffp-contract=off), where the device's and the C library's sin / cos may differ in the last bit.  The
+// dense point-to-plane ICP (DESIGN.md §3.14) builds its rotation with them.  Method: the classic fdlibm / musl argument
+// reduction by pi/2 in up to three rounds of a 33 + 33 + 33 + 53-bit split of pi/2, then their minimax kernels on
+// [-pi/4, pi/4]; within 1 ulp of a correctly rounded result over the range.
+namespace ghicp_sc {
+constexpr double INVPIO2 = 6.36619772367581382433e-01, TOINT = 6755399441055744.0;   // 2 / pi, 1.5 * 2^52
+constexpr double PIO2_1 = 1.57079632673412561417e+00, PIO2_1T = 6.07710050650619224932e-11;
+constexpr double PIO2_2 = 6.07710050630396597660e-11, PIO2_2T = 2.02226624879595063154e-21;
+constexpr double PIO2_3 = 2.02226624871116645580e-21, PIO2_3T = 8.47842766036889956997e-32;
+constexpr double S1 = -1.66666666666666324348e-01, S2 = 8.33333333332248946124e-03, S3 = -1.98412698298579493134e-04,
+                 S4 = 2.75573137070700676789e-06, S5 = -2.50507602534068634195e-08, S6 = 1.58969099521155010221e-10;
+constexpr double C1 = 4.16666666666666019037e-02, C2 = -1.38888888888741095749e-03, C3 = 2.48015872894767294178e-05,
+                 C4 = -2.75573143513906633035e-07, C5 = 2.08757232129817482790e-09, C6 = -1.13596475577881948265e-11;
+// sin(x + y) and cos(x + y) for |x + y| <= pi/4, |y| tiny against x
+GHICP_HD inline double ksin(double x, double y) {
+  const double z = x * x, w = z * z;
+  const double r = (S2 + z * (S3 + z * S4)) + (z * w) * (S5 + z * S6);
+  const double v = z * x;
+  return x - (((z * (0.5 * y - v * r)) - y) - v * S1);
+}
+GHICP_HD inline double kcos(double x, double y) {
+  const double z = x * x, w = z * z;
+  const double r = z * (C1 + z * (C2 + z * C3)) + (w * w) * (C4 + z * (C5 + z * C6));
+  const double hz = 0.5 * z, u = 1.0 - hz;
+  return u + (((1.0 - u) - hz) + (z * r - x * y));
+}
+// x = n pi/2 + (y0 + y1), |y0 + y1| <= pi/4 (about); returns n mod 4
+GHICP_HD inline int rem_pio2(double x, double &y0, double &y1) {
+  const double fn = (x * INVPIO2 + TOINT) - TOINT;   // x / (pi/2) rounded to the nearest integer
+  double r = x - fn * PIO2_1;                        // exact: fn * PIO2_1 has at most 53 bits for |fn| < 2^20
+  double w = fn * PIO2_1T;
+  y0 = r - w;
+  const double ax = x < 0.0 ? -x : x;
+  if ((y0 < 0.0 ? -y0 : y0) < ax * 0x1p-16) {        // cancellation: second round, good to 118 bits
+    double t = r;
+    w = fn * PIO2_2;
+    r = t - w;
+    w = fn * PIO2_2T - ((t - r) - w);
+    y0 = r - w;
+    if ((y0 < 0.0 ? -y0 : y0) < ax * 0x1p-49) {      // third round, 151 bits
+      t = r;
+      w = fn * PIO2_3;
+      r = t - w;
+      w = fn * PIO2_3T - ((t - r) - w);
+      y0 = r - w;
+    }
+  }
+  y1 = (r - y0) - w;
+  const double q = fn - 4.0 * (double)(long long)(fn * 0.25);   // fn mod 4 in -3 .. 3 (exact)
+  return ((int)q + 4) & 3;
+}
+}  // namespace ghicp_sc
+
+GHICP_HD inline void det_sincos(double x, double &s, double &c) {
+  using namespace ghicp_sc;
+  const double ax = x < 0.0 ? -x : x;
+  if (!(ax <= 1048576.0)) { s = c = (x - x) / (x - x); return; }   // NaN (also for +-inf and NaN)
+  if (ax < 0x1p-26) { s = x; c = 1.0; return; }                    // subnormals and tiny angles: exact to the last bit
+  double y0 = x, y1 = 0.0;
+  int n = 0;
+  if (ax > 0.78539816339744827900) n = rem_pio2(x, y0, y1);   // beyond pi/4
+  const double sn = ksin(y0, y1), cs = kcos(y0, y1);
+  switch (n) {
+    case 0: s = sn; c = cs; break;
+    case 1: s = cs; c = -sn; break;
+    case 2: s = -sn; c = -cs; break;
+    default: s = -cs; c = sn; break;
+  }
+}
+
 // CRegistration::LLS_4DOF (src/common_reg.cpp:623-775) from the 12 moments
 //   acc = { W, Sx, Sy, Sz, SX, SY, SZ, Q = sum w (x^2 + y^2), sum w xX, sum w yX, sum w xY, sum w yY }
 // (x, y, z source; X, Y, Z target).  Per Gauss-Newton step the reference's normal equations (:661-689) are

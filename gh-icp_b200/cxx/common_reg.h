@@ -12,12 +12,18 @@
 //   invTransform         (src/common_reg.cpp:358-370)  the reference's "not mathematically" inverse, kept as it is
 //   icp_reg              (src/common_reg.cpp:44-107)   PCL's point-to-point IterativeClosestPoint from the identity, with the
 //                                                      reciprocal and trimmed options, by ghicp_cloud_icp (DESIGN.md §3.13)
+//   ptplicp_reg          (src/common_reg.cpp:123-199)  PCL's IterativeClosestPointWithNormals (point-to-plane LLS) with the same
+//                                                      options against the target's k-NN normals, by ghicp_cloud_icp with
+//                                                      metric 1 (DESIGN.md §3.14); the source's normals take no part in PCL's
+//                                                      estimate and are not computed
 // Differences, deliberate: clouds are ghicp::Cloud (cloud_io.h) and fpfhFeaturePtr the stand-in of ghicp_types.h; the
 // transform is Eigen::Matrix4f when Eigen is on the include path, else the column-major ghicp::Matrix4f; the SAC-IA is the
 // deterministic one of DESIGN.md §3.11 instead of PCL's std::rand()-driven one; no CPU path (without a CUDA device both
 // members throw).  The fitness of the last Coarsereg_FPFHSAC or icp_reg, which the reference prints, is kept
-// (getFitnessScore).  icp_reg prints its lines to std::cout only (the reference also logs them through glog).
-// Not provided: the other PCL ICP wrappers (ptplicp_reg, gicp_reg), LLS_4DOF / SVD_6DOF and CSTRAN_4DOF / CSTRAN_7DOF.
+// (getFitnessScore).  icp_reg and ptplicp_reg print their lines to std::cout only (the reference also logs them through
+// glog).  ptplicp_reg writes TransformedSource and returns true, where the reference aligns into a local cloud (:141, :182)
+// and leaves the caller's untouched, and falls off the end of the function without a return value (:199).
+// Not provided: the other PCL ICP wrapper (gicp_reg), LLS_4DOF / SVD_6DOF and CSTRAN_4DOF / CSTRAN_7DOF.
 #pragma once
 #include <algorithm>
 #include <ctime>
@@ -89,10 +95,30 @@ class CRegistration {
   bool icp_reg(const Cloud &SourceCloud, const Cloud &TargetCloud, Cloud &TransformedSource, Matrix4f &transformationS2T,
                int max_iter, bool use_reciprocal_correspondence, bool use_trimmed_rejector, float thre_dis,
                float min_overlap_for_reg) {
+    return run_icp(SourceCloud, TargetCloud, TransformedSource, transformationS2T, max_iter, use_reciprocal_correspondence,
+                   use_trimmed_rejector, thre_dis, 0, 0, min_overlap_for_reg);
+  }
+
+  // :123-199 — point-to-plane ICP of SourceCloud onto TargetCloud from the identity against TargetCloud's k-NN normals
+  // (k = covariance_K, 3..32; transformation epsilon 1e-8, fitness epsilon 1e-5); the trimmed rejector as icp_reg.
+  bool ptplicp_reg(const Cloud &SourceCloud, const Cloud &TargetCloud, Cloud &TransformedSource, Matrix4f &transformationS2T,
+                   int max_iter, bool use_reciprocal_correspondence, bool use_trimmed_rejector, float thre_dis, int covariance_K,
+                   float min_overlap_for_reg) {
+    return run_icp(SourceCloud, TargetCloud, TransformedSource, transformationS2T, max_iter, use_reciprocal_correspondence,
+                   use_trimmed_rejector, thre_dis, 1, covariance_K, min_overlap_for_reg);
+  }
+
+ private:
+  // icp_reg (metric 0) and ptplicp_reg (metric 1, normal_k)
+  bool run_icp(const Cloud &SourceCloud, const Cloud &TargetCloud, Cloud &TransformedSource, Matrix4f &transformationS2T,
+               int max_iter, bool use_reciprocal_correspondence, bool use_trimmed_rejector, float thre_dis, int metric, int normal_k,
+               float min_overlap_for_reg) {
+    const char *who = metric == 1 ? "CRegistration::ptplicp_reg: " : "CRegistration::icp_reg: ";
     const clock_t t0 = clock();
     ghicp_icp_params p{};
     p.max_iterations = max_iter; p.reciprocal = use_reciprocal_correspondence ? 1 : 0;
-    p.transformation_epsilon = 1e-8; p.fitness_epsilon = 1e-5;   // :86, :88
+    p.transformation_epsilon = 1e-8; p.fitness_epsilon = 1e-5;   // :86, :88 (:166, :168)
+    p.metric = metric; p.normal_k = normal_k;
     if (use_trimmed_rejector) {
       const float overlap_ratio = calOverlap(SourceCloud, TargetCloud, thre_dis);
       if (overlap_ratio < min_overlap_for_reg) {
@@ -106,21 +132,24 @@ class CRegistration {
     ghicp_icp_result r{};
     if (ghicp_cloud_icp(0, SourceCloud.xyz.data(), n, TargetCloud.xyz.data(), (int)TargetCloud.size(), nullptr, &p, &r, moved.data(),
                         nullptr, nullptr) < 0)
-      throw std::runtime_error(std::string("CRegistration::icp_reg: ") + ghicp_last_error(nullptr));
+      throw std::runtime_error(std::string(who) + ghicp_last_error(nullptr));
     for (int i = 0; i < 16; ++i) transformationS2T.data()[i] = (float)r.Rt[i];
     TransformedSource.xyz = moved;
     fitness_ = r.fitness;
     icp_result_ = r;
     const clock_t t1 = clock();
-    std::cout << "Point-to-Point ICP done in " << float(t1 - t0) / CLOCKS_PER_SEC << " s" << std::endl;
+    std::cout << (metric == 1 ? "Point-to-Plane" : "Point-to-Point") << " ICP done in " << float(t1 - t0) / CLOCKS_PER_SEC << " s"
+              << std::endl;
     for (int i = 0; i < 4; ++i) {
       for (int j = 0; j < 4; ++j) std::cout << (j ? " " : "") << transformationS2T(i, j);
       std::cout << std::endl;
     }
     std::cout << "The fitness score of this registration is " << fitness_ << std::endl;
-    std::cout << "-----------------------------------------------------------------------------" << std::endl;
+    if (metric == 0) std::cout << "-----------------------------------------------------------------------------" << std::endl;
     return true;
   }
+
+ public:
 
   // :294-317 — (0.01 + #{points of Cloud1 with a Cloud2 point at d2 < thre_dis^2}) / |Cloud1|, as the reference's float
   float calOverlap(const Cloud &Cloud1, const Cloud &Cloud2, float thre_dis) {

@@ -39,6 +39,8 @@ transform, and returns the refined one; info["icp"] describes the refinement and
 With "trimmed_thre_dis" the trimmed rejector's ratio is calOverlap at that start pose, where the reference's icp_reg measures
 it on the unmoved source (it starts from the identity); with `evaluate`, info["evaluation"] scores the refined transform.
 The default None leaves the result and info as they were.  icp_reg(source, target, ...) is CRegistration::icp_reg itself.
+refine may also carry "metric": "plane" (default "point") and "covariance_k" (default 20): point-to-plane ICP against the
+target's k-NN normals (DESIGN.md §3.14); ptplicp_reg(source, target, ...) is CRegistration::ptplicp_reg itself.
 
 coarsereg_fpfh_sac(source_xyz, target_xyz, search_radius) is CRegistration::Coarsereg_FPFHSAC (src/common_reg.cpp:393-423):
 radius FPFH on every point of both clouds, then SAC-IA with correspondence randomness 15.
@@ -163,16 +165,22 @@ def _evaluate_kw(evaluate):
 def _refine_kw(refine):
     if refine is None:
         return None
-    if not isinstance(refine, dict) or "max_iter" not in refine or set(refine) - {"max_iter", "reciprocal", "trimmed_thre_dis"}:
-        raise capi.GhicpError(-1, "refine must be a dict {max_iter, reciprocal (optional), trimmed_thre_dis (optional)}")
+    keys = {"max_iter", "reciprocal", "trimmed_thre_dis", "metric", "covariance_k"}
+    if not isinstance(refine, dict) or "max_iter" not in refine or set(refine) - keys:
+        raise capi.GhicpError(-1, "refine must be a dict {max_iter, reciprocal (optional), trimmed_thre_dis (optional), "
+                                  "metric ('point' or 'plane', optional), covariance_k (optional)}")
+    metric = refine.get("metric", "point")
+    if metric not in capi.ICP_METRICS:
+        raise capi.GhicpError(-1, f"refine: metric must be 'point' or 'plane', not {metric!r}")
     return dict(max_iter=int(refine["max_iter"]), reciprocal=bool(refine.get("reciprocal", False)),
-                thre_dis=refine.get("trimmed_thre_dis"))
+                thre_dis=refine.get("trimmed_thre_dis"), metric=metric, normal_k=int(refine.get("covariance_k", 20)))
 
 
 def _refine(Rt, kw, info, ratio_at, icp_from):
     """ICP from Rt (icp_from(guess, **cloud_icp options)); the trimmed ratio is calOverlap at Rt (ratio_at(Rt, thre_dis))."""
     rho = 0.0 if kw["thre_dis"] is None else float(ratio_at(Rt, float(kw["thre_dis"])))
-    Rt_icp, icp_info = icp_from(Rt, max_iterations=kw["max_iter"], reciprocal=kw["reciprocal"], trim_ratio=min(rho, 1.0))
+    Rt_icp, icp_info = icp_from(Rt, max_iterations=kw["max_iter"], reciprocal=kw["reciprocal"], trim_ratio=min(rho, 1.0),
+                                metric=kw["metric"], normal_k=kw["normal_k"])
     info["icp"] = dict(icp_info, Rt_before=Rt, trim_ratio=rho)
     return Rt_icp
 
@@ -194,6 +202,29 @@ def icp_reg(source_xyz, target_xyz, max_iter, use_reciprocal_correspondence, use
     Rt, info = capi.cloud_icp(S, T, None, max_iterations=max_iter, reciprocal=use_reciprocal_correspondence,
                               trim_ratio=min(rho, 1.0), transformation_epsilon=1e-8, fitness_epsilon=1e-5, return_moved=True,
                               device=device)
+    if use_trimmed_rejector:
+        info["overlap_ratio"] = rho
+    return Rt, info
+
+
+def ptplicp_reg(source_xyz, target_xyz, max_iter, use_reciprocal_correspondence, use_trimmed_rejector, thre_dis, covariance_K,
+                min_overlap_for_reg=0.0, device=0):
+    """CRegistration::ptplicp_reg (src/common_reg.cpp:123-199) on the GPU: point-to-plane ICP of the source onto the target
+    from the identity against the target's k-NN normals (k = covariance_K, 3..32), transformation epsilon 1e-8 and fitness
+    epsilon 1e-5 (capi.cloud_icp with metric="plane", DESIGN.md §3.14).  The source's normals, which the reference also
+    computes, take no part in PCL's estimate and are not computed.  With use_trimmed_rejector the ratio is
+    calOverlap(source, target, thre_dis) of the unmoved source, and the call returns None below min_overlap_for_reg.  Returns
+    (Rt 4x4, info with the transformed source under "moved"; info["overlap_ratio"] when trimmed), as icp_reg."""
+    S = np.ascontiguousarray(source_xyz, dtype=np.float32).reshape(-1, 3)
+    T = np.ascontiguousarray(target_xyz, dtype=np.float32).reshape(-1, 3)
+    rho = 0.0
+    if use_trimmed_rejector:
+        rho = cal_overlap(S, T, thre_dis, device=device)
+        if rho < min_overlap_for_reg:
+            return None
+    Rt, info = capi.cloud_icp(S, T, None, max_iterations=max_iter, reciprocal=use_reciprocal_correspondence,
+                              trim_ratio=min(rho, 1.0), transformation_epsilon=1e-8, fitness_epsilon=1e-5, return_moved=True,
+                              device=device, metric="plane", normal_k=covariance_K)
     if use_trimmed_rejector:
         info["overlap_ratio"] = rho
     return Rt, info

@@ -55,7 +55,8 @@ enum ghicp_status {
   GHICP_E_NCCL = -4,   /* NCCL error / NCCL not loadable */
   GHICP_E_NOCONV = -5, /* ghicp_run hit max_iter without converging */
   GHICP_E_NODEV = -6,  /* no CUDA device: the product path has NO CPU fallback */
-  GHICP_W_FEW_PAIRS = 1 /* cor < min_cor (include/ghicp_reg.h:36, src/ghicp_reg.cpp:796-797) */
+  GHICP_W_FEW_PAIRS = 1, /* cor < min_cor (include/ghicp_reg.h:36, src/ghicp_reg.cpp:796-797) */
+  GHICP_W_SINGULAR = 2   /* point-to-plane ICP: the normal equations of an iteration were singular (GHICP_ICP_SINGULAR) */
 };
 
 /* Constructor arguments of ghicp::GHRegistration (include/ghicp_reg.h:77-81) + Energyfunction::init
@@ -355,13 +356,19 @@ int ghicp_prep_overlap(const ghicp_prep *a, const ghicp_prep *b, const double Rt
  * and then the floor(trim_ratio * pairs) closest ones, fits the float32 Umeyama of the loop to FP64 two-pass moments of the
  * kept pairs, and stops on the first of: max_iterations, a transform within transformation_epsilon of the identity, an
  * absolute (1e-12) or relative (fitness_epsilon) change of the pairs' mean squared distance, or fewer than 3 pairs.  Sums are
- * in double in a fixed order: two calls give identical bits.  Non-finite source and target points take no part. */
-enum ghicp_icp_state {   /* PCL's DefaultConvergenceCriteria::ConvergenceState values */
+ * in double in a fixed order: two calls give identical bits.  Non-finite source and target points take no part.
+ * Point-to-plane (metric = 1, DESIGN.md §3.14): CRegistration::ptplicp_reg (src/common_reg.cpp:123-199), PCL's
+ * IterativeClosestPointWithNormals with TransformationEstimationPointToPlaneLLS.  The same loop, but each step solves PCL's
+ * point-to-plane normal equations (centred on the kept source points' mean, FP64 fixed-order sums) against the target's k-NN
+ * normals (PCL NormalEstimation with k = normal_k, viewpoint 0, non-finite normals replaced by (0.577, 0.577, 0.577) as
+ * CheckNormals does).  A singular system stops the loop with GHICP_ICP_SINGULAR. */
+enum ghicp_icp_state {   /* PCL's DefaultConvergenceCriteria::ConvergenceState values, then SINGULAR */
   GHICP_ICP_ITERATIONS = 1,
   GHICP_ICP_TRANSFORM = 2,
   GHICP_ICP_ABS_MSE = 3,
   GHICP_ICP_REL_MSE = 4,
-  GHICP_ICP_NO_CORRESPONDENCES = 5
+  GHICP_ICP_NO_CORRESPONDENCES = 5,
+  GHICP_ICP_SINGULAR = 7           /* metric 1: 3 or more pairs but no solution (e.g. every normal parallel); F unchanged */
 };
 typedef struct ghicp_icp_params {
   int max_iterations;              /* >= 1 (icp_reg's max_iter) */
@@ -369,7 +376,9 @@ typedef struct ghicp_icp_params {
   float trim_ratio;                /* CorrespondenceRejectorTrimmed::setOverlapRatio, 0 = no rejector, else (0, 1] */
   double transformation_epsilon;   /* >= 0; icp_reg: 1e-8 */
   double fitness_epsilon;          /* >= 0; icp_reg: 1e-5 */
-  int reserved[4];
+  int metric;                      /* 0 = point-to-point (§3.13), 1 = point-to-plane (§3.14) */
+  int normal_k;                    /* metric 1: the target normals' k, 3..32 (ptplicp_reg's covariance_K); ignored by metric 0 */
+  int reserved[2];
 } ghicp_icp_params;
 typedef struct ghicp_icp_result {
   double Rt[16];                   /* column-major: the float32 accumulated transform widened (the guess when no step ran) */
@@ -377,19 +386,22 @@ typedef struct ghicp_icp_result {
   double fitness;                  /* PCL's getFitnessScore: §3.12 fitness of the source moved by Rt, max_range = +inf */
   int iterations, converged, state, cor;          /* state: ghicp_icp_state; cor: the last iteration's kept pairs */
   long long cells_visited, candidates;            /* work of every nearest-neighbour query of every iteration */
-  float stage_ms[4];                              /* target grid (0 when cached), iterations, fitness, total */
+  float stage_ms[4];                              /* target grid (+ normals for metric 1; 0 when cached), iterations, fitness,
+                                                     total */
 } ghicp_icp_result;
 /* src_xyz [n_s][3], tgt_xyz [n_t][3] (host arrays); guess column-major (NULL = identity), rounded once to float32; moved [n_s][3]
  * (may be NULL) receives the source moved by Rt (PCL's align output); cor_trace / mse_trace [max_iterations] (may be NULL)
  * receive each iteration's kept pairs and mean squared distance (entries past `iterations` are left as they are).  Fewer than
- * 3 pairs returns GHICP_W_FEW_PAIRS with the result filled in (converged = 0, Rt = the transform so far).  Argument errors
- * (NULL, n <= 0, no finite source or target point, max_iterations < 1, trim_ratio outside [0, 1] or NaN, a negative or NaN
- * epsilon, a non-finite guess, handles on different devices) return GHICP_E_ARG and write nothing; out of memory returns
- * GHICP_E_NOMEM and writes nothing. */
+ * 3 pairs returns GHICP_W_FEW_PAIRS, a singular point-to-plane system GHICP_W_SINGULAR, each with the result filled in
+ * (converged = 0, Rt = the transform so far).  Argument errors (NULL, n <= 0, no finite source or target point,
+ * max_iterations < 1, trim_ratio outside [0, 1] or NaN, a negative or NaN epsilon, a non-finite guess, a metric other than 0
+ * or 1, metric 1 with normal_k outside 3..32, handles on different devices) return GHICP_E_ARG and write nothing; out of
+ * memory returns GHICP_E_NOMEM and writes nothing. */
 int ghicp_cloud_icp(int device, const float *src_xyz, int n_s, const float *tgt_xyz, int n_t, const double guess[16],
                     const ghicp_icp_params *p, ghicp_icp_result *out, float *moved, int *cor_trace, double *mse_trace);
 /* the down-sampled clouds of two pipeline results, device to device; the target's grid is the one ghicp_prep_overlap keeps
- * (built by whichever call comes first, stage_ms[0] = 0 when it already exists) */
+ * (built by whichever call comes first, stage_ms[0] = 0 when it already exists).  Metric 1 also keeps the target's normals
+ * and their k there, under the same lock: a later call with the same normal_k reuses them, another k replaces them. */
 int ghicp_prep_icp(const ghicp_prep *source, const ghicp_prep *target, const double guess[16], const ghicp_icp_params *p,
                    ghicp_icp_result *out);
 
