@@ -20,5 +20,5 @@ from . import synth  # noqa: F401
 from . import capi  # noqa: F401
 from . import pipeline  # noqa: F401
 from .pipeline import (  # noqa: F401
-    register_clouds, transform_cloud, coarsereg_fpfh_sac, cal_overlap, evaluate_registration, icp_reg, ptplicp_reg,
+    register_clouds, transform_cloud, coarsereg_fpfh_sac, cal_overlap, evaluate_registration, icp_reg, ptplicp_reg, gicp_reg,
 )

@@ -15,7 +15,7 @@ FT_BSC, FT_ROPS, FT_FPFH, FT_NONE = 0, 1, 2, 3   # include/utility.h:51-57
 CT_NN, CT_NNR, CT_KM = 0, 1, 2                   # include/utility.h:59-64
 
 GHICP_W_FEW_PAIRS = 1
-GHICP_W_SINGULAR = 2   # point-to-plane ICP: a singular system stopped the loop
+GHICP_W_SINGULAR = 2   # point-to-plane ICP or GICP: a singular system stopped the loop
 # ghicp_solver_type (include/ghicp_b200.h): SVD is the reference's estimator, the others are opt-in extensions
 SOLVER_SVD, SOLVER_WEIGHTED_SVD, SOLVER_POINT_TO_PLANE, SOLVER_YAW_4DOF = 0, 1, 2, 3
 
@@ -197,11 +197,11 @@ def _overlap_out(r):
 
 
 class IcpParams(C.Structure):
-    """ghicp_icp_params (include/ghicp_b200.h): point-to-point (metric 0, DESIGN.md §3.13) or point-to-plane (metric 1, §3.14)
-    ICP."""
+    """ghicp_icp_params (include/ghicp_b200.h): point-to-point (metric 0, DESIGN.md §3.13), point-to-plane (metric 1, §3.14)
+    or Generalized (metric 2, §3.15) ICP."""
     _fields_ = [("max_iterations", C.c_int), ("reciprocal", C.c_int), ("trim_ratio", C.c_float),
                 ("transformation_epsilon", C.c_double), ("fitness_epsilon", C.c_double), ("metric", C.c_int), ("normal_k", C.c_int),
-                ("reserved", C.c_int * 2)]
+                ("rotation_epsilon", C.c_double)]
 
 
 class IcpResult(C.Structure):
@@ -211,14 +211,15 @@ class IcpResult(C.Structure):
 
 
 ICP_STATES = {1: "ITERATIONS", 2: "TRANSFORM", 3: "ABS_MSE", 4: "REL_MSE", 5: "NO_CORRESPONDENCES", 7: "SINGULAR"}   # ghicp_icp_state
-ICP_METRICS = {"point": 0, "plane": 1}   # ghicp_icp_params.metric
+ICP_METRICS = {"point": 0, "plane": 1, "gicp": 2}   # ghicp_icp_params.metric
 
 
-def _icp_params(max_iterations, reciprocal, trim_ratio, transformation_epsilon, fitness_epsilon, metric="point", normal_k=20):
+def _icp_params(max_iterations, reciprocal, trim_ratio, transformation_epsilon, fitness_epsilon, metric="point", normal_k=20,
+                rotation_epsilon=1e-6):
     if metric not in ICP_METRICS:
-        raise GhicpError(-1, f"icp: metric must be 'point' or 'plane', not {metric!r}")
+        raise GhicpError(-1, f"icp: metric must be 'point', 'plane' or 'gicp', not {metric!r}")
     return IcpParams(int(max_iterations), int(bool(reciprocal)), float(trim_ratio), float(transformation_epsilon),
-                     float(fitness_epsilon), ICP_METRICS[metric], int(normal_k))
+                     float(fitness_epsilon), ICP_METRICS[metric], int(normal_k), float(rotation_epsilon))
 
 
 def _icp_out(r, rc):
@@ -335,16 +336,17 @@ class Prep:
         return _overlap_out(r)
 
     def icp(self, target, guess=None, max_iterations=50, reciprocal=False, trim_ratio=0.0, transformation_epsilon=1e-8,
-            fitness_epsilon=1e-5, metric="point", normal_k=20):
+            fitness_epsilon=1e-5, metric="point", normal_k=20, rotation_epsilon=1e-6):
         """cloud_icp of this down-sampled cloud onto `target`'s, device to device (ghicp_prep_icp).  The target's grid is the one
         overlap() keeps (its stage_ms["grid"] is 0 once either has built it); with metric="plane" the target also keeps its
-        normals for that normal_k (stage_ms["grid"] is 0 again on a second call with the same k).  Returns (Rt, info) as
+        normals for that normal_k (stage_ms["grid"] is 0 again on a second call with the same k), with metric="gicp" both
+        results keep theirs (one set per result, shared by the metrics and by either role).  Returns (Rt, info) as
         cloud_icp."""
         keep, gp = _overlap_rt(guess)
         r = IcpResult()
         rc = check(lib().ghicp_prep_icp(self.h, target.h, gp, C.byref(_icp_params(max_iterations, reciprocal, trim_ratio,
                                                                                    transformation_epsilon, fitness_epsilon, metric,
-                                                                                   normal_k)),
+                                                                                   normal_k, rotation_epsilon)),
                                         C.byref(r)))
         del keep
         return _icp_out(r, rc)
@@ -570,15 +572,19 @@ def cloud_overlap(A, B, Rt=None, thre_dis=None, max_range=float("inf"), fitness=
 
 
 def cloud_icp(S, T, guess=None, max_iterations=50, reciprocal=False, trim_ratio=0.0, transformation_epsilon=1e-8,
-              fitness_epsilon=1e-5, return_moved=False, trace=False, device=0, metric="point", normal_k=20):
+              fitness_epsilon=1e-5, return_moved=False, trace=False, device=0, metric="point", normal_k=20, rotation_epsilon=1e-6):
     """Point-to-point ICP of source S onto target T on the GPU, DESIGN.md §3.13: PCL's IterativeClosestPoint as
     CRegistration::icp_reg configures it (src/common_reg.cpp:44-107), starting from `guess` (4x4, None = identity).
     reciprocal = setUseReciprocalCorrespondences; trim_ratio > 0 adds CorrespondenceRejectorTrimmed with that overlap ratio.
     metric="plane" estimates each step point-to-plane against T's k-NN normals (k = normal_k, 3..32), DESIGN.md §3.14: PCL's
     IterativeClosestPointWithNormals as CRegistration::ptplicp_reg configures it (src/common_reg.cpp:123-199).
+    metric="gicp" runs Generalized ICP, DESIGN.md §3.15: PCL's GeneralizedIterativeClosestPoint as CRegistration::gicp_reg
+    configures it (src/common_reg.cpp:217-284), with both clouds' k-NN normals as covariances, a Gauss-Newton inner loop, and
+    PCL's GICP stop (max_iterations, or no transform entry moved by more than rotation_epsilon / transformation_epsilon);
+    fitness_epsilon is not read, and reciprocal / trim_ratio apply as for the other metrics.
     Returns (Rt 4x4 mapping S onto T, info: iterations, converged, state (ITERATIONS, TRANSFORM, ABS_MSE, REL_MSE,
-    NO_CORRESPONDENCES or, point-to-plane only, SINGULAR), cor and mse of the last iteration, fitness = PCL's getFitnessScore,
-    warnings (GHICP_W_FEW_PAIRS when fewer than 3 pairs were left, GHICP_W_SINGULAR for a singular point-to-plane system),
+    NO_CORRESPONDENCES or, point-to-plane and GICP only, SINGULAR), cor and mse of the last iteration, fitness = PCL's
+    getFitnessScore, warnings (GHICP_W_FEW_PAIRS when fewer than 3 pairs were left, GHICP_W_SINGULAR for a singular system),
     work counters, stage_ms); + "moved" (S moved by Rt) with return_moved, + "cor_trace" / "mse_trace" per iteration with
     trace."""
     fpp = C.POINTER(C.c_float)
@@ -591,7 +597,7 @@ def cloud_icp(S, T, guess=None, max_iterations=50, reciprocal=False, trim_ratio=
     r = IcpResult()
     rc = check(lib().ghicp_cloud_icp(device, S.ctypes.data_as(fpp), len(S), T.ctypes.data_as(fpp), len(T), gp,
                                      C.byref(_icp_params(max_iterations, reciprocal, trim_ratio, transformation_epsilon,
-                                                         fitness_epsilon, metric, normal_k)), C.byref(r),
+                                                         fitness_epsilon, metric, normal_k, rotation_epsilon)), C.byref(r),
                                      None if moved is None else moved.ctypes.data_as(fpp), None if cor_tr is None else _ip(cor_tr),
                                      None if mse_tr is None else _dp(mse_tr)))
     del keep

@@ -5,7 +5,9 @@
 // the host from one small read-back per iteration.  There is NO CPU fallback: without a CUDA device
 // every entry point fails with GHICP_E_NODEV.
 #include <algorithm>
+#include <cfloat>
 #include <cmath>
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -1274,9 +1276,9 @@ struct ghicp_prep {
   float stage_ms[5] = {0, 0, 0, 0, 0};
   FpfhStats fpfh_stats;
   OverlapTarget *ov_target = nullptr;   // the down-sampled cloud's grid as an overlap target, after ghicp_prep_overlap
-  DevBuf<float> icp_nrm;                // [n_down][3] k-NN normals of point-to-plane ICP, after ghicp_prep_icp with metric 1
+  DevBuf<float> icp_nrm;                // [n_down][3] k-NN normals, after ghicp_prep_icp with metric 1 (target) or 2 (either)
   int icp_nrm_k = 0;                    // their k (0: none)
-  std::mutex ov_mu;                     // guards ov_target and the normals: concurrent first calls on one target build once
+  std::mutex ov_mu;                     // guards ov_target and the normals: concurrent first calls on one result build once
 };
 
 int ghicp_prep_destroy(ghicp_prep *h) {
@@ -1715,7 +1717,9 @@ int ghicp_prep_overlap(const ghicp_prep *a, const ghicp_prep *b, const double Rt
   return cuda_status(prep_overlap_run(a, tb, Rt, thre_dis, max_range, want_fitness, out), "prep_overlap");
 }
 
-// ---- point-to-point and point-to-plane ICP on the dense clouds -------------------------------------------------------------
+// ---- point-to-point, point-to-plane and Generalized ICP on the dense clouds ------------------------------------------------
+static_assert(offsetof(ghicp_icp_params, rotation_epsilon) == 40 && sizeof(ghicp_icp_params) == 48,
+              "ghicp_icp_params: rotation_epsilon took the place of reserved[2]; the layout must not move");
 static bool icp_params_ok(const ghicp_icp_params *p, const double *guess, const char *who) {
   const bool ok = p && p->max_iterations >= 1 && p->trim_ratio >= 0.f && p->trim_ratio <= 1.f &&   // false for NaN
                   p->transformation_epsilon >= 0.0 && p->fitness_epsilon >= 0.0;
@@ -1723,8 +1727,11 @@ static bool icp_params_ok(const ghicp_icp_params *p, const double *guess, const 
     set_error(nullptr, std::string(who) + ": max_iterations must be >= 1, trim_ratio in [0, 1], the epsilons >= 0");
     return false;
   }
-  if (p->metric != 0 && !(p->metric == 1 && p->normal_k >= 3 && p->normal_k <= 32)) {
-    set_error(nullptr, std::string(who) + ": metric must be 0 (point-to-point) or 1 (point-to-plane, with normal_k in 3..32)");
+  const bool k_ok = p->normal_k >= 3 && p->normal_k <= 32;
+  if (p->metric != 0 && !(p->metric == 1 && k_ok) &&
+      !(p->metric == 2 && k_ok && p->rotation_epsilon > 0.0 && p->rotation_epsilon <= DBL_MAX)) {   // false for NaN
+    set_error(nullptr, std::string(who) + ": metric must be 0 (point-to-point), 1 (point-to-plane, with normal_k in 3..32) or 2 "
+                                          "(GICP, with normal_k in 3..32 and a finite rotation_epsilon > 0)");
     return false;
   }
   return overlap_rt_ok(guess, who);
@@ -1739,12 +1746,13 @@ static cudaError_t cloud_icp_run(const float *src, int n_s, const float *src_fin
                                  const double *guess, const ghicp_icp_params *p, ghicp_icp_result *out, float *moved, int *cor_trace,
                                  double *mse_trace) {
   StageEvents<4> ev;
-  DevBuf<float> d_all, d_fin, d_t, d_nrm;
+  DevBuf<float> d_all, d_fin, d_t, d_nrm, d_nrm_s;
   ghicp_icp_result r{};
   CUDA_TRY(ev.create());
   CUDA_TRY(d_all.alloc(3 * (size_t)n_s)); CUDA_TRY(d_t.alloc(3 * (size_t)n_t));
   if (src_fin != src) CUDA_TRY(d_fin.alloc(3 * (size_t)ns_fin));
-  if (p->metric == 1) CUDA_TRY(d_nrm.alloc(3 * (size_t)n_t));
+  if (p->metric != 0) CUDA_TRY(d_nrm.alloc(3 * (size_t)n_t));
+  if (p->metric == 2) CUDA_TRY(d_nrm_s.alloc(3 * (size_t)ns_fin));
   CUDA_TRY(cudaMemcpyAsync(d_all.get(), src, 3 * (size_t)n_s * sizeof(float), cudaMemcpyHostToDevice, 0));
   if (src_fin != src) CUDA_TRY(cudaMemcpyAsync(d_fin.get(), src_fin, 3 * (size_t)ns_fin * sizeof(float), cudaMemcpyHostToDevice, 0));
   CUDA_TRY(cudaMemcpyAsync(d_t.get(), tgt, 3 * (size_t)n_t * sizeof(float), cudaMemcpyHostToDevice, 0));
@@ -1753,10 +1761,12 @@ static cudaError_t cloud_icp_run(const float *src, int n_s, const float *src_fin
   CUDA_TRY(overlap_target_build(d_t.get(), n_t, &t));
   std::vector<int> cor(cor_trace ? p->max_iterations : 0);
   std::vector<double> mse(mse_trace ? p->max_iterations : 0);
-  cudaError_t e = p->metric == 1 ? prep_knn_normals(0, d_t.get(), n_t, p->normal_k, d_nrm.get()) : cudaSuccess;
+  const float *d_src = src_fin != src ? d_fin.get() : d_all.get();
+  cudaError_t e = p->metric != 0 ? prep_knn_normals(0, d_t.get(), n_t, p->normal_k, d_nrm.get()) : cudaSuccess;
+  if (e == cudaSuccess && p->metric == 2) e = prep_knn_normals(0, d_src, ns_fin, p->normal_k, d_nrm_s.get());
   if (e == cudaSuccess)
-    e = icp_run(src_fin != src ? d_fin.get() : d_all.get(), ns_fin, d_all.get(), n_s, t, d_t.get(), d_nrm.get(), guess, p, ev[1],
-                ev[2], &r, moved, cor_trace ? cor.data() : nullptr, mse_trace ? mse.data() : nullptr);
+    e = icp_run(d_src, ns_fin, d_all.get(), n_s, t, d_t.get(), d_nrm.get(), d_nrm_s.get(), guess, p, ev[1], ev[2], &r, moved,
+                cor_trace ? cor.data() : nullptr, mse_trace ? mse.data() : nullptr);
   overlap_target_free(t);
   CUDA_TRY(e);
   CUDA_TRY(cudaEventRecord(ev[3], 0));
@@ -1787,26 +1797,47 @@ int ghicp_cloud_icp(int device, const float *src_xyz, int n_s, const float *tgt_
   return icp_warnings(out);
 }
 
-static cudaError_t prep_icp_run(const ghicp_prep *s, ghicp_prep *tb, const double *guess, const ghicp_icp_params *p,
+// a pipeline result's k-NN normals for k, kept on it (the caller holds its ov_mu); *built = false when they were already
+// there.  New normals go into a fresh buffer: the cache changes only once they exist.
+static cudaError_t prep_icp_normals(ghicp_prep *h, int k, bool *built) {
+  *built = h->icp_nrm_k != k;
+  if (!*built) return cudaSuccess;
+  DevBuf<float> nrm;
+  CUDA_TRY(nrm.alloc(3 * (size_t)h->n_down));
+  CUDA_TRY(prep_knn_normals(0, h->d_down.get(), h->n_down, k, nrm.get()));
+  h->icp_nrm = std::move(nrm);
+  h->icp_nrm_k = k;
+  return cudaSuccess;
+}
+
+// the caches and the loop, under the locks prep_icp_run holds; *cached: the grid and every normal needed were there
+static cudaError_t prep_icp_locked(ghicp_prep *sb, ghicp_prep *tb, const double *guess, const ghicp_icp_params *p,
+                                   StageEvents<4> &ev, ghicp_icp_result *r, bool *cached) {
+  bool built = false;
+  *cached = tb->ov_target != nullptr;
+  if (!*cached) CUDA_TRY(overlap_target_build(tb->d_down.get(), tb->n_down, &tb->ov_target));
+  if (p->metric != 0) { CUDA_TRY(prep_icp_normals(tb, p->normal_k, &built)); *cached = *cached && !built; }
+  if (p->metric == 2) { CUDA_TRY(prep_icp_normals(sb, p->normal_k, &built)); *cached = *cached && !built; }
+  return icp_run(sb->d_down.get(), sb->n_down, sb->d_down.get(), sb->n_down, tb->ov_target, tb->d_down.get(), tb->icp_nrm.get(),
+                 sb->icp_nrm.get(), guess, p, ev[1], ev[2], r, nullptr, nullptr, nullptr);
+}
+
+static cudaError_t prep_icp_run(ghicp_prep *sb, ghicp_prep *tb, const double *guess, const ghicp_icp_params *p,
                                 ghicp_icp_result *out) {
   StageEvents<4> ev;
   ghicp_icp_result r{};
   CUDA_TRY(ev.create());
   CUDA_TRY(cudaEventRecord(ev[0], 0));
-  std::lock_guard<std::mutex> lk(tb->ov_mu);   // the grid ghicp_prep_overlap keeps, and the normals, under its lock
-  bool cached = tb->ov_target != nullptr;
-  if (!cached) CUDA_TRY(overlap_target_build(tb->d_down.get(), tb->n_down, &tb->ov_target));
-  if (p->metric == 1 && tb->icp_nrm_k != p->normal_k) {
-    // into a fresh buffer: the cache changes only once the new normals exist
-    DevBuf<float> nrm;
-    CUDA_TRY(nrm.alloc(3 * (size_t)tb->n_down));
-    CUDA_TRY(prep_knn_normals(0, tb->d_down.get(), tb->n_down, p->normal_k, nrm.get()));
-    tb->icp_nrm = std::move(nrm);
-    tb->icp_nrm_k = p->normal_k;
-    cached = false;
+  // the grid ghicp_prep_overlap keeps, and the normals, under the target's lock; GICP also keeps the source's normals, under
+  // both locks taken together (std::scoped_lock avoids the deadlock of (a, b) and (b, a) at once; one lock when a == b)
+  bool cached = false;
+  if (p->metric == 2 && sb != tb) {
+    std::scoped_lock lk(tb->ov_mu, sb->ov_mu);
+    CUDA_TRY(prep_icp_locked(sb, tb, guess, p, ev, &r, &cached));
+  } else {
+    std::scoped_lock lk(tb->ov_mu);
+    CUDA_TRY(prep_icp_locked(sb, tb, guess, p, ev, &r, &cached));
   }
-  CUDA_TRY(icp_run(s->d_down.get(), s->n_down, s->d_down.get(), s->n_down, tb->ov_target, tb->d_down.get(), tb->icp_nrm.get(), guess,
-                   p, ev[1], ev[2], &r, nullptr, nullptr, nullptr));
   CUDA_TRY(cudaEventRecord(ev[3], 0));
   CUDA_TRY(cudaStreamSynchronize(0));
   if (!cached) r.stage_ms[0] = ev.ms(0, 1);
@@ -1823,8 +1854,9 @@ int ghicp_prep_icp(const ghicp_prep *source, const ghicp_prep *target, const dou
   if (source->device != target->device) { set_error(nullptr, "prep_icp: the two pipeline results live on different devices"); return GHICP_E_ARG; }
   if (!icp_params_ok(p, guess, "prep_icp")) return GHICP_E_ARG;
   if (int rc = enter_device(source->device, "prep_icp")) return rc;
-  ghicp_prep *tb = const_cast<ghicp_prep *>(target);   // the grid is a cache of the target's down-sampled cloud, not its state
-  if (int rc = cuda_status(prep_icp_run(source, tb, guess, p, out), "prep_icp")) return rc;
+  // the grid and the normals are caches of the down-sampled clouds, not the results' state
+  ghicp_prep *sb = const_cast<ghicp_prep *>(source), *tb = const_cast<ghicp_prep *>(target);
+  if (int rc = cuda_status(prep_icp_run(sb, tb, guess, p, out), "prep_icp")) return rc;
   return icp_warnings(out);
 }
 

@@ -22,6 +22,19 @@
 //   k_icp_solve_pl      one thread: chol_solve<6>, t = t' - omega x m, det_sincos, PCL's constructTransformationMatrix in double
 //                       rounded once to float32, then k_icp_solve's F <- T F and convergence; a singular system stops the loop
 // The target's normals (prep_knn_normals) are computed once per call, or kept on a pipeline result.
+// Generalized ICP (metric 2, DESIGN.md §3.15: the reference's CRegistration::gicp_reg, src/common_reg.cpp:217-284, PCL's
+// GeneralizedIterativeClosestPoint) keeps the correspondence stages, with k_icp_query<true> dropping pairs at d2 >= 1e12, and
+// replaces the estimate by a Gauss-Newton minimisation of the Mahalanobis objective for the fixed pairs:
+//   k_icp_sum<1>        as above: the kept pairs' count and sum q (-> the centre m)
+//   k_gicp_begin        one thread: icp_begin, F_0 = F, R = F's rotation
+//   k_gicp_mahal        M_i = gicp_mahalanobis(R, N_s,i, N_t,j) once per outer iteration, 6 doubles per pair
+//   k_gicp_pass x 20    one inner step per launch: the 28 FP64 sums of J^T M J, J^T M r0, r0^T M r0 at F_j over k_icp_sum's
+//                       point blocks and tree, then the last CTA to finish (an integer ticket) adds the blocks' partial sums
+//                       in block order and runs gicp_step on one thread: accept or reject, chol_solve<6>, F_{j+1} = dT F_j;
+//                       once the inner loop has ended the remaining launches return at once
+//   k_gicp_end          one thread: F, then max_iterations and PCL's transformation delta
+//   k_icp_move          W = F P, from the unmoved source
+// Both clouds' normals (prep_knn_normals) are computed once per call, or kept on the pipeline results.
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
@@ -56,6 +69,19 @@ struct IcpDev {
 };
 struct IcpSum { double v[9]; unsigned long long n; };   // pass 1: s, q, sum d; pass 2: sum (q - mu_q)(s - mu_s)^T
 constexpr int IC_PL = 27;            // point-to-plane sums: the upper triangle of sum r r^T (row order), then sum r b
+constexpr int IC_G = 28;             // GICP sums: the upper triangle of J^T M J (row order), J^T M r0, r0^T M r0
+constexpr int GICP_INNER = 20;       // PCL's max_inner_iterations_
+constexpr double GICP_GATE = 1e12;   // gicp_reg's corr_dist_threshold 1e6, squared: a pair is kept when d2 < this
+struct GicpCtl {                     // the inner loop's state, on the device
+  float Fs[16];                      // F at the start of the outer iteration (row-major float32)
+  float Fj[16];                      // F_j: the transform the next pass evaluates
+  float Fp[16];                      // F_{j-1}
+  double R[9];                       // Fs's rotation, widened
+  double m[3];                       // the centre: the kept target points' mean
+  double fprev;                      // f_{j-1}
+  int j, done;                       // the next pass's step; 1 once the inner loop has ended (the later passes return at once)
+  unsigned ticket;                   // CTAs of the running pass that have written their partial sums
+};
 
 __device__ __forceinline__ void icp_move(const float *m, float x, float y, float z, float *o) {
   o[0] = ((m[0] * x + m[1] * y) + m[2] * z) + m[3];
@@ -94,7 +120,9 @@ __device__ __forceinline__ void icp_add_work(unsigned long long cells, unsigned 
   if ((threadIdx.x & 31) == 0 && (cells | cand)) { atomicAdd(work, cells); atomicAdd(work + 1, cand); }
 }
 
-// j(i) and d_i: the nearest target point of W_i in (d2, index) order, -1 / +inf for a non-finite W_i
+// j(i) and d_i: the nearest target point of W_i in (d2, index) order, -1 / +inf for a non-finite W_i; GATE (GICP): no pair
+// unless (double)d_i < 1e12
+template <bool GATE>
 __global__ void __launch_bounds__(IC_T) k_icp_query(const float *__restrict__ W, long long n, const int *__restrict__ perm,
                                                     const OvGrid G, int *__restrict__ corr, float *__restrict__ d2, IcpDev *dev) {
   const long long t = (long long)blockIdx.x * IC_T + threadIdx.x;
@@ -103,8 +131,9 @@ __global__ void __launch_bounds__(IC_T) k_icp_query(const float *__restrict__ W,
     const long long i = perm[t];
     const GridRegs r = grid_regs(G.g);   // per-thread registers, see k_pca
     int j = -1;
-    d2[i] = ov_nearest<true>(r, G, W[3 * i], W[3 * i + 1], W[3 * i + 2], (double)INFINITY, -1.f, cells, cand, j);
-    corr[i] = j;
+    const float d = ov_nearest<true>(r, G, W[3 * i], W[3 * i + 1], W[3 * i + 2], (double)INFINITY, -1.f, cells, cand, j);
+    d2[i] = d;
+    corr[i] = GATE && !((double)d < GICP_GATE) ? -1 : j;
   }
   icp_add_work(cells, cand, dev->h.work);
 }
@@ -223,9 +252,10 @@ __global__ void __launch_bounds__(IC_RED_T) k_icp_total(const IcpSum *__restrict
 // point-to-plane pass 2: the 27 sums of the kept pairs' centred rows (m = the kept source mean of pass 1), the same point
 // blocks and per-thread order as k_icp_sum; each of the 27 components then goes through k_icp_sum's halving tree in turn
 // (one 2 KB shared array instead of 55 KB for all of them at once; tests/harness/icp_oracle.cpp restates it)
-__device__ void icp_tree_pl(double *sh, const double (&v)[IC_PL], double *out) {
+template <int NC>
+__device__ void icp_tree_pl(double *sh, const double (&v)[NC], double *out) {
 #pragma unroll
-  for (int c = 0; c < IC_PL; ++c) {
+  for (int c = 0; c < NC; ++c) {
     sh[threadIdx.x] = v[c];
     __syncthreads();
     for (int w = IC_RED_T / 2; w > 0; w >>= 1) {
@@ -285,13 +315,17 @@ __device__ unsigned long long icp_begin(IcpDev *dev, const IcpSum *__restrict__ 
   for (int i = 0; i < 16; ++i) dev->T[i] = (i % 5 == 0) ? 1.f : 0.f;
   return c;
 }
+// the float32 product T F of the loop (row-major), each entry ((a0 + a1) + a2) + a3
+__device__ __forceinline__ void icp_compose(const float (&T)[16], const float *F, float (&out)[16]) {
+  for (int r = 0; r < 4; ++r)
+    for (int cc = 0; cc < 4; ++cc)
+      out[r * 4 + cc] = ((T[r * 4] * F[cc] + T[r * 4 + 1] * F[4 + cc]) + T[r * 4 + 2] * F[8 + cc]) + T[r * 4 + 3] * F[12 + cc];
+}
 // F <- T_k F, and DefaultConvergenceCriteria with max_iterations_similar_transforms = 0
 __device__ void icp_step(IcpDev *dev, const float (&T)[16], int k, int max_it, double eps_t, double eps_f) {
   IcpHead &h = dev->h;
   float F[16];
-  for (int r = 0; r < 4; ++r)
-    for (int cc = 0; cc < 4; ++cc)
-      F[r * 4 + cc] = ((T[r * 4] * h.F[cc] + T[r * 4 + 1] * h.F[4 + cc]) + T[r * 4 + 2] * h.F[8 + cc]) + T[r * 4 + 3] * h.F[12 + cc];
+  icp_compose(T, h.F, F);
   for (int i = 0; i < 16; ++i) { dev->T[i] = T[i]; h.F[i] = F[i]; }
   if (k >= max_it) { h.state = GHICP_ICP_ITERATIONS; return; }
   const double cosa = 0.5 * ((((double)T[0] + (double)T[5]) + (double)T[10]) - 1.0);
@@ -346,24 +380,194 @@ __global__ void k_icp_solve_pl(IcpDev *dev, const IcpSum *__restrict__ m1, const
   icp_step(dev, T, k, max_it, eps_t, eps_f);
 }
 
+// ---- Generalized ICP (metric 2) ---------------------------------------------------------------------------------------------
+// PCL's GICP convergence measure between two float32 transforms: the largest |a_kl - b_kl| (float32 difference), scaled by
+// 1 / eps_r in the 3 x 3 rotation block and by 1 / eps_t elsewhere (a NaN product, eps_t = 0 against no change, is skipped)
+__device__ double gicp_delta(const float *a, const float *b, double eps_t, double eps_r) {
+  const double rr = 1.0 / eps_r, rt = 1.0 / eps_t;
+  double d = 0.0;
+  for (int k = 0; k < 4; ++k)
+    for (int l = 0; l < 4; ++l) {
+      const double c = (k < 3 && l < 3 ? rr : rt) * (double)fabsf(a[4 * k + l] - b[4 * k + l]);
+      if (c > d) d = c;
+    }
+  return d;
+}
+
+// one thread, once per outer iteration after k_icp_sum<1>: the pairs, F_0 = F, R, the centre m
+__global__ void k_gicp_begin(IcpDev *dev, GicpCtl *g, const IcpSum *__restrict__ m1) {
+  const unsigned long long c = icp_begin(dev, m1);
+  g->j = 0;
+  g->done = c < 3;
+  if (c < 3) { dev->h.state = GHICP_ICP_NO_CORRESPONDENCES; return; }
+  for (int i = 0; i < 16; ++i) { g->Fs[i] = dev->h.F[i]; g->Fj[i] = dev->h.F[i]; }
+  for (int r = 0; r < 3; ++r)
+    for (int cc = 0; cc < 3; ++cc) g->R[3 * r + cc] = (double)dev->h.F[4 * r + cc];
+  for (int a = 0; a < 3; ++a) g->m[a] = m1->v[3 + a] / (double)c;
+}
+
+// the pairs' metric for the whole outer iteration, [n][6] (rows of dropped points are left as they are); the passes read it
+// back rather than recompute it from the two normals: measured faster per outer iteration in 7 of 8 cases on an H100
+// (DESIGN.md §3.15)
+__global__ void k_gicp_mahal(const float *__restrict__ Ns, const float *__restrict__ Nt, const int *__restrict__ corr, long long n,
+                             const GicpCtl *g, double *__restrict__ Mst) {
+  const long long p = (long long)blockIdx.x * IC_T + threadIdx.x;
+  if (p >= n || g->done) return;
+  const int j = corr[p];
+  if (j >= 0) gicp_mahalanobis(g->R, Ns + 3 * p, Nt + 3 * (size_t)j, Mst + 6 * p);
+}
+
+// one thread: the inner step on the pass's totals (acc) at F_j.  f_j > f_{j-1} rejects F_j (back to F_{j-1}) and ends the
+// inner loop; else H x = -g by chol_solve<6>, t = t' - omega x m, dT = PCL's constructTransformationMatrix in double rounded
+// once to float32, F_{j+1} = dT F_j; the loop ends when PCL's delta(F_{j+1}, F_j) < 1 or after 20 steps.  A system chol_solve
+// refuses, an angle beyond det_sincos's range or a non-finite t stops the outer loop (SINGULAR) with F unchanged.
+__device__ void gicp_step(IcpDev *dev, GicpCtl *g, const double *acc, double eps_t, double eps_r) {
+  const double f = acc[IC_G - 1];
+  if (g->j > 0 && f > g->fprev) {
+    for (int i = 0; i < 16; ++i) g->Fj[i] = g->Fp[i];
+    g->done = 1;
+    return;
+  }
+  double A[6][6], b[6], x[6] = {0, 0, 0, 0, 0, 0};
+  int e = 0;
+  for (int i = 0; i < 6; ++i)
+    for (int j = i; j < 6; ++j) { A[i][j] = acc[e]; A[j][i] = acc[e]; ++e; }
+  for (int i = 0; i < 6; ++i) b[i] = -acc[21 + i];
+  const double *m = g->m;
+  bool ok = chol_solve<6>(A, b, x);
+  const double al = x[0], be = x[1], ga = x[2];
+  const double t[3] = {x[3] - (be * m[2] - ga * m[1]), x[4] - (ga * m[0] - al * m[2]), x[5] - (al * m[1] - be * m[0])};
+  for (int i = 0; i < 3; ++i) ok = ok && fabs(x[i]) <= 1048576.0 && fabs(t[i]) <= DBL_MAX;   // false for NaN
+  if (!ok) { dev->h.state = GHICP_ICP_SINGULAR; g->done = 1; return; }
+  double sa, ca, sb, cb, sg, cg;
+  det_sincos(al, sa, ca); det_sincos(be, sb, cb); det_sincos(ga, sg, cg);
+  const float T[16] = {(float)(cg * cb), (float)((-sg) * ca + (cg * sb) * sa), (float)(sg * sa + (cg * sb) * ca), (float)t[0],
+                       (float)(sg * cb), (float)(cg * ca + (sg * sb) * sa), (float)((-cg) * sa + (sg * sb) * ca), (float)t[1],
+                       (float)(-sb), (float)(cb * sa), (float)(cb * ca), (float)t[2],
+                       0.f, 0.f, 0.f, 1.f};
+  float Fn[16];
+  icp_compose(T, g->Fj, Fn);
+  const bool small = gicp_delta(Fn, g->Fj, eps_t, eps_r) < 1.0;
+  for (int i = 0; i < 16; ++i) { g->Fp[i] = g->Fj[i]; g->Fj[i] = Fn[i]; }
+  g->fprev = f;
+  g->j += 1;
+  if (small || g->j >= GICP_INNER) g->done = 1;
+}
+
+// One inner step: the 28 sums at F_j (W = F_j P in place, icp_move's formula), thread t of block b over the kept points
+// b*CHUNK + t, + t + T, ... and each component through the halving tree (k_icp_sum_pl's order); then the last CTA to take a
+// ticket adds the blocks' sums as k_icp_total_pl does (block order, not arrival order: the same bits whichever CTA is last)
+// and runs gicp_step.  Per kept pair, in double from the float32 inputs: r0 = w - q, u = w - m, J = [-[u]x, I] (the
+// residual linearised as r0 + omega x u + t'), H += J^T M J, g += J^T M r0, f += r0^T M r0, M = k_gicp_mahal's.
+__global__ void __launch_bounds__(IC_RED_T) k_gicp_pass(const float *__restrict__ P, const float *__restrict__ Q,
+                                                        const double *__restrict__ Mst, const int *__restrict__ corr, long long n,
+                                                        int nb, GicpCtl *g, IcpDev *dev, double *__restrict__ part, double eps_t,
+                                                        double eps_r) {
+  __shared__ double sh[IC_RED_T];
+  __shared__ double tot[IC_G];
+  __shared__ int last;
+  if (g->done) return;   // the inner loop has ended: the same for every thread of the launch
+  const long long p0 = (long long)blockIdx.x * IC_RED_CHUNK, p1 = min(p0 + IC_RED_CHUNK, n);
+  double v[IC_G];
+#pragma unroll
+  for (int c = 0; c < IC_G; ++c) v[c] = 0.0;
+  float F[16];
+  for (int i = 0; i < 16; ++i) F[i] = g->Fj[i];
+  double m[3];
+  for (int a = 0; a < 3; ++a) m[a] = g->m[a];
+  for (long long p = p0 + threadIdx.x; p < p1; p += IC_RED_T) {
+    const int j = corr[p];
+    if (j < 0) continue;
+    float w[3];
+    icp_move(F, P[3 * p], P[3 * p + 1], P[3 * p + 2], w);
+    double M[6];
+    for (int a = 0; a < 6; ++a) M[a] = Mst[6 * p + a];
+    const double q[3] = {(double)Q[3 * (size_t)j], (double)Q[3 * (size_t)j + 1], (double)Q[3 * (size_t)j + 2]};
+    const double r[3] = {(double)w[0] - q[0], (double)w[1] - q[1], (double)w[2] - q[2]};
+    const double u[3] = {(double)w[0] - m[0], (double)w[1] - m[1], (double)w[2] - m[2]};
+    // the rotation columns of J: e_x x u, e_y x u, e_z x u
+    const double J[3][3] = {{0.0, -u[2], u[1]}, {u[2], 0.0, -u[0]}, {-u[1], u[0], 0.0}};
+    double MJ[3][3], Mr[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      MJ[c][0] = (M[0] * J[c][0] + M[1] * J[c][1]) + M[2] * J[c][2];
+      MJ[c][1] = (M[1] * J[c][0] + M[3] * J[c][1]) + M[4] * J[c][2];
+      MJ[c][2] = (M[2] * J[c][0] + M[4] * J[c][1]) + M[5] * J[c][2];
+    }
+    Mr[0] = (M[0] * r[0] + M[1] * r[1]) + M[2] * r[2];
+    Mr[1] = (M[1] * r[0] + M[3] * r[1]) + M[4] * r[2];
+    Mr[2] = (M[2] * r[0] + M[4] * r[1]) + M[5] * r[2];
+    const double Mi[3][3] = {{M[0], M[1], M[2]}, {M[1], M[3], M[4]}, {M[2], M[4], M[5]}};
+    int e = 0;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+#pragma unroll
+      for (int c = a; c < 3; ++c) v[e++] += (J[a][0] * MJ[c][0] + J[a][1] * MJ[c][1]) + J[a][2] * MJ[c][2];
+#pragma unroll
+      for (int c = 0; c < 3; ++c) v[e++] += MJ[a][c];
+    }
+#pragma unroll
+    for (int a = 0; a < 3; ++a)
+#pragma unroll
+      for (int c = a; c < 3; ++c) v[e++] += Mi[a][c];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) v[21 + a] += (J[a][0] * Mr[0] + J[a][1] * Mr[1]) + J[a][2] * Mr[2];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) v[24 + a] += Mr[a];
+    v[27] += (r[0] * Mr[0] + r[1] * Mr[1]) + r[2] * Mr[2];
+  }
+  icp_tree_pl(sh, v, part + (size_t)IC_G * blockIdx.x);
+  if (threadIdx.x == 0) {
+    __threadfence();   // this block's sums before its ticket
+    last = atomicAdd(&g->ticket, 1u) == (unsigned)(nb - 1);
+  }
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+#pragma unroll
+  for (int c = 0; c < IC_G; ++c) v[c] = 0.0;
+  for (int b = threadIdx.x; b < nb; b += IC_RED_T)
+#pragma unroll
+    for (int c = 0; c < IC_G; ++c) v[c] += __ldcg(part + (size_t)IC_G * b + c);
+  icp_tree_pl(sh, v, tot);
+  if (threadIdx.x == 0) {
+    g->ticket = 0u;
+    gicp_step(dev, g, tot, eps_t, eps_r);
+  }
+}
+
+// one thread, after the inner steps: F, then k >= max_iterations (ITERATIONS) and PCL's delta(F_0, F) < 1 (TRANSFORM);
+// NO_CORRESPONDENCES and SINGULAR leave F as it was
+__global__ void k_gicp_end(IcpDev *dev, const GicpCtl *g, int k, int max_it, double eps_t, double eps_r) {
+  IcpHead &h = dev->h;
+  if (h.state != 0) return;
+  for (int i = 0; i < 16; ++i) h.F[i] = g->Fj[i];
+  if (k >= max_it) { h.state = GHICP_ICP_ITERATIONS; return; }
+  if (gicp_delta(g->Fj, g->Fs, eps_t, eps_r) < 1.0) h.state = GHICP_ICP_TRANSFORM;
+}
+
 inline int iblk(long long n, int t) { return (int)((n + t - 1) / t); }
 
 }  // namespace
 
 cudaError_t icp_run(const float *d_src, int n_src, const float *d_all, int n_all, const OverlapTarget *t, const float *d_tgt,
-                    const float *d_nrm, const double *guess, const ghicp_icp_params *p, cudaEvent_t ev_iter, cudaEvent_t ev_fit,
-                    ghicp_icp_result *out, float *h_moved, int *h_cor, double *h_mse) {
+                    const float *d_nrm, const float *d_nrm_s, const double *guess, const ghicp_icp_params *p, cudaEvent_t ev_iter,
+                    cudaEvent_t ev_fit, ghicp_icp_result *out, float *h_moved, int *h_cor, double *h_mse) {
   const long long n = n_src, nt = t->n;
-  const bool recip = p->reciprocal != 0, trim = p->trim_ratio > 0.f, plane = p->metric == 1;
+  const bool recip = p->reciprocal != 0, trim = p->trim_ratio > 0.f, plane = p->metric == 1, gicp = p->metric == 2;
   const int nb = iblk(n, IC_RED_CHUNK);
   DevBuf<float> W, d2, moved; DevBuf<int> corr, perm, rev, list; DevBuf<pu64> keys; DevBuf<unsigned char> flag;
-  DevBuf<IcpDev> dev; DevBuf<IcpSum> part, tot; DevBuf<double> part_pl, tot_pl;
+  DevBuf<IcpDev> dev; DevBuf<IcpSum> part, tot; DevBuf<double> part_pl, tot_pl, Mst; DevBuf<GicpCtl> ctl;
   // every workspace of the loop first: running out of memory returns before anything is written (the reciprocal option's
   // grid over W is the exception: prep_point_grid allocates it every iteration, from the same pool)
   CUDA_TRY(W.alloc(3 * (size_t)n)); CUDA_TRY(d2.alloc((size_t)n)); CUDA_TRY(corr.alloc((size_t)n));
   CUDA_TRY(perm.alloc((size_t)n)); CUDA_TRY(keys.alloc((size_t)n));
   CUDA_TRY(dev.alloc(1)); CUDA_TRY(part.alloc((size_t)nb)); CUDA_TRY(tot.alloc(2));
   if (plane) { CUDA_TRY(part_pl.alloc((size_t)IC_PL * nb)); CUDA_TRY(tot_pl.alloc(IC_PL)); }
+  if (gicp) {
+    CUDA_TRY(part_pl.alloc((size_t)IC_G * nb)); CUDA_TRY(ctl.alloc(1)); CUDA_TRY(Mst.alloc(6 * (size_t)n));
+    CUDA_TRY(cudaMemsetAsync(ctl.get(), 0, sizeof(GicpCtl), 0));
+  }
   if (recip) { CUDA_TRY(rev.alloc((size_t)nt)); CUDA_TRY(list.alloc((size_t)nt)); CUDA_TRY(flag.alloc((size_t)nt)); }
   if (h_moved) CUDA_TRY(moved.alloc(3 * (size_t)n_all));
   IcpDev h0{};
@@ -382,7 +586,8 @@ cudaError_t icp_run(const float *d_src, int n_src, const float *d_all, int n_all
   for (;; ++k) {
     GHICP_LAUNCH(k_icp_keys, iblk(n, IC_T), IC_T, 0, 0, W.get(), n, G, keys.get(), perm.get());
     CUDA_TRY(prep_sort_pairs(0, keys.get(), perm.get(), n_src));
-    GHICP_LAUNCH(k_icp_query, iblk(n, IC_T), IC_T, 0, 0, W.get(), n, perm.get(), G, corr.get(), d2.get(), D);
+    if (gicp) GHICP_LAUNCH(k_icp_query<true>, iblk(n, IC_T), IC_T, 0, 0, W.get(), n, perm.get(), G, corr.get(), d2.get(), D);
+    else GHICP_LAUNCH(k_icp_query<false>, iblk(n, IC_T), IC_T, 0, 0, W.get(), n, perm.get(), G, corr.get(), d2.get(), D);
     if (recip) {
       CUDA_TRY(cudaMemsetAsync(flag.get(), 0, (size_t)nt, 0));
       CUDA_TRY(cudaMemsetAsync(&D->n_rev, 0, sizeof(int), 0));
@@ -401,7 +606,15 @@ cudaError_t icp_run(const float *d_src, int n_src, const float *d_all, int n_all
     }
     GHICP_LAUNCH(k_icp_sum<1>, nb, IC_RED_T, 0, 0, W.get(), d_tgt, corr.get(), d2.get(), n, nullptr, part.get());
     GHICP_LAUNCH(k_icp_total, 1, IC_RED_T, 0, 0, part.get(), nb, tot.get());
-    if (plane) {
+    if (gicp) {
+      GicpCtl *C = ctl.get();
+      const double et = p->transformation_epsilon, er = p->rotation_epsilon;
+      GHICP_LAUNCH(k_gicp_begin, 1, 1, 0, 0, D, C, tot.get());
+      GHICP_LAUNCH(k_gicp_mahal, iblk(n, IC_T), IC_T, 0, 0, d_nrm_s, d_nrm, corr.get(), n, C, Mst.get());
+      for (int j = 0; j < GICP_INNER; ++j)   // no read-back: the passes after the inner loop's end return at once
+        GHICP_LAUNCH(k_gicp_pass, nb, IC_RED_T, 0, 0, d_src, d_tgt, Mst.get(), corr.get(), n, nb, C, D, part_pl.get(), et, er);
+      GHICP_LAUNCH(k_gicp_end, 1, 1, 0, 0, D, C, k, p->max_iterations, et, er);
+    } else if (plane) {
       GHICP_LAUNCH(k_icp_sum_pl, nb, IC_RED_T, 0, 0, W.get(), d_tgt, d_nrm, corr.get(), n, tot.get(), part_pl.get());
       GHICP_LAUNCH(k_icp_total_pl, 1, IC_RED_T, 0, 0, part_pl.get(), nb, tot_pl.get());
       GHICP_LAUNCH(k_icp_solve_pl, 1, 1, 0, 0, D, tot.get(), tot_pl.get(), k, p->max_iterations, p->transformation_epsilon,
@@ -412,7 +625,8 @@ cudaError_t icp_run(const float *d_src, int n_src, const float *d_all, int n_all
       GHICP_LAUNCH(k_icp_solve, 1, 1, 0, 0, D, tot.get(), tot.get() + 1, k, p->max_iterations, p->transformation_epsilon,
                    p->fitness_epsilon);
     }
-    GHICP_LAUNCH(k_icp_move, iblk(n, IC_T), IC_T, 0, 0, W.get(), W.get(), n, D->T);
+    if (gicp) GHICP_LAUNCH(k_icp_move, iblk(n, IC_T), IC_T, 0, 0, d_src, W.get(), n, D->h.F);   // W = F P, as PCL moves its output
+    else GHICP_LAUNCH(k_icp_move, iblk(n, IC_T), IC_T, 0, 0, W.get(), W.get(), n, D->T);
     CUDA_TRY(cudaGetLastError());
     // the one read-back of an iteration
     CUDA_TRY(cudaMemcpyAsync(&hh, &D->h, sizeof(hh), cudaMemcpyDeviceToHost, 0));

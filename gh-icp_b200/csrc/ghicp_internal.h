@@ -500,14 +500,15 @@ void overlap_target_free(OverlapTarget *t);
 cudaError_t overlap_run(const float *d_a, int n_a, const OverlapTarget *t, const double *Rt, float thre_dis, double max_range,
                         int want_fitness, cudaEvent_t ev_queries, ghicp_overlap_result *out, float *h_d2_out);
 
-// ICP on the dense clouds (ghicp_icp.cu): point-to-point (p->metric 0, DESIGN.md §3.13) or point-to-plane (1, §3.14).
-// d_src [n_src][3] = the finite source points (the loop's), d_all [n_all][3] = the whole source (fitness and h_moved); t = the
-// target's grid over d_tgt; d_nrm [n_tgt][3] = the target's normals (prep_knn_normals; read by metric 1 only); parameters
-// already checked.  Fills every field of out but stage_ms; h_moved, h_cor, h_mse (host, may be null) receive the moved source
-// and the per-iteration traces.  ev_iter / ev_fit (may be null) are recorded before the first iteration and before the fitness.
+// ICP on the dense clouds (ghicp_icp.cu): point-to-point (p->metric 0, DESIGN.md §3.13), point-to-plane (1, §3.14) or
+// Generalized ICP (2, §3.15).  d_src [n_src][3] = the finite source points (the loop's), d_all [n_all][3] = the whole source
+// (fitness and h_moved); t = the target's grid over d_tgt; d_nrm [n_tgt][3] = the target's normals (prep_knn_normals; read
+// by metrics 1 and 2), d_nrm_s [n_src][3] = d_src's normals (metric 2 only); parameters already checked.  Fills every field
+// of out but stage_ms; h_moved, h_cor, h_mse (host, may be null) receive the moved source and the per-iteration traces.
+// ev_iter / ev_fit (may be null) are recorded before the first iteration and before the fitness.
 cudaError_t icp_run(const float *d_src, int n_src, const float *d_all, int n_all, const OverlapTarget *t, const float *d_tgt,
-                    const float *d_nrm, const double *guess, const ghicp_icp_params *p, cudaEvent_t ev_iter, cudaEvent_t ev_fit, ghicp_icp_result *out,
-                    float *h_moved, int *h_cor, double *h_mse);
+                    const float *d_nrm, const float *d_nrm_s, const double *guess, const ghicp_icp_params *p, cudaEvent_t ev_iter,
+                    cudaEvent_t ev_fit, ghicp_icp_result *out, float *h_moved, int *h_cor, double *h_mse);
 
 // glue of the device-resident pipeline (ghicp_prep_run)
 cudaError_t prep_gather_points(cudaStream_t st, const float *d_xyz, const int *d_idx, int m, float *d_out);

@@ -141,6 +141,32 @@ GHICP_HD inline void det_sincos(double x, double &s, double &c) {
   }
 }
 
+// Generalized ICP's per-pair metric (DESIGN.md §3.15): M = (R C_s R^T + C_t)^-1 with C = I - (1 - eps) n n^T, eps = 0.001
+// (PCL's gicp_epsilon: the neighbourhood covariance with its singular values replaced by (1, 1, eps)), from the source and
+// target k-NN normals ns, nt and R = the rotation of the transform at the start of the iteration (row-major, widened from
+// float32).  All in double in a fixed order, so the kernel and the oracle agree bit for bit without FMA contraction.  The
+// sum has eigenvalues >= 2 eps: M is positive definite.  M = {m00, m01, m02, m11, m12, m22}.
+constexpr double GICP_EPSILON = 1e-3;
+GHICP_HD inline void gicp_mahalanobis(const double R[9], const float ns[3], const float nt[3], double M[6]) {
+  const double e = 1.0 - GICP_EPSILON;
+  const double a[3] = {(double)ns[0], (double)ns[1], (double)ns[2]}, b[3] = {(double)nt[0], (double)nt[1], (double)nt[2]};
+  double Cs[9], RC[9], S[6];
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c) Cs[3 * r + c] = (r == c ? 1.0 : 0.0) - e * (a[r] * a[c]);
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c) RC[3 * r + c] = (R[3 * r] * Cs[c] + R[3 * r + 1] * Cs[3 + c]) + R[3 * r + 2] * Cs[6 + c];
+  int q = 0;
+  for (int r = 0; r < 3; ++r)
+    for (int c = r; c < 3; ++c)   // (R C_s R^T)_rc + (C_t)_rc
+      S[q++] = ((RC[3 * r] * R[3 * c] + RC[3 * r + 1] * R[3 * c + 1]) + RC[3 * r + 2] * R[3 * c + 2]) +
+               ((r == c ? 1.0 : 0.0) - e * (b[r] * b[c]));
+  // the inverse of the symmetric S by its cofactors
+  const double c00 = S[3] * S[5] - S[4] * S[4], c01 = S[2] * S[4] - S[1] * S[5], c02 = S[1] * S[4] - S[2] * S[3];
+  const double c11 = S[0] * S[5] - S[2] * S[2], c12 = S[1] * S[2] - S[0] * S[4], c22 = S[0] * S[3] - S[1] * S[1];
+  const double det = (S[0] * c00 + S[1] * c01) + S[2] * c02;
+  M[0] = c00 / det; M[1] = c01 / det; M[2] = c02 / det; M[3] = c11 / det; M[4] = c12 / det; M[5] = c22 / det;
+}
+
 // CRegistration::LLS_4DOF (src/common_reg.cpp:623-775) from the 12 moments
 //   acc = { W, Sx, Sy, Sz, SX, SY, SZ, Q = sum w (x^2 + y^2), sum w xX, sum w yX, sum w xY, sum w yY }
 // (x, y, z source; X, Y, Z target).  Per Gauss-Newton step the reference's normal equations (:661-689) are

@@ -16,14 +16,20 @@
 //                                                      options against the target's k-NN normals, by ghicp_cloud_icp with
 //                                                      metric 1 (DESIGN.md §3.14); the source's normals take no part in PCL's
 //                                                      estimate and are not computed
+//   gicp_reg             (src/common_reg.cpp:217-284)  PCL's GeneralizedIterativeClosestPoint over both clouds' k-NN normals,
+//                                                      by ghicp_cloud_icp with metric 2 (DESIGN.md §3.15); the reciprocal and
+//                                                      trimmed options do not reach the loop, as in PCL's GICP (:213-215), and
+//                                                      use_trimmed_rejector only refuses a low overlap ratio
 // Differences, deliberate: clouds are ghicp::Cloud (cloud_io.h) and fpfhFeaturePtr the stand-in of ghicp_types.h; the
 // transform is Eigen::Matrix4f when Eigen is on the include path, else the column-major ghicp::Matrix4f; the SAC-IA is the
 // deterministic one of DESIGN.md §3.11 instead of PCL's std::rand()-driven one; no CPU path (without a CUDA device both
 // members throw).  The fitness of the last Coarsereg_FPFHSAC or icp_reg, which the reference prints, is kept
-// (getFitnessScore).  icp_reg and ptplicp_reg print their lines to std::cout only (the reference also logs them through
-// glog).  ptplicp_reg writes TransformedSource and returns true, where the reference aligns into a local cloud (:141, :182)
-// and leaves the caller's untouched, and falls off the end of the function without a return value (:199).
-// Not provided: the other PCL ICP wrapper (gicp_reg), LLS_4DOF / SVD_6DOF and CSTRAN_4DOF / CSTRAN_7DOF.
+// (getFitnessScore).  icp_reg, ptplicp_reg and gicp_reg print their lines to std::cout only (the reference also logs them
+// through glog; gicp_reg's fitness warning above 5000, a glog warning there, is printed as a line).  ptplicp_reg writes
+// TransformedSource and returns true, where the reference aligns into a local cloud (:141, :182) and leaves the caller's
+// untouched, and falls off the end of the function without a return value (:199); gicp_reg returns true where the reference
+// falls off the end too (:284).
+// Not provided: LLS_4DOF / SVD_6DOF and CSTRAN_4DOF / CSTRAN_7DOF.
 #pragma once
 #include <algorithm>
 #include <ctime>
@@ -108,24 +114,37 @@ class CRegistration {
                    use_trimmed_rejector, thre_dis, 1, covariance_K, min_overlap_for_reg);
   }
 
+  // :217-284 — Generalized ICP of SourceCloud onto TargetCloud from the identity with both clouds' k-NN normals as
+  // covariances (k = covariance_K, 3..32; transformation epsilon 1e-8, rotation epsilon 1e-6).  PCL's GICP ignores the
+  // reciprocal option and the rejectors: the loop runs without them, and use_trimmed_rejector only returns false when
+  // calOverlap(SourceCloud, TargetCloud, thre_dis) is below min_overlap_for_reg.
+  bool gicp_reg(const Cloud &SourceCloud, const Cloud &TargetCloud, Cloud &TransformedSource, Matrix4f &transformationS2T,
+                int max_iter, bool use_reciprocal_correspondence, bool use_trimmed_rejector, float thre_dis, int covariance_K,
+                float min_overlap_for_reg) {
+    (void)use_reciprocal_correspondence;
+    return run_icp(SourceCloud, TargetCloud, TransformedSource, transformationS2T, max_iter, false, use_trimmed_rejector,
+                   thre_dis, 2, covariance_K, min_overlap_for_reg);
+  }
+
  private:
-  // icp_reg (metric 0) and ptplicp_reg (metric 1, normal_k)
+  // icp_reg (metric 0), ptplicp_reg (metric 1, normal_k) and gicp_reg (metric 2, normal_k; the overlap ratio gates only)
   bool run_icp(const Cloud &SourceCloud, const Cloud &TargetCloud, Cloud &TransformedSource, Matrix4f &transformationS2T,
                int max_iter, bool use_reciprocal_correspondence, bool use_trimmed_rejector, float thre_dis, int metric, int normal_k,
                float min_overlap_for_reg) {
-    const char *who = metric == 1 ? "CRegistration::ptplicp_reg: " : "CRegistration::icp_reg: ";
+    const char *who = metric == 2 ? "CRegistration::gicp_reg: " : (metric == 1 ? "CRegistration::ptplicp_reg: " : "CRegistration::icp_reg: ");
     const clock_t t0 = clock();
     ghicp_icp_params p{};
     p.max_iterations = max_iter; p.reciprocal = use_reciprocal_correspondence ? 1 : 0;
-    p.transformation_epsilon = 1e-8; p.fitness_epsilon = 1e-5;   // :86, :88 (:166, :168)
+    p.transformation_epsilon = 1e-8; p.fitness_epsilon = 1e-5;   // :86, :88 (:166, :168; :263)
     p.metric = metric; p.normal_k = normal_k;
+    p.rotation_epsilon = 1e-6;                                   // :265, read by metric 2 only
     if (use_trimmed_rejector) {
       const float overlap_ratio = calOverlap(SourceCloud, TargetCloud, thre_dis);
       if (overlap_ratio < min_overlap_for_reg) {
         std::cout << "The overlap ratio is too small. This registration would not be done." << std::endl;
         return false;
       }
-      p.trim_ratio = std::min(1.0f, overlap_ratio);   // setOverlapRatio clamps to [0, 1]
+      if (metric != 2) p.trim_ratio = std::min(1.0f, overlap_ratio);   // setOverlapRatio clamps to [0, 1]
     }
     const int n = (int)SourceCloud.size();
     std::vector<float> moved(3 * (size_t)n);
@@ -138,14 +157,15 @@ class CRegistration {
     fitness_ = r.fitness;
     icp_result_ = r;
     const clock_t t1 = clock();
-    std::cout << (metric == 1 ? "Point-to-Plane" : "Point-to-Point") << " ICP done in " << float(t1 - t0) / CLOCKS_PER_SEC << " s"
-              << std::endl;
+    std::cout << (metric == 2 ? "GICP" : (metric == 1 ? "Point-to-Plane ICP" : "Point-to-Point ICP")) << " done in "
+              << float(t1 - t0) / CLOCKS_PER_SEC << " s" << std::endl;
     for (int i = 0; i < 4; ++i) {
       for (int j = 0; j < 4; ++j) std::cout << (j ? " " : "") << transformationS2T(i, j);
       std::cout << std::endl;
     }
     std::cout << "The fitness score of this registration is " << fitness_ << std::endl;
-    if (metric == 0) std::cout << "-----------------------------------------------------------------------------" << std::endl;
+    if (metric == 2 && fitness_ > 5000) std::cout << "The fitness score of this registration is a bit too large" << std::endl;
+    if (metric != 1) std::cout << "-----------------------------------------------------------------------------" << std::endl;
     return true;
   }
 

@@ -41,6 +41,10 @@ it on the unmoved source (it starts from the identity); with `evaluate`, info["e
 The default None leaves the result and info as they were.  icp_reg(source, target, ...) is CRegistration::icp_reg itself.
 refine may also carry "metric": "plane" (default "point") and "covariance_k" (default 20): point-to-plane ICP against the
 target's k-NN normals (DESIGN.md §3.14); ptplicp_reg(source, target, ...) is CRegistration::ptplicp_reg itself.
+"metric": "gicp" refines with Generalized ICP over both clouds' k-NN normals (DESIGN.md §3.15), honouring "reciprocal" and
+"trimmed_thre_dis" as the other metrics do: the library's own extension, the "G-ICP with trimmed property" the reference's
+author was working on (PCL's GICP ignores both, src/common_reg.cpp:213-215); gicp_reg(source, target, ...) is
+CRegistration::gicp_reg itself, with both options off in the loop as PCL has them.
 
 coarsereg_fpfh_sac(source_xyz, target_xyz, search_radius) is CRegistration::Coarsereg_FPFHSAC (src/common_reg.cpp:393-423):
 radius FPFH on every point of both clouds, then SAC-IA with correspondence randomness 15.
@@ -168,10 +172,10 @@ def _refine_kw(refine):
     keys = {"max_iter", "reciprocal", "trimmed_thre_dis", "metric", "covariance_k"}
     if not isinstance(refine, dict) or "max_iter" not in refine or set(refine) - keys:
         raise capi.GhicpError(-1, "refine must be a dict {max_iter, reciprocal (optional), trimmed_thre_dis (optional), "
-                                  "metric ('point' or 'plane', optional), covariance_k (optional)}")
+                                  "metric ('point', 'plane' or 'gicp', optional), covariance_k (optional)}")
     metric = refine.get("metric", "point")
     if metric not in capi.ICP_METRICS:
-        raise capi.GhicpError(-1, f"refine: metric must be 'point' or 'plane', not {metric!r}")
+        raise capi.GhicpError(-1, f"refine: metric must be 'point', 'plane' or 'gicp', not {metric!r}")
     return dict(max_iter=int(refine["max_iter"]), reciprocal=bool(refine.get("reciprocal", False)),
                 thre_dis=refine.get("trimmed_thre_dis"), metric=metric, normal_k=int(refine.get("covariance_k", 20)))
 
@@ -226,6 +230,28 @@ def ptplicp_reg(source_xyz, target_xyz, max_iter, use_reciprocal_correspondence,
                               trim_ratio=min(rho, 1.0), transformation_epsilon=1e-8, fitness_epsilon=1e-5, return_moved=True,
                               device=device, metric="plane", normal_k=covariance_K)
     if use_trimmed_rejector:
+        info["overlap_ratio"] = rho
+    return Rt, info
+
+
+def gicp_reg(source_xyz, target_xyz, max_iter, use_reciprocal_correspondence, use_trimmed_rejector, thre_dis, covariance_K,
+             min_overlap_for_reg=0.0, device=0):
+    """CRegistration::gicp_reg (src/common_reg.cpp:217-284) on the GPU: Generalized ICP of the source onto the target from the
+    identity with both clouds' k-NN normals as covariances (k = covariance_K, 3..32), transformation epsilon 1e-8 and rotation
+    epsilon 1e-6 (capi.cloud_icp with metric="gicp", DESIGN.md §3.15).  PCL's GICP ignores the reciprocal option and the
+    correspondence rejectors, so the loop runs without them whatever use_reciprocal_correspondence says; use_trimmed_rejector
+    only gates the call: the ratio calOverlap(source, target, thre_dis) of the unmoved source below min_overlap_for_reg returns
+    None.  Returns (Rt 4x4, info with the transformed source under "moved"; info["overlap_ratio"] when trimmed), as icp_reg."""
+    S = np.ascontiguousarray(source_xyz, dtype=np.float32).reshape(-1, 3)
+    T = np.ascontiguousarray(target_xyz, dtype=np.float32).reshape(-1, 3)
+    rho = None
+    if use_trimmed_rejector:
+        rho = cal_overlap(S, T, thre_dis, device=device)
+        if rho < min_overlap_for_reg:
+            return None
+    Rt, info = capi.cloud_icp(S, T, None, max_iterations=max_iter, reciprocal=False, trim_ratio=0.0, transformation_epsilon=1e-8,
+                              return_moved=True, device=device, metric="gicp", normal_k=covariance_K, rotation_epsilon=1e-6)
+    if rho is not None:
         info["overlap_ratio"] = rho
     return Rt, info
 

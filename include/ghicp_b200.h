@@ -56,7 +56,7 @@ enum ghicp_status {
   GHICP_E_NOCONV = -5, /* ghicp_run hit max_iter without converging */
   GHICP_E_NODEV = -6,  /* no CUDA device: the product path has NO CPU fallback */
   GHICP_W_FEW_PAIRS = 1, /* cor < min_cor (include/ghicp_reg.h:36, src/ghicp_reg.cpp:796-797) */
-  GHICP_W_SINGULAR = 2   /* point-to-plane ICP: the normal equations of an iteration were singular (GHICP_ICP_SINGULAR) */
+  GHICP_W_SINGULAR = 2   /* point-to-plane ICP or GICP: the normal equations of an iteration were singular (GHICP_ICP_SINGULAR) */
 };
 
 /* Constructor arguments of ghicp::GHRegistration (include/ghicp_reg.h:77-81) + Energyfunction::init
@@ -361,24 +361,36 @@ int ghicp_prep_overlap(const ghicp_prep *a, const ghicp_prep *b, const double Rt
  * IterativeClosestPointWithNormals with TransformationEstimationPointToPlaneLLS.  The same loop, but each step solves PCL's
  * point-to-plane normal equations (centred on the kept source points' mean, FP64 fixed-order sums) against the target's k-NN
  * normals (PCL NormalEstimation with k = normal_k, viewpoint 0, non-finite normals replaced by (0.577, 0.577, 0.577) as
- * CheckNormals does).  A singular system stops the loop with GHICP_ICP_SINGULAR. */
+ * CheckNormals does).  A singular system stops the loop with GHICP_ICP_SINGULAR.
+ * Generalized ICP (metric = 2, DESIGN.md §3.15): CRegistration::gicp_reg (src/common_reg.cpp:217-284), PCL's
+ * GeneralizedIterativeClosestPoint.  The same pairs, gated at d2 < 1e12 (gicp_reg's corr_dist_threshold 1e6, squared); each
+ * point's covariance is I - 0.999 n n^T from the k-NN normals of both clouds (k = normal_k, the source's on the unmoved
+ * source), and each iteration minimises PCL's objective sum r^T (R C_s R^T + C_t)^-1 r / c for those pairs by up to 20
+ * Gauss-Newton steps (FP64 fixed-order sums, a step that raises the objective is undone) where PCL runs its BFGS.  The loop
+ * stops at max_iterations, or when no entry of the transform moved by more than rotation_epsilon (the 3 x 3 block) or
+ * transformation_epsilon (the translation) in the iteration (TRANSFORM), PCL's GICP criterion; fitness_epsilon is not read.
+ * Gauss-Newton has no damping: when the first step of an iteration raises the objective it is undone, the transform has not
+ * moved, and the call reports TRANSFORM (converged = 1) from where that iteration started, which the result alone does not
+ * tell apart from a real convergence (a damped or backtracking step is a possible follow-up).
+ * A singular system stops it with GHICP_ICP_SINGULAR, the transform as it was at the start of that iteration.  Unlike PCL's
+ * GICP, which ignores them, reciprocal and trim_ratio apply (gicp_reg passes them as off). */
 enum ghicp_icp_state {   /* PCL's DefaultConvergenceCriteria::ConvergenceState values, then SINGULAR */
   GHICP_ICP_ITERATIONS = 1,
-  GHICP_ICP_TRANSFORM = 2,
+  GHICP_ICP_TRANSFORM = 2,         /* metric 2: also when an iteration's first step was undone (see above) */
   GHICP_ICP_ABS_MSE = 3,
   GHICP_ICP_REL_MSE = 4,
   GHICP_ICP_NO_CORRESPONDENCES = 5,
-  GHICP_ICP_SINGULAR = 7           /* metric 1: 3 or more pairs but no solution (e.g. every normal parallel); F unchanged */
+  GHICP_ICP_SINGULAR = 7           /* metrics 1, 2: 3 or more pairs but no solution (e.g. every normal parallel); F unchanged */
 };
 typedef struct ghicp_icp_params {
   int max_iterations;              /* >= 1 (icp_reg's max_iter) */
   int reciprocal;                  /* setUseReciprocalCorrespondences */
   float trim_ratio;                /* CorrespondenceRejectorTrimmed::setOverlapRatio, 0 = no rejector, else (0, 1] */
   double transformation_epsilon;   /* >= 0; icp_reg: 1e-8 */
-  double fitness_epsilon;          /* >= 0; icp_reg: 1e-5 */
-  int metric;                      /* 0 = point-to-point (§3.13), 1 = point-to-plane (§3.14) */
-  int normal_k;                    /* metric 1: the target normals' k, 3..32 (ptplicp_reg's covariance_K); ignored by metric 0 */
-  int reserved[2];
+  double fitness_epsilon;          /* >= 0; icp_reg: 1e-5; not read by metric 2 */
+  int metric;                      /* 0 = point-to-point (§3.13), 1 = point-to-plane (§3.14), 2 = Generalized ICP (§3.15) */
+  int normal_k;                    /* metrics 1, 2: the normals' k, 3..32 (covariance_K); ignored by metric 0 */
+  double rotation_epsilon;         /* metric 2: finite, > 0 (gicp_reg: 1e-6); ignored by metrics 0 and 1 */
 } ghicp_icp_params;
 typedef struct ghicp_icp_result {
   double Rt[16];                   /* column-major: the float32 accumulated transform widened (the guess when no step ran) */
@@ -386,22 +398,24 @@ typedef struct ghicp_icp_result {
   double fitness;                  /* PCL's getFitnessScore: §3.12 fitness of the source moved by Rt, max_range = +inf */
   int iterations, converged, state, cor;          /* state: ghicp_icp_state; cor: the last iteration's kept pairs */
   long long cells_visited, candidates;            /* work of every nearest-neighbour query of every iteration */
-  float stage_ms[4];                              /* target grid (+ normals for metric 1; 0 when cached), iterations, fitness,
-                                                     total */
+  float stage_ms[4];                              /* target grid (+ the target's normals for metric 1, both clouds' for
+                                                     metric 2; 0 when all cached), iterations, fitness, total */
 } ghicp_icp_result;
 /* src_xyz [n_s][3], tgt_xyz [n_t][3] (host arrays); guess column-major (NULL = identity), rounded once to float32; moved [n_s][3]
  * (may be NULL) receives the source moved by Rt (PCL's align output); cor_trace / mse_trace [max_iterations] (may be NULL)
  * receive each iteration's kept pairs and mean squared distance (entries past `iterations` are left as they are).  Fewer than
- * 3 pairs returns GHICP_W_FEW_PAIRS, a singular point-to-plane system GHICP_W_SINGULAR, each with the result filled in
- * (converged = 0, Rt = the transform so far).  Argument errors (NULL, n <= 0, no finite source or target point,
- * max_iterations < 1, trim_ratio outside [0, 1] or NaN, a negative or NaN epsilon, a non-finite guess, a metric other than 0
- * or 1, metric 1 with normal_k outside 3..32, handles on different devices) return GHICP_E_ARG and write nothing; out of
- * memory returns GHICP_E_NOMEM and writes nothing. */
+ * 3 pairs returns GHICP_W_FEW_PAIRS, a singular point-to-plane or GICP system GHICP_W_SINGULAR, each with the result filled
+ * in (converged = 0, Rt = the transform so far).  Argument errors (NULL, n <= 0, no finite source or target point,
+ * max_iterations < 1, trim_ratio outside [0, 1] or NaN, a negative or NaN epsilon, a non-finite guess, a metric other than
+ * 0, 1 or 2, metric 1 or 2 with normal_k outside 3..32, metric 2 without a finite rotation_epsilon > 0, handles on different
+ * devices) return GHICP_E_ARG and write nothing; out of memory returns GHICP_E_NOMEM and writes nothing. */
 int ghicp_cloud_icp(int device, const float *src_xyz, int n_s, const float *tgt_xyz, int n_t, const double guess[16],
                     const ghicp_icp_params *p, ghicp_icp_result *out, float *moved, int *cor_trace, double *mse_trace);
 /* the down-sampled clouds of two pipeline results, device to device; the target's grid is the one ghicp_prep_overlap keeps
  * (built by whichever call comes first, stage_ms[0] = 0 when it already exists).  Metric 1 also keeps the target's normals
- * and their k there, under the same lock: a later call with the same normal_k reuses them, another k replaces them. */
+ * and their k there, under the same lock: a later call with the same normal_k reuses them, another k replaces them.  Metric
+ * 2 keeps both results' normals that way (each result holds one set, whichever metric or role asked for it) and takes both
+ * locks together, so that calls on (a, b) and (b, a) from two host threads cannot deadlock; source == target is allowed. */
 int ghicp_prep_icp(const ghicp_prep *source, const ghicp_prep *target, const double guess[16], const ghicp_icp_params *p,
                    ghicp_icp_result *out);
 

@@ -1,9 +1,10 @@
 """Stage times of point-to-point ICP on the dense clouds (ghicp_icp.cu, DESIGN.md §3.13) on the synthetic scan pairs
 (synth.scan_pair), down-sampled at 0.05 m on the device as tools/bench_overlap.py scores them.  --metric plane times
 point-to-plane ICP (§3.14) instead, with the target normals' k = --normal-k, and adds the one-time normal estimation
-(normals_ms: the first point-to-plane call's stage_ms["grid"], the target's grid being cached by then).
+(normals_ms: the first point-to-plane call's stage_ms["grid"], the target's grid being cached by then).  --metric gicp times
+Generalized ICP (§3.15), whose normals_ms covers both clouds' normals.
 
-    python tools/bench_icp.py [--points 1000000 5000000] [--reps 3] [--voxel 0.05] [--metric point|plane] [--normal-k 20]
+    python tools/bench_icp.py [--points 1000000 5000000] [--reps 3] [--voxel 0.05] [--metric point|plane|gicp] [--normal-k 20]
 
 Per scan size: the target grid build, then from the truth perturbed by 2 degrees / 0.5 m and from the truth itself, with and
 without reciprocal correspondences, with and without the trimmed rejector (ratio = calOverlap at the start within 0.3 m):
@@ -37,10 +38,10 @@ def main():
     ap.add_argument("--voxel", type=float, default=0.05)
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--max-iter", type=int, default=50)
-    ap.add_argument("--metric", choices=["point", "plane"], default="point")
+    ap.add_argument("--metric", choices=["point", "plane", "gicp"], default="point")
     ap.add_argument("--normal-k", type=int, default=20)
     args = ap.parse_args()
-    mkw = {} if args.metric == "point" else dict(metric="plane", normal_k=args.normal_k)
+    mkw = {} if args.metric == "point" else dict(metric=args.metric, normal_k=args.normal_k)
     import ghicp_b200 as g
     if g.device_count() <= 0:
         raise SystemExit("bench_icp.py: no CUDA device (the product has no CPU fallback)")
@@ -58,7 +59,7 @@ def main():
         run = dict(points=n, n_source_down=ps.n_down, n_target_down=pt.n_down, cases=[])
         try:
             run["grid_ms"] = ps.overlap(pt, None, thre_dis=0.3)["stage_ms"]["grid"]   # the first call on the target builds it
-            if mkw:   # the first point-to-plane call estimates the target's normals (the grid is cached by now)
+            if mkw:   # the first point-to-plane (GICP) call estimates the target's (both clouds') normals; the grid is cached
                 run["normals_ms"] = ps.icp(pt, None, max_iterations=1, **mkw)[1]["stage_ms"]["grid"]
             for start, G0 in (("2deg_0.5m", off @ G), ("truth", G)):
                 ov = [ps.overlap(pt, G0, thre_dis=0.3) for _ in range(args.reps + 1)][1:]
