@@ -1302,7 +1302,7 @@ static cudaError_t prep_run_stages(const float *xyz, int n, const ghicp_prep_par
   CUDA_TRY(cudaEventRecord(ev[1], 0));
   int n_down = 0, n_kp = 0, rounds = 0;
   CUDA_TRY(prep_voxel_downsample(0, d_xyz.get(), n, p->voxel_size, d_keep.get(), &n_down));
-  if (n_down <= 0) return cudaErrorInvalidValue;
+  if (n_down <= 0) { h->n_down = 0; return cudaSuccess; }   // no finite point: ghicp_prep_run refuses the cloud
   CUDA_TRY(h->d_down.alloc(3 * (size_t)n_down));
   CUDA_TRY(prep_gather_points(0, d_xyz.get(), d_keep.get(), n_down, h->d_down.get()));
   CUDA_TRY(cudaEventRecord(ev[2], 0));
@@ -1349,6 +1349,7 @@ int ghicp_prep_run(int device, const float *xyz, int n, const ghicp_prep_params 
   ghicp_prep *h = new ghicp_prep();
   h->device = device; h->n = n; h->side = side;
   if ((rc = cuda_status(prep_run_stages(xyz, n, p, bsc_pairs, want_bsc, h), "prep_run"))) { ghicp_prep_destroy(h); return rc; }
+  if (h->n_down <= 0) { ghicp_prep_destroy(h); set_error(nullptr, "prep_run: the cloud has no finite point"); return GHICP_E_ARG; }
   *out = h;
   return GHICP_OK;
 }

@@ -11,6 +11,8 @@ typedef unsigned long long pu64;
 __device__ __forceinline__ pu64 cell_key(int cx, int cy, int cz) { return ((pu64)cx << 42) | ((pu64)cy << 21) | (pu64)cz; }
 __device__ __forceinline__ int cell_coord(float v, float mn, float inv) { const int c = (int)floorf((v - mn) * inv); return c < 0 ? 0 : c; }
 inline int cell_coord_host(float v, float mn, float inv) { const float f = (v - mn) * inv; const int c = (int)floorf(f); return c < 0 ? 0 : c; }
+// Non-finite points take no part in the pre-processing (DESIGN.md §3.8): they bound no box, own no cell and find no neighbour.
+__host__ __device__ __forceinline__ bool finite3(float x, float y, float z) { return isfinite(x) && isfinite(y) && isfinite(z); }
 
 struct GridArgs {
   const float *xyz; const int *ids;      // point of position k = xyz[ids ? ids[k] : k]
@@ -74,7 +76,8 @@ struct GridBufs {   // the device arrays GridArgs points into
 struct PointGrid {
   GridArgs g{};
   int gx = 0, gy = 0, gz = 0;
-  float mx[3] = {0.f, 0.f, 0.f};         // bounding-box maximum (the minimum is g.mnx, g.mny, g.mnz)
+  float mx[3] = {0.f, 0.f, 0.f};         // maximum of the finite points' box (the minimum is g.mnx, g.mny, g.mnz)
+  int nfin = 0;                          // finite points
   double cell = 0.0, slack = 0.0;
   GridBufs buf;
 };

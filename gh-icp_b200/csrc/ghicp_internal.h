@@ -513,7 +513,7 @@ cudaError_t icp_run(const float *d_src, int n_src, const float *d_all, int n_all
 // glue of the device-resident pipeline (ghicp_prep_run)
 cudaError_t prep_gather_points(cudaStream_t st, const float *d_xyz, const int *d_idx, int m, float *d_out);
 cudaError_t prep_kp_coords(cudaStream_t st, const float *d_xyz, const int *d_kp, int nkp, double *d_soa);
-cudaError_t prep_bounds(cudaStream_t st, const float *d_xyz, int n, float mn[3], float mx[3]);
+cudaError_t prep_bounds(cudaStream_t st, const float *d_xyz, int n, float mn[3], float mx[3], int *nfin = nullptr);
 
 // ---- streaming path (ghicp_stream.cu) -----------------------------------------------------------
 cudaError_t launch_stream_prep(Ctx *c, const CostParams &cp, int for_km_gate);

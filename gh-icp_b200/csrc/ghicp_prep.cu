@@ -142,43 +142,53 @@ __device__ void sym3_eig_f32(const float c[6], float lam[3]) {
 }
 
 // ---- kernels ------------------------------------------------------------------------------------------------------------
-// bounding box of the points ids[k] (or all points when ids == nullptr): ordered-uint atomics, warp-reduced first
-__global__ void k_bbox(const float *__restrict__ xyz, const int *__restrict__ ids, int n, unsigned *__restrict__ mn,
-                       unsigned *__restrict__ mx) {
-  unsigned lo[3] = {0xffffffffu, 0xffffffffu, 0xffffffffu}, hi[3] = {0u, 0u, 0u};
+// bounding box of the finite points ids[k] (or of all points when ids == nullptr): ordered-uint atomics, warp-reduced
+// first.  box[6] counts the finite points, box[7] is the smallest k of a finite point.  Non-finite points are left out (f2ord
+// would order +NaN above +inf and make the maximum NaN).
+__global__ void k_bbox(const float *__restrict__ xyz, const int *__restrict__ ids, int n, unsigned *__restrict__ box) {
+  unsigned lo[3] = {0xffffffffu, 0xffffffffu, 0xffffffffu}, hi[3] = {0u, 0u, 0u}, cnt = 0u, first = 0xffffffffu;
   for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
     const float *p = xyz + 3 * (size_t)(ids ? ids[k] : k);
+    if (!finite3(p[0], p[1], p[2])) continue;
+    ++cnt; first = (unsigned)k < first ? (unsigned)k : first;
 #pragma unroll
     for (int a = 0; a < 3; ++a) { const unsigned u = f2ord(p[a]); lo[a] = u < lo[a] ? u : lo[a]; hi[a] = u > hi[a] ? u : hi[a]; }
   }
 #pragma unroll
-  for (int a = 0; a < 3; ++a) {
+  for (int o = 16; o > 0; o >>= 1) {
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
+    for (int a = 0; a < 3; ++a) {
       const unsigned l = __shfl_xor_sync(0xffffffffu, lo[a], o), h = __shfl_xor_sync(0xffffffffu, hi[a], o);
       lo[a] = l < lo[a] ? l : lo[a]; hi[a] = h > hi[a] ? h : hi[a];
     }
-    if ((threadIdx.x & 31) == 0) { atomicMin(&mn[a], lo[a]); atomicMax(&mx[a], hi[a]); }
+    const unsigned f = __shfl_xor_sync(0xffffffffu, first, o);
+    cnt += __shfl_xor_sync(0xffffffffu, cnt, o); first = f < first ? f : first;
+  }
+  if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+    for (int a = 0; a < 3; ++a) { atomicMin(&box[a], lo[a]); atomicMax(&box[3 + a], hi[a]); }
+    if (cnt) { atomicAdd(&box[6], cnt); atomicMin(&box[7], first); }
   }
 }
-// voxel id of every point, float32 arithmetic as include/filter.hpp:54-63
+// voxel id of every point, float32 arithmetic as include/filter.hpp:54-63; a non-finite point gets id 0
 __global__ void k_voxel_keys(const float *__restrict__ xyz, int n, float mnx, float mny, float mnz, float inv, pu64 mul_vx,
                              pu64 mul_vy, pu64 *__restrict__ keys, int *__restrict__ vals) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const pu64 vx = (pu64)floorf((xyz[3 * (size_t)i] - mnx) * inv);
-  const pu64 vy = (pu64)floorf((xyz[3 * (size_t)i + 1] - mny) * inv);
-  const pu64 vz = (pu64)floorf((xyz[3 * (size_t)i + 2] - mnz) * inv);
-  keys[i] = vx * mul_vx + vy * mul_vy + vz;
+  const float x = xyz[3 * (size_t)i], y = xyz[3 * (size_t)i + 1], z = xyz[3 * (size_t)i + 2];
   vals[i] = i;
+  if (!finite3(x, y, z)) { keys[i] = 0ull; return; }   // joins the voxel-0 run, which is never emitted
+  const pu64 vx = (pu64)floorf((x - mnx) * inv), vy = (pu64)floorf((y - mny) * inv), vz = (pu64)floorf((z - mnz) * inv);
+  keys[i] = vx * mul_vx + vy * mul_vy + vz;
 }
-// grid cell of the points ids[k] (or k): key + position k
+// grid cell of the points ids[k] (or k): key + position k; non-finite points share the last key
 __global__ void k_cell_keys(const float *__restrict__ xyz, const int *__restrict__ ids, int n, float mnx, float mny, float mnz,
                             float inv, pu64 *__restrict__ keys, int *__restrict__ vals) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
   const float *p = xyz + 3 * (size_t)(ids ? ids[k] : k);
-  keys[k] = cell_key(cell_coord(p[0], mnx, inv), cell_coord(p[1], mny, inv), cell_coord(p[2], mnz, inv));
+  keys[k] = finite3(p[0], p[1], p[2]) ? cell_key(cell_coord(p[0], mnx, inv), cell_coord(p[1], mny, inv), cell_coord(p[2], mnz, inv))
+                                      : ~0ull;   // after every cell a walk reads (no distance to it is < r2 anyway)
   vals[k] = k;
 }
 // heads of the runs of equal keys in a sorted array (flags[n] = 0 so that the scan yields the total)
@@ -189,12 +199,13 @@ __global__ void k_run_heads(const pu64 *__restrict__ keys, int n, int skip_zero_
   const bool head = i == 0 || keys[i] != keys[i - 1];
   flags[i] = (head && !(skip_zero_key && keys[i] == 0ull)) ? 1 : 0;
 }
-// voxel filter output: [point 0 (the reference's phantom voxel-0 entry)] + the first (smallest) index of every run
+// voxel filter output: [the first finite point (the reference's phantom voxel-0 entry)] + the first (smallest) index of
+// every run
 __global__ void k_voxel_emit(const int *__restrict__ vals, const int *__restrict__ flags, const int *__restrict__ pos, int n,
-                             int base, int *__restrict__ out) {
+                             int head, int *__restrict__ out) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i == 0 && base == 1) out[0] = 0;
-  if (i < n && flags[i]) out[base + pos[i]] = vals[i];
+  if (i == 0) out[0] = head;
+  if (i < n && flags[i]) out[1 + pos[i]] = vals[i];
 }
 // table of occupied cells: ucell[u] = key, cstart[u] = first position in the sorted order (cstart[nu] = n)
 __global__ void k_cell_table(const pu64 *__restrict__ keys, const int *__restrict__ flags, const int *__restrict__ pos, int n,
@@ -234,6 +245,10 @@ __global__ void k_pca(const GridArgs g, int n, float *__restrict__ lam, double *
   const GridRegs r = grid_regs(g);
   const int i = r.order[t];   // threads of a warp take points of the same cell: same 27 runs, loads broadcast instead of scattered
   const float qx = g.xyz[3 * (size_t)i], qy = g.xyz[3 * (size_t)i + 1], qz = g.xyz[3 * (size_t)i + 2];
+  if (!finite3(qx, qy, qz)) {   // no neighbour: the outputs of an empty neighbourhood, never a keypoint
+    pt_num[i] = 0; lam[3 * (size_t)i] = 0.f; lam[3 * (size_t)i + 1] = 0.f; lam[3 * (size_t)i + 2] = 0.f; curvature[i] = 0.0;
+    return;
+  }
   const int cx = cell_coord(qx, g.mnx, g.inv), cy = cell_coord(qy, g.mny, g.inv), cz = cell_coord(qz, g.mnz, g.inv);
   int cnt = 0;
   double sd[3] = {0, 0, 0}, sdd[6] = {0, 0, 0, 0, 0, 0};
@@ -350,18 +365,29 @@ __global__ void k_gather_sorted(const float *__restrict__ xyz, const int *__rest
 
 inline int blocks(int n) { return (n + PT - 1) / PT; }
 
+// Bounding box of the finite points ids[k] (k < n; all points when ids == nullptr), their number and the smallest such k
+// (n when none).  Without a finite point the box is the origin, so that every grid built on it stays defined.
+struct FiniteBox { float mn[3], mx[3]; int nfin, first; };
+cudaError_t finite_box(cudaStream_t st, const float *d_xyz, const int *d_ids, int n, FiniteBox *b) {
+  DevBuf<unsigned> d_box; unsigned h[8];
+  const unsigned init[8] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u, 0u, 0xffffffffu};
+  CUDA_TRY(d_box.alloc(8));
+  CUDA_TRY(cudaMemcpyAsync(d_box.get(), init, sizeof(init), cudaMemcpyHostToDevice, st));
+  GHICP_LAUNCH(k_bbox, n < GHICP_SMS * 8 * PT ? blocks(n) : GHICP_SMS * 8, PT, 0, st, d_xyz, d_ids, n, d_box.get());
+  CUDA_TRY(cudaMemcpyAsync(h, d_box.get(), sizeof(h), cudaMemcpyDeviceToHost, st)); CUDA_TRY(cudaStreamSynchronize(st));
+  b->nfin = (int)h[6]; b->first = b->nfin ? (int)h[7] : n;
+  for (int a = 0; a < 3; ++a) { b->mn[a] = b->nfin ? ord2f(h[a]) : 0.f; b->mx[a] = b->nfin ? ord2f(h[3 + a]) : 0.f; }
+  return cudaSuccess;
+}
+
 // uniform grid over the points ids[k] (k < n); *out receives the device arrays g points into
 cudaError_t build_grid(cudaStream_t st, const float *d_xyz, const int *d_ids, int n, float cell, GridArgs *g, GridBufs *out) {
-  DevBuf<unsigned> d_box; unsigned h_box[6];
   DevBuf<pu64> d_keys; DevBuf<int> d_flags, d_pos;
   GridBufs b;
+  FiniteBox box;
   int nu = 0;
-  CUDA_TRY(d_box.alloc(6));
-  const unsigned init[6] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u};
-  CUDA_TRY(cudaMemcpyAsync(d_box.get(), init, sizeof(init), cudaMemcpyHostToDevice, st));
-  GHICP_LAUNCH(k_bbox, n < GHICP_SMS * 8 * PT ? blocks(n) : GHICP_SMS * 8, PT, 0, st, d_xyz, d_ids, n, d_box.get(), d_box.get() + 3);
-  CUDA_TRY(cudaMemcpyAsync(h_box, d_box.get(), sizeof(h_box), cudaMemcpyDeviceToHost, st)); CUDA_TRY(cudaStreamSynchronize(st));
-  g->mnx = ord2f(h_box[0]); g->mny = ord2f(h_box[1]); g->mnz = ord2f(h_box[2]);
+  CUDA_TRY(finite_box(st, d_xyz, d_ids, n, &box));
+  g->mnx = box.mn[0]; g->mny = box.mn[1]; g->mnz = box.mn[2];
   g->inv = 1.0f / cell; g->r2 = cell * cell;
   CUDA_TRY(d_keys.alloc((size_t)n)); CUDA_TRY(b.order.alloc((size_t)n)); CUDA_TRY(d_flags.alloc((size_t)n + 1)); CUDA_TRY(d_pos.alloc((size_t)n + 1));
   GHICP_LAUNCH(k_cell_keys, blocks(n), PT, 0, st, d_xyz, d_ids, n, g->mnx, g->mny, g->mnz, g->inv, d_keys.get(), b.order.get());
@@ -383,16 +409,13 @@ cudaError_t build_grid(cudaStream_t st, const float *d_xyz, const int *d_ids, in
 
 // CFilter::voxelfilter on device arrays: d_out (capacity n + 1) receives the kept indices in output order
 cudaError_t prep_voxel_downsample(cudaStream_t st, const float *d_xyz, int n, float voxel_size, int *d_out, int *n_out) {
-  DevBuf<unsigned> d_box; unsigned h_box[6];
   DevBuf<pu64> d_keys; DevBuf<int> d_vals, d_flags, d_pos;
+  FiniteBox box;
   *n_out = 0;
   if (n <= 0) return cudaSuccess;
-  CUDA_TRY(d_box.alloc(6));
-  const unsigned init[6] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u};
-  CUDA_TRY(cudaMemcpyAsync(d_box.get(), init, sizeof(init), cudaMemcpyHostToDevice, st));
-  GHICP_LAUNCH(k_bbox, n < GHICP_SMS * 8 * PT ? blocks(n) : GHICP_SMS * 8, PT, 0, st, d_xyz, (const int *)nullptr, n, d_box.get(), d_box.get() + 3);
-  CUDA_TRY(cudaMemcpyAsync(h_box, d_box.get(), sizeof(h_box), cudaMemcpyDeviceToHost, st)); CUDA_TRY(cudaStreamSynchronize(st));
-  const float mn[3] = {ord2f(h_box[0]), ord2f(h_box[1]), ord2f(h_box[2])}, mx[3] = {ord2f(h_box[3]), ord2f(h_box[4]), ord2f(h_box[5])};
+  CUDA_TRY(finite_box(st, d_xyz, nullptr, n, &box));   // pcl::removeNaNFromPointCloud, then pcl::getMinMax3D
+  if (box.nfin == 0) return cudaSuccess;
+  const float *mn = box.mn, *mx = box.mx;
   const float inv = 1.0f / voxel_size;                                   // include/filter.hpp:30
   const float gy = mx[1] - mn[1], gz = mx[2] - mn[2];                    // :36
   const pu64 max_vy = (pu64)(ceilf(gy * inv) + 1), max_vz = (pu64)(ceilf(gz * inv) + 1);   // :39-40
@@ -400,12 +423,13 @@ cudaError_t prep_voxel_downsample(cudaStream_t st, const float *d_xyz, int n, fl
   CUDA_TRY(d_keys.alloc((size_t)n)); CUDA_TRY(d_vals.alloc((size_t)n)); CUDA_TRY(d_flags.alloc((size_t)n + 1)); CUDA_TRY(d_pos.alloc((size_t)n + 1));
   GHICP_LAUNCH(k_voxel_keys, blocks(n), PT, 0, st, d_xyz, n, mn[0], mn[1], mn[2], inv, mul_vx, mul_vy, d_keys.get(), d_vals.get());
   CUDA_TRY(sort_pairs(d_keys.get(), d_vals.get(), n, st));          // stable: ascending index inside a voxel
-  // the reference's phantom entries {voxel 0, index 0} (:52) put point 0 first and absorb the real voxel-0 run
+  // the reference's phantom entries {voxel 0, index 0} (:52) put point 0 of the finite cloud first and absorb the real voxel-0
+  // run (and the non-finite points)
   GHICP_LAUNCH(k_run_heads, blocks(n + 1), PT, 0, st, d_keys.get(), n, 1, d_flags.get());
   CUDA_TRY(exclusive_scan(d_flags.get(), d_pos.get(), n, st));
   int runs = 0;
   CUDA_TRY(cudaMemcpyAsync(&runs, d_pos.get() + n, sizeof(int), cudaMemcpyDeviceToHost, st)); CUDA_TRY(cudaStreamSynchronize(st));
-  GHICP_LAUNCH(k_voxel_emit, blocks(n), PT, 0, st, d_vals.get(), d_flags.get(), d_pos.get(), n, 1, d_out);
+  GHICP_LAUNCH(k_voxel_emit, blocks(n), PT, 0, st, d_vals.get(), d_flags.get(), d_pos.get(), n, box.first, d_out);
   CUDA_TRY(cudaStreamSynchronize(st));
   *n_out = runs + 1;
   return cudaSuccess;
@@ -482,16 +506,14 @@ cudaError_t prep_kp_coords(cudaStream_t st, const float *d_xyz, const int *d_kp,
   GHICP_LAUNCH(k_kp_coords, blocks(nkp), PT, 0, st, d_xyz, d_kp, nkp, d_soa);
   return cudaSuccess;
 }
-// pcl::getMinMax3D of a device cloud (the bounding box the driver takes its bbx_magnitude from, test/ghicp_main.cpp:91-93)
-cudaError_t prep_bounds(cudaStream_t st, const float *d_xyz, int n, float mn[3], float mx[3]) {
-  DevBuf<unsigned> d_box; unsigned h_box[6];
+// pcl::getMinMax3D of the finite points of a device cloud (the bounding box the driver takes its bbx_magnitude from,
+// test/ghicp_main.cpp:91-93); *nfin (may be null) receives their number
+cudaError_t prep_bounds(cudaStream_t st, const float *d_xyz, int n, float mn[3], float mx[3], int *nfin) {
+  FiniteBox box;
   if (n <= 0) return cudaErrorInvalidValue;
-  CUDA_TRY(d_box.alloc(6));
-  const unsigned init[6] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u};
-  CUDA_TRY(cudaMemcpyAsync(d_box.get(), init, sizeof(init), cudaMemcpyHostToDevice, st));
-  GHICP_LAUNCH(k_bbox, n < GHICP_SMS * 8 * PT ? blocks(n) : GHICP_SMS * 8, PT, 0, st, d_xyz, (const int *)nullptr, n, d_box.get(), d_box.get() + 3);
-  CUDA_TRY(cudaMemcpyAsync(h_box, d_box.get(), sizeof(h_box), cudaMemcpyDeviceToHost, st)); CUDA_TRY(cudaStreamSynchronize(st));
-  for (int a = 0; a < 3; ++a) { mn[a] = ord2f(h_box[a]); mx[a] = ord2f(h_box[3 + a]); }
+  CUDA_TRY(finite_box(st, d_xyz, nullptr, n, &box));
+  for (int a = 0; a < 3; ++a) { mn[a] = box.mn[a]; mx[a] = box.mx[a]; }
+  if (nfin) *nfin = box.nfin;
   return cudaSuccess;
 }
 
@@ -611,8 +633,8 @@ __global__ void __launch_bounds__(BSC_T) k_bsc(const BscArgs a) {
   const float qx = g.xyz[3 * (size_t)p], qy = g.xyz[3 * (size_t)p + 1], qz = g.xyz[3 * (size_t)p + 2];
   if (tid < BSC_RUNS) {   // one contiguous run of the sorted points per grid column (x, y): its cells z - 1 .. z + 1
     const int cx = cell_coord(qx, g.mnx, g.inv) + tid / 3 - 1, cy = cell_coord(qy, g.mny, g.inv) + tid % 3 - 1;
-    int lo = 0, hi = 0;
-    if (cx >= 0 && cy >= 0) column_run(g, cx, cy, cell_coord(qz, g.mnz, g.inv), lo, hi);
+    int lo = 0, hi = 0;   // a non-finite keypoint walks nothing: fewer than 3 neighbours below
+    if (cx >= 0 && cy >= 0 && finite3(qx, qy, qz)) column_run(g, cx, cy, cell_coord(qz, g.mnz, g.inv), lo, hi);
     s_lo[tid] = lo; s_pre[tid + 1] = hi - lo;
   }
   for (int c = tid; c < cells; c += BSC_T) { s_num_lo[c] = 0u; s_num_hi[c] = 0u; s_dep_lo[c] = 0u; s_dep_hi[c] = 0u; }
@@ -898,52 +920,56 @@ __global__ void k_knn(const KnnArgs a) {
     const GridRegs r = grid_regs(a.g);   // per-thread registers, see k_pca
     const int i = r.order[t];            // threads of a warp take points of the same cell (see k_pca)
     const float qx = a.g.xyz[3 * (size_t)i], qy = a.g.xyz[3 * (size_t)i + 1], qz = a.g.xyz[3 * (size_t)i + 2];
-    const int cx = cell_coord(qx, a.g.mnx, a.g.inv), cy = cell_coord(qy, a.g.mny, a.g.inv), cz = cell_coord(qz, a.g.mnz, a.g.inv);
     const int k = a.k, gx = a.gx, gy = a.gy, gz = a.gz;
-    pu64 key[FPFH_KMAX];
-#pragma unroll
-    for (int j = 0; j < FPFH_KMAX; ++j) key[j] = (j < FPFH_KMAX - k) ? 0ull : ~0ull;
-    long long cand = 0;
-    int rmax = cx;                       // the ring that reaches the far side of the grid on every axis
-    rmax = max(rmax, gx - cx); rmax = max(rmax, cy); rmax = max(rmax, gy - cy); rmax = max(rmax, cz); rmax = max(rmax, gz - cz);
-    bool done = false;
-    for (int ring = 0; ring <= FPFH_RING_CAP && !done; ++ring) {
-      for (int dx = -ring; dx <= ring; ++dx) {
-        const int x = cx + dx;
-        if (x < 0 || x > gx) continue;
-        for (int dy = -ring; dy <= ring; ++dy) {
-          const int y = cy + dy;
-          if (y < 0 || y > gy) continue;
-          if (max(abs(dx), abs(dy)) == ring) {   // a column on the ring's wall: its whole z-range
-            const int zlo = max(cz - ring, 0), zhi = min(cz + ring, gz);
-            if (zlo <= zhi) knn_column(r, x, y, zlo, zhi, qx, qy, qz, key, cand);
-          } else {                               // inside the wall: the floor and the ceiling cell
-            if (cz - ring >= 0) knn_column(r, x, y, cz - ring, cz - ring, qx, qy, qz, key, cand);
-            if (cz + ring <= gz) knn_column(r, x, y, cz + ring, cz + ring, qx, qy, qz, key, cand);
-          }
-        }
-      }
-      if (ring >= rmax) { done = true; break; }
-      // every point of an unvisited cell lies at least (ring - slack) cell edges away on some axis
-      const double lb = ((double)ring - a.slack) * a.cell;
-      if (lb > 0.0 && key[FPFH_KMAX - 1] != ~0ull && (double)knn_key_d2(key[FPFH_KMAX - 1]) < lb * lb * (1.0 - 1e-5)) done = true;
-    }
-    if (!done) {   // far outlier (or a grid too fine for this cloud): exact by exhaustion
+    if (!finite3(qx, qy, qz)) {   // a non-finite point's list is itself at distance 0: an isolated point's zero histogram
+      for (int j = 0; j < k; ++j) { a.nb_idx[(size_t)i * k + j] = i; a.nb_d2[(size_t)i * k + j] = 0.f; }
+    } else {
+      const int cx = cell_coord(qx, a.g.mnx, a.g.inv), cy = cell_coord(qy, a.g.mny, a.g.inv), cz = cell_coord(qz, a.g.mnz, a.g.inv);
+      pu64 key[FPFH_KMAX];
 #pragma unroll
       for (int j = 0; j < FPFH_KMAX; ++j) key[j] = (j < FPFH_KMAX - k) ? 0ull : ~0ull;
-      for (int s = 0; s < a.n; ++s) knn_insert(key, knn_key(knn_d2(qx, qy, qz, r.sorted[s]), r.order[s]));
-      cand += a.n;
-      atomicAdd(&s_fb, 1);
-    }
-#pragma unroll
-    for (int j = 0; j < FPFH_KMAX; ++j) {
-      const int jj = j - (FPFH_KMAX - k);
-      if (jj >= 0) {
-        a.nb_idx[(size_t)i * k + jj] = (int)(unsigned)key[j];
-        a.nb_d2[(size_t)i * k + jj] = knn_key_d2(key[j]);
+      long long cand = 0;
+      int rmax = cx;                       // the ring that reaches the far side of the grid on every axis
+      rmax = max(rmax, gx - cx); rmax = max(rmax, cy); rmax = max(rmax, gy - cy); rmax = max(rmax, cz); rmax = max(rmax, gz - cz);
+      bool done = false;
+      for (int ring = 0; ring <= FPFH_RING_CAP && !done; ++ring) {
+        for (int dx = -ring; dx <= ring; ++dx) {
+          const int x = cx + dx;
+          if (x < 0 || x > gx) continue;
+          for (int dy = -ring; dy <= ring; ++dy) {
+            const int y = cy + dy;
+            if (y < 0 || y > gy) continue;
+            if (max(abs(dx), abs(dy)) == ring) {   // a column on the ring's wall: its whole z-range
+              const int zlo = max(cz - ring, 0), zhi = min(cz + ring, gz);
+              if (zlo <= zhi) knn_column(r, x, y, zlo, zhi, qx, qy, qz, key, cand);
+            } else {                               // inside the wall: the floor and the ceiling cell
+              if (cz - ring >= 0) knn_column(r, x, y, cz - ring, cz - ring, qx, qy, qz, key, cand);
+              if (cz + ring <= gz) knn_column(r, x, y, cz + ring, cz + ring, qx, qy, qz, key, cand);
+            }
+          }
+        }
+        if (ring >= rmax) { done = true; break; }
+        // every point of an unvisited cell lies at least (ring - slack) cell edges away on some axis
+        const double lb = ((double)ring - a.slack) * a.cell;
+        if (lb > 0.0 && key[FPFH_KMAX - 1] != ~0ull && (double)knn_key_d2(key[FPFH_KMAX - 1]) < lb * lb * (1.0 - 1e-5)) done = true;
       }
+      if (!done) {   // far outlier (or a grid too fine for this cloud): exact by exhaustion
+#pragma unroll
+        for (int j = 0; j < FPFH_KMAX; ++j) key[j] = (j < FPFH_KMAX - k) ? 0ull : ~0ull;
+        for (int s = 0; s < a.n; ++s) knn_insert(key, knn_key(knn_d2(qx, qy, qz, r.sorted[s]), r.order[s]));
+        cand += a.n;
+        atomicAdd(&s_fb, 1);
+      }
+#pragma unroll
+      for (int j = 0; j < FPFH_KMAX; ++j) {
+        const int jj = j - (FPFH_KMAX - k);
+        if (jj >= 0) {
+          a.nb_idx[(size_t)i * k + jj] = (int)(unsigned)key[j];
+          a.nb_d2[(size_t)i * k + jj] = knn_key_d2(key[j]);
+        }
+      }
+      atomicAdd(&s_cand, (unsigned long long)cand);
     }
-    atomicAdd(&s_cand, (unsigned long long)cand);
   }
   __syncthreads();
   if (threadIdx.x == 0) { atomicAdd(a.cand, s_cand); atomicAdd(a.fallbacks, s_fb); }
@@ -968,13 +994,15 @@ struct CsrLists {
   __device__ __forceinline__ float dist2(size_t e) const { return knn_key_d2(key[e]); }
 };
 
-// NormalEstimation::computePointNormal + flipNormalTowardsViewpoint (viewpoint 0) of point i over its list
+// NormalEstimation::computePointNormal + flipNormalTowardsViewpoint (viewpoint 0) of point i over its list; a non-finite point
+// (whose list is not read) or one with fewer than 3 neighbours gets a NaN normal and status 1
 template <class L>
 __device__ __forceinline__ void est_normal(const float *__restrict__ xyz, int i, const L &l, float *__restrict__ nrm,
                                            int *__restrict__ status) {
-  const int k = l.count((size_t)i);
-  const size_t b = l.first((size_t)i);
   const float qx = xyz[3 * (size_t)i], qy = xyz[3 * (size_t)i + 1], qz = xyz[3 * (size_t)i + 2];
+  const bool fin = finite3(qx, qy, qz);
+  const int k = fin ? l.count((size_t)i) : 0;
+  const size_t b = fin ? l.first((size_t)i) : 0;
   if (k < 3) {
     const float nan = __uint_as_float(0x7fc00000u);
     nrm[3 * (size_t)i] = nan; nrm[3 * (size_t)i + 1] = nan; nrm[3 * (size_t)i + 2] = nan;
@@ -1136,9 +1164,10 @@ struct RadWalk {
   int rings; float r2;
 };
 
-// calls f(sorted position, d2) for every point of N_r(q) in walk order (not sorted)
+// calls f(sorted position, d2) for every point of N_r(q) in walk order (not sorted); N_r of a non-finite q is empty
 template <class F>
 __device__ __forceinline__ void rad_walk(const GridRegs &r, const RadWalk &w, float qx, float qy, float qz, F &&f) {
+  if (!finite3(qx, qy, qz)) return;
   const int cx = cell_coord(qx, w.g.mnx, w.g.inv), cy = cell_coord(qy, w.g.mny, w.g.inv), cz = cell_coord(qz, w.g.mnz, w.g.inv);
   const int R = w.rings, zlo = max(cz - R, 0), zhi = cz + R;
   for (int x = max(cx - R, 0); x <= cx + R; ++x)
@@ -1151,13 +1180,15 @@ __device__ __forceinline__ void rad_walk(const GridRegs &r, const RadWalk &w, fl
     }
 }
 
-// need[q] = 1 for every q in N_r(idx[t]) (the points whose SPFH the requested histograms read)
+// need[q] = 1 for every q in N_r(idx[t]) (the points whose SPFH the requested histograms read) and for idx[t] itself, which
+// gives every requested point a list row (an empty one when it is not finite; a finite point is in its own N_r anyway)
 __global__ void k_rad_mark(const RadWalk w, const int *__restrict__ idx, int nidx, int *__restrict__ need) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= nidx) return;
   GridRegs r = grid_regs(w.g);   // per-thread registers, see k_pca
   r.r2 = w.r2;
   const float *q = w.g.xyz + 3 * (size_t)idx[t];
+  need[idx[t]] = 1;
   rad_walk(r, w, q[0], q[1], q[2], [&](int s, float) { need[r.order[s]] = 1; });
 }
 // need[q] = 1 for every entry of the lists of rows [0, m)
@@ -1202,11 +1233,15 @@ __global__ void k_rad_fill(const RadWalk w, const int *__restrict__ rows, int m,
   pu64 *out = key + off[t];
   rad_walk(r, w, q[0], q[1], q[2], [&](int s, float d2) { *out++ = knn_key(d2, r.order[s]); });
 }
-// normals of every point: over its N_rn list where one was built (row_of >= 0), NaN with status 2 elsewhere
+// normals of every point: over its N_rn list where one was built (row_of >= 0), NaN with status 1 at a non-finite point, NaN
+// with status 2 elsewhere
 __global__ void k_rad_normals(const float *__restrict__ xyz, int n, const CsrLists l, float *__restrict__ nrm, int *__restrict__ status) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  if (l.row[i] >= 0) { est_normal(xyz, i, l, nrm, status); return; }
+  if (l.row[i] >= 0 || !finite3(xyz[3 * (size_t)i], xyz[3 * (size_t)i + 1], xyz[3 * (size_t)i + 2])) {
+    est_normal(xyz, i, l, nrm, status);
+    return;
+  }
   const float nan = __uint_as_float(0x7fc00000u);
   nrm[3 * (size_t)i] = nan; nrm[3 * (size_t)i + 1] = nan; nrm[3 * (size_t)i + 2] = nan;
   if (status) status[i] = 2;
@@ -1282,7 +1317,7 @@ cudaError_t prep_point_grid(cudaStream_t st, const float *d_xyz, int n, int ke, 
   float mn[3], mx[3];
   *out = PointGrid();
   if (n <= 0 || ke <= 0) return cudaErrorInvalidValue;
-  CUDA_TRY(prep_bounds(st, d_xyz, n, mn, mx));
+  CUDA_TRY(prep_bounds(st, d_xyz, n, mn, mx, &out->nfin));
   // Cell edge from the data: a volume guess (k points per cell if the cloud filled its box), then corrected once by the
   // observed mean occupancy of the occupied cells assuming a surface (occupancy ~ edge^2), aiming at 0.4 k per cell —
   // enough for the k nearest to lie within one ring.  The results do not depend on it; the work per query does.
@@ -1315,15 +1350,18 @@ cudaError_t prep_point_grid(cudaStream_t st, const float *d_xyz, int n, int ke, 
 cudaError_t prep_sort_pairs(cudaStream_t st, pu64 *keys, int *vals, int n) { return sort_pairs(keys, vals, n, st); }
 
 // FPFH histograms at d_idx [nidx] (all points when d_idx == nullptr) of the cloud d_xyz [n][3]; d_normals [n][3] receives
-// every point's normal, d_status [n] (may be null) 1 where fewer than 3 neighbours exist, d_nb_idx / d_nb_d2 [n][min(k, n)]
-// (may be null) the k-NN lists.  ev_mid (may be null) is recorded between the k-NN + normals and the SPFH + FPFH stages.
+// every point's normal, d_status [n] (may be null) 1 where fewer than 3 neighbours exist or the point is not finite,
+// d_nb_idx / d_nb_d2 [n][k_eff] (may be null) the k-NN lists, k_eff = min(k, the number of finite points).  ev_mid (may be null) is recorded between the k-NN + normals and the SPFH + FPFH stages.
 // cell_scale multiplies the data-derived cell edge (test hook).
 namespace {
-// The k-NN stage of the FPFH estimator: the grid, the k_eff-NN lists of every point (nb_idx / nb_d2 [n][ke]) and their work
-// counters (cand, fb), all allocated before the first launch; then k_knn and k_normals.
-cudaError_t knn_normals(cudaStream_t st, const float *d_xyz, int n, int ke, float cell_scale, PointGrid *pg, DevBuf<int> *nb_idx,
-                        DevBuf<float> *nb_d2, DevBuf<pu64> *cand, DevBuf<int> *fb, float *d_normals, int *d_status) {
-  CUDA_TRY(prep_point_grid(st, d_xyz, n, ke, cell_scale, 0.0, pg));
+// The k-NN stage of the FPFH estimator: the grid, the k_eff-NN lists of every point (nb_idx / nb_d2 [n][*ke]) and their work
+// counters (cand, fb), all allocated before the first launch; then k_knn and k_normals.  k_eff = min(k, finite points): the
+// lists of the finite points hold finite points only.
+cudaError_t knn_normals(cudaStream_t st, const float *d_xyz, int n, int k, float cell_scale, PointGrid *pg, DevBuf<int> *nb_idx,
+                        DevBuf<float> *nb_d2, DevBuf<pu64> *cand, DevBuf<int> *fb, float *d_normals, int *d_status, int *ke_out) {
+  CUDA_TRY(prep_point_grid(st, d_xyz, n, k < n ? k : n, cell_scale, 0.0, pg));
+  const int ke = k < pg->nfin ? k : pg->nfin;
+  *ke_out = ke;
   KnnArgs a{};
   a.g = pg->g; a.n = n; a.k = ke;
   a.gx = pg->gx; a.gy = pg->gy; a.gz = pg->gz;
@@ -1349,8 +1387,9 @@ __global__ void k_check_normals(float *__restrict__ nrm, int n) {
 cudaError_t prep_knn_normals(cudaStream_t st, const float *d_xyz, int n, int k, float *d_normals) {
   PointGrid pg;
   DevBuf<int> nb_idx, d_fb; DevBuf<float> nb_d2; DevBuf<pu64> d_cand;
+  int ke = 0;
   if (n <= 0 || k < 3 || k > FPFH_KMAX) return cudaErrorInvalidValue;
-  CUDA_TRY(knn_normals(st, d_xyz, n, k < n ? k : n, 0.f, &pg, &nb_idx, &nb_d2, &d_cand, &d_fb, d_normals, nullptr));
+  CUDA_TRY(knn_normals(st, d_xyz, n, k, 0.f, &pg, &nb_idx, &nb_d2, &d_cand, &d_fb, d_normals, nullptr, &ke));
   GHICP_LAUNCH(k_check_normals, blocks(n), PT, 0, st, d_normals, n);
   return cudaGetLastError();
 }
@@ -1362,8 +1401,8 @@ cudaError_t prep_fpfh(cudaStream_t st, const float *d_xyz, int n, const int *d_i
   DevBuf<int> nb_idx, need, d_fb; DevBuf<float> nb_d2, spfh; DevBuf<pu64> d_cand;
   if (stats) *stats = FpfhStats{};
   if (n <= 0 || k < 3 || k > FPFH_KMAX) return cudaErrorInvalidValue;
-  const int ke = k < n ? k : n;
-  CUDA_TRY(knn_normals(st, d_xyz, n, ke, cell_scale, &pg, &nb_idx, &nb_d2, &d_cand, &d_fb, d_normals, d_status));
+  int ke = 0;
+  CUDA_TRY(knn_normals(st, d_xyz, n, k, cell_scale, &pg, &nb_idx, &nb_d2, &d_cand, &d_fb, d_normals, d_status, &ke));
   if (d_nb_idx) CUDA_TRY(cudaMemcpyAsync(d_nb_idx, nb_idx.get(), sizeof(int) * (size_t)n * ke, cudaMemcpyDeviceToDevice, st));
   if (d_nb_d2) CUDA_TRY(cudaMemcpyAsync(d_nb_d2, nb_d2.get(), sizeof(float) * (size_t)n * ke, cudaMemcpyDeviceToDevice, st));
   if (ev_mid) CUDA_TRY(cudaEventRecord(ev_mid, st));

@@ -193,15 +193,19 @@ int ghicp_rigid_fit_ex(int device, int solver, const double *s, const double *t,
 /* ---- pre-processing on the GPU (SURVEY.md §8f row N1; BASELINE.json configs 4 / 5) ------------------------------
  * The steps of test/ghicp_main.cpp:86-100 that produce the keypoints the loop consumes.  xyz = [n][3] float32 (PCL
  * points are float32).  Where the reference's result is implementation-defined (unstable std::sort) or delegated to PCL,
- * the canonical definitions documented in oracle/ghicp_prep_oracle.cpp apply. */
+ * the canonical definitions documented in oracle/ghicp_prep_oracle.cpp apply.
+ * Non-finite points (NaN or infinite in any coordinate, as in an organised scan) take no part in any pre-processing entry
+ * point: each returns what it returns on the cloud's finite points, indices mapped back to xyz (pcl::removeNaNFromPointCloud,
+ * then the reference).  What that means per entry point is stated with it. */
 /* CFilter::voxelfilter (include/filter.hpp:28-88): one point per occupied voxel — the one with the smallest index — in
- * ascending voxel-id order, preceded by point 0 (the reference's phantom voxel-0 entries, :52 + :66).
- * out_idx: capacity n + 1. */
+ * ascending voxel-id order, preceded by point 0 (the reference's phantom voxel-0 entries, :52 + :66).  A non-finite point is
+ * never emitted; the phantom entry is the first finite point; without a finite point *n_out = 0.  out_idx: capacity n + 1. */
 int ghicp_voxel_downsample(int device, const float *xyz, int n, float voxel_size, int *out_idx, int *n_out);
 /* CKeypointDetect::keypointDetectionBasedOnCurvature (include/keypoint_detect.hpp:27-51): radius PCA of every point
  * (include/pca.h:133-250), pruneUnstablePoints (:132-147, ratio_max = 0.65 and min_pts = 20 in ghicp_main.cpp:96-97),
  * non-maximum suppression by curvature (:149-191).  kp_idx (capacity n): keypoint indices in the reference's output order
- * (descending curvature).  lam [n][3] (eigenvalues, descending), curvature [n], pt_num [n] may be NULL. */
+ * (descending curvature).  lam [n][3] (eigenvalues, descending), curvature [n], pt_num [n] may be NULL.  A non-finite point
+ * has lam = 0, curvature = 0, pt_num = 0, is nobody's neighbour and is never a keypoint. */
 int ghicp_detect_keypoints(int device, const float *xyz, int n, float radius, float ratio_max, int min_pts, float nms_radius,
                            int *kp_idx, int *n_kp, float *lam, double *curvature, int *pt_num);
 
@@ -213,7 +217,8 @@ int ghicp_detect_keypoints(int device, const float *xyz, int n, float radius, fl
  * xyz [n][3] float32; kp_idx [nkp] indices into xyz; pairs [side^2][2] = the sampling pattern (sample_pattern.txt of the
  * reference, :107-116; ghicp_bsc_default_pattern for side 7).  features = [V][nkp][ceil(9 side^2 / 8)] bytes, V = 1
  * (dof_type 0), 2 (1..4) or 4 (> 4) — the layout ghicp_set_bsc takes.  lrf [nkp][12] (x, y, z axis, origin of variant 0)
- * and status [nkp] (0 ok, 1 = fewer than 3 neighbours: descriptor zero) may be NULL.  voxel_side_num <= 9.
+ * and status [nkp] (0 ok, 1 = fewer than 3 neighbours or a non-finite keypoint: descriptor zero) may be NULL.  Non-finite
+ * points are nobody's neighbour.  voxel_side_num <= 9.
  * Eigenvector signs (Eigen::EigenSolver's are implementation-defined) follow "largest component positive"; see DESIGN.md
  * §3.9 for the float32 accumulation tolerance against the reference. */
 int ghicp_bsc_extract(int device, const float *xyz, int n, const int *kp_idx, int nkp, float extract_radius, int voxel_side_num,
@@ -225,7 +230,10 @@ int ghicp_bsc_default_pattern(int voxel_side_num, int *pairs);
  * The reference's driver runs, per cloud, voxel filter -> curvature keypoints -> BSC encoder (test/ghicp_main.cpp:89-116)
  * and hands the keypoint coordinates + descriptors to GHRegistration (:143-151).  ghicp_prep_run uploads the raw cloud ONCE
  * and chains the three stages on the device (each stage = the stand-alone entry point above, same results bit for bit);
- * nothing but the keypoint set ever needs to come back, and ghicp_set_from_prep moves even that device to device.
+ * nothing but the keypoint set ever needs to come back, and ghicp_set_from_prep moves even that device to device.  A cloud
+ * with non-finite points gives bit for bit what its finite points give: n_down, the down-sampled cloud, keypoints, the
+ * bounding box, BSC and FPFH (the down-sampled cloud holds finite points only).  A cloud without a finite point (or n <= 0)
+ * leaves nothing to register: ghicp_prep_run returns GHICP_E_ARG and *out stays NULL.
  * stage_ms [5] = {host->device copy, voxel filter, keypoints, BSC encoder, total} from CUDA events. */
 typedef struct ghicp_prep_params {
   float voxel_size;           /* CFilter::voxelfilter resolution (:89-90) */
@@ -256,7 +264,8 @@ int ghicp_set_from_prep(ghicp_ctx *ctx, const ghicp_prep *source, const ghicp_pr
  * k-NN in ascending (distance, index) order, smallest-eigenvector normals flipped towards the origin, 3 x 11 bin SPFH, the
  * 1 / d^2 weighted FPFH without the point's own SPFH).  xyz [n][3] float32; idx [nidx] = the points whose histograms are
  * wanted (NULL: every point, nidx ignored); k in 3..32 (the reference uses 20); fpfh [nidx][33].  normals [n][3] (NaN
- * where status = 1, i.e. fewer than 3 points in the cloud) and status [n] may be NULL.  The histogram at a point depends
+ * where status = 1, i.e. fewer than 3 finite points in the cloud or a non-finite point) and status [n] may be NULL.
+ * Non-finite points are nobody's neighbour (k_eff = min(k, finite points)); their own histogram row is zero.  The histogram at a point depends
  * only on its neighbours, so a subset equals the same rows of the whole-cloud result. */
 int ghicp_fpfh_extract(int device, const float *xyz, int n, const int *idx, int nidx, int k, float *fpfh, float *normals,
                        int *status);
@@ -272,7 +281,8 @@ int ghicp_prep_fpfh_stats(const ghicp_prep *h, long long *candidates, int *queri
  * setRadiusSearch) computes it (DESIGN.md §3.10, "Radius neighbourhoods"): N_r(p) = every point q with d2(p, q) < r*r (float32,
  * the query and its duplicates included) in ascending (d2, index) order; normals over N_normal_radius (NaN, status 1, with
  * fewer than 3 points), SPFH and FPFH over N_feature_radius.  Arguments and outputs as ghicp_fpfh_extract; with idx given,
- * only what those histograms read is computed and the other normals are NaN with status 2.  Radii must be positive and
+ * only what those histograms read is computed and the other normals are NaN with status 2.  A non-finite point is nobody's
+ * neighbour and has a NaN normal, status 1 and a zero histogram row.  Radii must be positive and
  * finite (GHICP_E_ARG).  The neighbour lists live in device memory: when they would exceed the budget (half the free device
  * memory at 16 bytes per entry) the call returns GHICP_E_NOMEM, with the entry count in the message, before writing any
  * output. */

@@ -18,6 +18,8 @@
 //   3. nonMaximaSuppression sorts by curvature with an unstable sort and a '>' comparator (:120-130, :151): canonical tie
 //      order = ascending point index.
 // Neighbourhood test: squared distance < radius^2 (FLANN's RadiusResultSet keeps dist < radius), the query point included.
+// Non-finite points take no part (pcl::removeNaNFromPointCloud, then the reference; indices stay those of the input): they
+// bound no box, own no cell, have no neighbour (pt_num 0, eigenvalues and curvature 0) and are never emitted.
 #include <algorithm>
 #include <cmath>
 #include <cstdint>
@@ -29,6 +31,8 @@
 namespace {
 
 typedef unsigned long long ull;
+
+bool finite3(const float *p) { return std::isfinite(p[0]) && std::isfinite(p[1]) && std::isfinite(p[2]); }
 
 // cyclic Jacobi on a symmetric 3x3 (float32), eigenvalues sorted descending.  c = {xx, xy, xz, yy, yz, zz}
 void sym3_eig_f32(const float c[6], float lam[3]) {
@@ -70,17 +74,18 @@ struct Grid {  // uniform grid, cell edge = radius; cells keyed by (cx << 42 | c
     minx = miny = minz = INFINITY;
     for (int k = 0; k < n; ++k) {
       const float *p = xyz + 3 * (size_t)(ids ? ids[k] : k);
-      minx = fminf(minx, p[0]); miny = fminf(miny, p[1]); minz = fminf(minz, p[2]);
+      if (finite3(p)) { minx = fminf(minx, p[0]); miny = fminf(miny, p[1]); minz = fminf(minz, p[2]); }
     }
     inv = 1.0f / radius;
     for (int k = 0; k < n; ++k) {
       const int i = ids ? ids[k] : k;
       const float *p = xyz + 3 * (size_t)i;
-      cells[key(coord(p[0], minx), coord(p[1], miny), coord(p[2], minz))].push_back(k);
+      if (finite3(p)) cells[key(coord(p[0], minx), coord(p[1], miny), coord(p[2], minz))].push_back(k);
     }
   }
   template <typename F>
   void for_neighbours(const float *q, F &&f) const {  // 27 cells, x slowest / z fastest, ascending position inside a cell
+    if (!finite3(q)) return;
     const int cx = coord(q[0], minx), cy = coord(q[1], miny), cz = coord(q[2], minz);
     for (int dx = -1; dx <= 1; ++dx)
       for (int dy = -1; dy <= 1; ++dy)
@@ -101,17 +106,21 @@ extern "C" {
 // CFilter::voxelfilter (include/filter.hpp:28-88).  xyz [n][3] float32.  out_idx (capacity n + 1) receives the indices of
 // the kept points in output order (ascending voxel id).  Returns their number.
 int orc_voxel_downsample(const float *xyz, int n, float voxel_size, int *out_idx) {
-  if (n <= 0) return 0;
+  int first = -1, nfin = 0;                                                            // the finite cloud: its size, its point 0
+  for (int i = 0; i < n; ++i) if (finite3(xyz + 3 * (size_t)i)) { if (first < 0) first = i; ++nfin; }
+  if (nfin == 0) return 0;
   const float inverse_voxel_size = 1.0f / voxel_size;                                  // :30
   float mn[3] = {INFINITY, INFINITY, INFINITY}, mx[3] = {-INFINITY, -INFINITY, -INFINITY};   // pcl::getMinMax3D, :33
   for (int i = 0; i < n; ++i)
-    for (int k = 0; k < 3; ++k) { mn[k] = fminf(mn[k], xyz[3 * (size_t)i + k]); mx[k] = fmaxf(mx[k], xyz[3 * (size_t)i + k]); }
+    if (finite3(xyz + 3 * (size_t)i))
+      for (int k = 0; k < 3; ++k) { mn[k] = fminf(mn[k], xyz[3 * (size_t)i + k]); mx[k] = fmaxf(mx[k], xyz[3 * (size_t)i + k]); }
   const float gap[3] = {mx[0] - mn[0], mx[1] - mn[1], mx[2] - mn[2]};                  // :36
   const ull max_vy = (ull)(ceilf(gap[1] * inverse_voxel_size) + 1);                    // :39-40
   const ull max_vz = (ull)(ceilf(gap[2] * inverse_voxel_size) + 1);
   const ull mul_vx = max_vy * max_vz, mul_vy = max_vz;                                 // :48-50
-  std::vector<std::pair<ull, unsigned>> id_pairs((size_t)n, {0ull, 0u});               // :52: n default entries ...
+  std::vector<std::pair<ull, unsigned>> id_pairs((size_t)nfin, {0ull, (unsigned)first});   // :52: n default entries ...
   for (int i = 0; i < n; ++i) {                                                        // :54-68: ... plus n real ones
+    if (!finite3(xyz + 3 * (size_t)i)) continue;
     const ull vx = (ull)floorf((xyz[3 * (size_t)i] - mn[0]) * inverse_voxel_size);
     const ull vy = (ull)floorf((xyz[3 * (size_t)i + 1] - mn[1]) * inverse_voxel_size);
     const ull vz = (ull)floorf((xyz[3 * (size_t)i + 2] - mn[2]) * inverse_voxel_size);

@@ -41,7 +41,7 @@ def fpfh(xyz, idx=None, k=20, all_normals=True):
     n = len(xyz)
     ia = None if idx is None else np.ascontiguousarray(idx, dtype=np.int32).reshape(-1)
     m = n if ia is None else len(ia)
-    ke = min(k, n)
+    ke = min(k, int(np.isfinite(xyz).all(axis=1).sum()))   # non-finite points take no part
     out = np.zeros((m, 33), np.float32)
     nrm = np.full((n, 3), np.nan, np.float32)
     st = np.full(n, -1, np.int32)

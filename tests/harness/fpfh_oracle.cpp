@@ -14,6 +14,8 @@
 //   SPFH      hist_incr = 100 / (k_eff - 1); per neighbour q != p (by index) computePairFeatures, pairs with |dp| == 0,
 //             |v| == 0 or a NaN normal skipped (still counted in k_eff - 1); PCL's acos(|a1|) > acos(|a2|) is |a1| < |a2|;
 //             f1 = atan2 in double, rounded to float; bins floor(11 * x) clamped to [0, 10]
+//   non-finite points take no part: k_eff = min(k, finite points), the lists of finite points hold finite points only; a
+//             non-finite point's list is itself k_eff times at d2 = 0, its normal NaN (status 1), its SPFH and FPFH zero
 //   FPFH      the neighbours with d2 != 0, weight 1 / d2 (float), per bin float sums in k-NN order, per block double sums,
 //             each block times (float)(100 / sum) when the sum is not 0; the point's own SPFH is not added
 // Float operation order of the pair features — the same text in gh-icp_b200/csrc/ghicp_prep.cu:
@@ -74,11 +76,16 @@ struct State {
   std::vector<float> nrm; std::vector<char> have_nrm;
   std::vector<float> spfh; std::vector<char> have_spfh;
 
-  const int *knn(int i) {   // brute force over the whole cloud
+  bool finite(int i) const { const float *p = xyz + 3 * (size_t)i; return std::isfinite(p[0]) && std::isfinite(p[1]) && std::isfinite(p[2]); }
+  const int *knn(int i) {   // brute force over the whole (finite) cloud
     if (!have_nb[i]) {
-      std::vector<std::pair<float, int>> all(n);
-      for (int p = 0; p < n; ++p) all[p] = {fpfh_d2(xyz + 3 * (size_t)i, xyz + 3 * (size_t)p), p};
-      std::partial_sort(all.begin(), all.begin() + k, all.end());
+      std::vector<std::pair<float, int>> all;
+      if (finite(i)) {
+        for (int p = 0; p < n; ++p) if (finite(p)) all.push_back({fpfh_d2(xyz + 3 * (size_t)i, xyz + 3 * (size_t)p), p});
+        std::partial_sort(all.begin(), all.begin() + k, all.end());
+      } else {
+        all.assign(k, {0.f, i});
+      }
       for (int j = 0; j < k; ++j) { nb[(size_t)i * k + j] = all[j].second; d2[(size_t)i * k + j] = all[j].first; }
       have_nb[i] = 1;
     }
@@ -88,7 +95,7 @@ struct State {
     if (!have_nrm[i]) {
       float *o = &nrm[3 * (size_t)i];
       const float *q = xyz + 3 * (size_t)i;
-      if (k < 3) {
+      if (k < 3 || !finite(i)) {
         o[0] = o[1] = o[2] = std::nanf("");
       } else {
         const int *l = knn(i);
@@ -196,7 +203,9 @@ int fpfh_oracle(const float *xyz, int n, const int *idx, int nidx, int k, int al
                 int *status, int *nb_idx, float *nb_d2, int *computed) {
   if (n <= 0 || k < 1) return -1;
   State S;
-  S.xyz = xyz; S.n = n; S.k = k < n ? k : n;
+  int nfin = 0;
+  for (int i = 0; i < n; ++i) nfin += std::isfinite(xyz[3 * (size_t)i]) && std::isfinite(xyz[3 * (size_t)i + 1]) && std::isfinite(xyz[3 * (size_t)i + 2]);
+  S.xyz = xyz; S.n = n; S.k = k < nfin ? k : nfin;
   S.nb.assign((size_t)n * S.k, -1); S.d2.assign((size_t)n * S.k, 0.f); S.have_nb.assign(n, 0);
   S.nrm.assign(3 * (size_t)n, 0.f); S.have_nrm.assign(n, 0);
   S.spfh.assign((size_t)n * 33, 0.f); S.have_spfh.assign(n, 0);
@@ -210,7 +219,7 @@ int fpfh_oracle(const float *xyz, int n, const int *idx, int nidx, int k, int al
     }
     if (S.have_nrm[i]) {
       if (normals) std::memcpy(normals + 3 * (size_t)i, &S.nrm[3 * (size_t)i], sizeof(float) * 3);
-      if (status) status[i] = S.k < 3 ? 1 : 0;
+      if (status) status[i] = (S.k < 3 || !S.finite(i)) ? 1 : 0;
     }
     if (computed) computed[i] = (S.have_nb[i] ? 1 : 0) | (S.have_nrm[i] ? 2 : 0);
   }
