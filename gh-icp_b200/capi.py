@@ -7,9 +7,6 @@ import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = os.path.join(_HERE, "libghicp_b200.so")
-# developer hook for kernel A/B runs (tools/build_variants.sh): another build of the SAME library; never set by the driver
-if os.environ.get("GHICP_B200_LIB"):
-    _LIB = os.environ["GHICP_B200_LIB"]
 
 FT_BSC, FT_ROPS, FT_FPFH, FT_NONE = 0, 1, 2, 3   # include/utility.h:51-57
 CT_NN, CT_NNR, CT_KM = 0, 1, 2                   # include/utility.h:59-64

@@ -13,6 +13,7 @@
 //
 // All tie-breaks are explicit (value, then smaller index), so the result does not depend on the
 // order in which atomics land.
+#include <algorithm>
 #include <climits>
 #include <cooperative_groups.h>
 #include <cstdio>
@@ -95,7 +96,6 @@ struct AucArgs {
   int *bid_obj; double *bid_val, *bid_aux;
   int *counters;  // [0],[1]: ping-pong list sizes, [2]: base list size
   double eps;
-  int profile;    // GHICP_AUCTION_DEBUG: per-size-class timing of the tail rounds into counters[16..31]
   // Reverse phase: stop as soon as D = sum of the prices of the objects still free (= the active list) fits the budget.
   // Dual eps-feasibility (profit_i + price_j >= g_ij - eps on every edge, equality on matched pairs) is an invariant of
   // the reverse rounds, so OPT - ours <= n*eps + D holds at EVERY round boundary: the rest of the displacement chains
@@ -106,8 +106,8 @@ struct AucArgs {
 constexpr double D_FX = 1048576.0;
 __device__ __forceinline__ unsigned long long d_fx(double p) { return p > 0.0 ? (unsigned long long)(p * D_FX) + 1ull : 0ull; }
 // counters (int[64]): [0],[1] list sizes, [2] base list size, [3] sticky round-limit flag, [4] cur, [5] rounds, [6] rounds
-// of the whole solve, [8..9] bids (u64), [10] grid rounds, [12..13] / [14..15] ns in tail / grid rounds, [16..31] tail
-// profile, [32..33] / [34..35] D of list 0 / 1 (u64 fixed point), [36] 1 = the reverse phase stopped on the D budget
+// of the whole solve, [8..9] bids (u64), [10] grid rounds, [32..33] / [34..35] D of list 0 / 1 (u64 fixed point), [36] 1 =
+// the reverse phase stopped on the D budget
 __device__ __forceinline__ unsigned long long *d_slot(int *counters, int which) {
   return reinterpret_cast<unsigned long long *>(&counters[32 + 2 * which]);
 }
@@ -126,17 +126,9 @@ __global__ void k_auc_init(int n_rows, int n_cols, const long long *rowptr, int 
 }
 
 __global__ void k_auc_phase_start(int n_rows, int n_cols, const long long *rowptr, int n_chunks, int *assign,
-                                  int *owner, double *profit, double *price, double relax) {
+                                  int *owner, double *profit) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n_cols) {
-    owner[i] = -1;
-    // Warm start: prices of the previous (coarser) phase sit up to eps_prev above the level at which their
-    // last owner is indifferent to staying unmatched; carried over unchanged those owners would all retire to
-    // their dummy at once and the (sequential) reverse auction would have to re-attract them one chain at a
-    // time.  Relaxing every price by eps_prev lets the parallel forward rounds redo that matching instead.
-    // Any non-negative starting prices are valid for the auction.
-    if (relax > 0.0) price[i] = fmax(0.0, price[i] - relax);
-  }
+  if (i < n_cols) owner[i] = -1;
   if (i < n_rows) {
     const bool has = rowptr[(size_t)(i + 1) * n_chunks] > rowptr[(size_t)i * n_chunks];
     assign[i] = has ? UNASSIGNED : DUMMY;
@@ -169,7 +161,6 @@ __global__ void k_rev_collect(int n_cols, const int *owner, const double *price,
 // reverse) phase: rounds with many active bidders use the whole grid with grid-wide barriers between
 // bid / resolve / commit; once the active set is small (the long price-war tail) CTA 0 runs the rounds
 // alone with __syncthreads, which removes the launch / grid-barrier latency from ~all of the rounds.
-// All mutable state is read with ld.global.cg (L2) so no stale L1 line is ever consumed.
 // ---------------------------------------------------------------------------------------------
 namespace cg = cooperative_groups;
 constexpr int PA_THREADS = 512;
@@ -179,14 +170,6 @@ constexpr int PA_SMALL = 1024;  // largest active set CTA 0 iterates alone (its 
 // L1-cached loads: inside CTA 0's tail rounds the CTA's own stores go through the same L1, and every full-grid phase starts
 // behind __threadfence() + grid.sync(), whose acquire makes the other CTAs' earlier stores visible to plain loads (CUDA's
 // grid-synchronisation guarantee).  Words that ATOMICS modify (bid keys, counters, D slots) are always read at L2.
-// GHICP_AUC_L2_LOADS keeps every state load at L2 (ld.global.cg), the round-1 behaviour, for A/B runs.
-#if defined(GHICP_AUC_L2_LOADS)
-__device__ __forceinline__ int ldcg_i(const int *p) { return __ldcg(p); }
-__device__ __forceinline__ double ldcg_d(const double *p) { return __ldcg(p); }
-#else
-__device__ __forceinline__ int ldcg_i(const int *p) { return *p; }
-__device__ __forceinline__ double ldcg_d(const double *p) { return *p; }
-#endif
 __device__ __forceinline__ int ldl2_i(const int *p) { return __ldcg(p); }   // counters (atomically updated): always L2
 __device__ __forceinline__ unsigned long long pack_key(float v, int who) {  // v > 0
   return ((unsigned long long)__float_as_uint(v) << 32) | (unsigned)(who + 1);
@@ -206,7 +189,7 @@ __device__ __forceinline__ void fwd_scan(const AucArgs &a, int i, int lane, long
 #pragma unroll
     for (int u = 0; u < 8; ++u) { j[u] = a.csr_col[k + 32 * u]; g[u] = a.csr_gain[k + 32 * u]; }
 #pragma unroll
-    for (int u = 0; u < 8; ++u) p[u] = ldcg_d(&a.price[j[u]]);
+    for (int u = 0; u < 8; ++u) p[u] = a.price[j[u]];
 #pragma unroll
     for (int u = 0; u < 8; ++u) {
       const double v = g[u] - p[u];
@@ -217,7 +200,7 @@ __device__ __forceinline__ void fwd_scan(const AucArgs &a, int i, int lane, long
   for (; k < ke; k += 32) {
     const int j = a.csr_col[k];
     const double g = a.csr_gain[k];
-    const double v = g - ldcg_d(&a.price[j]);
+    const double v = g - a.price[j];
     if (v > t.best || (v == t.best && t.idx >= 0 && tie_less(i, j, t.idx))) bgain = g;
     top2_push_h(t, v, j, i);
   }
@@ -243,9 +226,9 @@ struct SlotsGlobal {
   int *o; double *v, *x;
   __device__ __forceinline__ void put(int k, int obj, double val, double aux) const { __stcg(&o[k], obj); __stcg(&v[k], val); __stcg(&x[k], aux); }
   __device__ __forceinline__ void none(int k) const { __stcg(&o[k], -1); }
-  __device__ __forceinline__ int obj(int k) const { return ldcg_i(&o[k]); }
-  __device__ __forceinline__ double val(int k) const { return ldcg_d(&v[k]); }
-  __device__ __forceinline__ double aux(int k) const { return ldcg_d(&x[k]); }
+  __device__ __forceinline__ int obj(int k) const { return o[k]; }
+  __device__ __forceinline__ double val(int k) const { return v[k]; }
+  __device__ __forceinline__ double aux(int k) const { return x[k]; }
 };
 struct SlotsShared {
   int *o; double *v, *x;
@@ -266,7 +249,7 @@ __device__ __forceinline__ void fwd_finish(const AucArgs &a, int i, const Top2 &
     sl.none(key);
   } else {
     const double wv = fmax(t.second, 0.0);
-    const double newprice = ldcg_d(&a.price[t.idx]) + (t.best - wv) + a.eps;
+    const double newprice = a.price[t.idx] + (t.best - wv) + a.eps;
     sl.put(key, t.idx, newprice, bgain);
     // One atomic decides the round's winner: the key orders bidders by their bid rounded to float32, then
     // by id.  ANY bidder may win a round as long as the price becomes its own (exact, double) bid: that is
@@ -285,10 +268,10 @@ __device__ __forceinline__ void fwd_bid_one(const AucArgs &a, int i, int lane, c
 // returns via append(): persons that stay / become unassigned
 template <typename S, typename Append>
 __device__ __forceinline__ void fwd_commit_one(const AucArgs &a, int i, const S &sl, int key, Append append) {
-  if (ldcg_i(&a.assign[i]) != UNASSIGNED) return;
+  if (a.assign[i] != UNASSIGNED) return;
   const int j = sl.obj(key);
   if (key_who(__ldcg(&a.bidmax[j])) == i) {
-    const int prev = ldcg_i(&a.owner[j]);
+    const int prev = a.owner[j];
     const double bv = sl.val(key);
     __stcg(&a.owner[j], i);
     __stcg(&a.price[j], bv);
@@ -309,13 +292,13 @@ __device__ __forceinline__ void rev_scan(const AucArgs &a, int j, int lane, long
 #pragma unroll
     for (int u = 0; u < 8; ++u) { i[u] = a.csc_row[k + 32 * u]; g[u] = a.csc_gain[k + 32 * u]; }
 #pragma unroll
-    for (int u = 0; u < 8; ++u) pr[u] = ldcg_d(&a.profit[i[u]]);
+    for (int u = 0; u < 8; ++u) pr[u] = a.profit[i[u]];
 #pragma unroll
     for (int u = 0; u < 8; ++u) top2_push_h(t, g[u] - pr[u], i[u], j);
   }
   for (; k < ke; k += 32) {
     const int i = a.csc_row[k];
-    top2_push_h(t, a.csc_gain[k] - ldcg_d(&a.profit[i]), i, j);
+    top2_push_h(t, a.csc_gain[k] - a.profit[i], i, j);
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
@@ -364,7 +347,7 @@ __device__ __forceinline__ void bid_serial(const AucArgs &a, int e, const S &sl,
 #pragma unroll
     for (int u = 0; u < 4; ++u) { x[u] = adj[k + u]; g[u] = gains[k + u]; }
 #pragma unroll
-    for (int u = 0; u < 4; ++u) p[u] = ldcg_d(&other[x[u]]);
+    for (int u = 0; u < 4; ++u) p[u] = other[x[u]];
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
       const double v = g[u] - p[u];
@@ -375,7 +358,7 @@ __device__ __forceinline__ void bid_serial(const AucArgs &a, int e, const S &sl,
   for (; k < ke; ++k) {
     const int x = adj[k];
     const double g = gains[k];
-    const double v = g - ldcg_d(&other[x]);
+    const double v = g - other[x];
     if (!REVERSE && (v > t.best || (v == t.best && t.idx >= 0 && tie_less(e, x, t.idx)))) bg = g;
     top2_push_h(t, v, x, e);
   }
@@ -387,20 +370,20 @@ __device__ __forceinline__ void rev_commit_one(const AucArgs &a, int j, const S 
   const int i = sl.obj(key);
   if (i < 0) return;
   if (key_who(__ldcg(&a.bidmax[i])) == j) {
-    const int old = ldcg_i(&a.assign[i]);
+    const int old = a.assign[i];
     const double dl = sl.val(key);
     __stcg(&a.assign[i], j);
     __stcg(&a.owner[j], i);
     __stcg(&a.price[j], sl.aux(key) - dl);
-    __stcg(&a.profit[i], ldcg_d(&a.profit[i]) + dl);
+    __stcg(&a.profit[i], a.profit[i] + dl);
     __stcg(&a.bidmax[i], 0ull);
     if (old >= 0) {
       __stcg(&a.owner[old], -1);
-      const double po = ldcg_d(&a.price[old]);
+      const double po = a.price[old];
       if (po > 0.0) append(old, po);
     }
   } else {
-    append(j, ldcg_d(&a.price[j]));
+    append(j, a.price[j]);
   }
 }
 
@@ -461,19 +444,11 @@ __global__ void __launch_bounds__(PA_THREADS, 2) k_auction_persistent(AucArgs a,
   const bool cut_on = REVERSE && a.d_budget_fx != 0ull;
   bool cut = false;
   int cur = 0, rounds = 0;
-  unsigned long long t_mark = 0, t_prev = 0;
-  int b_prev = 0;
-#if defined(GHICP_EMU_HOST)
-  auto now_ns = []() { return 0ull; };   // host emulation: no device timer
-#else
-  auto now_ns = []() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; };
-#endif
   while (true) {
     const int n = ldl2_i(&a.counters[cur]);
     if (n == 0 || rounds >= max_rounds) break;
     // every thread of the grid reads the same D (written before the last grid barrier): a uniform decision
     if (cut_on && __ldcg(d_slot(a.counters, cur)) <= a.d_budget_fx) { cut = true; break; }
-    if (gtid == 0) t_mark = now_ns();
     if (n <= small_n) {
       // ---- tail: CTA 0 alone, block-level barriers only; the active lists and the bid slots live in shared memory
       if (blockIdx.x == 0) {
@@ -488,14 +463,7 @@ __global__ void __launch_bounds__(PA_THREADS, 2) k_auction_persistent(AucArgs a,
           if (cut_on && s_D <= a.d_budget_fx) break;   // the outer loop re-reads the same D and stops
           const int *list = s_list[sc];
           int *next = s_list[sc ^ 1];
-          if (threadIdx.x == 0) {
-            s_next = 0; s_Dnext = 0ull; atomicAdd((unsigned long long *)&a.counters[8], (unsigned long long)m);
-            if (a.profile) {   // GHICP_AUCTION_DEBUG: time and rounds per active-set size class
-              const unsigned long long tn = now_ns();
-              if (t_prev) { atomicAdd((unsigned long long *)&a.counters[16 + 2 * b_prev], tn - t_prev); atomicAdd((unsigned long long *)&a.counters[24 + 2 * b_prev], 1ull); }
-              t_prev = tn; b_prev = m == 1 ? 0 : (m <= 16 ? 1 : (m <= 64 ? 2 : 3));
-            }
-          }
+          if (threadIdx.x == 0) { s_next = 0; s_Dnext = 0ull; atomicAdd((unsigned long long *)&a.counters[8], (unsigned long long)m); }
           if (m <= NW / 2) {
             // very few bidders: split every adjacency list over G warps so one round costs one short scan
             const int G = NW / m;
@@ -520,8 +488,8 @@ __global__ void __launch_bounds__(PA_THREADS, 2) k_auction_persistent(AucArgs a,
                     __stcg(&a.profit[i], 0.0);
                   } else {
                     const int j = t.idx;
-                    const double newprice = ldcg_d(&a.price[j]) + (t.best - fmax(t.second, 0.0)) + a.eps;
-                    const int prev = ldcg_i(&a.owner[j]);
+                    const double newprice = a.price[j] + (t.best - fmax(t.second, 0.0)) + a.eps;
+                    const int prev = a.owner[j];
                     __stcg(&a.owner[j], i);
                     __stcg(&a.price[j], newprice);
                     __stcg(&a.assign[i], j);
@@ -535,14 +503,14 @@ __global__ void __launch_bounds__(PA_THREADS, 2) k_auction_persistent(AucArgs a,
                   } else {
                     const int who = t.idx;
                     const double delta = fmin(t.best, (t.best - t.second) + a.eps);
-                    const int old = ldcg_i(&a.assign[who]);
+                    const int old = a.assign[who];
                     __stcg(&a.assign[who], j);
                     __stcg(&a.owner[j], who);
                     __stcg(&a.price[j], t.best - delta);
-                    __stcg(&a.profit[who], ldcg_d(&a.profit[who]) + delta);
+                    __stcg(&a.profit[who], a.profit[who] + delta);
                     if (old >= 0) {
                       __stcg(&a.owner[old], -1);
-                      const double po = ldcg_d(&a.price[old]);
+                      const double po = a.price[old];
                       if (po > 0.0) { next[0] = old; s_next = 1; s_Dnext = d_fx(po); }
                     }
                   }
@@ -597,7 +565,6 @@ __global__ void __launch_bounds__(PA_THREADS, 2) k_auction_persistent(AucArgs a,
       }
       __threadfence();
       grid.sync();
-      if (gtid == 0) atomicAdd((unsigned long long *)&a.counters[12], now_ns() - t_mark);  // ns in tail mode
       cur = ldl2_i(&a.counters[4]);
       rounds = ldl2_i(&a.counters[5]);
       continue;
@@ -617,13 +584,13 @@ __global__ void __launch_bounds__(PA_THREADS, 2) k_auction_persistent(AucArgs a,
       if (16ll * n <= tw) G = 16; else if (8ll * n <= tw) G = 8; else if (4ll * n <= tw) G = 4; else if (2ll * n <= tw) G = 2;
     }
     if (short_rows == 1 || (short_rows == 2 && n > 3 * gwarps)) {
-      for (int w = gtid; w < n; w += gthreads) { const int e = ldcg_i(&list[w]); bid_serial<REVERSE>(a, e, gsl, e); }
+      for (int w = gtid; w < n; w += gthreads) { const int e = list[w]; bid_serial<REVERSE>(a, e, gsl, e); }
     } else if (G > 1) {
       const int gpc = NW / G, grp = warp / G, slice = warp % G;
       const int w = blockIdx.x * gpc + grp;   // n <= gridDim.x * gpc by the choice of G
       int e = -1;
       if (w < n) {
-        e = ldcg_i(&list[w]);
+        e = list[w];
         Top2 t; double bg;
         split_scan<REVERSE>(a, e, G, slice, lane, t, bg);
         if (lane == 0) { s_pt[warp] = t; s_pg[warp] = bg; }
@@ -636,14 +603,14 @@ __global__ void __launch_bounds__(PA_THREADS, 2) k_auction_persistent(AucArgs a,
       }
     } else {
       for (int w = gwarp; w < n; w += gwarps) {
-        const int e = ldcg_i(&list[w]);
+        const int e = list[w];
         if (REVERSE) rev_offer_one(a, e, lane, gsl, e); else fwd_bid_one(a, e, lane, gsl, e);
       }
     }
     __threadfence();
     grid.sync();
     for (int w = gtid; w < n; w += gthreads) {
-      const int e = ldcg_i(&list[w]);
+      const int e = list[w];
       auto app = [&](int x, double p) {
         __stcg(&next[atomicAdd(&a.counters[cur ^ 1], 1)], x);
         if (REVERSE) atomicAdd(d_slot(a.counters, cur ^ 1), d_fx(p));
@@ -652,7 +619,6 @@ __global__ void __launch_bounds__(PA_THREADS, 2) k_auction_persistent(AucArgs a,
     }
     __threadfence();
     grid.sync();
-    if (gtid == 0) atomicAdd((unsigned long long *)&a.counters[14], now_ns() - t_mark);  // ns in full-grid rounds
     cur ^= 1;
     ++rounds;
   }
@@ -708,65 +674,97 @@ cudaError_t launch_build_csc(Ctx *c, int n_rows, int n_cols, long long nnz) {
   return cudaGetLastError();
 }
 
-// eps of the single forward phase from zero prices (sparse graphs): free objects keep price 0 there (D = 0), so the whole
-// optimality budget n*eps_final goes to eps.  One definition for km_auction and km_auction_settled: the two routes of an
-// iteration must produce the same matching.
-static double single_phase_eps(double eps_final) {
-  double f = 0.95;
-  if (const char *ov = getenv("GHICP_AUCTION_EPS1")) { const double v = atof(ov); if (v > 0.0 && v <= 1.0) f = v; }
-  return f * eps_final;
-}
+// The settled route (km_auction_settled) and the general route (km_auction) must produce the same matching on the same
+// graph: both fill the arguments, start the solve and launch the rounds through the functions below.
 
-// The settled loop's auction: ONE forward phase at eps_final/2 from zero prices (the sparse-graph schedule of
-// km_auction: every object that ever received a bid stays owned, free objects keep price 0, D = 0, no reverse phase),
-// enqueued without reading anything back.  Correct on any graph; chosen by the caller when last iteration's graph
-// was sparse.
-int km_auction_settled(Ctx *c, int n_rows, int n_cols, long long nnz_hint, double eps_final) {
-  cudaStream_t st = c->stream;
+// eps of the single forward phase from zero prices (sparse graphs): free objects keep price 0 there (D = 0), so the whole
+// optimality budget n*eps_final goes to eps.
+static double single_phase_eps(double eps_final) { return 0.95 * eps_final; }
+
+static AucArgs auc_args(const Ctx *c, double eps) {
   AucArgs a{};
   a.rowptr = c->d_rowptr; a.n_chunks = c->n_chunks; a.csr_col = c->d_csr_col; a.csr_gain = c->d_csr_gain;
   a.colptr = c->d_colptr; a.csc_row = c->d_csc_row; a.csc_gain = c->d_csc_gain;
   a.price = c->d_price; a.profit = c->d_profit; a.assign = c->d_assign; a.owner = c->d_owner;
   a.bidmax = c->d_bidmax; a.bidwin = c->d_bidwin; a.bid_obj = c->d_bid_obj; a.bid_val = c->d_bid_val;
   a.bid_aux = c->d_bid_aux; a.counters = c->d_counters;
-  a.eps = single_phase_eps(eps_final); a.profile = 0; a.d_budget_fx = 0ull;
-  const int nmax = n_rows > n_cols ? n_rows : n_cols;
-  const int gmax = (nmax + 255) / 256;
-  int *base_list = c->d_flags;  // free during KM
-  cudaMemsetAsync(c->d_counters, 0, sizeof(int) * 64, st);
-  GHICP_LAUNCH(k_auc_init, gmax, 256, 0, st, n_rows, n_cols, c->d_rowptr, c->n_chunks, c->d_price, base_list, c->d_counters,
-                                   c->d_bidmax, c->d_bidwin, nmax);
-  cudaMemsetAsync(c->d_bid_obj, 0xff, sizeof(int) * (size_t)nmax, st);  // -1
-  GHICP_LAUNCH(k_auc_phase_start, gmax, 256, 0, st, n_rows, n_cols, c->d_rowptr, c->n_chunks, c->d_assign, c->d_owner,
-                                          c->d_profit, c->d_price, 0.0);
-  c->launches += 2;
-  cudaMemcpyAsync(c->d_list[0], base_list, sizeof(int) * (size_t)n_rows, cudaMemcpyDeviceToDevice, st);
-  cudaMemcpyAsync(&c->d_counters[0], &c->d_counters[2], sizeof(int), cudaMemcpyDeviceToDevice, st);
-  static int blocks_per_sm = 0;
-  int n_sm = GHICP_SMS;
-  cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, c->device);
+  a.eps = eps;
+  return a;
+}
+
+static int *base_list(Ctx *c) { return c->d_flags; }  // free during KM
+
+// Start of a solve: counters zeroed, every price 0, the rows with candidates collected in the base list, no bids
+static void auc_solve_start(Ctx *c, int n_rows, int n_cols) {
+  const int nmax = std::max(n_rows, n_cols);
+  cudaMemsetAsync(c->d_counters, 0, sizeof(int) * 64, c->stream);
+  GHICP_LAUNCH(k_auc_init, (nmax + 255) / 256, 256, 0, c->stream, n_rows, n_cols, c->d_rowptr, c->n_chunks, c->d_price,
+               base_list(c), c->d_counters, c->d_bidmax, c->d_bidwin, nmax);
+  c->launches++;
+  cudaMemsetAsync(c->d_bid_obj, 0xff, sizeof(int) * (size_t)nmax, c->stream);  // -1
+}
+
+// Start of a forward phase: every object free, every row with candidates unassigned and active (list 0 = the base list)
+static void auc_phase_start(Ctx *c, int n_rows, int n_cols) {
+  const int nmax = std::max(n_rows, n_cols);
+  GHICP_LAUNCH(k_auc_phase_start, (nmax + 255) / 256, 256, 0, c->stream, n_rows, n_cols, c->d_rowptr, c->n_chunks,
+               c->d_assign, c->d_owner, c->d_profit);
+  c->launches++;
+  cudaMemcpyAsync(c->d_list[0], base_list(c), sizeof(int) * (size_t)n_rows, cudaMemcpyDeviceToDevice, c->stream);
+  cudaMemcpyAsync(&c->d_counters[0], &c->d_counters[2], sizeof(int), cudaMemcpyDeviceToDevice, c->stream);
+}
+
+// How the rounds run for adjacency lists of average length avg.  small_n: CTA 0 takes over the rounds alone once the active
+// set is this small, i.e. once the expected work of a round (bidders x avg) is small enough that grid-wide barriers would
+// dominate (long lists: a grid round gives every bidder up to 16 warps, CTA 0 alone only pays below ~16 bidders).
+// short_rows: 1 = one thread walks a bidder's list (short lists), 2 = the same for medium lists once the bidders outnumber
+// the warps, 0 = one or more warps per bidder.
+struct RoundShape { int small_n, short_rows; };
+static RoundShape round_shape(double avg) {
+  const int sn = (int)(8192.0 / (avg > 1.0 ? avg : 1.0));
+  return {std::min(std::max(sn, 16), PA_SMALL), avg <= 4.0 ? 1 : (avg <= 32.0 ? 2 : 0)};
+}
+
+// One persistent cooperative launch that runs a whole forward (REVERSE = false) or reverse phase from list 0
+template <bool REVERSE>
+static int launch_rounds(Ctx *c, const AucArgs &a, RoundShape rs) {
+  static int blocks_per_sm = 0;   // all CTAs must be co-resident
   if (blocks_per_sm == 0) {
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, k_auction_persistent<false>, PA_THREADS, 0);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, k_auction_persistent<REVERSE>, PA_THREADS, 0);
     if (blocks_per_sm < 1) blocks_per_sm = 1;
   }
-  const double avg_row = (double)nnz_hint / (n_rows > 0 ? n_rows : 1);
-  int sn = (int)(8192.0 / (avg_row > 1.0 ? avg_row : 1.0));
-  sn = sn < 16 ? 16 : (sn > PA_SMALL ? PA_SMALL : sn);
+  int n_sm = GHICP_SMS;
+  cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, c->device);
+  const dim3 grid(n_sm * blocks_per_sm);
   int *l0 = c->d_list[0], *l1 = c->d_list[1];
-  int mr = 4000000;
-  int sr = avg_row <= 4.0 ? 1 : (avg_row <= 32.0 ? 2 : 0);   // one thread per bidder (2: only when bidders outnumber warps)
-  void *args[] = {(void *)&a, (void *)&l0, (void *)&l1, (void *)&mr, (void *)&sn, (void *)&sr};
+  int max_rounds = 4000000;
 #if defined(GHICP_EMU_HOST)
-  (void)args;
-  emu::launch_cooperative(dim3(n_sm * blocks_per_sm), dim3(PA_THREADS), [&] { k_auction_persistent<false>(a, l0, l1, mr, sn, sr); });
-  cudaError_t e = cudaSuccess;
+  // host emulation: all blocks of the (small) grid run as fibers, the grid barrier is a rendezvous
+  emu::launch_cooperative(grid, dim3(PA_THREADS), [&] { k_auction_persistent<REVERSE>(a, l0, l1, max_rounds, rs.small_n, rs.short_rows); });
+  const cudaError_t e = cudaSuccess;
 #else
-  cudaError_t e = cudaLaunchCooperativeKernel((void *)k_auction_persistent<false>, dim3(n_sm * blocks_per_sm), dim3(PA_THREADS),
-                                              args, 0, st);
+  void *args[] = {(void *)&a, (void *)&l0, (void *)&l1, (void *)&max_rounds, (void *)&rs.small_n, (void *)&rs.short_rows};
+  const cudaError_t e = cudaLaunchCooperativeKernel((void *)k_auction_persistent<REVERSE>, grid, dim3(PA_THREADS), args, 0, c->stream);
 #endif
-  if (e != cudaSuccess) { set_error(c, std::string("auction (settled) launch: ") + cudaGetErrorString(e)); return GHICP_E_CUDA; }
+  if (e != cudaSuccess) {
+    set_error(c, std::string(REVERSE ? "auction reverse launch: " : "auction forward launch: ") + cudaGetErrorString(e));
+    return GHICP_E_CUDA;
+  }
   c->launches++;
-  cudaMemcpyAsync(c->h_counters, c->d_counters, sizeof(int) * 8, cudaMemcpyDeviceToHost, st);
+  return GHICP_OK;
+}
+
+// The settled loop's auction: ONE forward phase at single_phase_eps from zero prices (the sparse-graph schedule of
+// km_auction: every object that ever received a bid stays owned, free objects keep price 0, D = 0, no reverse phase),
+// enqueued without reading anything back.  Correct on any graph; chosen by the caller when last iteration's graph
+// was sparse.
+int km_auction_settled(Ctx *c, int n_rows, int n_cols, long long nnz_hint, double eps_final) {
+  auc_solve_start(c, n_rows, n_cols);
+  auc_phase_start(c, n_rows, n_cols);
+  int rc;
+  if ((rc = launch_rounds<false>(c, auc_args(c, single_phase_eps(eps_final)), round_shape((double)nnz_hint / std::max(n_rows, 1)))))
+    return rc;
+  cudaMemcpyAsync(c->h_counters, c->d_counters, sizeof(int) * 8, cudaMemcpyDeviceToHost, c->stream);
   return GHICP_OK;
 }
 int km_auction_settled_result(Ctx *c, KmResult *res) {   // after the iteration's stream synchronize
@@ -777,21 +775,9 @@ int km_auction_settled_result(Ctx *c, KmResult *res) {   // after the iteration'
 
 int km_auction(Ctx *c, int n_rows, int n_cols, long long nnz, double eps_final, double max_gain, KmResult *res) {
   cudaStream_t st = c->stream;
-  AucArgs a{};
-  a.rowptr = c->d_rowptr; a.n_chunks = c->n_chunks; a.csr_col = c->d_csr_col; a.csr_gain = c->d_csr_gain;
-  a.colptr = c->d_colptr; a.csc_row = c->d_csc_row; a.csc_gain = c->d_csc_gain;
-  a.price = c->d_price; a.profit = c->d_profit; a.assign = c->d_assign; a.owner = c->d_owner;
-  a.bidmax = c->d_bidmax; a.bidwin = c->d_bidwin; a.bid_obj = c->d_bid_obj; a.bid_val = c->d_bid_val;
-  a.bid_aux = c->d_bid_aux; a.counters = c->d_counters;
-  const int nmax = n_rows > n_cols ? n_rows : n_cols;
-  const int gmax = (nmax + 255) / 256;
-  int *base_list = c->d_flags;  // free during KM
-
-  cudaMemsetAsync(c->d_counters, 0, sizeof(int) * 64, st);
-  GHICP_LAUNCH(k_auc_init, gmax, 256, 0, st, n_rows, n_cols, c->d_rowptr, c->n_chunks, c->d_price, base_list, c->d_counters,
-                                   c->d_bidmax, c->d_bidwin, nmax);
-  c->launches++;
-  cudaMemsetAsync(c->d_bid_obj, 0xff, sizeof(int) * (size_t)nmax, st);  // -1
+  AucArgs a = auc_args(c, 0.0);
+  const int nmax = std::max(n_rows, n_cols);
+  auc_solve_start(c, n_rows, n_cols);
 
   // Split of the optimality budget n*eps_final: eps_last = epsf*eps_final for the forward phases (n*eps_last), the rest
   // for D = the prices of objects left free (the reverse phase runs while D exceeds it and stops as soon as it fits).
@@ -800,19 +786,17 @@ int km_auction(Ctx *c, int n_rows, int n_cols, long long nnz, double eps_final, 
   // whose budget n*KM_eps is below a handful of prices anyway and where the larger eps shortens the price wars instead
   // (measured, whole registration: config 4 (2.6k keypoints) 441 / 482 / 209 / 217 ms and config 5 (12.5k) 1549 / 765 / 731 / 839 ms
   // at f = 0.1 / 0.5 / 0.75 / 0.9)
-  double epsf = (eps_final * (double)nmax >= 250.0) ? 0.1 : 0.75;
-  if (const char *ov = getenv("GHICP_AUCTION_EPSF")) { const double v = atof(ov); if (v > 0.0 && v < 1.0) epsf = v; }
+  const double epsf = (eps_final * (double)nmax >= 250.0) ? 0.1 : 0.75;
   const double d_budget = (1.0 - epsf) * eps_final * (double)nmax;
   a.d_budget_fx = getenv("GHICP_AUCTION_NOCUT") ? 0ull : (unsigned long long)(d_budget * D_FX);
   // epsilon schedule
   std::vector<double> eps_list;
   {
     // Optimality bound at termination: OPT - ours <= n*eps_last + D  (D = prices of objects left free).
-    // eps_last = eps_final/2 leaves a budget of n*eps_final/2 for D, so the reverse auction (whose rounds are
+    // eps_last = epsf*eps_final leaves a budget of n*(1 - epsf)*eps_final for D, so the reverse auction (whose rounds are
     // long sequential displacement chains) only runs when D exceeds that budget.
     const double eps_last = epsf * eps_final;
     double e0 = max_gain / 4.0;
-    if (const char *ov = getenv("GHICP_AUCTION_EPS0")) e0 = atof(ov);  // experiment hook: first epsilon (0 = single phase)
     while (e0 > eps_last * 1.0000001) { eps_list.push_back(e0); e0 /= 5.0; }
     eps_list.push_back(eps_last);
   }
@@ -822,60 +806,17 @@ int km_auction(Ctx *c, int n_rows, int n_cols, long long nnz, double eps_final, 
   const bool single_phase = nnz <= (long long)(1.5 * (double)nmax) && getenv("GHICP_AUCTION_SCALING") == nullptr;
   if (nnz == 0 || single_phase) eps_list.assign(1, single_phase_eps(eps_final));
 
-  int rounds = 0;
-  const int max_rounds = 4000000;
-  // persistent cooperative launch geometry (all CTAs must be co-resident)
-  static int coop_blocks_per_sm[2] = {0, 0};
-  int n_sm = GHICP_SMS;
-  cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, c->device);
-  if (coop_blocks_per_sm[0] == 0) {
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&coop_blocks_per_sm[0], k_auction_persistent<false>, PA_THREADS, 0);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&coop_blocks_per_sm[1], k_auction_persistent<true>, PA_THREADS, 0);
-    if (coop_blocks_per_sm[0] < 1) coop_blocks_per_sm[0] = 1;
-    if (coop_blocks_per_sm[1] < 1) coop_blocks_per_sm[1] = 1;
-  }
-  // CTA 0 takes over the rounds alone once the expected work of a round (active bidders x average
-  // adjacency length) is small enough that grid-wide barriers would dominate
-  const double avg_row = (double)nnz / (n_rows > 0 ? n_rows : 1), avg_col = (double)nnz / (n_cols > 0 ? n_cols : 1);
-  // (long adjacency lists: a grid round gives every bidder up to 16 warps, CTA 0 alone only pays below ~16 bidders)
-  int small_fwd = (int)(8192.0 / (avg_row > 1.0 ? avg_row : 1.0));
-  int small_rev = (int)(8192.0 / (avg_col > 1.0 ? avg_col : 1.0));
-  small_fwd = small_fwd < 16 ? 16 : (small_fwd > PA_SMALL ? PA_SMALL : small_fwd);
-  small_rev = small_rev < 16 ? 16 : (small_rev > PA_SMALL ? PA_SMALL : small_rev);
-  if (const char *ov = getenv("GHICP_AUCTION_SMALL")) {   // experiment / test hook: 0 = grid rounds only
-    small_fwd = small_rev = atoi(ov);
-    if (small_fwd > PA_SMALL) small_fwd = small_rev = PA_SMALL;
-  }
+  RoundShape fwd = round_shape((double)nnz / std::max(n_rows, 1)), rev = round_shape((double)nnz / std::max(n_cols, 1));
+  if (const char *ov = getenv("GHICP_AUCTION_SMALL"))   // test hook: 0 = grid rounds only
+    fwd.small_n = rev.small_n = std::min(atoi(ov), PA_SMALL);
   const bool debug = getenv("GHICP_AUCTION_DEBUG") != nullptr;
-  a.profile = debug ? 1 : 0;
-  const double relax_factor = getenv("GHICP_AUCTION_RELAX") ? atof(getenv("GHICP_AUCTION_RELAX")) : 0.0;
-  int last_rounds = 0;
+  int last_rounds = 0, rc;
   bool ran_reverse = false;
   for (size_t ph = 0; ph < eps_list.size(); ++ph) {
     a.eps = eps_list[ph];
-    GHICP_LAUNCH(k_auc_phase_start, gmax, 256, 0, st, n_rows, n_cols, c->d_rowptr, c->n_chunks, c->d_assign, c->d_owner,
-                                            c->d_profit, c->d_price, ph > 0 ? relax_factor * eps_list[ph - 1] : 0.0);
-    c->launches++;
-    cudaMemcpyAsync(c->d_list[0], base_list, sizeof(int) * (size_t)n_rows, cudaMemcpyDeviceToDevice, st);
-    cudaMemcpyAsync(&c->d_counters[0], &c->d_counters[2], sizeof(int), cudaMemcpyDeviceToDevice, st);
+    auc_phase_start(c, n_rows, n_cols);
     cudaMemsetAsync(&c->d_counters[1], 0, sizeof(int), st);
-    {
-      int *l0 = c->d_list[0], *l1 = c->d_list[1];
-      int mr = max_rounds;
-      int sn = small_fwd;
-      int sr = avg_row <= 4.0 ? 1 : (avg_row <= 32.0 ? 2 : 0);   // short / medium adjacency lists: one thread per bidder
-      void *args[] = {(void *)&a, (void *)&l0, (void *)&l1, (void *)&mr, (void *)&sn, (void *)&sr};
-#if defined(GHICP_EMU_HOST)
-      (void)args;   // host emulation: all blocks of the (small) grid run as fibers, the grid barrier is a rendezvous
-      emu::launch_cooperative(dim3(n_sm * coop_blocks_per_sm[0]), dim3(PA_THREADS), [&] { k_auction_persistent<false>(a, l0, l1, mr, sn, sr); });
-      cudaError_t e = cudaSuccess;
-#else
-      cudaError_t e = cudaLaunchCooperativeKernel((void *)k_auction_persistent<false>, dim3(n_sm * coop_blocks_per_sm[0]),
-                                                  dim3(PA_THREADS), args, 0, st);
-#endif
-      if (e != cudaSuccess) { set_error(c, std::string("auction forward launch: ") + cudaGetErrorString(e)); return GHICP_E_CUDA; }
-      c->launches++;
-    }
+    if ((rc = launch_rounds<false>(c, a, fwd))) return rc;
     // reverse: objects left free with a positive price.  Complementary slackness for free objects only
     // matters for the final optimality bound, so intermediate phases skip it (their leftover prices are
     // just the next phase's starting prices).
@@ -889,68 +830,43 @@ int km_auction(Ctx *c, int n_rows, int n_cols, long long nnz, double eps_final, 
       cudaMemcpyAsync(&D_fx_host, d_D, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st);
       cudaMemcpyAsync(c->h_counters, c->d_counters, sizeof(int) * 8, cudaMemcpyDeviceToHost, st);  // final, unless the reverse runs
       cudaStreamSynchronize(st);
-      const double D = (double)D_fx_host / D_FX, budget = d_budget;
-      need_reverse = D > budget;
-      if (debug) fprintf(stderr, "[auction] free-object price sum D = %.4f, budget %.4f -> reverse %s\n", D, budget, need_reverse ? "yes" : "skipped");
+      const double D = (double)D_fx_host / D_FX;
+      need_reverse = D > d_budget;
+      if (debug) fprintf(stderr, "[auction] free-object price sum D = %.4f, budget %.4f -> reverse %s\n", D, d_budget, need_reverse ? "yes" : "skipped");
     }
     if (need_reverse) {
-    ran_reverse = true;
-    // the column-wise copy of the graph is only read by the reverse rounds: built here, on demand (a settled loop, one
-    // forward phase from zero prices, never gets here)
-    { cudaError_t e = launch_build_csc(c, n_rows, n_cols, nnz); if (e != cudaSuccess) { set_error(c, std::string("auction: CSC build: ") + cudaGetErrorString(e)); return GHICP_E_CUDA; } }
-    cudaMemsetAsync(&c->d_counters[0], 0, sizeof(int) * 2, st);
-    cudaMemsetAsync(&c->d_counters[32], 0, sizeof(int) * 5, st);   // D of both lists, the budget-stop flag
-    GHICP_LAUNCH(k_rev_collect, gmax, 256, 0, st, n_cols, c->d_owner, c->d_price, c->d_list[0], c->d_counters, 0);
-    c->launches++;
-    cudaMemsetAsync(c->d_bid_obj, 0xff, sizeof(int) * (size_t)nmax, st);
-    {
-      int *l0 = c->d_list[0], *l1 = c->d_list[1];
-      int mr = max_rounds;
-      int sn = small_rev;
-      int sr = avg_col <= 4.0 ? 1 : (avg_col <= 32.0 ? 2 : 0);
-      void *args[] = {(void *)&a, (void *)&l0, (void *)&l1, (void *)&mr, (void *)&sn, (void *)&sr};
-#if defined(GHICP_EMU_HOST)
-      (void)args;
-      emu::launch_cooperative(dim3(n_sm * coop_blocks_per_sm[1]), dim3(PA_THREADS), [&] { k_auction_persistent<true>(a, l0, l1, mr, sn, sr); });
-      cudaError_t e = cudaSuccess;
-#else
-      cudaError_t e = cudaLaunchCooperativeKernel((void *)k_auction_persistent<true>, dim3(n_sm * coop_blocks_per_sm[1]),
-                                                  dim3(PA_THREADS), args, 0, st);
-#endif
-      if (e != cudaSuccess) { set_error(c, std::string("auction reverse launch: ") + cudaGetErrorString(e)); return GHICP_E_CUDA; }
+      ran_reverse = true;
+      // the column-wise copy of the graph is only read by the reverse rounds: built here, on demand (a settled loop, one
+      // forward phase from zero prices, never gets here)
+      { cudaError_t e = launch_build_csc(c, n_rows, n_cols, nnz); if (e != cudaSuccess) { set_error(c, std::string("auction: CSC build: ") + cudaGetErrorString(e)); return GHICP_E_CUDA; } }
+      cudaMemsetAsync(&c->d_counters[0], 0, sizeof(int) * 2, st);
+      cudaMemsetAsync(&c->d_counters[32], 0, sizeof(int) * 5, st);   // D of both lists, the budget-stop flag
+      GHICP_LAUNCH(k_rev_collect, (nmax + 255) / 256, 256, 0, st, n_cols, c->d_owner, c->d_price, c->d_list[0], c->d_counters, 0);
       c->launches++;
-    }
-    cudaMemsetAsync(c->d_bid_obj, 0xff, sizeof(int) * (size_t)nmax, st);
+      cudaMemsetAsync(c->d_bid_obj, 0xff, sizeof(int) * (size_t)nmax, st);
+      if ((rc = launch_rounds<true>(c, a, rev))) return rc;
+      cudaMemsetAsync(c->d_bid_obj, 0xff, sizeof(int) * (size_t)nmax, st);
     }
     if (debug) {
       cudaMemcpyAsync(c->h_counters, c->d_counters, sizeof(int) * 64, cudaMemcpyDeviceToHost, st);
       cudaStreamSynchronize(st);
-      fprintf(stderr, "[auction] phase %zu eps %.5f rounds %d (cum %d, grid rounds %d) bids(cum) %llu small_fwd %d  tail %.2f ms grid %.2f ms (cum)\n", ph, a.eps,
-              c->h_counters[6] - last_rounds, c->h_counters[6], c->h_counters[10],
-              *(unsigned long long *)&c->h_counters[8], small_fwd, *(unsigned long long *)&c->h_counters[12] * 1e-6,
-              *(unsigned long long *)&c->h_counters[14] * 1e-6);
+      fprintf(stderr, "[auction] phase %zu eps %.5f rounds %d (cum %d, grid rounds %d) bids(cum) %llu\n", ph, a.eps,
+              c->h_counters[6] - last_rounds, c->h_counters[6], c->h_counters[10], *(unsigned long long *)&c->h_counters[8]);
       last_rounds = c->h_counters[6];
-      const unsigned long long *pb = (const unsigned long long *)&c->h_counters[16];
-      fprintf(stderr, "[auction]   tail rounds by active-set size (cum): m=1: %llu in %.2f ms | 2-16: %llu in %.2f ms | 17-64: %llu in %.2f ms | >64: %llu in %.2f ms\n",
-              pb[4], pb[0] * 1e-6, pb[5], pb[1] * 1e-6, pb[6], pb[2] * 1e-6, pb[7], pb[3] * 1e-6);
       if (need_reverse)
         fprintf(stderr, "[auction]   reverse %s: %d objects still free with a positive price, D left %.3f (budget %.3f)\n",
                 c->h_counters[36] ? "stopped on the D budget" : "ran to completion", c->h_counters[c->h_counters[4] & 1],
                 (double)*(unsigned long long *)&c->h_counters[32 + 2 * (c->h_counters[4] & 1)] / D_FX, d_budget);
     }
   }
-  {
-    cudaError_t e = cudaSuccess;
-    if (ran_reverse || debug) {
-      cudaMemcpyAsync(c->h_counters, c->d_counters, sizeof(int) * 8, cudaMemcpyDeviceToHost, st);
-      e = cudaStreamSynchronize(st);
-    }
+  if (ran_reverse || debug) {
+    cudaMemcpyAsync(c->h_counters, c->d_counters, sizeof(int) * 8, cudaMemcpyDeviceToHost, st);
+    const cudaError_t e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) { set_error(c, std::string("auction: ") + cudaGetErrorString(e)); return GHICP_E_CUDA; }
-    rounds = c->h_counters[6];
-    if (c->h_counters[3] != 0) { set_error(c, "auction: round limit exceeded"); return GHICP_E_NOCONV; }
   }
-  if (res) { res->rounds = rounds; res->phases = (int)eps_list.size(); }
-  cudaError_t e = cudaGetLastError();
+  if (c->h_counters[3] != 0) { set_error(c, "auction: round limit exceeded"); return GHICP_E_NOCONV; }
+  if (res) { res->rounds = c->h_counters[6]; res->phases = (int)eps_list.size(); }
+  const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { set_error(c, std::string("auction: ") + cudaGetErrorString(e)); return GHICP_E_CUDA; }
   return GHICP_OK;
 }

@@ -468,10 +468,7 @@ __global__ void k_ff_seed(FfArgs a, const int *__restrict__ prev_row_idx, const 
 // registers); the CTA walks FF_ROWS source rows, FF_RB at a time through shared memory.  One row's record is read from shared
 // memory once (broadcast LDS.128) and serves both columns: the two 33-term dots are the two independent instruction
 // streams, and the operand traffic per pair is half of the one-column form (ncu, round 2: LSU 31 % of the issue slots there).
-#ifndef GHICP_FF_CPT
-#define GHICP_FF_CPT 2
-#endif
-constexpr int FF_CPT = GHICP_FF_CPT;   // columns per thread (1 = the round-1 form, for A/B builds)
+constexpr int FF_CPT = 2;   // columns per thread
 template <bool PRE, bool COLS>
 __global__ void __launch_bounds__(FF_THREADS, 2) k_ff_sweep(const FfArgs a) {
   __shared__ __align__(16) float s_rec[FF_RB][FF_REC];

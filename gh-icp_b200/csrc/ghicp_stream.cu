@@ -34,25 +34,16 @@ constexpr int ST_PANEL = 32 * ST_CPL;             // columns per warp
 constexpr int ST_CTA_COLS = ST_WARPS * ST_PANEL;  // 2048
 constexpr int ST_RB = 256;                        // source rows per CTA (upper bound; StreamArgs::rb is what a launch uses)
 constexpr int ST_RB_MIN = 64;
-// tuning knobs (compile-time; tools/build_variants.sh builds A/B libraries with other values)
-#ifndef GHICP_ST_RING_KB
-#define GHICP_ST_RING_KB 12
-#endif
-#ifndef GHICP_ST_QPS
-#define GHICP_ST_QPS 4
-#endif
-#ifndef GHICP_ST_MINB
-#define GHICP_ST_MINB 2
-#endif
+constexpr int ST_CTAS_PER_SM = 2;                 // k_stream's residency bound, and the slots stream_rows_per_cta fills
 constexpr int ST_UNROLL = FD_QUAD;   // rows per batch = one quad block of the packed plane (part of its format)
 constexpr unsigned INF_BITS = 0x7f800000u;
-// TMA staging of the FD plane: every warp runs its own ring of stages in at most GHICP_ST_RING_KB; a stage holds ST_QPS
+// TMA staging of the FD plane: every warp runs its own ring of stages in at most ST_RING_BYTES; a stage holds ST_QPS
 // consecutive quad blocks of the warp's 256-column panel (fd_block_bytes(hb) = 1152 / 1280 / 1536 B each), brought in by ONE
 // cp.async.bulk (TMA engine, UBLKCP) and signalled on one mbarrier per stage.  No registers are tied up by loads in flight.
 // Four quads per stage (two stages) measured fastest on the H100: fewer, larger copies beat more bytes in flight.
-constexpr int ST_RING_BYTES = GHICP_ST_RING_KB * 1024;   // per warp
+constexpr int ST_RING_BYTES = 12 * 1024;   // per warp
 constexpr int ST_DYN_SMEM = ST_WARPS * ST_RING_BYTES;
-constexpr int ST_QPS = GHICP_ST_QPS;                     // quad blocks (batches) per stage
+constexpr int ST_QPS = 4;                  // quad blocks (batches) per stage
 template <int HB> __host__ __device__ constexpr int st_quad_bytes() { return FD_LOW_BYTES + 128 * HB; }
 template <int HB> __host__ __device__ constexpr int st_stage_bytes() { return ST_QPS * st_quad_bytes<HB>(); }
 template <int HB> __host__ __device__ constexpr int st_stages() { return ST_RING_BYTES / st_stage_bytes<HB>(); }
@@ -582,7 +573,7 @@ __device__ __forceinline__ void sweep(const StreamArgs &a, const float4 *s_S4, c
 
 // two CTAs per SM: the FD variants are held there by their 2 x 96 KB rings anyway, and a tighter bound only costs spills
 template <int MODE, bool HAS_FD, bool STATS, int HB, bool X2>
-__global__ void __launch_bounds__(ST_THREADS, GHICP_ST_MINB) k_stream(const StreamArgs a) {
+__global__ void __launch_bounds__(ST_THREADS, ST_CTAS_PER_SM) k_stream(const StreamArgs a) {
   __shared__ __align__(16) float s_S8[X2 ? ST_RB * 8 : 8];
 #if defined(GHICP_EMU_HOST)
   unsigned char *s_ring = reinterpret_cast<unsigned char *>(emu::dyn_smem());   // host emulation: the launch's dynamic shared memory
@@ -849,15 +840,13 @@ static StreamArgs make_args(Ctx *c, const CostParams &cp) {
 // Source rows per CTA.  The grid is (column blocks) x (row blocks) CTAs of equal cost, two resident per SM: with 256 rows a
 // sharded rank's last wave is mostly empty (6250 rows x 50k columns: 625 CTAs on 296 slots = 3 waves for 2.1 waves of
 // work).  Pick the height (multiple of the batch, 64 ... 256) that minimises waves x rows — 180 rows in that example:
-// 875 CTAs, 2.96 waves.  GHICP_STREAM_RB overrides (tests).
+// 875 CTAs, 2.96 waves.
 static int stream_rows_per_cta(const Ctx *c) {
-  static const int forced = getenv("GHICP_STREAM_RB") ? atoi(getenv("GHICP_STREAM_RB")) : 0;
-  if (forced >= ST_RB_MIN && forced <= ST_RB) return forced / ST_UNROLL * ST_UNROLL;
   static int slots = 0;
   if (slots == 0) {
     int n_sm = GHICP_SMS;
     cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, c->device);
-    slots = 2 * (n_sm > 0 ? n_sm : GHICP_SMS);
+    slots = ST_CTAS_PER_SM * (n_sm > 0 ? n_sm : GHICP_SMS);
   }
   const long long gx = (c->M + ST_CTA_COLS - 1) / ST_CTA_COLS;
   const int nloc = c->nloc > 0 ? c->nloc : 1;
