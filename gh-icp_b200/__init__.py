@@ -12,7 +12,7 @@ from .capi import (  # noqa: F401
     GhicpError, IterStats, Config, lib, lib_path, build_library, device_count,
     km_solve, rigid_fit, rigid_fit_ex, comm_unique_id, voxel_downsample, detect_keypoints,
     bsc_extract, bsc_default_pattern, read_sample_pattern, Prep, PrepParams, fpfh_extract, fpfh_extract_radius, sac_ia,
-    cloud_overlap, OverlapResult, cloud_icp,
+    cloud_overlap, OverlapResult, cloud_icp, sor_filter, SorResult,
     SOLVER_SVD, SOLVER_WEIGHTED_SVD, SOLVER_POINT_TO_PLANE, SOLVER_YAW_4DOF,
 )
 from .registration import GHRegistration, Keypoints, Energyfunction  # noqa: F401

@@ -75,7 +75,7 @@ EXPORTS = ["ghicp_abi_version", "ghicp_device_count", "ghicp_last_error", "ghicp
            "ghicp_host_alloc", "ghicp_host_free", "ghicp_fpfh_extract", "ghicp_prep_fpfh", "ghicp_prep_get_fpfh",
            "ghicp_prep_fpfh_stats", "ghicp_sac_ia", "ghicp_prep_sac_ia", "ghicp_set_initial_transform",
            "ghicp_fpfh_extract_radius", "ghicp_prep_fpfh_radius", "ghicp_cloud_overlap", "ghicp_prep_overlap",
-           "ghicp_cloud_icp", "ghicp_prep_icp"]
+           "ghicp_cloud_icp", "ghicp_prep_icp", "ghicp_sor_filter", "ghicp_prep_run_sor", "ghicp_prep_sor_info"]
 
 
 def lib():
@@ -140,6 +140,9 @@ def lib():
     L.ghicp_prep_overlap.argtypes = [vp, vp, dp, C.c_float, C.c_double, C.c_int, C.POINTER(OverlapResult)]
     L.ghicp_cloud_icp.argtypes = [C.c_int, fpp, C.c_int, fpp, C.c_int, dp, C.POINTER(IcpParams), C.POINTER(IcpResult), fpp, ip, dp]
     L.ghicp_prep_icp.argtypes = [vp, vp, dp, C.POINTER(IcpParams), C.POINTER(IcpResult)]
+    L.ghicp_sor_filter.argtypes = [C.c_int, fpp, C.c_int, C.c_int, C.c_double, ip, fpp, C.POINTER(SorResult)]
+    L.ghicp_prep_run_sor.argtypes = [C.c_int, fpp, C.c_int, C.POINTER(PrepParams), ip, C.c_int, C.c_double, C.POINTER(vp)]
+    L.ghicp_prep_sor_info.argtypes = [vp, C.POINTER(SorResult), ip, fpp]
     _lib = L
     return L
 
@@ -227,6 +230,31 @@ def _icp_out(r, rc):
                     stage_ms=dict(grid=ms[0], iterations=ms[1], fitness=ms[2], total=ms[3]))
 
 
+class SorResult(C.Structure):
+    """ghicp_sor_result (include/ghicp_b200.h): statistical outlier removal, DESIGN.md §3.16."""
+    _fields_ = [("n_finite", C.c_int), ("n_kept", C.c_int), ("k_eff", C.c_int), ("fallbacks", C.c_int), ("mean", C.c_double),
+                ("stddev", C.c_double), ("threshold", C.c_double), ("candidates", C.c_longlong), ("stage_ms", C.c_float * 5)]
+
+
+def _sor_out(r):
+    ms = list(r.stage_ms)
+    return dict(n_finite=r.n_finite, n_kept=r.n_kept, k_eff=r.k_eff, mean=r.mean, stddev=r.stddev, threshold=r.threshold,
+                candidates=r.candidates, fallbacks=r.fallbacks,
+                stage_ms=dict(grid=ms[0], distances=ms[1], statistics=ms[2], compaction=ms[3], total=ms[4]))
+
+
+def _sor_args(sor):
+    """None -> (0, 0.0), the ABI's "no filter"; else the (mean_k, std_mul) pair, mean_k in 1..128 and std_mul finite (mean_k 0
+    would silently mean "no filter" to the ABI)."""
+    if sor is None:
+        return 0, 0.0
+    mean_k, std_mul = sor
+    mean_k, std_mul = int(mean_k), float(std_mul)
+    if not 1 <= mean_k <= 128 or not np.isfinite(std_mul):
+        raise GhicpError(-1, f"sor: mean_k must be in 1..128 and std_mul finite, not ({mean_k}, {std_mul})")
+    return mean_k, std_mul
+
+
 class PrepParams(C.Structure):
     """ghicp_prep_params (include/ghicp_b200.h): the driver's per-cloud parameters (test/ghicp_main.cpp:89-116)."""
     _fields_ = [("voxel_size", C.c_float), ("neighborhood_radius", C.c_float), ("ratio_max", C.c_float), ("min_pts", C.c_int),
@@ -235,10 +263,13 @@ class PrepParams(C.Structure):
 
 class Prep:
     """Device-resident pipeline result of ONE cloud (ghicp_prep_run): voxel filter -> curvature keypoints -> BSC encoder,
-    the raw cloud uploaded once, nothing copied back unless asked for."""
+    the raw cloud uploaded once, nothing copied back unless asked for.  sor = (mean_k, std_mul) removes statistical outliers
+    from the down-sampled cloud between the voxel filter and the keypoints (ghicp_prep_run_sor, see sor_filter); `sor_info`
+    then holds the filter's result, with the down-sampled size before it ("n_voxel") and its time ("ms").  sor=None (the
+    default) runs no filter and sor_info is None."""
 
     def __init__(self, xyz, voxel_size, neighborhood_radius, nms_radius, bsc_radius=0.0, dof_type=0, ratio_max=0.65, min_pts=20,
-                 side=7, pairs=None, device=0):
+                 side=7, pairs=None, device=0, sor=None):
         xyz = np.ascontiguousarray(xyz, dtype=np.float32)
         self.params = PrepParams(voxel_size, neighborhood_radius, ratio_max, min_pts, nms_radius, bsc_radius, side, dof_type)
         pr = None
@@ -246,8 +277,14 @@ class Prep:
             pr = bsc_default_pattern(side) if pairs is None else np.ascontiguousarray(pairs, dtype=np.int32)
         self.h = C.c_void_p()
         self.side = side
-        check(lib().ghicp_prep_run(device, xyz.ctypes.data_as(C.POINTER(C.c_float)), len(xyz), C.byref(self.params),
-                                   None if pr is None else _ip(pr), C.byref(self.h)))
+        mean_k, std_mul = _sor_args(sor)
+        check(lib().ghicp_prep_run_sor(device, xyz.ctypes.data_as(C.POINTER(C.c_float)), len(xyz), C.byref(self.params),
+                                       None if pr is None else _ip(pr), mean_k, std_mul, C.byref(self.h)))
+        self.sor_info = None
+        if sor is not None:
+            r, nv, ms = SorResult(), C.c_int(0), C.c_float(0)
+            check(lib().ghicp_prep_sor_info(self.h, C.byref(r), C.byref(nv), C.byref(ms)))
+            self.sor_info = dict(_sor_out(r), n_voxel=nv.value, ms=ms.value)
         nd, nk, nv = C.c_int(0), C.c_int(0), C.c_int(0)
         mn, mx, ms = np.zeros(3, np.float32), np.zeros(3, np.float32), np.zeros(5, np.float32)
         fpp = C.POINTER(C.c_float)
@@ -437,6 +474,26 @@ def voxel_downsample(xyz, voxel_size, device=0):
     check(lib().ghicp_voxel_downsample(device, xyz.ctypes.data_as(C.POINTER(C.c_float)), len(xyz), voxel_size, _ip(out),
                                        C.byref(m)))
     return out[:m.value].copy()
+
+
+def sor_filter(xyz, mean_k=50, std_mul=1.0, return_distances=False, device=0):
+    """CFilter::SORFilter (include/filter.hpp:90-102; PCL's StatisticalOutlierRemoval) on the GPU, DESIGN.md §3.16: a finite
+    point is kept unless its mean distance to its mean_k (1..128) nearest other finite points exceeds mean + std_mul * stddev
+    of those distances; non-finite points are never kept.  Returns (kept indices ascending, info: n_finite, n_kept, k_eff,
+    mean, stddev, threshold, candidates, fallbacks, stage_ms); + info["distances"] [n] float32 (NaN for non-finite points)
+    with return_distances."""
+    xyz = np.ascontiguousarray(xyz, dtype=np.float32).reshape(-1, 3)
+    n = len(xyz)
+    out = np.zeros(max(n, 1), np.int32)
+    dist = np.zeros(n, np.float32) if return_distances else None
+    r = SorResult()
+    fpp = C.POINTER(C.c_float)
+    check(lib().ghicp_sor_filter(device, xyz.ctypes.data_as(fpp), n, int(mean_k), float(std_mul), _ip(out),
+                                 None if dist is None else dist.ctypes.data_as(fpp), C.byref(r)))
+    info = _sor_out(r)
+    if dist is not None:
+        info["distances"] = dist
+    return out[:r.n_kept].copy(), info
 
 
 def detect_keypoints(xyz, radius, ratio_max=0.65, min_pts=20, nms_radius=None, device=0):

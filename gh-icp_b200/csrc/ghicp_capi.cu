@@ -1203,6 +1203,27 @@ int ghicp_voxel_downsample(int device, const float *xyz, int n, float voxel_size
   return cuda_status(voxel_downsample_run(xyz, n, voxel_size, out_idx, n_out), "voxel_downsample");
 }
 
+static bool sor_args_ok(int mean_k, double std_mul) { return mean_k >= 1 && mean_k <= 128 && std::isfinite(std_mul); }
+static cudaError_t sor_filter_run(const float *xyz, int n, int mean_k, double std_mul, int *out_idx, float *mean_dist,
+                                  ghicp_sor_result *r) {
+  DevBuf<float> d_xyz, d_dist; DevBuf<int> d_out;
+  ghicp_sor_result res;
+  CUDA_TRY(d_xyz.alloc(3 * (size_t)n)); CUDA_TRY(d_dist.alloc((size_t)n)); CUDA_TRY(d_out.alloc((size_t)n));
+  CUDA_TRY(cudaMemcpy(d_xyz.get(), xyz, 3 * (size_t)n * sizeof(float), cudaMemcpyHostToDevice));
+  CUDA_TRY(prep_sor_filter(0, d_xyz.get(), n, mean_k, std_mul, d_out.get(), d_dist.get(), &res));
+  if (res.n_kept > 0) CUDA_TRY(cudaMemcpy(out_idx, d_out.get(), (size_t)res.n_kept * sizeof(int), cudaMemcpyDeviceToHost));
+  if (mean_dist) CUDA_TRY(cudaMemcpy(mean_dist, d_dist.get(), (size_t)n * sizeof(float), cudaMemcpyDeviceToHost));
+  *r = res;
+  return cudaSuccess;
+}
+int ghicp_sor_filter(int device, const float *xyz, int n, int mean_k, double std_mul, int *out_idx, float *mean_dist,
+                     ghicp_sor_result *r) {
+  if (!xyz || !out_idx || !r || n < 0 || !sor_args_ok(mean_k, std_mul)) { set_error(nullptr, "sor_filter: bad argument"); return GHICP_E_ARG; }
+  if (int rc = enter_device(device, "sor_filter")) return rc;
+  if (n == 0) { *r = ghicp_sor_result{}; return GHICP_OK; }
+  return cuda_status(sor_filter_run(xyz, n, mean_k, std_mul, out_idx, mean_dist, r), "sor_filter");
+}
+
 static cudaError_t detect_keypoints_run(const float *xyz, int n, float radius, float ratio_max, int min_pts, float nms_radius,
                                         int *kp_idx, int *n_kp, float *lam, double *curvature, int *pt_num) {
   DevBuf<float> d_xyz, d_lam; DevBuf<double> d_curv; DevBuf<int> d_cnt, d_kp;
@@ -1274,6 +1295,10 @@ struct ghicp_prep {
   DevBuf<float> d_fpfh;           // [n_kp][33] after ghicp_prep_fpfh
   float bbox_min[3] = {0, 0, 0}, bbox_max[3] = {0, 0, 0};
   float stage_ms[5] = {0, 0, 0, 0, 0};
+  bool sor = false;                     // made by ghicp_prep_run_sor with the filter on
+  ghicp_sor_result sor_result{};
+  int n_voxel = 0;                      // the down-sampled cloud's size before the filter
+  float sor_ms = 0.f;
   FpfhStats fpfh_stats;
   OverlapTarget *ov_target = nullptr;   // the down-sampled cloud's grid as an overlap target, after ghicp_prep_overlap
   DevBuf<float> icp_nrm;                // [n_down][3] k-NN normals, after ghicp_prep_icp with metric 1 (target) or 2 (either)
@@ -1289,11 +1314,12 @@ int ghicp_prep_destroy(ghicp_prep *h) {
   return GHICP_OK;
 }
 
+// events: 0 start, 1 uploaded, 2 voxel filter, 3 outlier filter (mean_k > 0; else right after 2), 4 keypoints, 5 end
 static cudaError_t prep_run_stages(const float *xyz, int n, const ghicp_prep_params *p, const int *bsc_pairs, bool want_bsc,
-                                   ghicp_prep *h) {
+                                   int sor_k, double sor_std, ghicp_prep *h) {
   const int side = h->side;
-  StageEvents<5> ev;
-  DevBuf<float> d_xyz, d_lam, d_lrf; DevBuf<double> d_curv;
+  StageEvents<6> ev;
+  DevBuf<float> d_xyz, d_lam, d_lrf, d_dist; DevBuf<double> d_curv;
   DevBuf<int> d_keep, d_cnt, d_kpbuf, d_pairs, d_status;
   CUDA_TRY(ev.create());
   CUDA_TRY(d_xyz.alloc(3 * (size_t)n)); CUDA_TRY(d_keep.alloc((size_t)n + 1));
@@ -1307,12 +1333,25 @@ static cudaError_t prep_run_stages(const float *xyz, int n, const ghicp_prep_par
   CUDA_TRY(prep_gather_points(0, d_xyz.get(), d_keep.get(), n_down, h->d_down.get()));
   CUDA_TRY(cudaEventRecord(ev[2], 0));
   d_xyz.reset(); d_keep.reset();
+  if (sor_k > 0) {   // the outlier filter on the down-sampled cloud; the kept points replace it
+    DevBuf<float> kept;
+    h->n_voxel = n_down;
+    CUDA_TRY(d_keep.alloc((size_t)n_down)); CUDA_TRY(d_dist.alloc((size_t)n_down));
+    CUDA_TRY(prep_sor_filter(0, h->d_down.get(), n_down, sor_k, sor_std, d_keep.get(), d_dist.get(), &h->sor_result));
+    n_down = h->sor_result.n_kept;
+    if (n_down <= 0) { h->n_down = 0; return cudaSuccess; }   // nothing kept: refused like a cloud without a finite point
+    CUDA_TRY(kept.alloc(3 * (size_t)n_down));
+    CUDA_TRY(prep_gather_points(0, h->d_down.get(), d_keep.get(), n_down, kept.get()));
+    h->d_down = std::move(kept);
+    d_keep.reset(); d_dist.reset();
+  }
+  CUDA_TRY(cudaEventRecord(ev[3], 0));
   CUDA_TRY(prep_bounds(0, h->d_down.get(), n_down, h->bbox_min, h->bbox_max));
   CUDA_TRY(d_lam.alloc(3 * (size_t)n_down)); CUDA_TRY(d_curv.alloc((size_t)n_down));
   CUDA_TRY(d_cnt.alloc((size_t)n_down)); CUDA_TRY(d_kpbuf.alloc((size_t)n_down));
   CUDA_TRY(prep_detect_keypoints(0, h->d_down.get(), n_down, p->neighborhood_radius, p->ratio_max, p->min_pts, p->nms_radius,
                                  d_lam.get(), d_curv.get(), d_cnt.get(), d_kpbuf.get(), &n_kp, &rounds));
-  CUDA_TRY(cudaEventRecord(ev[3], 0));
+  CUDA_TRY(cudaEventRecord(ev[4], 0));
   h->n_down = n_down; h->n_kp = n_kp;
   if (n_kp > 0) {
     CUDA_TRY(h->d_kp.alloc((size_t)n_kp));
@@ -1329,14 +1368,20 @@ static cudaError_t prep_run_stages(const float *xyz, int n, const ghicp_prep_par
                                 h->d_bits.get(), d_lrf.get(), d_status.get()));
     }
   }
-  CUDA_TRY(cudaEventRecord(ev[4], 0));
+  CUDA_TRY(cudaEventRecord(ev[5], 0));
   CUDA_TRY(cudaStreamSynchronize(0));
-  for (int k = 0; k < 4; ++k) h->stage_ms[k] = ev.ms(k, k + 1);
-  h->stage_ms[4] = ev.ms(0, 4);
+  h->stage_ms[0] = ev.ms(0, 1); h->stage_ms[1] = ev.ms(1, 2); h->stage_ms[2] = ev.ms(3, 4); h->stage_ms[3] = ev.ms(4, 5);
+  h->stage_ms[4] = ev.ms(0, 5);
+  h->sor_ms = ev.ms(2, 3);
   return cudaSuccess;
 }
 int ghicp_prep_run(int device, const float *xyz, int n, const ghicp_prep_params *p, const int *bsc_pairs, ghicp_prep **out) {
-  if (!xyz || !p || !out || n <= 0 || !(p->voxel_size > 0.f) || !(p->neighborhood_radius > 0.f) || !(p->nms_radius > 0.f)) {
+  return ghicp_prep_run_sor(device, xyz, n, p, bsc_pairs, 0, 0.0, out);
+}
+int ghicp_prep_run_sor(int device, const float *xyz, int n, const ghicp_prep_params *p, const int *bsc_pairs, int mean_k,
+                       double std_mul, ghicp_prep **out) {
+  if (!xyz || !p || !out || n <= 0 || !(p->voxel_size > 0.f) || !(p->neighborhood_radius > 0.f) || !(p->nms_radius > 0.f) ||
+      (mean_k != 0 && !sor_args_ok(mean_k, std_mul))) {
     set_error(nullptr, "prep_run: bad argument");
     return GHICP_E_ARG;
   }
@@ -1347,10 +1392,23 @@ int ghicp_prep_run(int device, const float *xyz, int n, const ghicp_prep_params 
   int rc;
   if ((rc = enter_device(device, "prep_run"))) return rc;
   ghicp_prep *h = new ghicp_prep();
-  h->device = device; h->n = n; h->side = side;
-  if ((rc = cuda_status(prep_run_stages(xyz, n, p, bsc_pairs, want_bsc, h), "prep_run"))) { ghicp_prep_destroy(h); return rc; }
-  if (h->n_down <= 0) { ghicp_prep_destroy(h); set_error(nullptr, "prep_run: the cloud has no finite point"); return GHICP_E_ARG; }
+  h->device = device; h->n = n; h->side = side; h->sor = mean_k > 0;
+  if ((rc = cuda_status(prep_run_stages(xyz, n, p, bsc_pairs, want_bsc, mean_k, std_mul, h), "prep_run"))) { ghicp_prep_destroy(h); return rc; }
+  if (h->n_down <= 0) {
+    const bool filtered = h->sor && h->n_voxel > 0;
+    ghicp_prep_destroy(h);
+    set_error(nullptr, filtered ? "prep_run: the outlier filter kept no point" : "prep_run: the cloud has no finite point");
+    return GHICP_E_ARG;
+  }
   *out = h;
+  return GHICP_OK;
+}
+
+int ghicp_prep_sor_info(const ghicp_prep *h, ghicp_sor_result *r, int *n_voxel, float *ms) {
+  if (!h || !h->sor) { set_error(nullptr, "prep_sor_info: the result was made without the outlier filter"); return GHICP_E_ARG; }
+  if (r) *r = h->sor_result;
+  if (n_voxel) *n_voxel = h->n_voxel;
+  if (ms) *ms = h->sor_ms;
   return GHICP_OK;
 }
 

@@ -510,6 +510,11 @@ cudaError_t icp_run(const float *d_src, int n_src, const float *d_all, int n_all
                     const float *d_nrm, const float *d_nrm_s, const double *guess, const ghicp_icp_params *p, cudaEvent_t ev_iter,
                     cudaEvent_t ev_fit, ghicp_icp_result *out, float *h_moved, int *h_cor, double *h_mse);
 
+// CFilter::SORFilter (ghicp_sor_filter, DESIGN.md §3.16) on device arrays, see ghicp_prep.cu: d_out (capacity n) receives the
+// kept indices, d_dist [n] every point's mean distance; *r every field.  mean_k in 1..128.
+cudaError_t prep_sor_filter(cudaStream_t st, const float *d_xyz, int n, int mean_k, double std_mul, int *d_out, float *d_dist,
+                            ghicp_sor_result *r);
+
 // glue of the device-resident pipeline (ghicp_prep_run)
 cudaError_t prep_gather_points(cudaStream_t st, const float *d_xyz, const int *d_idx, int m, float *d_out);
 cudaError_t prep_kp_coords(cudaStream_t st, const float *d_xyz, const int *d_kp, int nkp, double *d_soa);

@@ -18,6 +18,7 @@
 // Sort / scan plumbing = CUB (library code; under the host emulation shim: std::stable_sort / a loop).
 #include <climits>
 #include <cmath>
+#include <cstdlib>
 #include <cstring>
 
 #include "ghicp_internal.h"
@@ -900,6 +901,7 @@ struct KnnArgs {
   int *nb_idx; float *nb_d2;        // [n][k]
   unsigned long long *cand;         // candidates examined, summed over all queries
   int *fallbacks;                   // queries that took the exhaustive scan
+  int *deferred, *n_deferred;       // optional: such queries are listed here instead (rows not written), for a wider scan
 };
 
 // cells (x, y, zlo .. zhi) = one run of the sorted order
@@ -954,16 +956,20 @@ __global__ void k_knn(const KnnArgs a) {
         if (lb > 0.0 && key[FPFH_KMAX - 1] != ~0ull && (double)knn_key_d2(key[FPFH_KMAX - 1]) < lb * lb * (1.0 - 1e-5)) done = true;
       }
       if (!done) {   // far outlier (or a grid too fine for this cloud): exact by exhaustion
-#pragma unroll
-        for (int j = 0; j < FPFH_KMAX; ++j) key[j] = (j < FPFH_KMAX - k) ? 0ull : ~0ull;
-        for (int s = 0; s < a.n; ++s) knn_insert(key, knn_key(knn_d2(qx, qy, qz, r.sorted[s]), r.order[s]));
-        cand += a.n;
         atomicAdd(&s_fb, 1);
+        if (a.deferred) {
+          a.deferred[atomicAdd(a.n_deferred, 1)] = i;
+        } else {
+#pragma unroll
+          for (int j = 0; j < FPFH_KMAX; ++j) key[j] = (j < FPFH_KMAX - k) ? 0ull : ~0ull;
+          for (int s = 0; s < a.n; ++s) knn_insert(key, knn_key(knn_d2(qx, qy, qz, r.sorted[s]), r.order[s]));
+          cand += a.n;
+        }
       }
 #pragma unroll
       for (int j = 0; j < FPFH_KMAX; ++j) {
         const int jj = j - (FPFH_KMAX - k);
-        if (jj >= 0) {
+        if (jj >= 0 && (done || !a.deferred)) {
           a.nb_idx[(size_t)i * k + jj] = (int)(unsigned)key[j];
           a.nb_d2[(size_t)i * k + jj] = knn_key_d2(key[j]);
         }
@@ -1534,6 +1540,328 @@ cudaError_t prep_fpfh_radius(cudaStream_t st, const float *d_xyz, int n, const i
                                         ev_normals, &s);
   if (stats) *stats = s;
   return e;
+}
+
+// =====================================================================================================================
+// Statistical outlier removal (DESIGN.md §3.16): CFilter::SORFilter (include/filter.hpp:90-102), PCL's
+// StatisticalOutlierRemoval, on the canonical definition stated with ghicp_sor_filter in include/ghicp_b200.h.
+//   k_knn + k_sor_listmean   k_eff <= 31: k_knn's k_eff + 1 nearest in registers, the point itself dropped, summed per thread
+//   k_sor_dist     larger k_eff: one warp per finite point, k_knn's ring walk (same grid, stopping bound and exhaustive fallback) over
+//                  batches of 32 candidates, one per lane.  The k_eff smallest (d2, index) keys, k_eff up to 128, stay sorted
+//                  in a per-warp list in shared memory; a batch's keys below the current k-th key are merged into it by rank.
+//                  Only the mean distance leaves the warp: one float per point, no [n][k] lists.
+//   k_sor_partial  fixed-order double sums of d (pass 0) or of (d - mean)^2 (pass 1), one per block of a fixed grid
+//   k_sor_finish   one block: the fixed-order sum of the partials -> mean (pass 0), stddev and threshold (pass 1)
+//   k_sor_flags + exclusive_scan + k_sor_emit: the kept indices, ascending
+// No floating-point atomics: two runs give the same bits.
+// =====================================================================================================================
+namespace {
+
+constexpr int SOR_KMAX = 128;       // largest mean_k
+constexpr int SOR_T = 256;          // 8 warps per block, one query each
+constexpr int SOR_DEFER_BLOCKS = 32;  // grid of the warp kernel over k_knn's deferred queries (rare: far outliers)
+constexpr int SOR_RED = 256;        // blocks of the partial sums = threads of the final sum (fixed: it fixes the summation order)
+
+struct SorArgs {
+  GridArgs g;
+  int n, nfin, k;                   // points; the finite ones = the first nfin sorted positions (non-finite ones sort last); k = k_eff
+  int gx, gy, gz;                   // largest occupied cell coordinate per axis
+  double cell, slack;               // as KnnArgs
+  float *dist;                      // [n]
+  unsigned long long *cand;         // candidates examined, summed over all queries
+  int *fallbacks;                   // queries that took the exhaustive scan
+  const int *qlist, *nq;            // optional: only the points qlist[0 .. *nq) (k_knn's deferred far outliers), grid-strided;
+                                    // their fallbacks were counted by k_knn
+};
+
+// Merge the lanes' candidate keys c into the warp's ascending list cur[0 .. k) (~0ull = empty slot), writing nxt and swapping.
+// Keys are distinct (d2, index) pairs, so every key's new slot is its rank in the union; slots >= k drop out.  Only keys
+// below the current k-th key (kth) take part.  Warp-uniform control flow; the __syncwarp orders the writes of nxt before
+// the next reads, and every read of cur before the next merge overwrites it.
+__device__ __forceinline__ void sor_merge(pu64 *&cur, pu64 *&nxt, int k, int lane, pu64 c, pu64 &kth) {
+  const unsigned acc = __ballot_sync(0xffffffffu, c < kth);
+  if (acc == 0u) return;
+  constexpr int E = SOR_KMAX / 32;  // list slots per lane: lane + 32 j
+  pu64 e[E];
+  int re[E];
+#pragma unroll
+  for (int j = 0; j < E; ++j) { const int t = lane + 32 * j; e[j] = t < k ? cur[t] : 0ull; re[j] = 0; }
+  int rb = 0;                       // accepted batch keys below c
+  for (unsigned m = acc; m; m &= m - 1) {
+    const pu64 b = __shfl_sync(0xffffffffu, c, __ffs(m) - 1);
+    rb += b < c ? 1 : 0;
+#pragma unroll
+    for (int j = 0; j < E; ++j) re[j] += b < e[j] ? 1 : 0;
+  }
+  if ((acc >> lane) & 1u) {
+    int lo = 0, hi = k;             // list keys below c
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (cur[mid] < c) lo = mid + 1; else hi = mid;
+    }
+    if (lo + rb < k) nxt[lo + rb] = c;
+  }
+#pragma unroll
+  for (int j = 0; j < E; ++j) {
+    const int t = lane + 32 * j;
+    if (t < k && t + re[j] < k) nxt[t + re[j]] = e[j];
+  }
+  __syncwarp();
+  pu64 *const tmp = cur; cur = nxt; nxt = tmp;
+  kth = cur[k - 1];
+}
+// sorted positions [s0, s1) as candidates of the query (point i), 32 per batch; the query itself is not its own neighbour
+__device__ __forceinline__ void sor_scan(const GridRegs &g, int s0, int s1, int i, float qx, float qy, float qz, int k, int lane,
+                                         pu64 *&cur, pu64 *&nxt, pu64 &kth) {
+  for (int b = s0; b < s1; b += 32) {
+    const int s = b + lane;
+    pu64 c = ~0ull;
+    if (s < s1) {
+      const int p = g.order[s];
+      if (p != i) c = knn_key(knn_d2(qx, qy, qz, g.sorted[s]), p);
+    }
+    sor_merge(cur, nxt, k, lane, c, kth);
+  }
+}
+__device__ __forceinline__ void sor_column(const GridRegs &g, int x, int y, int zlo, int zhi, int i, float qx, float qy, float qz,
+                                           int k, int lane, pu64 *&cur, pu64 *&nxt, pu64 &kth, long long &cand) {
+  const int s0 = g.cstart[lower_cell(g, cell_key(x, y, zlo))], s1 = g.cstart[lower_cell(g, cell_key(x, y, zhi) + 1)];
+  cand += s1 - s0;
+  sor_scan(g, s0, s1, i, qx, qy, qz, k, lane, cur, nxt, kth);
+}
+__device__ __forceinline__ void sor_reset(pu64 *cur, int k, int lane, pu64 &kth) {
+  for (int t = lane; t < k; t += 32) cur[t] = ~0ull;
+  __syncwarp();
+  kth = ~0ull;
+}
+
+__global__ void __launch_bounds__(SOR_T) k_sor_dist(const SorArgs a) {
+  __shared__ pu64 s_list[SOR_T / 32][2][SOR_KMAX];
+  __shared__ unsigned long long s_cand;
+  __shared__ int s_fb;
+  if (threadIdx.x == 0) { s_cand = 0ull; s_fb = 0; }
+  __syncthreads();
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int t = blockIdx.x * (SOR_T / 32) + w;   // sorted position: the warps of a block take points of the same cells
+  if (!a.qlist && t >= a.nfin && t < a.n && lane == 0) a.dist[a.g.order[t]] = __uint_as_float(0x7fc00000u);   // non-finite
+  const int nq = a.qlist ? *a.nq : a.nfin;
+  const int step = a.qlist ? gridDim.x * (SOR_T / 32) : nq;   // without a list: at most one query per warp
+  const GridRegs r = grid_regs(a.g);     // per-thread registers, see k_pca
+  for (int q = t; q < nq; q += step) {
+    const int i = a.qlist ? a.qlist[q] : r.order[q];
+    const float qx = a.g.xyz[3 * (size_t)i], qy = a.g.xyz[3 * (size_t)i + 1], qz = a.g.xyz[3 * (size_t)i + 2];
+    const int k = a.k;
+    float d = 0.f;                       // k_eff = 0 (one finite point): distance 0
+    long long cand = 0;
+    bool fb = false;
+    if (k > 0) {
+      pu64 *cur = s_list[w][0], *nxt = s_list[w][1], kth;
+      sor_reset(cur, k, lane, kth);
+      const int cx = cell_coord(qx, a.g.mnx, a.g.inv), cy = cell_coord(qy, a.g.mny, a.g.inv), cz = cell_coord(qz, a.g.mnz, a.g.inv);
+      const int gx = a.gx, gy = a.gy, gz = a.gz;
+      int rmax = cx;                     // the ring that reaches the far side of the grid on every axis
+      rmax = max(rmax, gx - cx); rmax = max(rmax, cy); rmax = max(rmax, gy - cy); rmax = max(rmax, cz); rmax = max(rmax, gz - cz);
+      bool done = false;
+      for (int ring = 0; ring <= FPFH_RING_CAP && !done; ++ring) {   // k_knn's walk
+        for (int dx = -ring; dx <= ring; ++dx) {
+          const int x = cx + dx;
+          if (x < 0 || x > gx) continue;
+          for (int dy = -ring; dy <= ring; ++dy) {
+            const int y = cy + dy;
+            if (y < 0 || y > gy) continue;
+            if (max(abs(dx), abs(dy)) == ring) {
+              const int zlo = max(cz - ring, 0), zhi = min(cz + ring, gz);
+              if (zlo <= zhi) sor_column(r, x, y, zlo, zhi, i, qx, qy, qz, k, lane, cur, nxt, kth, cand);
+            } else {
+              if (cz - ring >= 0) sor_column(r, x, y, cz - ring, cz - ring, i, qx, qy, qz, k, lane, cur, nxt, kth, cand);
+              if (cz + ring <= gz) sor_column(r, x, y, cz + ring, cz + ring, i, qx, qy, qz, k, lane, cur, nxt, kth, cand);
+            }
+          }
+        }
+        if (ring >= rmax) { done = true; break; }
+        const double lb = ((double)ring - a.slack) * a.cell;
+        if (lb > 0.0 && kth != ~0ull && (double)knn_key_d2(kth) < lb * lb * (1.0 - 1e-5)) done = true;
+      }
+      if (!done) {                       // far outlier: exact by exhaustion over the finite points
+        sor_reset(cur, k, lane, kth);
+        sor_scan(r, 0, a.nfin, i, qx, qy, qz, k, lane, cur, nxt, kth);
+        cand += a.nfin;
+        fb = true;
+      }
+      // square roots in parallel into the spare list, then one lane sums them in ascending d2 order
+      for (int j = lane; j < k; j += 32) nxt[j] = (pu64)__double_as_longlong(sqrt((double)knn_key_d2(cur[j])));
+      __syncwarp();
+      double s = 0.0;
+      for (int j = 0; j < k && lane == 0; ++j) s += __longlong_as_double((long long)nxt[j]);
+      d = (float)(s / (double)k);
+    }
+    if (lane == 0) {
+      a.dist[i] = d;
+      atomicAdd(&s_cand, (unsigned long long)cand);
+      if (fb && !a.qlist) atomicAdd(&s_fb, 1);
+    }
+    __syncwarp();                        // the next query's reset overwrites the lists lane 0 has just read
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) { atomicAdd(a.cand, s_cand); atomicAdd(a.fallbacks, s_fb); }
+}
+
+// pass 0: sum of d, pass 1: sum of (d - mean)^2, over the finite points (d not NaN) of this block's fixed share, tree-reduced
+__global__ void __launch_bounds__(SOR_RED) k_sor_partial(const float *__restrict__ dist, int n, const double *__restrict__ stats,
+                                                         int pass, double *__restrict__ partial) {
+  __shared__ double s[SOR_RED];
+  const double mean = pass ? stats[0] : 0.0;
+  double acc = 0.0;
+  for (int i = blockIdx.x * SOR_RED + threadIdx.x; i < n; i += SOR_RED * SOR_RED) {
+    const float d = dist[i];
+    if (d == d) { const double v = (double)d - mean; acc += pass ? v * v : v; }
+  }
+  s[threadIdx.x] = acc;
+  __syncthreads();
+  for (int o = SOR_RED / 2; o > 0; o >>= 1) {
+    if ((int)threadIdx.x < o) s[threadIdx.x] += s[threadIdx.x + o];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) partial[blockIdx.x] = s[0];
+}
+// one block: stats[0] = mean (pass 0); stats[1] = stddev, stats[2] = threshold (pass 1)
+__global__ void __launch_bounds__(SOR_RED) k_sor_finish(const double *__restrict__ partial, int nfin, double std_mul, int pass,
+                                                        double *__restrict__ stats) {
+  __shared__ double s[SOR_RED];
+  s[threadIdx.x] = partial[threadIdx.x];
+  __syncthreads();
+  for (int o = SOR_RED / 2; o > 0; o >>= 1) {
+    if ((int)threadIdx.x < o) s[threadIdx.x] += s[threadIdx.x + o];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    if (pass == 0) {
+      stats[0] = s[0] / (double)nfin;
+    } else {
+      const double sd = nfin > 1 ? sqrt(s[0] / (double)(nfin - 1)) : 0.0;
+      stats[1] = sd;
+      stats[2] = stats[0] + std_mul * sd;
+    }
+  }
+}
+// flags[i] = point i is kept (finite, d not above the threshold); flags[n] = 0
+__global__ void k_sor_flags(const float *__restrict__ dist, int n, const double *__restrict__ stats, int *__restrict__ flags) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i > n) return;
+  const float d = i < n ? dist[i] : 0.f;
+  flags[i] = (i < n && d == d && !((double)d > stats[2])) ? 1 : 0;
+}
+__global__ void k_sor_emit(const int *__restrict__ flags, const int *__restrict__ pos, int n, int *__restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n && flags[i]) out[pos[i]] = i;
+}
+// The small-k path: d_p from k_knn's ascending (d2, index) list of k + 1 entries.  The list holds the k + 1 nearest of all
+// finite points, p itself included unless k + 1 duplicates of p with smaller indices fill it; dropping p (or, without it, the
+// last entry) leaves the k nearest OTHER points, whose square roots are added in list order as k_sor_dist adds them.
+__global__ void k_sor_listmean(const float *__restrict__ xyz, int n, const int *__restrict__ nb_idx, const float *__restrict__ nb_d2,
+                               int k, float *__restrict__ dist) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  if (!finite3(xyz[3 * (size_t)i], xyz[3 * (size_t)i + 1], xyz[3 * (size_t)i + 2])) { dist[i] = __uint_as_float(0x7fc00000u); return; }
+  const size_t b = (size_t)i * (k + 1);
+  double s = 0.0;
+  for (int j = 0, taken = 0; j <= k && taken < k; ++j) {
+    if (nb_idx[b + j] == i) continue;
+    s += sqrt((double)nb_d2[b + j]);
+    ++taken;
+  }
+  dist[i] = k > 0 ? (float)(s / (double)k) : 0.f;
+}
+// GHICP_SOR_FORCE_WARP=1 (test and benchmark hook) runs k_sor_dist at every k, so that both paths can be checked and timed at
+// the same small k; results do not change, only the time does
+bool sor_force_warp() {
+  const char *e = getenv("GHICP_SOR_FORCE_WARP");
+  return e && e[0] == '1';
+}
+
+}  // namespace
+
+// ghicp_sor_filter on device arrays: d_out (capacity n) receives the kept indices, d_dist [n] every point's mean distance
+// (NaN for a non-finite point); r every field.  The grid build allocates, launches and reads back its box and cell count;
+// every later buffer is allocated before the distance kernels, and the one read-back after them, before the final
+// synchronise, brings the kept count (with the statistics and work counters).  The distances come from k_knn's register
+// top-k (k_eff + 1 <= FPFH_KMAX: its [n][k_eff + 1] lists, at most 1.3 GB at 5 M points, are summed by k_sor_listmean) or
+// from k_sor_dist (larger k, no lists); both give the same bits, and at the k where both run k_knn is the faster
+// (tools/bench_sor.py times both).
+cudaError_t prep_sor_filter(cudaStream_t st, const float *d_xyz, int n, int mean_k, double std_mul, int *d_out, float *d_dist,
+                            ghicp_sor_result *r) {
+  StageEvents<5> ev;
+  PointGrid pg;
+  DevBuf<double> d_part, d_stats; DevBuf<int> d_flags, d_pos, d_fb, nb_idx, d_def; DevBuf<pu64> d_cand; DevBuf<float> nb_d2;
+  *r = ghicp_sor_result{};
+  if (n <= 0) return cudaSuccess;
+  if (mean_k < 1 || mean_k > SOR_KMAX) return cudaErrorInvalidValue;
+  CUDA_TRY(ev.create());
+  CUDA_TRY(cudaEventRecord(ev[0], st));
+  CUDA_TRY(prep_point_grid(st, d_xyz, n, mean_k + 1 < n ? mean_k + 1 : n, 0.f, 0.0, &pg));
+  const int nfin = pg.nfin, k = nfin > 0 ? (mean_k < nfin - 1 ? mean_k : nfin - 1) : 0;
+  CUDA_TRY(d_part.alloc(SOR_RED)); CUDA_TRY(d_stats.alloc(3));
+  CUDA_TRY(d_flags.alloc((size_t)n + 1)); CUDA_TRY(d_pos.alloc((size_t)n + 1));
+  CUDA_TRY(d_cand.alloc(1)); CUDA_TRY(d_fb.alloc(1));
+  const bool lists = k + 1 <= FPFH_KMAX && !sor_force_warp();
+  if (lists && nfin > 0) {
+    CUDA_TRY(nb_idx.alloc((size_t)n * (k + 1))); CUDA_TRY(nb_d2.alloc((size_t)n * (k + 1)));
+    CUDA_TRY(d_def.alloc((size_t)nfin + 1));
+    CUDA_TRY(cudaMemsetAsync(d_def.get() + nfin, 0, sizeof(int), st));   // the deferred count
+  }
+  CUDA_TRY(cudaMemsetAsync(d_stats.get(), 0, 3 * sizeof(double), st));
+  CUDA_TRY(cudaMemsetAsync(d_cand.get(), 0, sizeof(pu64), st)); CUDA_TRY(cudaMemsetAsync(d_fb.get(), 0, sizeof(int), st));
+  CUDA_TRY(cudaEventRecord(ev[1], st));
+  SorArgs a{};
+  a.g = pg.g; a.n = n; a.nfin = nfin; a.k = k;
+  a.gx = pg.gx; a.gy = pg.gy; a.gz = pg.gz;
+  a.cell = pg.cell; a.slack = pg.slack;
+  a.dist = d_dist; a.cand = d_cand.get(); a.fallbacks = d_fb.get();
+  if (lists) {
+    if (nfin > 0) {
+      KnnArgs b{};
+      b.g = pg.g; b.n = n; b.k = k + 1;
+      b.gx = pg.gx; b.gy = pg.gy; b.gz = pg.gz;
+      b.cell = pg.cell; b.slack = pg.slack;
+      b.nb_idx = nb_idx.get(); b.nb_d2 = nb_d2.get(); b.cand = d_cand.get(); b.fallbacks = d_fb.get();
+      b.deferred = d_def.get(); b.n_deferred = d_def.get() + nfin;
+      GHICP_LAUNCH(k_knn, blocks(n), PT, 0, st, b);
+    }
+    GHICP_LAUNCH(k_sor_listmean, blocks(n), PT, 0, st, d_xyz, n, nb_idx.get(), nb_d2.get(), k, d_dist);
+    if (nfin > 0) {   // the far outliers k_knn deferred: the warp kernel's 32-lane scan instead of one thread's
+      a.qlist = d_def.get(); a.nq = d_def.get() + nfin;
+      GHICP_LAUNCH(k_sor_dist, SOR_DEFER_BLOCKS, SOR_T, 0, st, a);
+    }
+  } else {
+    GHICP_LAUNCH(k_sor_dist, (n + SOR_T / 32 - 1) / (SOR_T / 32), SOR_T, 0, st, a);
+  }
+  CUDA_TRY(cudaEventRecord(ev[2], st));
+  if (nfin > 0)
+    for (int pass = 0; pass < 2; ++pass) {
+      GHICP_LAUNCH(k_sor_partial, SOR_RED, SOR_RED, 0, st, d_dist, n, d_stats.get(), pass, d_part.get());
+      GHICP_LAUNCH(k_sor_finish, 1, SOR_RED, 0, st, d_part.get(), nfin, std_mul, pass, d_stats.get());
+    }
+  CUDA_TRY(cudaEventRecord(ev[3], st));
+  GHICP_LAUNCH(k_sor_flags, blocks(n + 1), PT, 0, st, d_dist, n, d_stats.get(), d_flags.get());
+  CUDA_TRY(exclusive_scan(d_flags.get(), d_pos.get(), n, st));
+  int kept = 0, fb = 0;
+  double stats[3];
+  pu64 cand = 0;
+  CUDA_TRY(cudaMemcpyAsync(&kept, d_pos.get() + n, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaMemcpyAsync(stats, d_stats.get(), sizeof(stats), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaMemcpyAsync(&cand, d_cand.get(), sizeof(cand), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaMemcpyAsync(&fb, d_fb.get(), sizeof(fb), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  nb_idx.reset(); nb_d2.reset(); d_def.reset();
+  if (kept > 0) GHICP_LAUNCH(k_sor_emit, blocks(n), PT, 0, st, d_flags.get(), d_pos.get(), n, d_out);
+  CUDA_TRY(cudaEventRecord(ev[4], st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  r->n_finite = nfin; r->n_kept = kept; r->k_eff = k; r->fallbacks = fb;
+  r->mean = stats[0]; r->stddev = stats[1]; r->threshold = stats[2];
+  r->candidates = (long long)cand;
+  for (int s = 0; s < 4; ++s) r->stage_ms[s] = ev.ms(s, s + 1);
+  r->stage_ms[4] = ev.ms(0, 4);
+  return cudaGetLastError();
 }
 
 }  // namespace ghicp_b200

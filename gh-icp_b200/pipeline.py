@@ -46,6 +46,13 @@ target's k-NN normals (DESIGN.md §3.14); ptplicp_reg(source, target, ...) is CR
 author was working on (PCL's GICP ignores both, src/common_reg.cpp:213-215); gicp_reg(source, target, ...) is
 CRegistration::gicp_reg itself, with both options off in the loop as PCL has them.
 
+sor = (mean_k, std_mul) removes statistical outliers (CFilter::SORFilter, capi.sor_filter, DESIGN.md §3.16) from each
+down-sampled cloud between the voxel filter and the keypoints, on the device pipeline (capi.Prep(sor=...)) and with
+`features` alike: isolated returns would otherwise stretch the bounding box that scales the loop's energy, and reach every
+later stage.  info["sor"] = {"target": ..., "source": ...} then holds each cloud's filter result (the keys of capi.Prep.sor_info
+on both branches).  The default None leaves
+the result and info as they were.
+
 coarsereg_fpfh_sac(source_xyz, target_xyz, search_radius) is CRegistration::Coarsereg_FPFHSAC (src/common_reg.cpp:393-423):
 radius FPFH on every point of both clouds, then SAC-IA with correspondence randomness 15.
 """
@@ -58,8 +65,12 @@ from .registration import Energyfunction, GHRegistration, Keypoints
 def register_clouds(target_xyz, source_xyz, resolution, neighborhood_radius, curvature_non_max_radius, corr_type=capi.CT_NN,
                     feature_type=capi.FT_NONE, features=None, weight_adjustment_ratio=1.1, weight_adjustment_step=0.1,
                     dof_type=6, estimated_IoU=0.5, max_iter=0, device=0, bsc_pattern=None, fpfh_k=20, initial_alignment=None,
-                    sac=None, fpfh_radius=None, evaluate=None, refine=None, **reg_kw):
+                    sac=None, fpfh_radius=None, evaluate=None, refine=None, sor=None, **reg_kw):
     ev_kw = _evaluate_kw(evaluate)
+    if sor is not None:
+        if len(sor) != 2:
+            raise capi.GhicpError(-1, "sor must be a (mean_k, std_mul) pair")
+        sor = capi._sor_args(sor)
     icp_kw = _refine_kw(refine)
     if initial_alignment not in (None, "fpfh_sac"):
         raise capi.GhicpError(-1, f"initial_alignment must be None or 'fpfh_sac', not {initial_alignment!r}")
@@ -76,8 +87,10 @@ def register_clouds(target_xyz, source_xyz, resolution, neighborhood_radius, cur
         # descriptors go device-to-device into the registration context (ghicp_prep_run + ghicp_set_from_prep)
         want_bsc = feature_type == capi.FT_BSC
         radius = curvature_non_max_radius if want_bsc else 0.0
-        pt = capi.Prep(T, resolution, neighborhood_radius, curvature_non_max_radius, radius, 0, pairs=bsc_pattern, device=device)       # :89-115
-        ps = capi.Prep(S, resolution, neighborhood_radius, curvature_non_max_radius, radius, dof_type, pairs=bsc_pattern, device=device)  # :116
+        pt = capi.Prep(T, resolution, neighborhood_radius, curvature_non_max_radius, radius, 0, pairs=bsc_pattern, device=device,
+                       sor=sor)                                                                                                    # :89-115
+        ps = capi.Prep(S, resolution, neighborhood_radius, curvature_non_max_radius, radius, dof_type, pairs=bsc_pattern, device=device,
+                       sor=sor)                                                                                                    # :116
         try:
             for name, pr in (("target", pt), ("source", ps)):
                 if pr.n_kp == 0:
@@ -103,6 +116,8 @@ def register_clouds(target_xyz, source_xyz, resolution, neighborhood_radius, cur
                         stage_ms=dict(target=pt.stage_ms, source=ps.stage_ms))
             if feature_type == capi.FT_FPFH:
                 info["fpfh_ms"] = dict(target=pt.fpfh_ms, source=ps.fpfh_ms)
+            if sor is not None:
+                info["sor"] = dict(target=pt.sor_info, source=ps.sor_info)
             if sac_info is not None:
                 info["sac"] = dict(sac_info, Rt=Rt0)
             if icp_kw is not None:
@@ -116,10 +131,14 @@ def register_clouds(target_xyz, source_xyz, resolution, neighborhood_radius, cur
         finally:
             pt.close(); ps.close()
         return Rt, info
-    down, kp_idx = {}, {}
+    down, kp_idx, sor_info = {}, {}, {}
     for name, P in (("T", T), ("S", S)):
         keep = capi.voxel_downsample(P, resolution, device=device)                       # :89-90
         D = np.ascontiguousarray(P[keep])
+        if sor is not None:
+            kept, sor_info[name] = capi.sor_filter(D, *sor, device=device)
+            sor_info[name].update(n_voxel=len(D), ms=sor_info[name]["stage_ms"]["total"])   # the keys of Prep.sor_info
+            D = np.ascontiguousarray(D[kept])
         kp, _, _, _ = capi.detect_keypoints(D, neighborhood_radius, 0.65, 20, curvature_non_max_radius, device=device)   # :96-100
         if len(kp) == 0:
             raise capi.GhicpError(-1, f"no keypoints in the {'target' if name == 'T' else 'source'} cloud: check the radii")
@@ -144,6 +163,8 @@ def register_clouds(target_xyz, source_xyz, resolution, neighborhood_radius, cur
     Rt, iterations = reg.ghicp_reg()
     info = dict(iterations=iterations, n_target_down=len(down["T"]), n_source_down=len(down["S"]), n_target_kp=len(kp_idx["T"]),
                 n_source_kp=len(kp_idx["S"]), bbx_magnitude=bbx, cor=len(reg.pairs()[0]))
+    if sor is not None:
+        info["sor"] = dict(target=sor_info["T"], source=sor_info["S"])
     if sac_info is not None:
         info["sac"] = sac_info
     if icp_kw is not None:

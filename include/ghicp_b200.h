@@ -209,6 +209,28 @@ int ghicp_voxel_downsample(int device, const float *xyz, int n, float voxel_size
 int ghicp_detect_keypoints(int device, const float *xyz, int n, float radius, float ratio_max, int min_pts, float nms_radius,
                            int *kp_idx, int *n_kp, float *lam, double *curvature, int *pt_num);
 
+/* CFilter::SORFilter (include/filter.hpp:90-102): PCL's StatisticalOutlierRemoval on the canonical definition of DESIGN.md
+ * §3.16.  Let F be the finite points, n_f = |F|, k_eff = min(mean_k, n_f - 1).  The mean distance d_p of p in F is the mean of
+ * sqrt((double)d2) over the k_eff smallest float32 d2 = (dx*dx + dy*dy) + dz*dz from p to the OTHER points of F (duplicates
+ * of p count, at 0), summed in double in ascending d2 order, divided by k_eff in double and rounded to float (0 when k_eff = 0).
+ * mean = sum d / n_f, stddev = sqrt(sum (d - mean)^2 / (n_f - 1)) (two-pass; 0 when n_f <= 1), threshold = mean + std_mul *
+ * stddev in double; p is kept unless (double)d_p > threshold, kept points in ascending index.  Non-finite points are nobody's
+ * neighbour, have no distance (NaN in mean_dist) and are never kept (pcl::removeNaNFromPointCloud first; PCL itself would keep
+ * NaN rows, with distance 0).  PCL's one-pass variance can go negative (NaN stddev, every point kept) on a cloud whose points
+ * all have about the same mean distance; the two-pass form cannot.  Sums are in double in a fixed order: two calls give
+ * identical bits.  mean_k in 1..128, std_mul finite (negative allowed, as in PCL); otherwise, for NULL xyz / out_idx / r or
+ * n < 0, GHICP_E_ARG.  A cloud without a finite point returns GHICP_OK with nothing kept (mean, stddev, threshold 0). */
+typedef struct ghicp_sor_result {
+  int n_finite, n_kept, k_eff;
+  int fallbacks;                 /* queries whose ring walk gave up and scanned every finite point (far outliers) */
+  double mean, stddev, threshold;
+  long long candidates;          /* points examined by every query together */
+  float stage_ms[5];             /* CUDA events: grid, distances, statistics, compaction, total */
+} ghicp_sor_result;
+/* xyz [n][3] (host); out_idx (capacity n) receives the kept indices, mean_dist [n] (may be NULL) every point's d_p */
+int ghicp_sor_filter(int device, const float *xyz, int n, int mean_k, double std_mul, int *out_idx, float *mean_dist,
+                     ghicp_sor_result *r);
+
 /* ---- BSC descriptor encoder on the GPU (SURVEY.md §8f row N2) -----------------------------------------------------
  * BSCEncoder<PointT>::extractBinaryFeatures (include/binary_feature_extraction.hpp:603-676, called at
  * test/ghicp_main.cpp:113-116 with voxel_side_num = 7, extract_radius = the keypoint NMS radius, dof_type 0 for the target
@@ -234,7 +256,8 @@ int ghicp_bsc_default_pattern(int voxel_side_num, int *pairs);
  * with non-finite points gives bit for bit what its finite points give: n_down, the down-sampled cloud, keypoints, the
  * bounding box, BSC and FPFH (the down-sampled cloud holds finite points only).  A cloud without a finite point (or n <= 0)
  * leaves nothing to register: ghicp_prep_run returns GHICP_E_ARG and *out stays NULL.
- * stage_ms [5] = {host->device copy, voxel filter, keypoints, BSC encoder, total} from CUDA events. */
+ * stage_ms [5] = {host->device copy, voxel filter, keypoints, BSC encoder, total} from CUDA events (the total includes the
+ * outlier filter of ghicp_prep_run_sor, which ghicp_prep_sor_info times). */
 typedef struct ghicp_prep_params {
   float voxel_size;           /* CFilter::voxelfilter resolution (:89-90) */
   float neighborhood_radius;  /* PCA radius (:96) */
@@ -247,6 +270,16 @@ typedef struct ghicp_prep_params {
 } ghicp_prep_params;
 typedef struct ghicp_prep ghicp_prep;
 int ghicp_prep_run(int device, const float *xyz, int n, const ghicp_prep_params *p, const int *bsc_pairs, ghicp_prep **out);
+/* ghicp_prep_run with ghicp_sor_filter (mean_k, std_mul) applied to the DOWN-SAMPLED cloud, between the voxel filter and
+ * the keypoints: the voxel filter evens a raw scan's range-dependent density first, so that the filter removes isolated
+ * returns rather than far-range surface.  The result's down-sampled cloud, bounding box, keypoints and everything derived
+ * from them are those of the kept points.  mean_k = 0 runs no filter (= ghicp_prep_run); otherwise mean_k in 1..128 and
+ * std_mul finite.  A filter that keeps nothing returns GHICP_E_ARG, as a cloud without a finite point does. */
+int ghicp_prep_run_sor(int device, const float *xyz, int n, const ghicp_prep_params *p, const int *bsc_pairs, int mean_k,
+                       double std_mul, ghicp_prep **out);
+/* the filter's result, the down-sampled cloud's size before it (n_voxel) and its time in ms (CUDA events); any output may
+ * be NULL.  GHICP_E_ARG for a result made without the filter. */
+int ghicp_prep_sor_info(const ghicp_prep *h, ghicp_sor_result *r, int *n_voxel, float *ms);
 int ghicp_prep_info(const ghicp_prep *h, int *n_down, int *n_kp, int *n_variants, float bbox_min[3], float bbox_max[3],
                     float stage_ms[5]);
 /* any of the outputs may be NULL: down_xyz [n_down][3], kp_idx [n_kp] (into the down-sampled cloud), kp_xyz [3][n_kp]
