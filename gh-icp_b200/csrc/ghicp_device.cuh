@@ -86,10 +86,19 @@ __device__ __forceinline__ double cd_exact(double ed, double fd, const CostParam
 // ---------------------------------------------------------------------------------------------
 // float32 3x3 SVD (one-sided Jacobi) and Umeyama from moments — PCL's
 // TransformationEstimationSVD → Eigen::umeyama (no scaling) as called at src/ghicp_reg.cpp:857-866.
+// A is first scaled by 2^-e, 2^e the power of two above its largest |entry| (JacobiSVD divides by the
+// largest entry too): the sweep's alpha * beta then neither overflows (points spread over more than
+// ~6e4 units) nor underflows, and every step commutes exactly with the power of two, so results are
+// bit-identical to the unscaled sweep wherever that one stayed in range.  Zero or non-finite A: e = 0.
 // ---------------------------------------------------------------------------------------------
 __device__ void svd3_f32(const float A[9], float U[9], float S[3], float V[9]) {
+  float amax = 0.f;
+  bool finite = true;
+  for (int i = 0; i < 9; ++i) { const float m = fabsf(A[i]); finite = finite && isfinite(m); amax = m > amax ? m : amax; }
+  int e = 0;
+  if (finite && amax > 0.f) frexpf(amax, &e);
   float a[9];
-  for (int i = 0; i < 9; ++i) a[i] = A[i];
+  for (int i = 0; i < 9; ++i) a[i] = ldexpf(A[i], -e);
   float v[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
   const float tol = 1e-7f;
   for (int sweep = 0; sweep < 30; ++sweep) {
@@ -162,6 +171,7 @@ __device__ void svd3_f32(const float A[9], float U[9], float S[3], float V[9]) {
     u[8] = u[0] * u[4] - u[3] * u[1];
   }
   for (int i = 0; i < 9; ++i) U[i] = u[i];
+  for (int k = 0; k < 3; ++k) S[k] = ldexpf(S[k], e);
 }
 __device__ __forceinline__ float det3_f32(const float m[9]) {
   return m[0] * (m[4] * m[8] - m[5] * m[7]) - m[1] * (m[3] * m[8] - m[5] * m[6]) +

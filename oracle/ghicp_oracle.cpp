@@ -45,10 +45,18 @@ static void init_lut() {
 // ---------------------------------------------------------------------------------------------
 // 3x3 float32 SVD by one-sided (Hestenes) Jacobi, singular values sorted descending like
 // Eigen::JacobiSVD.  A = U diag(S) V^T, row-major 3x3.  V is a product of rotations / column swaps.
+// Like JacobiSVD, A is first divided by its scale: by 2^e, the power of two above its largest |entry|, which
+// every step commutes with exactly (bit-identical results wherever the unscaled sweep stayed in range; no
+// overflow of alpha * beta past ~6e4 units of spread).  Zero or non-finite A is left unscaled.
 // ---------------------------------------------------------------------------------------------
 static void svd3_f32(const float A[9], float U[9], float S[3], float V[9]) {
+  float amax = 0.f;
+  bool finite = true;
+  for (int i = 0; i < 9; ++i) { const float m = std::fabs(A[i]); finite = finite && std::isfinite(m); amax = m > amax ? m : amax; }
+  int e = 0;
+  if (finite && amax > 0.f) std::frexp(amax, &e);
   float a[9];
-  for (int i = 0; i < 9; ++i) a[i] = A[i];
+  for (int i = 0; i < 9; ++i) a[i] = std::ldexp(A[i], -e);
   float v[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
   const float tol = 1e-7f;
   for (int sweep = 0; sweep < 30; ++sweep) {
@@ -128,6 +136,7 @@ static void svd3_f32(const float A[9], float U[9], float S[3], float V[9]) {
     u[8] = u[0] * u[4] - u[3] * u[1];
   }
   for (int i = 0; i < 9; ++i) U[i] = u[i];
+  for (int k = 0; k < 3; ++k) S[k] = std::ldexp(S[k], e);
 }
 
 static inline float det3_f32(const float m[9]) {

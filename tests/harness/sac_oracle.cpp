@@ -33,8 +33,13 @@ using namespace ghicp_sac;
 
 // ---- float32 SVD / Umeyama: the same text as the device code (gh-icp_b200/csrc/ghicp_device.cuh) and oracle/ghicp_oracle.cpp
 void svd3_f32(const float A[9], float U[9], float S[3], float V[9]) {
+  float amax = 0.f;   // scale by 2^-e, 2^e the power of two above max |A_ij| (zero or non-finite A: e = 0)
+  bool finite = true;
+  for (int i = 0; i < 9; ++i) { const float m = std::fabs(A[i]); finite = finite && std::isfinite(m); amax = m > amax ? m : amax; }
+  int e = 0;
+  if (finite && amax > 0.f) std::frexp(amax, &e);
   float a[9];
-  for (int i = 0; i < 9; ++i) a[i] = A[i];
+  for (int i = 0; i < 9; ++i) a[i] = std::ldexp(A[i], -e);
   float v[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
   const float tol = 1e-7f;
   for (int sweep = 0; sweep < 30; ++sweep) {
@@ -107,6 +112,7 @@ void svd3_f32(const float A[9], float U[9], float S[3], float V[9]) {
     u[8] = u[0] * u[4] - u[3] * u[1];
   }
   for (int i = 0; i < 9; ++i) U[i] = u[i];
+  for (int k = 0; k < 3; ++k) S[k] = std::ldexp(S[k], e);
 }
 float det3_f32(const float m[9]) {
   return m[0] * (m[4] * m[8] - m[5] * m[7]) - m[1] * (m[3] * m[8] - m[5] * m[6]) + m[2] * (m[3] * m[7] - m[4] * m[6]);
@@ -181,6 +187,11 @@ void move(const float R[9], const float t[3], const float *p, float o[3]) {
 }  // namespace
 
 extern "C" {
+
+// the float32 Umeyama of the hypotheses (and of icp_oracle.cpp's steps) on given float32 moments: R row-major [9], t [3]
+void sac_oracle_umeyama(const float *mu_s, const float *mu_d, const float *sigma, float *R, float *t) {
+  umeyama_f32(mu_s, mu_d, sigma, R, t);
+}
 
 // the k_eff nearest target histograms of the source histograms idx[m] (ascending (d2, index)); returns k_eff
 int sac_oracle_feat_knn(const float *Fs, const int *idx, int m, const float *Ft, int nt, int k, int *out) {

@@ -36,6 +36,7 @@ def lib():
                                  ip, ip, ip, fp, u64p, dp, dp, ip]
         L.sac_oracle_feat_knn.argtypes = [fp, ip, C.c_int, fp, C.c_int, C.c_int, ip]
         L.sac_oracle_nearest.argtypes = [fp, C.c_int, fp, C.c_int, fp, C.c_float, fp]
+        L.sac_oracle_umeyama.argtypes = [fp, fp, fp, fp, fp]
         _lib = L
     return _lib
 
@@ -83,6 +84,16 @@ def nearest(P, Q, rt12, threshold):
     lib().sac_oracle_nearest(P.ctypes.data_as(fp), len(P), Q.ctypes.data_as(fp), len(Q), rt12.ctypes.data_as(fp), threshold,
                              out.ctypes.data_as(fp))
     return out
+
+
+def umeyama(mu_s, mu_d, sigma):
+    """The oracle's float32 Umeyama on float32 moments (sigma row-major 3x3): (R 3x3, t) as float32."""
+    mu_s, mu_d = np.ascontiguousarray(mu_s, np.float32), np.ascontiguousarray(mu_d, np.float32)
+    sigma = np.ascontiguousarray(sigma, np.float32).reshape(9)
+    R, t = np.zeros(9, np.float32), np.zeros(3, np.float32)
+    lib().sac_oracle_umeyama(mu_s.ctypes.data_as(fp), mu_d.ctypes.data_as(fp), sigma.ctypes.data_as(fp), R.ctypes.data_as(fp),
+                             t.ctypes.data_as(fp))
+    return R.reshape(3, 3), t
 
 
 def build_emu_harness(out_dir):
