@@ -1,5 +1,6 @@
 // ghicp_grid.cuh — the cell-sorted uniform point grid of the pre-processing kernels (ghicp_prep.cu: radius PCA, NMS, the
-// FPFH k-NN) and of the SAC-IA scoring (ghicp_sac.cu), which runs exact nearest-neighbour queries against the same index.
+// FPFH k-NN, SOR) and of the SAC-IA scoring (ghicp_sac.cu), which runs exact nearest-neighbour queries against the same
+// index, and the ring walk those exact searches share.
 // Points are sorted by cell key; ucell lists the occupied cells in key order and cstart their first sorted position.
 #pragma once
 #include "ghicp_internal.h"
@@ -67,18 +68,61 @@ __device__ __forceinline__ float knn_d2(float qx, float qy, float qz, const floa
   return (dx * dx + dy * dy) + dz * dz;
 }
 
-// A grid over all n points of d_xyz with the cell rule of the FPFH k-NN (k_eff neighbours wanted per query), for ring
-// searches: gx / gy / gz = the largest occupied cell coordinate per axis, slack = cells of margin for the float32 rounding
-// of cell_coord.
+// A grid for ring searches as the kernels read it (prep_point_grid).
+struct RingGrid {
+  GridArgs g;
+  int gm[3];                             // largest occupied cell coordinate per axis
+  float mx[3];                           // maximum of the finite points' box (the minimum is g.mnx, g.mny, g.mnz)
+  double cell, slack;                    // cell edge; cells of margin for the float32 rounding of cell_coord
+};
+
+// The ring walk of the exact nearest-neighbour searches (k_knn, k_sor_dist, SAC-IA's sac_nn_d2) from the cell (cx, cy, cz):
+// rings 0, 1, ... of grid columns, dx then dy; a column on the ring's wall is its whole z-range clipped to the grid, one
+// inside the wall its floor cell, then its ceiling cell.  col(s0, s1) receives each column's run [s0, s1) of sorted
+// positions.  After each ring the walk is settled once the ring reaches the far side of the grid on every axis, or once
+// bound() (a squared distance; +inf while nothing bounds the search) lies below every point of an unvisited cell, which is at
+// least (ring - slack) cell edges away on some axis.  The (1 - 1e-5) margin is far more than the float32 rounding of knn_d2,
+// and it is what keeps the results exact.  Returns false when rings 0 .. cap did not settle it.
+// The scalar geometry is read once into locals (see GridRegs); the columns go through the per-thread copy r.
+template <class Col, class Bound>
+__device__ __forceinline__ bool ring_walk(const GridRegs &r, const RingGrid &G, int cx, int cy, int cz, int cap, Col &&col,
+                                          Bound &&bound) {
+  const int gx = G.gm[0], gy = G.gm[1], gz = G.gm[2];
+  const double cell = G.cell, slack = G.slack;
+  int rmax = cx;                         // the ring that reaches the far side of the grid on every axis
+  rmax = max(rmax, gx - cx); rmax = max(rmax, cy); rmax = max(rmax, gy - cy); rmax = max(rmax, cz); rmax = max(rmax, gz - cz);
+  for (int ring = 0; ring <= cap; ++ring) {
+    for (int dx = -ring; dx <= ring; ++dx) {
+      const int x = cx + dx;
+      if (x < 0 || x > gx) continue;
+      for (int dy = -ring; dy <= ring; ++dy) {
+        const int y = cy + dy;
+        if (y < 0 || y > gy) continue;
+        const bool wall = max(abs(dx), abs(dy)) == ring;
+        for (int zs = 0; zs < (wall ? 1 : 2); ++zs) {
+          int zlo, zhi;
+          if (wall) { zlo = max(cz - ring, 0); zhi = min(cz + ring, gz); }
+          else { zlo = zhi = zs == 0 ? cz - ring : cz + ring; if (zlo < 0 || zlo > gz) continue; }
+          if (zlo > zhi) continue;
+          col(r.cstart[lower_cell(r, cell_key(x, y, zlo))], r.cstart[lower_cell(r, cell_key(x, y, zhi) + 1)]);
+        }
+      }
+    }
+    if (ring >= rmax) return true;
+    const double lb = ((double)ring - slack) * cell;
+    if (lb > 0.0 && bound() < lb * lb * (1.0 - 1e-5)) return true;
+  }
+  return false;
+}
+
 struct GridBufs {   // the device arrays GridArgs points into
   DevBuf<int> order, cstart; DevBuf<pu64> ucell; DevBuf<float4> sorted;
 };
+// A grid over all n points of d_xyz with the cell rule of the FPFH k-NN (k_eff neighbours wanted per query), for ring
+// searches, and the device arrays it reads.
 struct PointGrid {
-  GridArgs g{};
-  int gx = 0, gy = 0, gz = 0;
-  float mx[3] = {0.f, 0.f, 0.f};         // maximum of the finite points' box (the minimum is g.mnx, g.mny, g.mnz)
+  RingGrid rg{};
   int nfin = 0;                          // finite points
-  double cell = 0.0, slack = 0.0;
   GridBufs buf;
 };
 // cell edge = the k-NN rule times cell_scale (if > 0), at least min_cell, at least the extent / 2^20 (21-bit key fields)

@@ -13,7 +13,7 @@
 //   k_icp_sum<1, 2>     two-pass FP64 moments of the kept pairs over fixed point blocks and a fixed tree (means first, then
 //   k_icp_total         the demeaned cross-covariance), as k_ov_reduce / k_ov_total: no floating-point atomic
 //   k_icp_solve         one thread: the float32 Umeyama of the loop, F <- T F, DefaultConvergenceCriteria
-//   k_icp_move          W <- T W (sac_move's formula)
+//   k_icp_move          W <- T W (ov_move's formula)
 // Point-to-plane (metric 1, DESIGN.md §3.14: the reference's CRegistration::ptplicp_reg, src/common_reg.cpp:123-199, PCL's
 // IterativeClosestPointWithNormals with TransformationEstimationPointToPlaneLLS) keeps every stage above but the estimate:
 //   k_icp_sum<1>        as above: the kept pairs' count, sum s (-> the centre m), sum d
@@ -101,23 +101,8 @@ __global__ void k_icp_move(const float *src, float *dst, long long n, const floa
 __global__ void k_icp_keys(const float *__restrict__ W, long long n, const OvGrid G, pu64 *__restrict__ keys, int *__restrict__ vals) {
   const long long t = (long long)blockIdx.x * IC_T + threadIdx.x;
   if (t >= n) return;
-  int c[3];
-  for (int k = 0; k < 3; ++k) {
-    const double f = floor(((double)W[3 * t + k] - G.mn[k]) / G.cell);
-    c[k] = !(f > 0.0) ? 0 : (f > (double)G.gm[k] ? G.gm[k] : (int)f);
-  }
-  keys[t] = cell_key(c[0], c[1], c[2]);
+  keys[t] = ov_cell_key(G, W + 3 * t);
   vals[t] = (int)t;
-}
-
-// warp-reduced integer work counters (every lane of the warp must call it)
-__device__ __forceinline__ void icp_add_work(unsigned long long cells, unsigned long long cand, unsigned long long *work) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    cells += __shfl_xor_sync(0xffffffffu, cells, o);
-    cand += __shfl_xor_sync(0xffffffffu, cand, o);
-  }
-  if ((threadIdx.x & 31) == 0 && (cells | cand)) { atomicAdd(work, cells); atomicAdd(work + 1, cand); }
 }
 
 // j(i) and d_i: the nearest target point of W_i in (d2, index) order, -1 / +inf for a non-finite W_i; GATE (GICP): no pair
@@ -129,13 +114,13 @@ __global__ void __launch_bounds__(IC_T) k_icp_query(const float *__restrict__ W,
   unsigned long long cells = 0ull, cand = 0ull;
   if (t < n) {
     const long long i = perm[t];
-    const GridRegs r = grid_regs(G.g);   // per-thread registers, see k_pca
+    const GridRegs r = grid_regs(G.rg.g);   // per-thread registers, see k_pca
     int j = -1;
     const float d = ov_nearest<true>(r, G, W[3 * i], W[3 * i + 1], W[3 * i + 2], (double)INFINITY, -1.f, cells, cand, j);
     d2[i] = d;
     corr[i] = GATE && !((double)d < GICP_GATE) ? -1 : j;
   }
-  icp_add_work(cells, cand, dev->h.work);
+  ov_add_work(cells, cand, dev->h.work);
 }
 
 // reciprocal: the distinct targets of the pairs, compacted into list[0 .. n_rev) (any order: results are stored per target)
@@ -160,12 +145,12 @@ __global__ void __launch_bounds__(IC_T) k_icp_rev(const float *__restrict__ Q, c
   unsigned long long cells = 0ull, cand = 0ull;
   if (t < dev->n_rev) {
     const int j = list[t];
-    const GridRegs r = grid_regs(Gw.g);
+    const GridRegs r = grid_regs(Gw.rg.g);
     int i = -1;
     ov_nearest<true>(r, Gw, Q[3 * (size_t)j], Q[3 * (size_t)j + 1], Q[3 * (size_t)j + 2], (double)INFINITY, -1.f, cells, cand, i);
     rev[j] = i;
   }
-  icp_add_work(cells, cand, dev->h.work);
+  ov_add_work(cells, cand, dev->h.work);
 }
 __global__ void k_icp_recip(int *__restrict__ corr, long long n, const int *__restrict__ rev) {
   const long long i = (long long)blockIdx.x * IC_T + threadIdx.x;

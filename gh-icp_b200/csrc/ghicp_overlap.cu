@@ -4,9 +4,10 @@
 //   target grid   B's cell-sorted grid (prep_point_grid, the k-NN cell rule with 8 points per cell): independent of the
 //                 threshold, so one grid serves every call on the same target (ghicp_prep_overlap keeps it)
 //   k_ov_keys     (fitness mode) the moved points' clamped B-cell keys, radix-sorted into the query order
-//   k_ov_query    the hot path: one exact nearest-neighbour query per point of A, a ring walk over B's grid like SAC-IA's
-//                 sac_nn_d2, but every column is culled by a lower bound on its distance (cell extents clipped to B's box)
-//                 and the walk stops once a true lower bound on every unvisited cell passes min(best, limit).  A query
+//   k_ov_query    the hot path: one exact nearest-neighbour query per point of A, a ring walk over B's grid like
+//                 ghicp_grid.cuh's ring_walk, but every column is culled by a lower bound on its distance (cell extents
+//                 clipped to B's box) and the walk stops once a true lower bound on every unvisited cell passes
+//                 min(best, limit).  A query
 //                 outside B's box walks only the cells that could hold a closer point.  Work counters: integer atomics.
 //   k_ov_reduce   counts and double sums over contiguous point blocks, each in a fixed tree order; k_ov_total sums the
 //   k_ov_total    blocks in a fixed order: two runs give identical bits, and no floating-point atomic is used
@@ -53,17 +54,12 @@ __global__ void __launch_bounds__(OV_T) k_ov_query(const OvArgs a, const OvGrid 
   unsigned long long cells = 0ull, cand = 0ull;
   if (t < a.n) {
     const long long i = a.perm ? (long long)a.perm[t] : t;
-    const GridRegs r = grid_regs(G.g);   // per-thread registers, see k_pca
+    const GridRegs r = grid_regs(G.rg.g);   // per-thread registers, see k_pca
     float x, y, z;
     ov_move(a.rt, a.A[3 * i], a.A[3 * i + 1], a.A[3 * i + 2], x, y, z);
     a.d2[i] = ov_nn_d2(r, G, x, y, z, a.lim, a.hit, cells, cand);
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    cells += __shfl_xor_sync(0xffffffffu, cells, o);
-    cand += __shfl_xor_sync(0xffffffffu, cand, o);
-  }
-  if ((threadIdx.x & 31) == 0 && (cells | cand)) { atomicAdd(a.work, cells); atomicAdd(a.work + 1, cand); }
+  ov_add_work(cells, cand, a.work);
 }
 
 // clamped B-cell key of each moved point of A, with its index (the cell order of the queries)
@@ -72,12 +68,7 @@ __global__ void k_ov_keys(const OvArgs a, const OvGrid G, pu64 *__restrict__ key
   if (t >= a.n) return;
   float v[3];
   ov_move(a.rt, a.A[3 * t], a.A[3 * t + 1], a.A[3 * t + 2], v[0], v[1], v[2]);
-  int c[3];
-  for (int k = 0; k < 3; ++k) {
-    const double f = floor(((double)v[k] - G.mn[k]) / G.cell);
-    c[k] = !(f > 0.0) ? 0 : (f > (double)G.gm[k] ? G.gm[k] : (int)f);
-  }
-  keys[t] = cell_key(c[0], c[1], c[2]);
+  keys[t] = ov_cell_key(G, v);
   vals[t] = (int)t;
 }
 

@@ -882,7 +882,7 @@ cudaError_t prep_bsc_extract(cudaStream_t st, const float *d_xyz, int n, const i
 // PCL is not pinned, so the definition is the canonical one restated in tests/harness/fpfh_oracle.cpp; these kernels and
 // that oracle agree bit for bit (k-NN lists, normals) and up to the double atan2 of the device math library (histograms).
 //   k_knn      exact k nearest neighbours of every point, ascending (d2, index): rings of grid columns outward from the
-//              query's cell (a column's z-range is one contiguous run of the cell-sorted points), stopped once the k-th
+//              query's cell (ring_walk; a column's z-range is one contiguous run of the cell-sorted points), stopped once the k-th
 //              distance is below a conservative bound on every unvisited cell, exhaustive scan past FPFH_RING_CAP rings
 //   k_normals  covariance of the k neighbours (k_pca's double sums), smallest eigenvector (bsc_jacobi3), flip to the origin
 //   k_spfh     3 x 11 bin SPFH of every point a requested histogram reads (all points for the whole-cloud call)
@@ -894,23 +894,13 @@ constexpr int FPFH_KMAX = 32;       // largest k: the top-k list lives in regist
 constexpr int FPFH_RING_CAP = 4;    // a query not settled after this many rings scans the whole cloud (far outliers)
 
 struct KnnArgs {
-  GridArgs g;
+  RingGrid rg;
   int n, k;                         // k = k_eff = min(k, n)
-  int gx, gy, gz;                   // largest occupied cell coordinate per axis
-  double cell, slack;               // cell edge; cells of margin for the float32 rounding of cell_coord
   int *nb_idx; float *nb_d2;        // [n][k]
   unsigned long long *cand;         // candidates examined, summed over all queries
   int *fallbacks;                   // queries that took the exhaustive scan
   int *deferred, *n_deferred;       // optional: such queries are listed here instead (rows not written), for a wider scan
 };
-
-// cells (x, y, zlo .. zhi) = one run of the sorted order
-__device__ __forceinline__ void knn_column(const GridRegs &g, int x, int y, int zlo, int zhi, float qx, float qy, float qz,
-                                           pu64 (&key)[FPFH_KMAX], long long &cand) {
-  const int s0 = g.cstart[lower_cell(g, cell_key(x, y, zlo))], s1 = g.cstart[lower_cell(g, cell_key(x, y, zhi) + 1)];
-  cand += s1 - s0;
-  for (int s = s0; s < s1; ++s) knn_insert(key, knn_key(knn_d2(qx, qy, qz, g.sorted[s]), g.order[s]));
-}
 
 __global__ void k_knn(const KnnArgs a) {
   __shared__ unsigned long long s_cand;
@@ -919,42 +909,25 @@ __global__ void k_knn(const KnnArgs a) {
   __syncthreads();
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t < a.n) {
-    const GridRegs r = grid_regs(a.g);   // per-thread registers, see k_pca
+    const GridArgs &g = a.rg.g;
+    const GridRegs r = grid_regs(g);     // per-thread registers, see k_pca
     const int i = r.order[t];            // threads of a warp take points of the same cell (see k_pca)
-    const float qx = a.g.xyz[3 * (size_t)i], qy = a.g.xyz[3 * (size_t)i + 1], qz = a.g.xyz[3 * (size_t)i + 2];
-    const int k = a.k, gx = a.gx, gy = a.gy, gz = a.gz;
+    const float qx = g.xyz[3 * (size_t)i], qy = g.xyz[3 * (size_t)i + 1], qz = g.xyz[3 * (size_t)i + 2];
+    const int k = a.k;
     if (!finite3(qx, qy, qz)) {   // a non-finite point's list is itself at distance 0: an isolated point's zero histogram
       for (int j = 0; j < k; ++j) { a.nb_idx[(size_t)i * k + j] = i; a.nb_d2[(size_t)i * k + j] = 0.f; }
     } else {
-      const int cx = cell_coord(qx, a.g.mnx, a.g.inv), cy = cell_coord(qy, a.g.mny, a.g.inv), cz = cell_coord(qz, a.g.mnz, a.g.inv);
+      const int cx = cell_coord(qx, g.mnx, g.inv), cy = cell_coord(qy, g.mny, g.inv), cz = cell_coord(qz, g.mnz, g.inv);
       pu64 key[FPFH_KMAX];
 #pragma unroll
       for (int j = 0; j < FPFH_KMAX; ++j) key[j] = (j < FPFH_KMAX - k) ? 0ull : ~0ull;
       long long cand = 0;
-      int rmax = cx;                       // the ring that reaches the far side of the grid on every axis
-      rmax = max(rmax, gx - cx); rmax = max(rmax, cy); rmax = max(rmax, gy - cy); rmax = max(rmax, cz); rmax = max(rmax, gz - cz);
-      bool done = false;
-      for (int ring = 0; ring <= FPFH_RING_CAP && !done; ++ring) {
-        for (int dx = -ring; dx <= ring; ++dx) {
-          const int x = cx + dx;
-          if (x < 0 || x > gx) continue;
-          for (int dy = -ring; dy <= ring; ++dy) {
-            const int y = cy + dy;
-            if (y < 0 || y > gy) continue;
-            if (max(abs(dx), abs(dy)) == ring) {   // a column on the ring's wall: its whole z-range
-              const int zlo = max(cz - ring, 0), zhi = min(cz + ring, gz);
-              if (zlo <= zhi) knn_column(r, x, y, zlo, zhi, qx, qy, qz, key, cand);
-            } else {                               // inside the wall: the floor and the ceiling cell
-              if (cz - ring >= 0) knn_column(r, x, y, cz - ring, cz - ring, qx, qy, qz, key, cand);
-              if (cz + ring <= gz) knn_column(r, x, y, cz + ring, cz + ring, qx, qy, qz, key, cand);
-            }
-          }
-        }
-        if (ring >= rmax) { done = true; break; }
-        // every point of an unvisited cell lies at least (ring - slack) cell edges away on some axis
-        const double lb = ((double)ring - a.slack) * a.cell;
-        if (lb > 0.0 && key[FPFH_KMAX - 1] != ~0ull && (double)knn_key_d2(key[FPFH_KMAX - 1]) < lb * lb * (1.0 - 1e-5)) done = true;
-      }
+      const bool done = ring_walk(r, a.rg, cx, cy, cz, FPFH_RING_CAP,
+          [&](int s0, int s1) {
+            cand += s1 - s0;
+            for (int s = s0; s < s1; ++s) knn_insert(key, knn_key(knn_d2(qx, qy, qz, r.sorted[s]), r.order[s]));
+          },
+          [&] { return key[FPFH_KMAX - 1] == ~0ull ? (double)INFINITY : (double)knn_key_d2(key[FPFH_KMAX - 1]); });
       if (!done) {   // far outlier (or a grid too fine for this cloud): exact by exhaustion
         atomicAdd(&s_fb, 1);
         if (a.deferred) {
@@ -1345,12 +1318,13 @@ cudaError_t prep_point_grid(cudaStream_t st, const float *d_xyz, int n, int ke, 
   if (cell < min_cell) cell = min_cell;
   if (cell < emax / 1048576.0) cell = emax / 1048576.0;   // cell coordinates stay below 2^20 (21-bit key fields)
   CUDA_TRY(build_grid(st, d_xyz, nullptr, n, (float)cell, &g, &out->buf));
-  out->g = g;
-  out->gx = cell_coord_host(mx[0], g.mnx, g.inv); out->gy = cell_coord_host(mx[1], g.mny, g.inv); out->gz = cell_coord_host(mx[2], g.mnz, g.inv);
-  for (int a = 0; a < 3; ++a) out->mx[a] = mx[a];
-  out->cell = (double)(float)cell;
-  const int gmax = out->gx > out->gy ? (out->gx > out->gz ? out->gx : out->gz) : (out->gy > out->gz ? out->gy : out->gz);
-  out->slack = 0.01 + (gmax + 2.0) / 1048576.0;
+  RingGrid &G = out->rg;
+  G.g = g;
+  G.gm[0] = cell_coord_host(mx[0], g.mnx, g.inv); G.gm[1] = cell_coord_host(mx[1], g.mny, g.inv); G.gm[2] = cell_coord_host(mx[2], g.mnz, g.inv);
+  for (int a = 0; a < 3; ++a) G.mx[a] = mx[a];
+  G.cell = (double)(float)cell;
+  const int gmax = G.gm[0] > G.gm[1] ? (G.gm[0] > G.gm[2] ? G.gm[0] : G.gm[2]) : (G.gm[1] > G.gm[2] ? G.gm[1] : G.gm[2]);
+  G.slack = 0.01 + (gmax + 2.0) / 1048576.0;
   return cudaSuccess;
 }
 cudaError_t prep_sort_pairs(cudaStream_t st, pu64 *keys, int *vals, int n) { return sort_pairs(keys, vals, n, st); }
@@ -1369,9 +1343,7 @@ cudaError_t knn_normals(cudaStream_t st, const float *d_xyz, int n, int k, float
   const int ke = k < pg->nfin ? k : pg->nfin;
   *ke_out = ke;
   KnnArgs a{};
-  a.g = pg->g; a.n = n; a.k = ke;
-  a.gx = pg->gx; a.gy = pg->gy; a.gz = pg->gz;
-  a.cell = pg->cell; a.slack = pg->slack;
+  a.rg = pg->rg; a.n = n; a.k = ke;
   CUDA_TRY(nb_idx->alloc((size_t)n * ke)); CUDA_TRY(nb_d2->alloc((size_t)n * ke));
   CUDA_TRY(cand->alloc(1)); CUDA_TRY(fb->alloc(1));
   CUDA_TRY(cudaMemsetAsync(cand->get(), 0, sizeof(pu64), st)); CUDA_TRY(cudaMemsetAsync(fb->get(), 0, sizeof(int), st));
@@ -1425,7 +1397,7 @@ cudaError_t prep_fpfh(cudaStream_t st, const float *d_xyz, int n, const int *d_i
     CUDA_TRY(cudaMemcpyAsync(&c, d_cand.get(), sizeof(c), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemcpyAsync(&fb, d_fb.get(), sizeof(fb), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
-    stats->candidates = (long long)c; stats->fallbacks = fb; stats->cell = (float)pg.cell; stats->queries = n;
+    stats->candidates = (long long)c; stats->fallbacks = fb; stats->cell = (float)pg.rg.cell; stats->queries = n;
   }
   return cudaGetLastError();
 }
@@ -1546,8 +1518,8 @@ cudaError_t prep_fpfh_radius(cudaStream_t st, const float *d_xyz, int n, const i
 // Statistical outlier removal (DESIGN.md §3.16): CFilter::SORFilter (include/filter.hpp:90-102), PCL's
 // StatisticalOutlierRemoval, on the canonical definition stated with ghicp_sor_filter in include/ghicp_b200.h.
 //   k_knn + k_sor_listmean   k_eff <= 31: k_knn's k_eff + 1 nearest in registers, the point itself dropped, summed per thread
-//   k_sor_dist     larger k_eff: one warp per finite point, k_knn's ring walk (same grid, stopping bound and exhaustive fallback) over
-//                  batches of 32 candidates, one per lane.  The k_eff smallest (d2, index) keys, k_eff up to 128, stay sorted
+//   k_sor_dist     larger k_eff: one warp per finite point, k_knn's grid, ring_walk with k_knn's cap and bound, and its
+//                  exhaustive fallback, over batches of 32 candidates, one per lane.  The k_eff smallest (d2, index) keys, k_eff up to 128, stay sorted
 //                  in a per-warp list in shared memory; a batch's keys below the current k-th key are merged into it by rank.
 //                  Only the mean distance leaves the warp: one float per point, no [n][k] lists.
 //   k_sor_partial  fixed-order double sums of d (pass 0) or of (d - mean)^2 (pass 1), one per block of a fixed grid
@@ -1563,11 +1535,9 @@ constexpr int SOR_DEFER_BLOCKS = 32;  // grid of the warp kernel over k_knn's de
 constexpr int SOR_RED = 256;        // blocks of the partial sums = threads of the final sum (fixed: it fixes the summation order)
 
 struct SorArgs {
-  GridArgs g;
+  RingGrid rg;
   int n, nfin, k;                   // points; the finite ones = the first nfin sorted positions (non-finite ones sort last); k = k_eff
-  int gx, gy, gz;                   // largest occupied cell coordinate per axis
-  double cell, slack;               // as KnnArgs
-  float *dist;                      // [n]
+  float *dist;                     // [n]
   unsigned long long *cand;         // candidates examined, summed over all queries
   int *fallbacks;                   // queries that took the exhaustive scan
   const int *qlist, *nq;            // optional: only the points qlist[0 .. *nq) (k_knn's deferred far outliers), grid-strided;
@@ -1623,12 +1593,6 @@ __device__ __forceinline__ void sor_scan(const GridRegs &g, int s0, int s1, int 
     sor_merge(cur, nxt, k, lane, c, kth);
   }
 }
-__device__ __forceinline__ void sor_column(const GridRegs &g, int x, int y, int zlo, int zhi, int i, float qx, float qy, float qz,
-                                           int k, int lane, pu64 *&cur, pu64 *&nxt, pu64 &kth, long long &cand) {
-  const int s0 = g.cstart[lower_cell(g, cell_key(x, y, zlo))], s1 = g.cstart[lower_cell(g, cell_key(x, y, zhi) + 1)];
-  cand += s1 - s0;
-  sor_scan(g, s0, s1, i, qx, qy, qz, k, lane, cur, nxt, kth);
-}
 __device__ __forceinline__ void sor_reset(pu64 *cur, int k, int lane, pu64 &kth) {
   for (int t = lane; t < k; t += 32) cur[t] = ~0ull;
   __syncwarp();
@@ -1643,13 +1607,14 @@ __global__ void __launch_bounds__(SOR_T) k_sor_dist(const SorArgs a) {
   __syncthreads();
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int t = blockIdx.x * (SOR_T / 32) + w;   // sorted position: the warps of a block take points of the same cells
-  if (!a.qlist && t >= a.nfin && t < a.n && lane == 0) a.dist[a.g.order[t]] = __uint_as_float(0x7fc00000u);   // non-finite
+  const GridArgs &g = a.rg.g;
+  if (!a.qlist && t >= a.nfin && t < a.n && lane == 0) a.dist[g.order[t]] = __uint_as_float(0x7fc00000u);   // non-finite
   const int nq = a.qlist ? *a.nq : a.nfin;
   const int step = a.qlist ? gridDim.x * (SOR_T / 32) : nq;   // without a list: at most one query per warp
-  const GridRegs r = grid_regs(a.g);     // per-thread registers, see k_pca
+  const GridRegs r = grid_regs(g);       // per-thread registers, see k_pca
   for (int q = t; q < nq; q += step) {
     const int i = a.qlist ? a.qlist[q] : r.order[q];
-    const float qx = a.g.xyz[3 * (size_t)i], qy = a.g.xyz[3 * (size_t)i + 1], qz = a.g.xyz[3 * (size_t)i + 2];
+    const float qx = g.xyz[3 * (size_t)i], qy = g.xyz[3 * (size_t)i + 1], qz = g.xyz[3 * (size_t)i + 2];
     const int k = a.k;
     float d = 0.f;                       // k_eff = 0 (one finite point): distance 0
     long long cand = 0;
@@ -1657,31 +1622,13 @@ __global__ void __launch_bounds__(SOR_T) k_sor_dist(const SorArgs a) {
     if (k > 0) {
       pu64 *cur = s_list[w][0], *nxt = s_list[w][1], kth;
       sor_reset(cur, k, lane, kth);
-      const int cx = cell_coord(qx, a.g.mnx, a.g.inv), cy = cell_coord(qy, a.g.mny, a.g.inv), cz = cell_coord(qz, a.g.mnz, a.g.inv);
-      const int gx = a.gx, gy = a.gy, gz = a.gz;
-      int rmax = cx;                     // the ring that reaches the far side of the grid on every axis
-      rmax = max(rmax, gx - cx); rmax = max(rmax, cy); rmax = max(rmax, gy - cy); rmax = max(rmax, cz); rmax = max(rmax, gz - cz);
-      bool done = false;
-      for (int ring = 0; ring <= FPFH_RING_CAP && !done; ++ring) {   // k_knn's walk
-        for (int dx = -ring; dx <= ring; ++dx) {
-          const int x = cx + dx;
-          if (x < 0 || x > gx) continue;
-          for (int dy = -ring; dy <= ring; ++dy) {
-            const int y = cy + dy;
-            if (y < 0 || y > gy) continue;
-            if (max(abs(dx), abs(dy)) == ring) {
-              const int zlo = max(cz - ring, 0), zhi = min(cz + ring, gz);
-              if (zlo <= zhi) sor_column(r, x, y, zlo, zhi, i, qx, qy, qz, k, lane, cur, nxt, kth, cand);
-            } else {
-              if (cz - ring >= 0) sor_column(r, x, y, cz - ring, cz - ring, i, qx, qy, qz, k, lane, cur, nxt, kth, cand);
-              if (cz + ring <= gz) sor_column(r, x, y, cz + ring, cz + ring, i, qx, qy, qz, k, lane, cur, nxt, kth, cand);
-            }
-          }
-        }
-        if (ring >= rmax) { done = true; break; }
-        const double lb = ((double)ring - a.slack) * a.cell;
-        if (lb > 0.0 && kth != ~0ull && (double)knn_key_d2(kth) < lb * lb * (1.0 - 1e-5)) done = true;
-      }
+      const int cx = cell_coord(qx, g.mnx, g.inv), cy = cell_coord(qy, g.mny, g.inv), cz = cell_coord(qz, g.mnz, g.inv);
+      const bool done = ring_walk(r, a.rg, cx, cy, cz, FPFH_RING_CAP,
+          [&](int s0, int s1) {
+            cand += s1 - s0;
+            sor_scan(r, s0, s1, i, qx, qy, qz, k, lane, cur, nxt, kth);
+          },
+          [&] { return kth == ~0ull ? (double)INFINITY : (double)knn_key_d2(kth); });
       if (!done) {                       // far outlier: exact by exhaustion over the finite points
         sor_reset(cur, k, lane, kth);
         sor_scan(r, 0, a.nfin, i, qx, qy, qz, k, lane, cur, nxt, kth);
@@ -1813,16 +1760,12 @@ cudaError_t prep_sor_filter(cudaStream_t st, const float *d_xyz, int n, int mean
   CUDA_TRY(cudaMemsetAsync(d_cand.get(), 0, sizeof(pu64), st)); CUDA_TRY(cudaMemsetAsync(d_fb.get(), 0, sizeof(int), st));
   CUDA_TRY(cudaEventRecord(ev[1], st));
   SorArgs a{};
-  a.g = pg.g; a.n = n; a.nfin = nfin; a.k = k;
-  a.gx = pg.gx; a.gy = pg.gy; a.gz = pg.gz;
-  a.cell = pg.cell; a.slack = pg.slack;
+  a.rg = pg.rg; a.n = n; a.nfin = nfin; a.k = k;
   a.dist = d_dist; a.cand = d_cand.get(); a.fallbacks = d_fb.get();
   if (lists) {
     if (nfin > 0) {
       KnnArgs b{};
-      b.g = pg.g; b.n = n; b.k = k + 1;
-      b.gx = pg.gx; b.gy = pg.gy; b.gz = pg.gz;
-      b.cell = pg.cell; b.slack = pg.slack;
+      b.rg = pg.rg; b.n = n; b.k = k + 1;
       b.nb_idx = nb_idx.get(); b.nb_d2 = nb_d2.get(); b.cand = d_cand.get(); b.fallbacks = d_fb.get();
       b.deferred = d_def.get(); b.n_deferred = d_def.get() + nfin;
       GHICP_LAUNCH(k_knn, blocks(n), PT, 0, st, b);

@@ -8,8 +8,8 @@
 //                    top-k in registers as sorted (d2, index) keys (the k_knn idiom)
 //   k_sac_estimate   one thread per hypothesis: the correspondence picks, FP64 moments, the hot path's float32 Umeyama
 //   k_sac_score      the hot path: a CTA per (block of hypotheses, chunk of source points in shared memory), one exact
-//                    nearest-neighbour query per (hypothesis, point) against the target's cell grid (ghicp_grid.cuh, the
-//                    grid and ring walk of k_knn with k = 1, stopped once the ring bound passes min(best, sqrt(thr))), the
+//                    nearest-neighbour query per (hypothesis, point) against the target's cell grid (ghicp_grid.cuh: the
+//                    grid and ring_walk of k_knn with k = 1, stopped once the ring bound passes min(best, sqrt(thr))), the
 //                    truncated error of each point as a 2^-32 fixed-point integer, warp-reduced, one 64-bit atomic per CTA
 //                    and hypothesis: the sums are exact in any order
 //   k_sac_pick       smallest (error, h) over the valid hypotheses
@@ -25,6 +25,7 @@
 #include "ghicp_internal.h"
 #include "ghicp_device.cuh"
 #include "ghicp_grid.cuh"
+#include "ghicp_ovwalk.cuh"
 #include "ghicp_sac.h"
 
 namespace ghicp_b200 {
@@ -56,13 +57,6 @@ struct SacArgs {
   int *corr;                          // [H][nsamp]
   float *rt;                          // [H][12]: R row-major, then t
   unsigned long long *err;            // [H] fixed-point error sums
-};
-
-struct SacGrid {   // the target grid (PointGrid) as the scoring kernels read it
-  GridArgs g;
-  int gx, gy, gz;
-  float mxx, mxy, mxz;
-  double cell, slack;
 };
 
 __global__ void k_sac_sample(const SacArgs a) {
@@ -169,55 +163,27 @@ __device__ __forceinline__ int sac_cell(float v, float mn, float inv, int gmax) 
   return !(f > 0.f) ? 0 : (f > (float)gmax ? gmax : (int)f);
 }
 // squared distance to the nearest target point when it is <= thr; otherwise some value > thr (the error term is 1 either way)
-__device__ float sac_nn_d2(const GridRegs &r, const SacGrid &G, float qx, float qy, float qz, float thr) {
+__device__ float sac_nn_d2(const GridRegs &r, const RingGrid &G, float qx, float qy, float qz, float thr) {
   {  // outside the box by more than sqrt(thr): no point can be within the threshold
-    const double ex = qx < G.g.mnx ? (double)G.g.mnx - qx : (qx > G.mxx ? (double)qx - G.mxx : 0.0);
-    const double ey = qy < G.g.mny ? (double)G.g.mny - qy : (qy > G.mxy ? (double)qy - G.mxy : 0.0);
-    const double ez = qz < G.g.mnz ? (double)G.g.mnz - qz : (qz > G.mxz ? (double)qz - G.mxz : 0.0);
+    const double ex = qx < G.g.mnx ? (double)G.g.mnx - qx : (qx > G.mx[0] ? (double)qx - G.mx[0] : 0.0);
+    const double ey = qy < G.g.mny ? (double)G.g.mny - qy : (qy > G.mx[1] ? (double)qy - G.mx[1] : 0.0);
+    const double ez = qz < G.g.mnz ? (double)G.g.mnz - qz : (qz > G.mx[2] ? (double)qz - G.mx[2] : 0.0);
     if ((ex * ex + ey * ey) + ez * ez > (double)thr * (1.0 + 1e-5)) return INFINITY;
   }
-  const int cx = sac_cell(qx, G.g.mnx, G.g.inv, G.gx), cy = sac_cell(qy, G.g.mny, G.g.inv, G.gy), cz = sac_cell(qz, G.g.mnz, G.g.inv, G.gz);
-  int rmax = cx;
-  rmax = max(rmax, G.gx - cx); rmax = max(rmax, cy); rmax = max(rmax, G.gy - cy); rmax = max(rmax, cz); rmax = max(rmax, G.gz - cz);
+  const int cx = sac_cell(qx, G.g.mnx, G.g.inv, G.gm[0]), cy = sac_cell(qy, G.g.mny, G.g.inv, G.gm[1]), cz = sac_cell(qz, G.g.mnz, G.g.inv, G.gm[2]);
   float best = INFINITY;
-  for (int ring = 0;; ++ring) {
-    for (int dx = -ring; dx <= ring; ++dx) {
-      const int x = cx + dx;
-      if (x < 0 || x > G.gx) continue;
-      for (int dy = -ring; dy <= ring; ++dy) {
-        const int y = cy + dy;
-        if (y < 0 || y > G.gy) continue;
-        const bool wall = max(abs(dx), abs(dy)) == ring;   // a column on the ring's wall: its whole z-range
-        for (int zs = 0; zs < (wall ? 1 : 2); ++zs) {       // inside the wall: the floor and the ceiling cell
-          int zlo, zhi;
-          if (wall) { zlo = max(cz - ring, 0); zhi = min(cz + ring, G.gz); }
-          else { zlo = zhi = zs == 0 ? cz - ring : cz + ring; if (zlo < 0 || zlo > G.gz) continue; }
-          if (zlo > zhi) continue;
-          const int s0 = r.cstart[lower_cell(r, cell_key(x, y, zlo))], s1 = r.cstart[lower_cell(r, cell_key(x, y, zhi) + 1)];
-          for (int s = s0; s < s1; ++s) {
-            const float d2 = knn_d2(qx, qy, qz, r.sorted[s]);
-            best = d2 < best ? d2 : best;
-          }
+  ring_walk(r, G, cx, cy, cz, INT_MAX,   // no cap: the walk settles by the last ring at the latest
+      [&](int s0, int s1) {
+        for (int s = s0; s < s1; ++s) {
+          const float d2 = knn_d2(qx, qy, qz, r.sorted[s]);
+          best = d2 < best ? d2 : best;
         }
-      }
-    }
-    if (ring >= rmax) break;
-    // every point of an unvisited cell lies at least (ring - slack) cell edges away on some axis
-    const double lb = ((double)ring - G.slack) * G.cell;
-    const double lim = best < thr ? (double)best : (double)thr;
-    if (lb > 0.0 && lim < lb * lb * (1.0 - 1e-5)) break;
-  }
+      },
+      [&] { return best < thr ? (double)best : (double)thr; });
   return best;
 }
 
-// x' = ((R00 x + R01 y) + R02 z) + t0, float32, every operation rounded separately
-__device__ __forceinline__ void sac_move(const float *rt, float x, float y, float z, float &ox, float &oy, float &oz) {
-  ox = ((rt[0] * x + rt[1] * y) + rt[2] * z) + rt[9];
-  oy = ((rt[3] * x + rt[4] * y) + rt[5] * z) + rt[10];
-  oz = ((rt[6] * x + rt[7] * y) + rt[8] * z) + rt[11];
-}
-
-__global__ void __launch_bounds__(SCORE_T) k_sac_score(const SacArgs a, const SacGrid G) {
+__global__ void __launch_bounds__(SCORE_T) k_sac_score(const SacArgs a, const RingGrid G) {
   __shared__ float s_p[SCORE_CHUNK * 3];
   __shared__ float s_rt[SCORE_HB * 12];
   __shared__ int s_ok[SCORE_HB];
@@ -235,7 +201,7 @@ __global__ void __launch_bounds__(SCORE_T) k_sac_score(const SacArgs a, const Sa
     unsigned long long acc = 0ull;
     for (int p = threadIdx.x; p < cnt; p += SCORE_T) {
       float x, y, z;
-      sac_move(s_rt + 12 * hb, s_p[3 * p], s_p[3 * p + 1], s_p[3 * p + 2], x, y, z);
+      ov_move(s_rt + 12 * hb, s_p[3 * p], s_p[3 * p + 1], s_p[3 * p + 2], x, y, z);
       acc += ghicp_sac::sac_term_fx(sac_nn_d2(r, G, x, y, z, a.thr), a.thr);
     }
 #pragma unroll
@@ -283,12 +249,12 @@ __global__ void __launch_bounds__(PICK_T) k_sac_pick(const SacArgs a, int *__res
 
 struct Rt12 { float v[12]; };
 // per source point: the nearest target distance under the chosen transform when within the threshold, else +inf
-__global__ void k_sac_fit(const SacArgs a, const SacGrid G, const Rt12 rt, float *__restrict__ d2o) {
+__global__ void k_sac_fit(const SacArgs a, const RingGrid G, const Rt12 rt, float *__restrict__ d2o) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= a.ns) return;
   const GridRegs r = grid_regs(G.g);
   float x, y, z;
-  sac_move(rt.v, a.P[3 * (size_t)i], a.P[3 * (size_t)i + 1], a.P[3 * (size_t)i + 2], x, y, z);
+  ov_move(rt.v, a.P[3 * (size_t)i], a.P[3 * (size_t)i + 1], a.P[3 * (size_t)i + 2], x, y, z);
   const float d2 = sac_nn_d2(r, G, x, y, z, a.thr);
   d2o[i] = d2 <= a.thr ? d2 : INFINITY;
 }
@@ -345,11 +311,8 @@ cudaError_t sac_run(const float *d_P, const float *d_Fs, int ns, const float *d_
   // about five rings once no point can come within the threshold.  The result does not depend on the cell edge.
   const int kcell = nt < 8 ? nt : 8;
   CUDA_TRY(prep_point_grid(0, d_Q, nt, kcell, 0.f, std::sqrt((double)a.thr) / 4.0, &pg));
-  SacGrid G{};
-  G.g = pg.g; G.gx = pg.gx; G.gy = pg.gy; G.gz = pg.gz; G.mxx = pg.mx[0]; G.mxy = pg.mx[1]; G.mxz = pg.mx[2];
-  G.cell = pg.cell; G.slack = pg.slack;
   dim3 grid((unsigned)nblk(H, SCORE_HB), (unsigned)nblk(ns, SCORE_CHUNK));
-  GHICP_LAUNCH(k_sac_score, grid, SCORE_T, 0, 0, a, G);
+  GHICP_LAUNCH(k_sac_score, grid, SCORE_T, 0, 0, a, pg.rg);
   CUDA_TRY(cudaEventRecord(ev[3], 0));
   GHICP_LAUNCH(k_sac_pick, 1, PICK_T, 0, 0, a, d_pick.get());
   CUDA_TRY(cudaEventRecord(ev[4], 0));
@@ -360,7 +323,7 @@ cudaError_t sac_run(const float *d_P, const float *d_Fs, int ns, const float *d_
   } else {   // no valid hypothesis: the identity, scored like any transform
     rt.v[0] = rt.v[4] = rt.v[8] = 1.f;
   }
-  GHICP_LAUNCH(k_sac_fit, nblk(ns, SAC_T), SAC_T, 0, 0, a, G, rt, d_d2.get());
+  GHICP_LAUNCH(k_sac_fit, nblk(ns, SAC_T), SAC_T, 0, 0, a, pg.rg, rt, d_d2.get());
   CUDA_TRY(cudaGetLastError());
   std::vector<float> d2((size_t)ns);
   CUDA_TRY(cudaMemcpyAsync(d2.data(), d_d2.get(), sizeof(float) * (size_t)ns, cudaMemcpyDeviceToHost, 0));
@@ -390,7 +353,7 @@ cudaError_t sac_run(const float *d_P, const float *d_Fs, int ns, const float *d_
     if (dbg->corr) CUDA_TRY(cudaMemcpy(dbg->corr, a.corr, sizeof(int) * (size_t)H * a.nsamp, cudaMemcpyDeviceToHost));
     if (dbg->rt) CUDA_TRY(cudaMemcpy(dbg->rt, a.rt, sizeof(float) * 12 * (size_t)H, cudaMemcpyDeviceToHost));
     if (dbg->err) CUDA_TRY(cudaMemcpy(dbg->err, a.err, sizeof(unsigned long long) * (size_t)H, cudaMemcpyDeviceToHost));
-    dbg->cell = pg.cell;
+    dbg->cell = pg.rg.cell;
   }
   return cudaSuccess;
 }
