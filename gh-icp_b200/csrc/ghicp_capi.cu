@@ -414,6 +414,7 @@ struct RouteResult {
   int stream_passes = 0;      // > 0: ev[4] / ev[5] were recorded around the route's main streaming pass
   long long candidates = 0;   // NN / NNR filter routes: candidates the filter passed to exact evaluation
   bool exact_redo = false;    // a filter route asks for the all-double redo of its cost stage (which then skips ev[1])
+  bool out_of_range = false;  // ... because its operands left the FP32 filter's window (StreamDev::out_of_range)
 };
 
 // Seed pre-pass (FP32 minima only) before an NN / NNR filter pass?  It keeps the refinement cheap whenever last iteration's
@@ -436,6 +437,7 @@ static int nn_tail(Ctx *c, const LoopScalars &ls, bool cols, double amb_rel, Rou
   CK(c, cudaMemcpyAsync(c->h_iter, c->d_iter, sizeof(DevIter), cudaMemcpyDeviceToHost, c->stream));
   CK(c, cudaStreamSynchronize(c->stream));
   r->candidates = c->last_cands = (long long)c->h_sdev->cand_count[0] + (cols ? c->h_sdev->cand_count[1] : 0);
+  r->out_of_range = c->h_sdev->out_of_range != 0;
   r->exact_redo = c->h_iter->overflow_any || (!cols && c->h_iter->ambiguous > 0);
   if (!r->exact_redo) c->have_prev = true;
   return GHICP_OK;
@@ -543,6 +545,12 @@ static int km_general_tail(Ctx *c, RouteResult *r, Fill fill) {
       CK(c, cudaMemcpyAsync(c->h_rowptr_cut + k, c->d_rowptr + std::min(c->N, k * c->shard), sizeof(long long),
                             cudaMemcpyDeviceToHost, c->stream));
   CK(c, cudaStreamSynchronize(c->stream));
+  if (c->h_iter->overflow_any) {
+    // only the streaming route sets it here (k_finalize_fast): its gate ran outside the FP32 filter's window, and nothing
+    // has been applied yet, so the all-double route takes the iteration over
+    r->exact_redo = r->out_of_range = true;
+    return GHICP_OK;
+  }
   const long long nnz = c->h_iter->nnz;
   const double penalty = c->h_iter->penalty;
   int rc;
@@ -709,7 +717,7 @@ static int host_tail(Ctx *c, const RouteResult &r, bool redone, ghicp_iter_stats
     out->ax = ax; out->ay = ay; out->az = az;
     out->nnz = r.nnz; out->km_rounds = r.kres.rounds; out->km_phases = r.kres.phases;
     out->gpu_launches = c->launches;
-    out->exact_fallback = (r.exact_redo ? 1 : 0) | (redone ? 2 : 0);
+    out->exact_fallback = (r.exact_redo ? 1 : 0) | (redone ? 2 : 0) | (r.out_of_range ? 4 : 0);
     float ms;
     cudaEventElapsedTime(&ms, c->ev[0], c->ev[1]); out->ms_cost = ms;
     cudaEventElapsedTime(&ms, c->ev[1], c->ev[2]); out->ms_corr = ms;

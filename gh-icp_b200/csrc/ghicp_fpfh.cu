@@ -622,15 +622,19 @@ __global__ void k_ff_publish(const FfArgs a, double *row_cd, int *row_idx, doubl
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k == 0) xstats[4 * rank + 2] = a.dev->overflow ? 1.0 : 0.0;   // travels with the statistics
   if (k >= a.row0 && k < a.row0 + a.nloc) {
+    // not found: every CD of the row is NaN or >= 9e20 (clouds of ~1e10 units) -> the reference scan, which starts at
+    // (9e20, 0) and takes a CD only when it is smaller, keeps (9e20, 0)
     const int j = a.rowidx[k];
-    const bool found = j != INT_MAX;   // not found: every CD of the row is NaN -> the reference scan keeps (9e20, 0)
-    row_cd[k] = found ? __longlong_as_double((long long)a.rowbest[k]) : MAXVALIUE;
+    const double v = __longlong_as_double((long long)a.rowbest[k]);
+    const bool found = j != INT_MAX && v < MAXVALIUE;
+    row_cd[k] = found ? v : MAXVALIUE;
     row_idx[k] = found ? j : 0;
   }
   if (col_cd && k < a.M) {
     const int i = a.colidx[k];
-    const bool found = i != INT_MAX;
-    col_cd[k] = found ? __longlong_as_double((long long)a.colbest[k]) : MAXVALIUE;
+    const double v = __longlong_as_double((long long)a.colbest[k]);
+    const bool found = i != INT_MAX && v < MAXVALIUE;
+    col_cd[k] = found ? v : MAXVALIUE;
     col_idx[k] = found ? i : 0;
   }
 }

@@ -209,7 +209,21 @@ struct StreamDev {  // device-resident scalars of the streaming path
   int overflow;          // some candidate did not fit below cand_cap
   unsigned long long nnz_valid;
   unsigned long long emit_count;  // KM: gate hits appended to the edge list by the count pass (may exceed its capacity)
+  int out_of_range;      // A * R^2 outside the window of k_margin's error bound (stream_in_window): all-double route
 };
+// Where the FP32 filter of ghicp_stream.cu keeps every operand and partial sum of d2' = A*|s - t|^2 a normal float (A = the
+// squared ED weight, R2 = the largest squared centred norm): A*R2 in [2^-80, 2^120] (the sums stay below 4*A*R2, the
+// rounding error 2^-150 of a subnormal and the flush of sqrt.approx.ftz stay far below the margin), |T.xyz| = 2*A*|t| below
+// 2^120, and R2 in [2^-100, 2^100] for the coordinates themselves.  A = 0 (BSC iteration 0: no ED term) is always inside.
+// About 10^-5 ... 10^10 units of cloud extent for the usual bbx_magnitude weight (bbx_magnitude ~ 3x the extent).
+constexpr double STREAM_WINDOW_LO = 0x1p-80, STREAM_WINDOW_HI = 0x1p120;
+__host__ __device__ inline bool stream_in_window(double A, double R2) {
+  if (!(R2 >= 0x1p-100 && R2 <= 0x1p100)) return false;
+  if (A == 0.0) return true;
+  const double P = A * R2;
+  return P >= STREAM_WINDOW_LO && P <= STREAM_WINDOW_HI && 4.0 * A * A * R2 <= 0x1p240;
+}
+
 struct StreamArgs {
   const unsigned char *fd;   // packed BSC FD plane (fd_at) or nullptr (no feature)
   size_t fd_rows;            // rows of the plane held by this context

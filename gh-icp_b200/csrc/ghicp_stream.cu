@@ -179,6 +179,9 @@ __global__ void k_prep(const double *__restrict__ s, const double *__restrict__ 
 // Error bound of the FP32 filter.  d2' carries <= 32*2^-24*A*R^2 absolute error (input roundings of
 // S, T + 1 add + 3 fma on magnitudes <= 4*A*R^2, R = max centred norm), so |sqrt(d2'_32) - a*dist| <=
 // sqrt(that); sqrt.approx, the fd FFMA and the float weight add 2^-21-relative terms.
+// The bound holds while every operand and partial sum is a normal float (STREAM_WINDOW_*): below it a rounding costs up to
+// 2^-150 absolutely and sqrt.approx.ftz flushes d2' to 0, above it S.w / T.w overflow and d2' becomes NaN.  Outside the
+// window StreamDev::out_of_range sends the iteration to the all-double route (exact_fallback bit 2).
 __global__ void k_margin(StreamDev *dev, double A, double a, double b, double fdmax, const DevIter *iter,
                          int use_iter_penalty, double rel_slack, double kappa) {
   const double R2 = (double)__uint_as_float(dev->r2max_bits);
@@ -189,6 +192,7 @@ __global__ void k_margin(StreamDev *dev, double A, double a, double b, double fd
   dev->cand_count[0] = 0;
   dev->cand_count[1] = 0;
   dev->overflow = 0;
+  dev->out_of_range = !stream_in_window(A, R2);
   dev->nnz_valid = 0;
   dev->emit_count = 0;
   if (use_iter_penalty) {
@@ -670,7 +674,7 @@ __global__ void k_resolve(const StreamArgs a, int which) {
 __global__ void k_publish(const StreamArgs a, double *row_cd, int *row_idx, double *col_cd, int *col_idx,
                           double *xstats, int rank) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k == 0) xstats[4 * rank + 2] = a.dev->overflow ? 1.0 : 0.0;  // travels with the statistics
+  if (k == 0) xstats[4 * rank + 2] = (a.dev->overflow || a.dev->out_of_range) ? 1.0 : 0.0;  // travels with the statistics
   if (k >= a.row0 && k < a.row0 + a.nloc) {
     row_cd[k] = __longlong_as_double((long long)a.rowbest[k]);
     const int j = a.rowidx[k];
@@ -685,7 +689,8 @@ __global__ void k_publish(const StreamArgs a, double *row_cd, int *row_idx, doub
 
 // fast statistics: this rank's partial sums of CD and CD^2 (the penalty rule runs in k_penalty)
 __global__ void __launch_bounds__(1024) k_finalize_fast(const double *__restrict__ part_stats, int n_parts,
-                                                        double *__restrict__ xstats, int rank, double kappa) {
+                                                        double *__restrict__ xstats, int rank, double kappa,
+                                                        const StreamDev *dev) {
   __shared__ double sm[2][32];
   double a0 = 0.0, a1 = 0.0;
   for (int p = threadIdx.x; p < n_parts; p += blockDim.x) { a0 += part_stats[2 * p]; a1 += part_stats[2 * p + 1]; }
@@ -699,7 +704,7 @@ __global__ void __launch_bounds__(1024) k_finalize_fast(const double *__restrict
     for (int w = 0; w < 32; ++w) { S1 += sm[0][w]; S2 += sm[1][w]; }
     xstats[4 * rank] = S1 / kappa;               // back from the filter's scaled domain
     xstats[4 * rank + 1] = S2 / (kappa * kappa);
-    xstats[4 * rank + 2] = 0.0;
+    xstats[4 * rank + 2] = dev->out_of_range ? 1.0 : 0.0;   // k_penalty: DevIter::overflow_any (KM general route: redo)
   }
 }
 // BSC iterations > 1: the penalty does not depend on this iteration's statistics (src/ghicp_reg.cpp:279-282)
@@ -752,7 +757,7 @@ __global__ void __launch_bounds__(256) k_emit_check(const StreamArgs a, const De
                                                     XBlockHdr *hdr, unsigned long long *__restrict__ xkey,
                                                     double *__restrict__ xgain, float *__restrict__ xfd, unsigned long long xcap) {
   const unsigned long long count = a.dev->emit_count;
-  const bool ovf = count > xcap || count > a.emit_cap;
+  const bool ovf = count > xcap || count > a.emit_cap || a.dev->out_of_range;
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     hdr->count = ovf ? 0ull : count;
     hdr->stats[0] = xstats_rank[0]; hdr->stats[1] = xstats_rank[1];
@@ -996,7 +1001,8 @@ cudaError_t launch_stream_resolve(Ctx *c, const CostParams &cp, bool with_cols) 
 }
 
 cudaError_t launch_finalize_fast(Ctx *c) {
-  GHICP_LAUNCH(k_finalize_fast, 1, 1024, 0, c->stream, c->d_part_stats, stream_num_parts_now(c), c->d_xstats, c->rank, c->kappa);
+  GHICP_LAUNCH(k_finalize_fast, 1, 1024, 0, c->stream, c->d_part_stats, stream_num_parts_now(c), c->d_xstats, c->rank, c->kappa,
+               c->d_sdev);
   c->launches++;
   return cudaGetLastError();
 }

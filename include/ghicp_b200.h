@@ -107,7 +107,9 @@ typedef struct ghicp_iter_stats {
   int km_phases;        /* KM: epsilon-scaling phases */
   int gpu_launches;     /* kernels launched by this call */
   int exact_fallback;   /* bit 0: this iteration re-ran its cost stage with the all-double kernels; bit 1: a settled KM
-                           iteration's candidate block overflowed and the iteration re-ran on the general route */
+                           iteration's candidate block overflowed and the iteration re-ran on the general route; bit 2: the
+                           redo of bit 0 was taken because the keypoints' scale put the FP32 filter's operands outside the
+                           float range its error bound holds in (None / BSC: roughly 1e-5 ... 1e10 units of extent) */
   float ms_cost, ms_corr, ms_solve, ms_total; /* CUDA-event stage times on the ctx stream */
   float ms_stream;      /* CUDA-event time of ONE streaming pass over the FD plane (the dominant kernel) */
   int stream_passes;    /* passes over the FD plane this iteration (1 NN/NNR, +1 seed pass, 2-3 KM) */
